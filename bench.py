@@ -4,7 +4,7 @@
 A "step" is one scheduling cycle: every pending PodGang of the snapshot goes through fit -> (score) -> admit -> commit
 and comes out admitted or rejected, with the result of the SEQUENTIAL priority-ordered pass (oracle/grove_oracle_seq.c).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--config C4] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--config C4] [--impl reference] [--dump-outputs DIR]
 
 `value`       whole-job admitted gangs / second, node table already resident in HBM (per step: device->device reset of
               the node table, then the cycle).
@@ -22,6 +22,8 @@ and comes out admitted or rejected, with the result of the SEQUENTIAL priority-o
 --config C4X  the part of the path that DOES shard: the score pass (K1 + K2) on a cluster 4x C4, node-range shards, one rank per
               GPU, ONE all-reduce of per-shard feasibility / capacity counts (NCCL); strong scaling, pairs scored per second.
 --config C5   steady-state churn (BASELINE.json config 5); C1..C3 the smaller configurations.
+--dump-outputs DIR   after the timed steps, what the last timed step computed (the arrays its caller receives) as DIR/<name>.npy,
+              float64, one column per field of a record; the inputs are seeded, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -46,7 +48,7 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 class ClockSampler:
@@ -84,6 +86,27 @@ class ClockSampler:
                 "reasons": reasons, "samples": len(sm)}
 
 
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """--dump-outputs: each array as out_dir/<name>.npy in float64 (exact for the u32 / i32 fields), a record array as one column
+    per flattened field.  Above DUMP_BYTES in all, every array keeps the same share of its rows, a fixed seeded sample in order."""
+    from numpy.lib import recfunctions as rf
+    os.makedirs(out_dir, exist_ok=True)
+    flat = {}
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        a = rf.structured_to_unstructured(a, dtype=np.float64) if a.dtype.names else a.astype(np.float64)
+        flat[name] = a.reshape(len(a), -1)
+    total = sum(a.nbytes for a in flat.values())
+    for name, a in flat.items():
+        if total > DUMP_BYTES:
+            keep = int(len(a) * DUMP_BYTES // total)
+            a = a[np.sort(np.random.default_rng(0).choice(len(a), keep, replace=False))]
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+
+
 def make_workload(name: str, replica: int = 0):
     """replica r > 0: an independent cluster of the same shape (rank-specific seed)"""
     cfg = synth.CONFIGS[name]() if replica == 0 or name == "C1" else synth.CONFIGS[name](seed=synth.SEED_BASE + int(name[1]) + 1000 * replica)
@@ -112,7 +135,7 @@ def workload_desc(name, n_nodes, n_gangs, n_cliques, n_gpus):
             "pairs_per_full_pass": int(n_nodes) * int(n_cliques),
             "semantics": "sequential pass in (priority desc, submission index asc) order",
             "parallelism": "1 cluster on 1 GPU" if n_gpus == 1 else f"replicas only: {n_gpus} independent clusters, one per GPU",
-            "l2": "inputs change every step (node table reset, claims rebuilt); the 126 MB L2 holds the working set by design"}
+            "l2": "inputs change every step (node table reset, claims rebuilt); the H100's 50 MB L2 holds the working set by design"}
 
 
 def prefix_sample(g, c, s, keep):
@@ -168,6 +191,9 @@ def run_reference(args):
         r = O.run_cycle(nodes, L, sg, sc, ss, threads=cores)
         adm = r["stats"]["gangs_admitted"]
     dt = (time.perf_counter() - t0) / args.steps
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"placements": r["placements"], "gang_status": r["status"],
+                                         "scope_domains": r["scope_status"], "nodes": r["nodes_after"]})
     val = adm / dt
     line = {
         "impl": "reference", "metric": "podgang_placements_per_sec", "value": val, "unit": "gangs/s",
@@ -181,22 +207,6 @@ def run_reference(args):
         "gpu_launches": 0,
     }
     print(json.dumps(line))
-
-
-def ncu_traffic():
-    """DRAM bytes (read + write) of one k_score launch over the whole C4 submission, from the committed `ncu --set full`
-    capture (profiles/r2_ncu_k_score_raw.csv); None when the capture is absent."""
-    import csv
-    for name in ("r2_ncu_k_score_raw.csv", "r1_ncu_k_score_raw.csv"):
-        try:
-            rows = list(csv.reader(open(os.path.join(ROOT, "profiles", name))))
-            h, units, vals = rows[0], rows[1], rows[2]
-            scale = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-            tot = sum(float(vals[h.index(k)].replace(",", "")) * scale[units[h.index(k)]] for k in ("dram__bytes_read.sum", "dram__bytes_write.sum"))
-            return tot, name
-        except (OSError, ValueError, KeyError, IndexError):
-            continue
-    return None, None
 
 
 def run_gpu(args):
@@ -259,6 +269,8 @@ def run_gpu(args):
         evals += st["evaluations"]
     sync()
     dt = time.perf_counter() - t0
+    if args.dump_outputs and rank == 0:   # read back before the e2e steps below run the cycle again
+        outs = {"placements": eng.placements(), "gang_status": eng.gang_status(), "scope_domains": eng.scope_domains(), "nodes": eng.nodes()}
     # e2e through the C ABI with host buffers
     for _ in range(max(1, args.warmup // 2)):
         step_e2e()
@@ -292,7 +304,6 @@ def run_gpu(args):
         eng.build_score_matrix()
     k2_ms = float(np.mean([eng.build_score_matrix() for _ in range(args.steps)]))
     achieved = k2_bytes / (k2_ms * 1e-3) / 1e9 if k2_ms > 0 else 0.0
-    traffic, traffic_src = ncu_traffic() if args.config == "C4" else (None, None)
     d2h = pl.nbytes + gs.nbytes
     ms_cycle = acc["ms_total"] / args.steps
     cpu = None
@@ -322,13 +333,13 @@ def run_gpu(args):
                 "h2d_bytes_per_step": int(h2d) * world, "d2h_bytes_per_step": int(d2h) * world},
         "gpu_launches": int(launches),
         "roofline": {"kernel": "k_score (K2 topology-distance score matrix), timed alone", "bound": "hbm", "achieved": achieved, "peak": peak,
-                     "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
-                     "traffic_note": None if traffic is None else f"DRAM read+write of one k_score launch over the whole submission, profiles/{traffic_src}",
+                     "unit": "GB/s", "frac": achieved / peak, "traffic": None,
                      "peak_source": peak_src, "algorithmic_bytes_per_launch": k2_bytes, "ms_per_launch": k2_ms,
                      "on_critical_path": False,
                      "note": "the admission (K3) derives its visiting order from the anchor's domain ranges and never reads the score matrix: K2 is "
                              "built on request (grove_build_score_matrix) and is not part of `value`; it is write-dominated (1 B written per 1/8 B read), "
-                             "so ~0.6 of the copy peak is its DRAM ceiling",
+                             "and the fit words it reads are shared by every clique of a signature and served from L2, so the algorithmic "
+                             "figure can exceed the DRAM peak: its DRAM traffic is the 1 B written per pair",
                      "whole_cycle": {"ms_device": ms_cycle,
                                      "frac_k2_bytes_model": (k2_bytes / (ms_cycle * 1e-3) / 1e9) / peak,
                                      "frac_survey_model_2.375B_per_pair": (2.375 * pairs / (ms_cycle * 1e-3) / 1e9) / peak,
@@ -339,6 +350,8 @@ def run_gpu(args):
         "kernel_ms_per_step": {k: v / args.steps for k, v in acc.items()},
         "cpu_baseline": cpu,
     }
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, outs)
     print(json.dumps(line))
     if dist is not None:
         dist.destroy_process_group()
@@ -426,7 +439,7 @@ def run_sharded(args):
             "config": {"workload": f"C4X: score pass (K1 + K2 + per-shard feasibility, no admission) on {len(nodes)} nodes / {len(g)} PodGangs / "
                                    f"{len(c)} PodCliques, 4-level tree; node-range shards cut at zone boundaries, one all-reduce(SUM) of int32[G + Q]",
                        "nodes": len(nodes), "gangs": len(g), "cliques": len(c), "pairs_per_full_pass": pairs,
-                       "parallelism": f"{world} node-range shard(s), one per GPU", "l2": "each step writes a score-matrix shard far larger than the 126 MB L2"},
+                       "parallelism": f"{world} node-range shard(s), one per GPU", "l2": "each step writes a score-matrix shard far larger than the H100's 50 MB L2"},
             "result": {"gangs_infeasible_from_snapshot": int(bad.sum()), "all_reduce_bytes": int(4 * (len(g) + len(c))),
                        "collective_s_per_step_max_over_ranks": s_coll, "shard_nodes_rank0": int(hi - lo), "score_matrix_bytes_total": int(pairs)},
             "clocks": clocks,
@@ -436,9 +449,11 @@ def run_sharded(args):
             "roofline": {"kernel": "k_fit + k_score over this rank's node range (grove_run_score_pass), slowest rank", "bound": "hbm", "achieved": ach,
                          "peak": peak, "unit": "GB/s", "frac": ach / peak, "traffic": None, "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": shard_bytes, "ms_per_launch": ms_kernel,
-                         "note": "1 B written + 1/8 B read per (clique, node) pair of the shard; the pass is write-dominated (~0.6 of the copy peak is its DRAM ceiling)"},
+                         "note": "1 B written + 1/8 B read per (clique, node) pair of the shard; the pass is write-dominated and its fit words are served from L2"},
             "cpu_baseline": None,
         }
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, {"shard_summary": total})
         print(json.dumps(line))
     if dist is not None:
         dist.destroy_process_group()
@@ -493,6 +508,8 @@ def run_churn(args):
         cpu_t += time.perf_counter() - tc; cpu_adm += r["stats"]["gangs_admitted"]
         same &= bool(np.array_equal(r["placements"], pl) and np.array_equal(r["status"], gs))
     clocks = sampler.stop()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"placements": pl, "gang_status": gs})
     ms_tick, ms_cyc = float(np.mean(t_tick)), float(np.mean(t_cycle))
     line = {
         "metric": "podgang_placements_per_sec", "value": adm / (sum(t_cycle) * 1e-3), "unit": "gangs/s", "n_gpus": 1,
@@ -524,7 +541,10 @@ def main():
     ap.add_argument("--config", default="C4", choices=sorted(synth.CONFIGS) + ["C5", "C4X"])
     ap.add_argument("--impl", default="grove_b200", choices=["grove_b200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 0)
     if args.impl == "reference":
         if args.config == "C4X":

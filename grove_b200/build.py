@@ -1,4 +1,4 @@
-"""In-tree build of libgrove_place.so (nvcc, sm_100a only)."""
+"""In-tree build of libgrove_place.so (nvcc, sm_90a only)."""
 from __future__ import annotations
 
 import os
@@ -12,7 +12,7 @@ DEPS = ["engine.cu", "kernels.cuh", "common.cuh", "tables.cuh", "fit.cuh", "scor
         os.path.join("..", "..", "include", "grove_place.h")]
 NVCC_FLAGS = [
     "-DGROVE_INLINE_ALL",
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall", "-Xcompiler", "-fopenmp", "-shared", "-cudart", "shared", "-lgomp",
 ]
 
@@ -28,7 +28,8 @@ def stale() -> bool:
     if not os.path.exists(LIB):
         return True
     t = os.path.getmtime(LIB)
-    return any(os.path.getmtime(os.path.join(CSRC, d)) > t for d in DEPS)
+    # this file holds the flags: a library built with other flags (another architecture) is stale too
+    return os.path.getmtime(__file__) > t or any(os.path.getmtime(os.path.join(CSRC, d)) > t for d in DEPS)
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
@@ -37,7 +38,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
         env = dict(os.environ)
-        env.pop("CC", None); env.pop("CXX", None)  # /opt/gcc wrappers in this image lack libgomp specs
+        env.pop("CC", None); env.pop("CXX", None)  # a CC/CXX wrapper without libgomp specs would break -fopenmp
         subprocess.check_call(cmd, env=env)
     return LIB
 

@@ -173,7 +173,7 @@ struct grove_engine {
   DevBuf<grove_placement_t> d_out;
   bool any_preferred = false;  // some gang / scope / clique carries a Preferred level
   uint32_t max_gang_pods = 0;
-  uint32_t n_sm = 148;
+  uint32_t n_sm = 132;  // H100 SXM; replaced by the device's own count at creation
   uint32_t cap_off[GROVE_MAX_LEVELS]{}, cap_stride = 0;
   bool dbg_on = false;
   DevBuf<uint32_t> d_dbg;

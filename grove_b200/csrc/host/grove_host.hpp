@@ -9,7 +9,7 @@
 //   CreatePodGroupsForPodGang                     .../components/podgang/podgang.go:165-186
 //   isBasePodGangScheduled / scheduling gates     operator/internal/controller/podclique/components/pod/syncflow.go:255-358
 //
-// (all paths relative to /root/reference).  Error convention: Go returns `error`; here every fallible
+// (all paths relative to ai-dynamo/grove).  Error convention: Go returns `error`; here every fallible
 // call returns std::optional<Error> (nullopt == nil), and Error carries the GroveError fields
 // (operator/internal/errors/errors.go:41-86).
 #pragma once

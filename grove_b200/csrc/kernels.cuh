@@ -1,4 +1,4 @@
-// kernels.cuh -- sm_100a kernels of the gang-placement cycle (umbrella include).
+// kernels.cuh -- sm_90a kernels of the gang-placement cycle (umbrella include).
 //
 //   tables.cuh   k_gather / k_scatter / k_update / k_anchor               table (un)packing
 //   fit.cuh      k_fit  K1  node x clique-signature resource-fit bitmap   (Filter; oracle: fit())

@@ -1,7 +1,7 @@
 """Kubernetes manifests -> packed tables (the data formats either side of the hot path).
 
 * Node manifests in the shape the reference's KWOK generator emits
-  (/root/reference operator/hack/infra_manager/kwok.py:74-117): allocatable {cpu, memory, pods[, nvidia.com/gpu]},
+  (ai-dynamo/grove operator/hack/infra_manager/kwok.py:74-117): allocatable {cpu, memory, pods[, nvidia.com/gpu]},
   topology labels, NoSchedule taints, spec.unschedulable.
 * PodGang manifests in the CRD's shape (scheduler/api/core/v1alpha1/podgang.go:51-131,
   crds/scheduler.grove.io_podgangs.yaml): podgroups[].{name, podReferences, minReplicas,
@@ -146,7 +146,7 @@ def podgangs_from_manifests(podgangs, requests, level_keys, priority_classes=Non
 
 # ------------------------------------------------------------------------------------------------
 # The producer: PodCliqueSet -> PodGang manifests (the Python counterpart of ComputeExpectedPodGangs in
-# grove_b200/csrc/host; /root/reference operator/internal/controller/podcliqueset/components/podgang/syncflow.go:145-371,
+# grove_b200/csrc/host; ai-dynamo/grove operator/internal/controller/podcliqueset/components/podgang/syncflow.go:145-371,
 # names from operator/api/common/namegen.go:70-117, PodGroups from .../podgang/podgang.go:165-186).
 # ------------------------------------------------------------------------------------------------
 def podgangs_from_pcs(pcs: dict, topology_levels, tas_enabled: bool = True):

@@ -2,8 +2,8 @@
 
 One cluster is ONE sequential dependency chain over ~1.6 MB of node state: a cycle is bound by the latency of its
 relaxation rounds, not by bytes or flops, so splitting it over GPUs would put a collective (>= 10-20 us on NVLink,
-per round) on a critical path whose rounds cost a few tens of microseconds -- measured in round 1: 1/2/4/8 GPUs
-went 1.94 -> 2.50 ms.  What does scale is the number of clusters: a scheduler instance per cluster (or per
+per round) on a critical path whose rounds cost a few tens of microseconds -- round 1 measured it: the cycle got
+slower as GPUs were added.  What does scale is the number of clusters: a scheduler instance per cluster (or per
 federated partition), one per GPU, no data-path collective.  This module is the thin orchestration of that: every
 rank runs its own cycle, and the only communication is the bookkeeping reduction (max time over ranks, sum of
 units) that bench.py reports.  It works with any torch.distributed backend (NCCL on the GPU box, gloo in the CPU

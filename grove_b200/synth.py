@@ -1,7 +1,7 @@
 """Synthetic cluster snapshots and pending-gang tables (measurement fixtures + e2e shapes).
 
 Node side restates the reference's KWOK fake-node generator: topology labels by integer division of
-the node index and a fixed allocatable (/root/reference operator/hack/infra_manager/kwok.py:55-117,
+the node index and a fixed allocatable (ai-dynamo/grove operator/hack/infra_manager/kwok.py:55-117,
 constants.py:65-67,195-197).  Gang side restates the structure the operator's PodGang builder emits
 for a PodCliqueSet -- a base gang per PCS replica holding standalone cliques plus the first
 minAvailable replicas of each scaling group, and one scaled gang per further scaling-group replica

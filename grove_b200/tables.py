@@ -2,7 +2,7 @@
 
 The record layouts are the wire format between the host side (a scheduler backend's cycle loop)
 and libgrove_place.so.  Field meanings follow the reference's PodGang schema
-(/root/reference scheduler/api/core/v1alpha1/podgang.go:51-131); see include/grove_place.h.
+(ai-dynamo/grove scheduler/api/core/v1alpha1/podgang.go:51-131); see include/grove_place.h.
 """
 from __future__ import annotations
 

@@ -1,5 +1,5 @@
 /*
- * grove_place.h -- C ABI of libgrove_place.so, the B200 gang-placement engine.
+ * grove_place.h -- C ABI of libgrove_place.so, the H100 (sm_90a) gang-placement engine.
  *
  * This is the drop-in boundary for the scheduling-cycle hot path named in
  * BASELINE.json (resource fit -> topology score -> all-or-nothing gang

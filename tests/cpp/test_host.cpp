@@ -1,5 +1,5 @@
 // Host-side mirror tests.  The producer cases are the reference's own table-driven vectors
-// (/root/reference operator/internal/controller/podcliqueset/components/podgang/syncflow_test.go:740-953
+// (ai-dynamo/grove operator/internal/controller/podcliqueset/components/podgang/syncflow_test.go:740-953
 // TestComputeExpectedPodGangs and :965-1420 TestComputeExpectedPodGangsWithTopologyConstraints),
 // transcribed: same inputs, same expected PodGang names, counts and topology keys.
 //   test_host cpu   producer + encoder (no GPU)        test_host gpu   + GpuBackend cycles on cuda:0

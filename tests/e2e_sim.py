@@ -1,4 +1,4 @@
-"""Replay harness for the reference's multi-step gang-scheduling suites (/root/reference
+"""Replay harness for the reference's multi-step gang-scheduling suites (ai-dynamo/grove
 operator/e2e/tests/gang_scheduling_test.go GS2-GS12): a kwok-shaped cluster whose nodes are cordoned and
 uncordoned step by step, PodCliqueSets that are scaled between scheduling passes, and a placement function
 (the oracle or the CUDA engine) run once per step over everything that is pending.

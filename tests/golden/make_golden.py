@@ -1,10 +1,9 @@
 """Regenerates tests/golden/*.npz.
 
-The reference (/root/reference, ai-dynamo/grove @ 08ad3b37) is Go, contains no scheduler and cannot
-be built or imported here, so there is no reference OUTPUT to record.  These fixtures are small
+The reference (ai-dynamo/grove @ 08ad3b37) is Go and contains no scheduler, so there is no reference OUTPUT to record.  These fixtures are small
 snapshots in the shapes of the reference's e2e suites and BASELINE.json configs together with the
 sequential oracle's answer (oracle/grove_oracle_seq.c) at the commit that generated them; they pin (a) the oracle against silent drift and
-(b) the CUDA path on the GPU box, where neither /root/reference nor this generator needs to run.
+(b) the CUDA path on the GPU, where neither the reference nor this generator needs to run.
 
     python tests/golden/make_golden.py
 """

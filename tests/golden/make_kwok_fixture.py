@@ -1,10 +1,9 @@
 """Generates tests/golden/kwok_nodes_60.json by RUNNING the reference's own KWOK node generator
-(/root/reference operator/hack/infra_manager/kwok.py: topology_labels :55-71, node_manifest :74-117)
-in this container.  The reference package imports `sh` (a CLI helper, not installed and not needed by
-the two pure functions used here); it is stubbed for the import only -- nothing under /root/reference
-is modified or copied.  The fixture travels to the GPU box; the reference does not.
+(ai-dynamo/grove operator/hack/infra_manager/kwok.py: topology_labels :55-71, node_manifest :74-117).  The reference package imports `sh` (a CLI helper, not installed and not needed by
+the two pure functions used here); it is stubbed for the import only -- nothing of the reference
+is modified or copied.  The tests read the fixture; they never need the reference.
 
-    python tests/golden/make_kwok_fixture.py
+    GROVE_REFERENCE=<checkout of ai-dynamo/grove @ 08ad3b37> python tests/golden/make_kwok_fixture.py
 """
 import json
 import os
@@ -12,7 +11,7 @@ import sys
 import types
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF = "/root/reference/operator/hack"
+REF = os.path.join(os.environ["GROVE_REFERENCE"], "operator", "hack")
 
 
 def main():

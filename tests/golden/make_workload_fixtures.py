@@ -1,6 +1,6 @@
 """Extract the PodCliqueSets of the reference's e2e / sample workloads into a small JSON fixture.
 
-    python tests/golden/make_workload_fixtures.py     (run in the build container: reads /root/reference)
+    GROVE_REFERENCE=<checkout of ai-dynamo/grove @ 08ad3b37> python tests/golden/make_workload_fixtures.py
 
 Only the fields a scheduler's input depends on are kept: per clique name / replicas / minAvailable / resource
 requests / node selector + tolerations (as a flag) / packDomain; per PodCliqueScalingGroup name / cliqueNames /
@@ -14,7 +14,7 @@ import os
 
 import yaml
 
-REF = "/root/reference/operator"
+REF = os.path.join(os.environ["GROVE_REFERENCE"], "operator")
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 

@@ -32,10 +32,10 @@ def test_library_exports_every_declared_symbol(built_lib):
     assert lib.grove_abi_version() == 2
 
 
-def test_library_is_sm100a_only(built_lib):
+def test_library_is_sm90a_only(built_lib):
     out = subprocess.run(["cuobjdump", "-lelf", built_lib], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_\d+a?", out))
-    assert archs == {"sm_100a"}, archs
+    assert archs == {"sm_90a"}, archs
 
 
 def test_struct_layouts_match_header(tmp_path):

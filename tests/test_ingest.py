@@ -1,6 +1,6 @@
 """Manifests -> tables, pinned on output of the reference's own KWOK node generator
 (tests/golden/kwok_nodes_60.json, made by tests/golden/make_kwok_fixture.py importing
-/root/reference operator/hack/infra_manager/kwok.py in the build container)."""
+ai-dynamo/grove operator/hack/infra_manager/kwok.py in the build container)."""
 import json
 import os
 

@@ -1,5 +1,5 @@
 """The oracle against the only placement OUTCOMES the reference pins: the live-cluster e2e suites
-(/root/reference operator/e2e/tests/gang_scheduling_test.go GS1-GS12, topology_test.go TAS2-TAS17),
+(ai-dynamo/grove operator/e2e/tests/gang_scheduling_test.go GS1-GS12, topology_test.go TAS2-TAS17),
 restated as properties over synthetic snapshots of the same shape (150 MiB nodes, 80/40/20/500 MiB
 pods, zone/block/rack/host labels).  Node-level choices below these properties are unpinned
 (DESIGN.md "Oracle").

@@ -1,4 +1,4 @@
-"""Preferred pack levels (/root/reference scheduler/api/core/v1alpha1/podgang.go:110-117): "best-effort
+"""Preferred pack levels (ai-dynamo/grove scheduler/api/core/v1alpha1/podgang.go:110-117): "best-effort
 topology constraint ... not binding on the scheduler ... Scheduler can fall back to higher topology levels
 (upto Required constraint) if preferred cannot be satisfied."  The operator never populates the field
 (syncflow.go:366-368 sets Required only) and no reference test exercises it, so these properties restate

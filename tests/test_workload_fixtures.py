@@ -1,5 +1,5 @@
 """The reference's own workload files, end to end: tests/golden/workloads.json (extracted from
-/root/reference operator/e2e/yaml/*.yaml and samples/simple/simple1.yaml by tests/golden/make_workload_fixtures.py)
+ai-dynamo/grove operator/e2e/yaml/*.yaml and samples/simple/simple1.yaml by tests/golden/make_workload_fixtures.py)
 -> producer (grove_b200/ingest.podgangs_from_pcs, the Python counterpart of ComputeExpectedPodGangs) -> PodGang
 manifests -> packed tables -> oracle, with the outcome each e2e suite asserts for its file."""
 import json
