@@ -693,6 +693,7 @@ __device__ __forceinline__ void score_unit(uint32_t req, uint32_t pref, int got,
 __global__ void __launch_bounds__(128) k_shape_plaus(Topo tp, Tables tb, Relax rx, const uint32_t* __restrict__ shape_rep) {
   __shared__ GangShared sh;
   __shared__ uint32_t s_bits;
+  cudaGridDependencySynchronize();   // (launched chained: engine.cu launch_chained)
   const uint32_t shape = blockIdx.y, l = blockIdx.z;
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5, slot = threadIdx.x & 3u;
   const uint32_t gi = shape_rep[shape];
@@ -739,37 +740,57 @@ __device__ __forceinline__ uint32_t eval_list_at(const Relax& rx, const Tables& 
   return tb.by_rank[rx.ctl[kEntryLo] + (i - nh - nl)];
 }
 
-// K3 launch forms: kW warps share ONE gang.  The candidates of the gang's level are pre-filtered 1024 at a time by all
-// warps (a lane each); the plausible ones are then attempted kW at a time, a warp each, and the lowest successful
-// candidate IN ORDER is the answer -- exactly what trying them one after the other gives, minus the waiting.  kW = 1
-// while a round has many gangs (what matters is gangs in flight), 4 / 8 when it has few (what matters is the
-// latency of the slowest gang: a round lasts as long as its slowest evaluation).
-// Two launches per round, side by side on two streams: the LIGHT gangs (the tail of the list: most gangs, answered by their
-// first or second candidate) a warp each -- every resident warp does useful work --, the HEAVY ones (the head: gangs whose
-// last evaluation needed many attempts) kW warps each.  A light evaluation that is still unanswered after `max_att` attempts
-// gives up (kEvalDeferred): the gang stays dirty and comes back as a heavy one next round, instead of holding the round up.
-// Writes the "nxt" scratch of the gang.
+// K3, one launch per round: CTAs of kEvalWarps warps take work items from a queue (ctl[kEvalNext]), in list order.  First the
+// HEAVY gangs (the head of the list: their last evaluation needed many attempts), an item each, evaluated by the whole CTA; then
+// the LIGHT ones (the tail of the list and the new entrants: most gangs, answered by their first or second candidate) in groups
+// of consecutive entries, a warp each.  Heavy first is longest-first list scheduling: a round lasts as long as its slowest
+// evaluation.  A light group holds as many entries as spread the light gangs over every CTA of the grid (at most kEvalWarps):
+// a round with a few hundred of them puts one warp on each SM rather than eight on a few.
+// A TEAM (the CTA, or one warp) evaluates one gang.  The candidates of the gang's level are pre-filtered 1024 at a time by all
+// its warps (a lane each); the plausible ones are then attempted a warp each, and the lowest successful candidate IN ORDER is the
+// answer -- exactly what trying them one after the other gives, minus the waiting.  A light evaluation that is still unanswered
+// after `max_att` attempts gives up (kEvalDeferred): the gang stays dirty and comes back as a heavy one next round, instead of
+// holding the round up.  Writes the "nxt" scratch of the gang.
+// Launched as a programmatic dependent of the kernel before it (engine.cu launch_chained): nothing is read before
+// cudaGridDependencySynchronize().
 constexpr uint32_t kEvalDeferred = 0xFFu;   // nxt_tstate: no result this round
-constexpr int kHeavyWarps = 8;
-template <bool kPref, int kW, bool kHeavy>
-__global__ void __launch_bounds__(kW * 32, kW == 1 ? 16 : 2) k_eval(Topo tp, Tables tb, Relax rx, uint32_t max_att) {
-  __shared__ GangShared shs[kW];
-  __shared__ int4 s_view[kW][kStageMax];
-  __shared__ uint32_t s_vflag[kW][kStageMax];
-  __shared__ __align__(16) uint8_t s_rk[kW][kStageMax + 256];
-  __shared__ uint32_t s_plaus[32];   // plausible candidates of the current 1024-candidate chunk, in order
-  __shared__ uint32_t s_cl[kW][32], s_ch[kW][32];   // node ranges of the first chunk's candidates (kW runs of 32)
-  __shared__ uint32_t s_win, s_ext, s_att, s_npl;
+constexpr int kEvalWarps = 8;
+template <bool kPref>
+__global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb, Relax rx, uint32_t max_att) {
+  __shared__ GangShared shs[kEvalWarps];
+  __shared__ int4 s_view[kEvalWarps][kStageMax];
+  __shared__ uint32_t s_vflag[kEvalWarps][kStageMax];
+  __shared__ __align__(16) uint8_t s_rk[kEvalWarps][kStageMax + 256];
+  // per team, in the row of its first warp w0: the plausible candidates of the current 1024-candidate chunk, in order; the
+  // winning attempt, the extent read, the attempts and the plausible candidates so far
+  __shared__ uint32_t s_plaus[kEvalWarps][32];
+  __shared__ uint32_t s_win[kEvalWarps], s_ext[kEvalWarps], s_att[kEvalWarps], s_npl[kEvalWarps];
+  __shared__ uint32_t s_cl[kEvalWarps][32], s_ch[kEvalWarps][32];   // node ranges of the first chunk's candidates: run c in row w0 + c
+  __shared__ uint32_t s_item;
+  cudaGridDependencySynchronize();
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const uint32_t n_eval = rx.ctl[kNEval], n_heavy = rx.ctl[kNHeavy];
   if (rx.ctl[kDone]) return;
+  const uint32_t n_eval = rx.ctl[kNEval], n_heavy = rx.ctl[kNHeavy];
+  const uint32_t n_light = n_eval - n_heavy;
+  const uint32_t grp = min(uint32_t(kEvalWarps), max(1u, (n_light + gridDim.x - 1u) / gridDim.x));   // light entries per item
+  const uint32_t n_items = n_heavy + (n_light + grp - 1u) / grp;
   GangShared& sh = shs[warp];
-  const uint32_t seg_lo = kHeavy ? 0u : n_heavy, seg_hi = kHeavy ? n_heavy : n_eval;
-  for (uint32_t ei = seg_lo + blockIdx.x; ei < seg_hi; ei += gridDim.x) {
+  for (;;) {
+    __syncthreads();   // the previous item's shared state is no longer read
+    if (threadIdx.x == 0) s_item = atomicAdd(rx.ctl + kEvalNext, 1u);
+    __syncthreads();
+    const uint32_t item = s_item;
+    if (item >= n_items) break;
+    const bool cta = item < n_heavy;                  // CTA-uniform
+    const uint32_t ei = cta ? item : n_heavy + (item - n_heavy) * grp + warp;
+    if (!cta && (warp >= grp || ei >= n_eval)) continue;
+    const uint32_t tw = cta ? uint32_t(kEvalWarps) : 1u;   // warps in the team
+    const uint32_t w0 = cta ? 0u : warp;                   // the team's first warp
+    const uint32_t wi = cta ? warp : 0u, tt = cta ? threadIdx.x : lane;   // warp / thread within the team
+    auto team_sync = [cta]() { if (cta) __syncthreads(); else __syncwarp(); };
     const uint32_t gi = eval_list_at(rx, tb, ei);
     const grove_gang_t gg = tb.gangs[gi];
     const GangInfo info = tb.ginfo[gi];
-    __syncthreads();   // the previous gang's shared state is no longer read
     // the gang's cliques and scopes (a lane each), the words of the re-evaluation shortcut and the base gang's rank are asked for
     // BEFORE anything looks at them: one L2 round trip for all of them instead of one per question
     const bool has_c = lane < gg.n_cliques, has_s = lane < gg.n_scopes;
@@ -789,10 +810,10 @@ __global__ void __launch_bounds__(kW * 32, kW == 1 ? 16 : 2) k_eval(Topo tp, Tab
       if (bs != GROVE_GANG_ADMITTED) trivial = GROVE_GANG_BASE_REJECTED;
     }
     if (trivial) {
-      if (threadIdx.x == 0) {
+      if (tt == 0) {
         rx.nxt_tstate[gi] = uint8_t(trivial); rx.nxt_n[gi] = 0; rx.nxt_info[gi] = 0xFFu; rx.nxt_glo[gi] = GROVE_NONE_U32; rx.nxt_extent[gi] = 0;
       }
-      for (uint32_t si = threadIdx.x; si < gg.n_scopes; si += kW * 32) { rx.nxt_sc_lvl[gg.scope_off + si] = 0xFFu; rx.nxt_sc_lo[gg.scope_off + si] = GROVE_NONE_U32; }
+      for (uint32_t si = tt; si < gg.n_scopes; si += tw * 32) { rx.nxt_sc_lvl[gg.scope_off + si] = 0xFFu; rx.nxt_sc_lo[gg.scope_off + si] = GROVE_NONE_U32; }
       continue;
     }
     GangRegs g;
@@ -812,8 +833,8 @@ __global__ void __launch_bounds__(kW * 32, kW == 1 ? 16 : 2) k_eval(Topo tp, Tab
       sh.Hlo[c] = 0; sh.Hhi[c] = 0; sh.c_got[c] = -1;
     }
     if (has_s) { sh.scopes[lane] = sc0; sh.s_got[lane] = -1; sh.s_lo[lane] = 0; }
-    if (threadIdx.x == 0) { s_win = GROVE_NONE_U32; s_ext = 0; s_att = 0; s_npl = 0; }
-    __syncthreads();
+    if (tt == 0) { s_win[w0] = GROVE_NONE_U32; s_ext[w0] = 0; s_att[w0] = 0; s_npl[w0] = 0; }
+    team_sync();
     // A candidate that failed in the gang's last evaluation fails again unless a claim was withdrawn inside it since: views only
     // shrink otherwise (claims are added, settled claims move into the committed state).  So a re-evaluation skips the
     // candidates in front of its last answer that no withdrawal touched -- gangs that meet a nearly full cluster would
@@ -836,13 +857,13 @@ __global__ void __launch_bounds__(kW * 32, kW == 1 ? 16 : 2) k_eval(Topo tp, Tab
     do {
       if (gl < 0) {
         staged = false;
-        if (warp == 0) {
+        if (wi == 0) {
           won = place_in(ev, gg.n_scopes, 0, tp.n, -1);
-          if (won) { g_got = -1; g_lo = 0; if (lane == 0) s_win = 0; }
-          if (lane == 0) s_att += 1;
+          if (won) { g_got = -1; g_lo = 0; if (lane == 0) s_win[w0] = 0; }
+          if (lane == 0) s_att[w0] += 1;
         }
-        __syncthreads();
-        done = s_win != GROVE_NONE_U32;
+        team_sync();
+        done = s_win[w0] != GROVE_NONE_U32;
       } else {
         // candidate domains of level gl in score order: up to kMaxPieces ranges of domain indices
         uint32_t r0[kMaxPieces], rcnt[kMaxPieces], D = 0;
@@ -861,10 +882,10 @@ __global__ void __launch_bounds__(kW * 32, kW == 1 ? 16 : 2) k_eval(Topo tp, Tab
           dl = __ldg(tp.dom_lo[gl] + d); dh = __ldg(tp.dom_hi[gl] + d);
           return d;
         };
-        // candidates are taken in chunks that grow (kW x 32, then up to 1024): most gangs succeed among the first few
-        for (uint32_t base = 0, nchunk = kW; base < D && !done && !gave_up; base += nchunk * 32, nchunk = min(32u, nchunk * 4u)) {
-          // pre-filter: nchunk runs of 32 candidates, dealt to the warps
-          for (uint32_t c = warp; c < nchunk; c += kW) {
+        // candidates are taken in chunks that grow (tw x 32, then up to 1024): most gangs succeed among the first few
+        for (uint32_t base = 0, nchunk = tw; base < D && !done && !gave_up; base += nchunk * 32, nchunk = min(32u, nchunk * 4u)) {
+          // pre-filter: nchunk runs of 32 candidates, dealt to the team's warps
+          for (uint32_t c = wi; c < nchunk; c += tw) {
             const uint32_t k = base + c * 32 + lane;
             bool plaus = false;
             if (k < D) {
@@ -877,7 +898,7 @@ __global__ void __launch_bounds__(kW * 32, kW == 1 ? 16 : 2) k_eval(Topo tp, Tab
               } else {
                 plaus = gang_plausible(tp, rx, sh, gg.n_scopes, dl, dh, gl, d);
               }
-              if (base == 0) { s_cl[c][lane] = dl; s_ch[c][lane] = dh; }
+              if (base == 0) { s_cl[w0 + c][lane] = dl; s_ch[w0 + c][lane] = dh; }   // (c < tw in the first chunk)
               if (plaus && k < fu) {   // failed last time: worth another attempt only if somebody withdrew a claim in there since
                 bool again = false;
                 for (uint32_t w = dl >> 5; w <= (dh - 1u) >> 5; ++w) again |= __ldg(rx.rem_round + w) >= le;
@@ -885,63 +906,61 @@ __global__ void __launch_bounds__(kW * 32, kW == 1 ? 16 : 2) k_eval(Topo tp, Tab
               }
             }
             const uint32_t b = __ballot_sync(kFull, plaus);
-            if (lane == 0) s_plaus[c] = b;
+            if (lane == 0) s_plaus[w0][c] = b;
           }
-          __syncthreads();
+          team_sync();
           uint32_t total = 0;
-          for (uint32_t c = 0; c < nchunk; ++c) total += __popc(s_plaus[c]);
-          if (threadIdx.x == 0) s_npl += total;
-          // attempts: kW plausible candidates at a time, in order, a warp each
-          // while a round has many gangs the very first candidate is attempted by one warp alone: it usually succeeds,
-          // and the other warps' attempts would be thrown away
-          for (uint32_t j0 = 0; j0 < total && !done; j0 += uint32_t(kW)) {
-            if (!kHeavy && max_att && s_att >= max_att) { gave_up = true; break; }   // CTA-uniform (read after a barrier)
-            const uint32_t j = j0 + warp;
+          for (uint32_t c = 0; c < nchunk; ++c) total += __popc(s_plaus[w0][c]);
+          if (tt == 0) s_npl[w0] += total;
+          // attempts: tw plausible candidates at a time, in order, a warp each
+          for (uint32_t j0 = 0; j0 < total && !done; j0 += tw) {
+            if (!cta && max_att && s_att[w0] >= max_att) { gave_up = true; break; }   // team-uniform (read after a barrier)
+            const uint32_t j = j0 + wi;
             bool ok = false; uint32_t dl = 0, dh = 0;
             if (j < total) {
               uint32_t rem = j, c = 0;   // the j-th set bit of the bitmap
-              for (; c + 1 < nchunk; ++c) { const uint32_t pc = __popc(s_plaus[c]); if (rem < pc) break; rem -= pc; }
-              uint32_t w = s_plaus[c];
+              for (; c + 1 < nchunk; ++c) { const uint32_t pc = __popc(s_plaus[w0][c]); if (rem < pc) break; rem -= pc; }
+              uint32_t w = s_plaus[w0][c];
               for (uint32_t i = 0; i < rem; ++i) w &= w - 1;
               const uint32_t kl = __ffs(w) - 1, k = base + c * 32 + kl;
-              if (base == 0) { dl = s_cl[c][kl]; dh = s_ch[c][kl]; } else cand(k, dl, dh);
+              if (base == 0) { dl = s_cl[w0 + c][kl]; dh = s_ch[w0 + c][kl]; } else cand(k, dl, dh);
               staged = dh - dl <= kStageMax;
               ok = staged ? place_in(evs, gg.n_scopes, dl, dh, gl) : place_in(ev, gg.n_scopes, dl, dh, gl);
-              if (lane == 0) { atomicAdd(&s_att, 1u); if (ok) atomicMin(&s_win, j); }
+              if (lane == 0) { atomicAdd(&s_att[w0], 1u); if (ok) atomicMin(&s_win[w0], j); }
               if (ok) k_won = k;
             }
-            __syncthreads();
-            const uint32_t win = s_win;
+            team_sync();
+            const uint32_t win = s_win[w0];
             if (win != GROVE_NONE_U32) { done = true; won = ok && win == j; if (won) { g_got = gl; g_lo = dl; } }
           }
-          __syncthreads();   // s_plaus is rewritten by the next chunk
+          team_sync();   // s_plaus is rewritten by the next chunk
         }
       }
     } while (kPref && !done && !gave_up && --gl >= gbase);
     // what any of the attempts may have read (attempts past the winner only widen it)
-    if (lane == 0) atomicMax(&s_ext, max(max(ev.ext, evs.ext), fu ? ext_word : 0u));   // skipped candidates were read by the last evaluation
-    __syncthreads();
-    if (threadIdx.x == 0) rx.last_att[gi] = uint8_t(gave_up ? 255u : min(254u, s_att));
+    if (lane == 0) atomicMax(&s_ext[w0], max(max(ev.ext, evs.ext), fu ? ext_word : 0u));   // skipped candidates were read by the last evaluation
+    team_sync();
+    if (tt == 0) rx.last_att[gi] = uint8_t(gave_up ? 255u : min(254u, s_att[w0]));
     if (gave_up) {   // no result this round: k_apply keeps the gang dirty
-      if (threadIdx.x == 0) rx.nxt_tstate[gi] = uint8_t(kEvalDeferred);
+      if (tt == 0) rx.nxt_tstate[gi] = uint8_t(kEvalDeferred);
       continue;
     }
-    if (rx.dbg && threadIdx.x == 0) {
+    if (rx.dbg && tt == 0) {
       const uint32_t cyc = uint32_t(clock64() - t0);
-      rx.dbg[gi * 8 + 0] += 1; rx.dbg[gi * 8 + 1] += s_npl; rx.dbg[gi * 8 + 2] += s_att;
-      rx.dbg[gi * 8 + 3] = max(rx.dbg[gi * 8 + 3], cyc); rx.dbg[gi * 8 + 4] = cyc; rx.dbg[gi * 8 + 5] = s_att; rx.dbg[gi * 8 + 6] = s_npl; rx.dbg[gi * 8 + 7] = rx.ctl[kRound];
+      rx.dbg[gi * 8 + 0] += 1; rx.dbg[gi * 8 + 1] += s_npl[w0]; rx.dbg[gi * 8 + 2] += s_att[w0];
+      rx.dbg[gi * 8 + 3] = max(rx.dbg[gi * 8 + 3], cyc); rx.dbg[gi * 8 + 4] = cyc; rx.dbg[gi * 8 + 5] = s_att[w0]; rx.dbg[gi * 8 + 6] = s_npl[w0]; rx.dbg[gi * 8 + 7] = rx.ctl[kRound];
       // warp 0's own phases, summed over the cycle: staging, sub-domain pre-filter, packing, attempts staged
       atomicAdd(rx.dbg + tb.G * 8 + 0, evs.t_stage); atomicAdd(rx.dbg + tb.G * 8 + 1, evs.t_pre); atomicAdd(rx.dbg + tb.G * 8 + 2, evs.t_pack);
       atomicAdd(rx.dbg + tb.G * 8 + 3, evs.n_stage); atomicAdd(rx.dbg + tb.G * 8 + 4, cyc); atomicAdd(rx.dbg + tb.G * 8 + 5, 1u);
       atomicAdd(rx.dbg + tb.G * 8 + 6, evs.t_st2); atomicAdd(rx.dbg + tb.G * 8 + 7, evs.t_st3);
     }
     if (!done) {
-      if (threadIdx.x == 0) {
+      if (tt == 0) {
         rx.last_eval[gi] = round_now; rx.fail_upto[gi] = kFull;   // every candidate failed
         rx.nxt_tstate[gi] = GROVE_GANG_REJECTED; rx.nxt_n[gi] = 0; rx.nxt_info[gi] = 0xFFu; rx.nxt_glo[gi] = GROVE_NONE_U32;
-        rx.nxt_extent[gi] = s_ext;
+        rx.nxt_extent[gi] = s_ext[w0];
       }
-      for (uint32_t si = threadIdx.x; si < gg.n_scopes; si += kW * 32) { rx.nxt_sc_lvl[gg.scope_off + si] = 0xFFu; rx.nxt_sc_lo[gg.scope_off + si] = GROVE_NONE_U32; }
+      for (uint32_t si = tt; si < gg.n_scopes; si += tw * 32) { rx.nxt_sc_lvl[gg.scope_off + si] = 0xFFu; rx.nxt_sc_lo[gg.scope_off + si] = GROVE_NONE_U32; }
       continue;
     }
     if (!won) continue;   // warp-uniform: the winner finishes alone
@@ -981,7 +1000,7 @@ __global__ void __launch_bounds__(kW * 32, kW == 1 ? 16 : 2) k_eval(Topo tp, Tab
       rx.nxt_tstate[gi] = GROVE_GANG_ADMITTED; rx.nxt_n[gi] = uint16_t(n_ent);
       rx.nxt_info[gi] = (g_got >= 0 ? uint32_t(g_got) : 0xFFu) | (num << 8) | (den << 20);
       rx.nxt_glo[gi] = g_got >= 0 ? g_lo : GROVE_NONE_U32;
-      rx.nxt_extent[gi] = max(max(ev.ext, evs.ext), s_ext);   // the surplus pass above may have read further
+      rx.nxt_extent[gi] = max(max(ev.ext, evs.ext), s_ext[w0]);   // the surplus pass above may have read further
     }
   }
 }

@@ -78,6 +78,7 @@ enum Ctl : uint32_t {
   kEntryLo,        // this round's new entrants are the ranks [kEntryLo, kHi): never evaluated, no list entry needed
   kNHeavyNext,     // the NEXT round's list counters, filled by k_detect while this round's are still being read
   kNLightNext,
+  kEvalNext,       // next work item of the round's k_eval queue (heavy gangs, then groups of light ones)
   kCtlWords = 24
 };
 

@@ -112,7 +112,6 @@ struct grove_engine {
   std::string err;
   cudaStream_t stream = nullptr;
   cudaStream_t stream_score = nullptr;  // K2 runs beside the relaxation (they only share the fit data)
-  cudaStream_t stream_heavy = nullptr;  // the heavy gangs of a round are evaluated beside the light ones
   cudaEvent_t ev_fit = nullptr, ev_score = nullptr, ev_s0 = nullptr, ev_s1 = nullptr;
   cudaEvent_t ev_nodes_up = nullptr, ev_tables_up = nullptr;  // the last upload out of the pinned node staging buffer / gang tables
   cudaEvent_t ev[10]{};
@@ -183,11 +182,10 @@ struct grove_engine {
   uint32_t tune_warp_ctas = 4;     // CTAs per SM of the warp-per-gang bookkeeping kernels (apply / detect / settle)
   uint32_t tune_batch = 3;         // rounds enqueued between two looks at the control words (GROVE_TUNE_AHEAD=0 / GROVE_DEBUG_ADMIT)
   uint32_t tune_ahead = 3;         // rounds kept in the queue while the host follows the relaxation through host-mapped progress words
-  uint32_t tune_eval_ctas = 0;     // k_eval CTAs per SM
-  uint32_t tune_heavy_att = 4;     // a gang whose last evaluation made this many attempts is heavy: kW warps next time
+  uint32_t tune_eval_ctas = 0;     // k_eval CTAs in all (0: tune_heavy_ctas per SM)
+  uint32_t tune_heavy_att = 4;     // a gang whose last evaluation made this many attempts is heavy: a whole k_eval CTA next time
   uint32_t tune_max_att = 3;       // a light (one-warp) evaluation gives up after this many attempts and comes back heavy
-  uint32_t tune_heavy_ctas = 2;    // heavy-form CTAs per SM
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+  uint32_t tune_heavy_ctas = 2;    // k_eval CTAs per SM: 2 fill the register file (8 warps x 128 registers each)
   bool tune_overlap = true;        // K2 on a second stream beside the relaxation (GROVE_TUNE_OVERLAP=0 serialises them, e.g. to time K2 alone)
   bool tune_score = false;         // K2 score matrix: false = materialised on request (grove_build_score_matrix / the row getters),
                                    // true = every cycle, on the second stream beside the relaxation
@@ -232,6 +230,20 @@ struct grove_engine {
   } while (0)
 
 static int32_t fail(grove_engine* e, int32_t code, const char* msg) { e->err = msg; return code; }
+
+// A kernel of the relaxation chain, launched as a programmatic dependent of the kernel before it on the stream: its CTAs are
+// launched and become resident while that kernel drains, and wait in cudaGridDependencySynchronize() -- the first statement of
+// every kernel launched this way -- until it has completed and its writes are visible.  Behind anything else on the stream
+// (a copy, a memset, an event) the launch is ordered as usual.
+template <typename... P, typename... A>
+static cudaError_t launch_chained(void (*k)(P...), dim3 grid, uint32_t block, cudaStream_t s, A&&... args) {
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t c{};
+  c.gridDim = grid; c.blockDim = dim3(block); c.dynamicSmemBytes = 0; c.stream = s; c.attrs = at; c.numAttrs = 1;
+  return cudaLaunchKernelEx(&c, k, std::forward<A>(args)...);
+}
 
 // ---------------------------------------------------------------------------------------------
 // topology: sort by label path, tree-ify ids, domain ranges.  Host side; runs only when labels change.
@@ -411,11 +423,9 @@ int32_t grove_engine_create(const grove_config_t* cfg, grove_engine_t** out) {
   cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);  // the latency-bound relaxation gets the SMs first
   if (cudaStreamCreateWithPriority(&e->stream, cudaStreamNonBlocking, prio_hi) != cudaSuccess) { delete e; return GROVE_ERR_CUDA; }
   if (cudaStreamCreateWithPriority(&e->stream_score, cudaStreamNonBlocking, prio_lo) != cudaSuccess) { delete e; return GROVE_ERR_CUDA; }
-  if (cudaStreamCreateWithPriority(&e->stream_heavy, cudaStreamNonBlocking, prio_hi) != cudaSuccess) { delete e; return GROVE_ERR_CUDA; }
   if (cudaEventCreateWithFlags(&e->ev_fit, cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&e->ev_score, cudaEventDisableTiming) != cudaSuccess ||
       cudaEventCreateWithFlags(&e->ev_nodes_up, cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&e->ev_tables_up, cudaEventDisableTiming) != cudaSuccess ||
       cudaEventCreateWithFlags(&e->ev_upd, cudaEventDisableTiming) != cudaSuccess ||
-      cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming) != cudaSuccess ||
       cudaEventCreate(&e->ev_s0) != cudaSuccess || cudaEventCreate(&e->ev_s1) != cudaSuccess) { delete e; return GROVE_ERR_CUDA; }
   for (auto& ev : e->ev) if (cudaEventCreate(&ev) != cudaSuccess) { delete e; return GROVE_ERR_CUDA; }
   if (e->h_ctl.ensure(kCtlWords) != cudaSuccess) { delete e; return GROVE_ERR_OOM; }
@@ -437,12 +447,9 @@ void grove_engine_destroy(grove_engine_t* e) {
   if (e->ev_nodes_up) cudaEventDestroy(e->ev_nodes_up);
   if (e->ev_tables_up) cudaEventDestroy(e->ev_tables_up);
   if (e->ev_upd) cudaEventDestroy(e->ev_upd);
-  if (e->ev_fork) cudaEventDestroy(e->ev_fork);
-  if (e->ev_join) cudaEventDestroy(e->ev_join);
   if (e->ev_score) cudaEventDestroy(e->ev_score);
   if (e->h_live) cudaFreeHost(e->h_live);
   if (e->stream_score) cudaStreamDestroy(e->stream_score);
-  if (e->stream_heavy) cudaStreamDestroy(e->stream_heavy);
   if (e->stream) cudaStreamDestroy(e->stream);
   delete e;
 }
@@ -892,7 +899,7 @@ static int32_t build_cap_tables(grove_engine* e, const Topo& tp, const Tables& t
     CU_TRY(e, cudaMemsetAsync(e->d_capmax.p, 0, sizeof(uint32_t) * size_t(e->n_sigs) * e->cap_stride, e->stream));
   }
   k_fit<<<gfit, 1024, 0, e->stream>>>(tp, tb, e->d_F.p, e->d_cap8.p, e->cap_stride ? e->d_capsum.p : nullptr, e->cap_stride ? e->d_capmax.p : nullptr);
-  k_clear_stale<<<(e->Npad / 4 + 255) / 256, 256, 0, e->stream>>>(rx, e->Npad / 4);
+  CU_TRY(e, launch_chained(k_clear_stale, (e->Npad / 4 + 255) / 256, 256, e->stream, rx, e->Npad / 4));
   if (e->shape_tables) {   // the candidate pre-filter of every gang shape over every domain of its candidate levels
     // only the levels some shape takes its candidates from (Preferred down to Required): a CTA that has nothing to do still
     // costs its launch, and the unit level alone would be tens of thousands of them
@@ -903,7 +910,7 @@ static int32_t build_cap_tables(grove_engine* e, const Topo& tp, const Tables& t
       const int first = g.preferred != GROVE_LEVEL_NONE && int(g.preferred) > base ? int(g.preferred) : base;
       for (int l = std::max(base, 0); l <= first && l < int(e->L); ++l) mx = std::max(mx, e->n_dom[l]);
     }
-    if (mx) k_shape_plaus<<<dim3((mx + 31) / 32, e->n_shapes, e->L), 128, 0, e->stream>>>(tp, tb, rx, e->d_shape_rep.p);
+    if (mx) CU_TRY(e, launch_chained(k_shape_plaus, dim3((mx + 31) / 32, e->n_shapes, e->L), 128, e->stream, tp, tb, rx, e->d_shape_rep.p));
     e->launches += 1;
   }
   CU_TRY(e, cudaGetLastError());
@@ -994,7 +1001,7 @@ static int32_t finish_cycle(grove_engine* e) {
 
 struct CycleGuard {   // every error exit of a cycle leaves the handle usable (ADVICE round 1: in_cycle stayed set)
   grove_engine* e; bool armed = true;
-  ~CycleGuard() { if (armed) { e->in_cycle = false; cudaStreamSynchronize(e->stream); cudaStreamSynchronize(e->stream_score); cudaStreamSynchronize(e->stream_heavy); } }
+  ~CycleGuard() { if (armed) { e->in_cycle = false; cudaStreamSynchronize(e->stream); cudaStreamSynchronize(e->stream_score); } }
 };
 
 int32_t grove_run_cycle(grove_engine_t* e, grove_cycle_stats_t* stats) {
@@ -1028,9 +1035,8 @@ int32_t grove_run_cycle(grove_engine_t* e, grove_cycle_stats_t* stats) {
     }
     CU_TRY(e, cudaEventRecord(e->ev[2], e->stream));
     const uint32_t W = rx.window;
-    const uint32_t per_sm = e->tune_eval_ctas ? e->tune_eval_ctas : 16u;
-    const uint32_t eval_ctas = std::max(1u, std::min(W, e->n_sm * per_sm));
-    const uint32_t heavy_ctas = std::max(1u, std::min(W, e->n_sm * e->tune_heavy_ctas));
+    // K3: CTAs that take work items from a queue; by default as many as are resident at once (heavy gangs take whole CTAs)
+    const uint32_t eval_ctas = std::max(1u, e->tune_eval_ctas ? e->tune_eval_ctas : std::min(W, e->n_sm * e->tune_heavy_ctas));
     const uint32_t warp_ctas = std::max(1u, std::min((W * 32 + 255) / 256, e->n_sm * e->tune_warp_ctas));
     // Rounds are enqueued `batch` at a time without waiting: every kernel returns at once when the cycle is over, so the
     // host only looks at the control words between batches (to rebuild the capacity tables when the settled prefix has
@@ -1042,27 +1048,17 @@ int32_t grove_run_cycle(grove_engine_t* e, grove_cycle_stats_t* stats) {
         CU_TRY(e, cudaMemsetAsync(e->d_add_stamp.p, 0xFF, sizeof(uint32_t) * e->Npad, e->stream));
         CU_TRY(e, cudaMemsetAsync(e->d_rem_stamp.p, 0xFF, sizeof(uint32_t) * e->words, e->stream));
       }
-      // heavy gangs (head of the list) on the second stream, kHeavyWarps warps each; light gangs (tail) a warp each
-      CU_TRY(e, cudaEventRecord(e->ev_fork, e->stream));
-      CU_TRY(e, cudaStreamWaitEvent(e->stream_heavy, e->ev_fork, 0));
-      if (e->any_preferred) {
-        k_eval<true, kHeavyWarps, true><<<heavy_ctas, kHeavyWarps * 32, 0, e->stream_heavy>>>(tp, tb, rx, 0);
-        k_eval<true, 1, false><<<eval_ctas, 32, 0, e->stream>>>(tp, tb, rx, e->tune_max_att);
-      } else {
-        k_eval<false, kHeavyWarps, true><<<heavy_ctas, kHeavyWarps * 32, 0, e->stream_heavy>>>(tp, tb, rx, 0);
-        k_eval<false, 1, false><<<eval_ctas, 32, 0, e->stream>>>(tp, tb, rx, e->tune_max_att);
-      }
-      CU_TRY(e, cudaEventRecord(e->ev_join, e->stream_heavy));
-      CU_TRY(e, cudaStreamWaitEvent(e->stream, e->ev_join, 0));
-      k_apply<<<warp_ctas, 256, 0, e->stream>>>(tb, rx);
-      k_detect<<<warp_ctas, 256, 0, e->stream>>>(tp, tb, rx, e->tune_refresh);
-      e->launches += 4;
+      // one stream-ordered chain: evaluate -> publish -> detect, each launched while the one before drains
+      CU_TRY(e, launch_chained(e->any_preferred ? k_eval<true> : k_eval<false>, eval_ctas, kEvalWarps * 32, e->stream, tp, tb, rx, e->tune_max_att));
+      CU_TRY(e, launch_chained(k_apply, warp_ctas, 256, e->stream, tb, rx));
+      CU_TRY(e, launch_chained(k_detect, warp_ctas, 256, e->stream, tp, tb, rx, e->tune_refresh));
+      e->launches += 3;
       ++next_round;
       return GROVE_OK;
     };
     auto fold = [&]() -> int32_t {   // the final gangs' claims -> committed state (relax.cuh k_fold)
-      k_fold<<<warp_ctas, 256, 0, e->stream>>>(tb, rx, e->d_nres.p);
-      k_fold_mark<<<1, 1, 0, e->stream>>>(rx);
+      CU_TRY(e, launch_chained(k_fold, warp_ctas, 256, e->stream, tb, rx, e->d_nres.p));
+      CU_TRY(e, launch_chained(k_fold_mark, 1, 1, e->stream, rx));
       e->launches += 2;
       CU_TRY(e, cudaGetLastError());
       return GROVE_OK;

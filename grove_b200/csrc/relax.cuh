@@ -142,6 +142,7 @@ __device__ __forceinline__ uint32_t run_length(const uint32_t* node, const uint1
 
 // one warp per evaluated gang: publish a changed result
 __global__ void __launch_bounds__(256) k_apply(Tables tb, Relax rx) {
+  cudaGridDependencySynchronize();   // (launched chained: engine.cu launch_chained)
   const uint32_t lane = threadIdx.x & 31;
   if (rx.ctl[kDone]) return;
   const uint32_t n_eval = rx.ctl[kNEval], round = rx.ctl[kRound];
@@ -209,6 +210,7 @@ __global__ void __launch_bounds__(256) k_apply(Tables tb, Relax rx) {
 // one warp per gang of the window: did its view change this round?
 __global__ void __launch_bounds__(256) k_detect(Topo tp, Tables tb, Relax rx, uint32_t refresh_every) {
   __shared__ bool s_last;
+  cudaGridDependencySynchronize();
   const uint32_t lane = threadIdx.x & 31;
   if (rx.ctl[kDone]) return;   // uniform over the grid: set only by the last CTA of an earlier launch
   const uint32_t front = rx.ctl[kFront], hi = rx.ctl[kHi], round = rx.ctl[kRound];
@@ -252,7 +254,7 @@ __global__ void __launch_bounds__(256) k_detect(Topo tp, Tables tb, Relax rx, ui
     if (dirty && lane == 0) {
       atomicMin(rx.ctl + kMinDirty, p);
       // the next round's list.  Longest first: a round lasts as long as its slowest evaluation, so the gangs whose last evaluation
-      // needed several attempts get kHeavyWarps warps (head of the list), the others a warp each (tail)
+      // needed several attempts get a whole k_eval CTA (head of the list, taken first), the others a warp each (tail)
       if (rx.last_att[g] >= rx.heavy_att) rx.eval_list[atomicAdd(rx.ctl + kNHeavyNext, 1u)] = g;
       else rx.eval_list[tb.G - 1u - atomicAdd(rx.ctl + kNLightNext, 1u)] = g;
     }
@@ -273,7 +275,7 @@ __global__ void __launch_bounds__(256) k_detect(Topo tp, Tables tb, Relax rx, ui
     rx.ctl[kEvals] += rx.ctl[kNEval];
     rx.ctl[kFront] = nf; rx.ctl[kHi] = h2; rx.ctl[kMinDirty] = h2; rx.ctl[kChanged] = 0;
     rx.ctl[kEntryLo] = old_hi; rx.ctl[kNHeavy] = nh; rx.ctl[kNLight] = nl; rx.ctl[kNEval] = nh + nl + (h2 - min(old_hi, h2));
-    rx.ctl[kNHeavyNext] = 0; rx.ctl[kNLightNext] = 0;
+    rx.ctl[kNHeavyNext] = 0; rx.ctl[kNLightNext] = 0; rx.ctl[kEvalNext] = 0;
     rx.ctl[kRound] += 1; rx.ctl[kRemAny] = kFull; rx.ctl[kCtaDone] = 0;
     rx.ctl[kDone] = nf >= G ? 1u : 0u;
     if (nf < G && nf - rx.ctl[kTablesAt] >= refresh_every) rx.ctl[kRefresh] = 1;
@@ -291,6 +293,7 @@ __global__ void __launch_bounds__(256) k_detect(Topo tp, Tables tb, Relax rx, ui
 // claims of final gangs are as good as committed for everybody who ranks after them, so the fold runs before a capacity-table
 // rebuild (the tables are built from the committed state) and when the cycle ends; k_fold_mark then moves the marker.
 __global__ void __launch_bounds__(256) k_fold(Tables tb, Relax rx, uint4* nres) {
+  cudaGridDependencySynchronize();
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t lo = rx.ctl[kFolded], hi = rx.ctl[kFront];
   const uint32_t nw = (gridDim.x * blockDim.x) >> 5;
@@ -314,10 +317,11 @@ __global__ void __launch_bounds__(256) k_fold(Tables tb, Relax rx, uint4* nres) 
     }
   }
 }
-__global__ void k_fold_mark(Relax rx) { rx.ctl[kFolded] = rx.ctl[kFront]; }
+__global__ void k_fold_mark(Relax rx) { cudaGridDependencySynchronize(); rx.ctl[kFolded] = rx.ctl[kFront]; }
 
 // after a capacity-table build: the tables describe every node again
 __global__ void k_clear_stale(Relax rx, uint32_t n_words) {
+  cudaGridDependencySynchronize();
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n_words) rx.nlive[i] &= ~0x80808080u;
   if (i == 0) { rx.ctl[kTablesAt] = rx.ctl[kFront]; rx.ctl[kRefresh] = 0; rx.ctl[kFoldAny] = 0; }
