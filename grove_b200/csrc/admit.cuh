@@ -142,7 +142,7 @@ __device__ __forceinline__ uint32_t visit_pos(const GangRegs& g, uint32_t n) {
 }
 
 // ---- the evaluator: the whole warp packs ONE candidate range ------------------------------------------
-template <bool kPref_>
+template <bool kPref_, bool kHolds>
 struct Ev {
   static constexpr bool kPref = kPref_;
   static constexpr bool kStaged = false;
@@ -175,13 +175,13 @@ struct Ev {
 #pragma unroll
           for (uint32_t s = 0; s < kClaimSlots; ++s) {
             const uint4 c = __ldg(line + s);
-            if (c.x >= g.rank && c.x != kClaimEmpty) { cpu += int(c.y); mem += int(c.z); gpu += int(c.w & 0xFFFFu); pods += int(c.w >> 16); }
+            if (gives_back<kHolds>(c.x, g.rank)) { cpu += int(c.y); mem += int(c.z); gpu += int(c.w & 0xFFFFu); pods += int(c.w >> 16); }
           }
         }
         if (live & kHasOvf) {
           for (uint32_t i = __ldg(rb.ovf_head + n); i; i = __ldg(rb.ovf_next + i - 1)) {
             const uint4 c = __ldg(rb.ovf_claim + i - 1);
-            if (c.x >= g.rank && c.x != kClaimEmpty) { cpu += int(c.y); mem += int(c.z); gpu += int(c.w & 0xFFFFu); pods += int(c.w >> 16); }
+            if (gives_back<kHolds>(c.x, g.rank)) { cpu += int(c.y); mem += int(c.z); gpu += int(c.w & 0xFFFFu); pods += int(c.w >> 16); }
           }
         }
       }
@@ -290,7 +290,7 @@ struct Ev {
 // instead of a chain of dependent L2 look-ups per 32 nodes.
 constexpr uint32_t kStageMax = 128;
 
-template <bool kPref_>
+template <bool kPref_, bool kHolds>
 struct EvS {
   static constexpr bool kPref = kPref_;
   static constexpr bool kStaged = true;   // node state in shared memory: an attempt costs less than the table look-ups that would skip it
@@ -334,7 +334,7 @@ struct EvS {
     for (uint32_t k = 0; k < kPer; ++k) {
       const uint32_t n = dl + k * 32u + lane;
       int cpu = int(r[k].x) - t[k].x, mem = int(r[k].y) - t[k].y, gpu = int(r[k].z & 0xFFFFu) - t[k].z, pods = int(r[k].z >> 16) - t[k].w;
-      if (live[k] && mr[k] >= g.rank) {   // a gang of a higher rank may hold a claim here: it is invisible to this one
+      if (live[k] && mr[k] >= g.rank) {   // a gang of a higher rank may hold a claim here (invisible to this one), or this gang its hold
         if (live[k] & 0x3Fu) {
           const uint4* line = rb.claims + size_t(n) * kClaimSlots;
           uint4 c[kClaimSlots];
@@ -342,12 +342,12 @@ struct EvS {
           for (uint32_t s = 0; s < kClaimSlots; ++s) c[s] = __ldg(line + s);
 #pragma unroll
           for (uint32_t s = 0; s < kClaimSlots; ++s)
-            if (c[s].x >= g.rank && c[s].x != kClaimEmpty) { cpu += int(c[s].y); mem += int(c[s].z); gpu += int(c[s].w & 0xFFFFu); pods += int(c[s].w >> 16); }
+            if (gives_back<kHolds>(c[s].x, g.rank)) { cpu += int(c[s].y); mem += int(c[s].z); gpu += int(c[s].w & 0xFFFFu); pods += int(c[s].w >> 16); }
         }
         if (live[k] & kHasOvf) {
           for (uint32_t i = __ldg(rb.ovf_head + n); i; i = __ldg(rb.ovf_next + i - 1)) {
             const uint4 c = __ldg(rb.ovf_claim + i - 1);
-            if (c.x >= g.rank && c.x != kClaimEmpty) { cpu += int(c.y); mem += int(c.z); gpu += int(c.w & 0xFFFFu); pods += int(c.w >> 16); }
+            if (gives_back<kHolds>(c.x, g.rank)) { cpu += int(c.y); mem += int(c.z); gpu += int(c.w & 0xFFFFu); pods += int(c.w >> 16); }
           }
         }
       }
@@ -755,7 +755,7 @@ __device__ __forceinline__ uint32_t eval_list_at(const Relax& rx, const Tables& 
 // cudaGridDependencySynchronize().
 constexpr uint32_t kEvalDeferred = 0xFFu;   // nxt_tstate: no result this round
 constexpr int kEvalWarps = 8;
-template <bool kPref>
+template <bool kPref, bool kHolds>
 __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb, Relax rx, uint32_t max_att) {
   __shared__ GangShared shs[kEvalWarps];
   __shared__ int4 s_view[kEvalWarps][kStageMax];
@@ -839,8 +839,8 @@ __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb,
     // shrink otherwise (claims are added, settled claims move into the committed state).  So a re-evaluation skips the
     // candidates in front of its last answer that no withdrawal touched -- gangs that meet a nearly full cluster would
     // otherwise re-run dozens of failing attempts every round.  (Single candidate level only.)
-    Ev<kPref> ev(tp, rx, sh, g, lane);                         // candidates of any size, node state from L2
-    EvS<kPref> evs(tp, rx, sh, g, lane, s_view[warp], s_vflag[warp], s_rk[warp]);         // candidates of <= kStageMax nodes, node state staged in shared memory
+    Ev<kPref, kHolds> ev(tp, rx, sh, g, lane);                         // candidates of any size, node state from L2
+    EvS<kPref, kHolds> evs(tp, rx, sh, g, lane, s_view[warp], s_vflag[warp], s_rk[warp]);         // candidates of <= kStageMax nodes, node state staged in shared memory
     bool staged = false;  // the winning attempt ran on evs
     bool won = false;     // this warp holds the answer
     bool done = false;    // CTA-uniform

@@ -15,6 +15,17 @@ constexpr uint32_t kClaimEmpty = 0xFFFFFFFFu;
 constexpr uint32_t kStale = 0x80u;            // nlive8 bit: committed state changed since the capacity tables were built
 constexpr uint32_t kHasOvf = 0x40u;           // nlive8 bit: the node has (had) claims in the overflow chain
 constexpr uint32_t kTagRounds = 254u;         // rounds per stamp epoch (stamps carry a round tag in their top byte)
+constexpr uint32_t kHold = 1u << 24;          // claim tag bit above the 24 rank bits: the claim is the HOLD of the gang of that rank
+                                              // (what the running gang it replaces holds on the node; grove_run_cycle_reuse)
+
+// Does the gang of rank `rank` give claim tag x back, i.e. not subtract it from its view?  The claims of the ranks after it, and
+// (kHolds: a cycle with holds) its own hold; every other hold is subtracted by everybody.  Without holds this is the plain rank
+// test: the kernels of an ordinary cycle are instantiated without the hold logic.
+template <bool kHolds>
+__device__ __forceinline__ bool gives_back(uint32_t x, uint32_t rank) {
+  if constexpr (kHolds) return (x >= rank && x < kHold) || x == (rank | kHold);   // (kClaimEmpty has the hold bit set)
+  else return x >= rank && x != kClaimEmpty;
+}
 
 struct GangInfo {     // 48 B, built on the host at submit time
   uint32_t anchor;    // sorted node index
@@ -141,6 +152,10 @@ struct Relax {
   const uint32_t* shape_bits; // [shapes][pl_words] candidate pre-filter per (gang shape, domain), bit pl_off[level] + d; null = not built
   uint32_t pl_off[GROVE_MAX_LEVELS], pl_words;
   uint32_t P, window, entry, heavy_att;   // heavy_att: attempts of its last evaluation from which a gang counts as heavy
+  // holds (grove_run_cycle_reuse): gang g owns records [hold_off[g], hold_off[g + 1]), one per node, x = sorted node, y = cpu,
+  // z = mem, w = gpu | pods << 16; hold_off == null: no gang has one
+  const uint32_t* hold_off; // [G + 1]
+  const uint4* hold;
   uint32_t* dbg;            // [G][8] optional per-gang evaluation statistics
   uint32_t* live;           // [kLiveWords] host-mapped: progress words the host polls (null: not available)
 };

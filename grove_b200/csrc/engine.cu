@@ -217,6 +217,11 @@ struct grove_engine {
   bool score_pass_valid = false;   // the capacity tables + T describe the loaded snapshot (grove_run_score_pass)
   uint32_t t_c0 = 0, t_cpr = 0;    // ... and T holds the 16-node chunks [t_c0, t_c0 + t_cpr) of every row
   DevBuf<uint32_t> d_sig_sum;
+  // holds of the replacement gangs of a grove_run_cycle_reuse (relax.cuh "holds"); holds_on only while such a cycle runs
+  DevBuf<uint32_t> d_hold_off;
+  DevBuf<uint4> d_hold;
+  uint32_t n_hold = 0;
+  bool holds_on = false;
 };
 
 
@@ -379,6 +384,7 @@ static Relax make_relax(grove_engine* e) {
   r.shape_bits = e->shape_tables ? e->d_shape_bits.p : nullptr; r.pl_words = e->pl_words;
   for (uint32_t l = 0; l < GROVE_MAX_LEVELS; ++l) r.pl_off[l] = e->pl_off[l];
   r.P = e->P; r.window = e->tune_window ? e->tune_window : (e->G ? e->G : 1u); r.entry = e->tune_entry ? e->tune_entry : r.window; r.heavy_att = e->tune_heavy_att;
+  r.hold_off = e->holds_on ? e->d_hold_off.p : nullptr; r.hold = e->d_hold.p;
   r.dbg = e->dbg_on ? e->d_dbg.p : nullptr;
   r.live = e->d_live;
   return r;
@@ -935,7 +941,9 @@ static int32_t cycle_begin(grove_engine* e) {
   CU_TRY(e, e->d_nxt_info.ensure(g1)); CU_TRY(e, e->d_nxt_glo.ensure(g1)); CU_TRY(e, e->d_nxt_extent.ensure(g1));
   CU_TRY(e, e->d_nxt_sc_lvl.ensure(s1)); CU_TRY(e, e->d_nxt_sc_lo.ensure(s1));
   CU_TRY(e, e->d_claims.ensure(size_t(N) * kClaimSlots)); CU_TRY(e, e->d_nlive.ensure(N / 4)); CU_TRY(e, e->d_ovf_head.ensure(N));
-  CU_TRY(e, e->d_ovf_next.ensure(4 * p1 + 1024)); CU_TRY(e, e->d_ovf_claim.ensure(4 * p1 + 1024));
+  // (the overflow pool takes the holds as well as the claims: a node's line may be full of both)
+  const size_t ovf = 4 * p1 + 1024 + (e->holds_on ? e->n_hold : 0u);
+  CU_TRY(e, e->d_ovf_next.ensure(ovf)); CU_TRY(e, e->d_ovf_claim.ensure(ovf));
   CU_TRY(e, e->d_ctot.ensure(N)); CU_TRY(e, e->d_cmaxr.ensure(N));
   CU_TRY(e, e->d_add_stamp.ensure(N)); CU_TRY(e, e->d_rem_stamp.ensure(e->words)); CU_TRY(e, e->d_rem_round.ensure(e->words));
   CU_TRY(e, e->d_last_eval.ensure(g1)); CU_TRY(e, e->d_fail_upto.ensure(g1));
@@ -1004,8 +1012,7 @@ struct CycleGuard {   // every error exit of a cycle leaves the handle usable (A
   ~CycleGuard() { if (armed) { e->in_cycle = false; cudaStreamSynchronize(e->stream); cudaStreamSynchronize(e->stream_score); } }
 };
 
-int32_t grove_run_cycle(grove_engine_t* e, grove_cycle_stats_t* stats) {
-  if (!e) return GROVE_ERR_INVALID_ARG;
+static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
   int32_t rc = cycle_begin(e);
   if (rc) return rc;
   CycleGuard guard{e};
@@ -1013,6 +1020,11 @@ int32_t grove_run_cycle(grove_engine_t* e, grove_cycle_stats_t* stats) {
   const uint32_t G = e->G;
   CU_TRY(e, cudaEventRecord(e->ev[8], e->stream));
   uint32_t rounds = 0;
+  if (G && e->holds_on) {   // the holds join the committed state (so every table built from it bounds every gang's view) as claims
+    k_hold_publish<<<(G * 32 + 255) / 256, 256, 0, e->stream>>>(tb, rx, e->d_nres.p);
+    CU_TRY(e, cudaGetLastError());
+    e->launches += 1;
+  }
   if (G) {
     // K1 + capacity tables over the cycle-start snapshot; K2 (score matrix) forks to the second stream
     CU_TRY(e, cudaEventRecord(e->ev[0], e->stream));
@@ -1049,15 +1061,15 @@ int32_t grove_run_cycle(grove_engine_t* e, grove_cycle_stats_t* stats) {
         CU_TRY(e, cudaMemsetAsync(e->d_rem_stamp.p, 0xFF, sizeof(uint32_t) * e->words, e->stream));
       }
       // one stream-ordered chain: evaluate -> publish -> detect, each launched while the one before drains
-      CU_TRY(e, launch_chained(e->any_preferred ? k_eval<true> : k_eval<false>, eval_ctas, kEvalWarps * 32, e->stream, tp, tb, rx, e->tune_max_att));
-      CU_TRY(e, launch_chained(k_apply, warp_ctas, 256, e->stream, tb, rx));
+      CU_TRY(e, launch_chained(e->holds_on ? (e->any_preferred ? k_eval<true, true> : k_eval<false, true>) : (e->any_preferred ? k_eval<true, false> : k_eval<false, false>), eval_ctas, kEvalWarps * 32, e->stream, tp, tb, rx, e->tune_max_att));
+      CU_TRY(e, launch_chained(e->holds_on ? k_apply<true> : k_apply<false>, warp_ctas, 256, e->stream, tb, rx));
       CU_TRY(e, launch_chained(k_detect, warp_ctas, 256, e->stream, tp, tb, rx, e->tune_refresh));
       e->launches += 3;
       ++next_round;
       return GROVE_OK;
     };
     auto fold = [&]() -> int32_t {   // the final gangs' claims -> committed state (relax.cuh k_fold)
-      CU_TRY(e, launch_chained(k_fold, warp_ctas, 256, e->stream, tb, rx, e->d_nres.p));
+      CU_TRY(e, launch_chained(e->holds_on ? k_fold<true> : k_fold<false>, warp_ctas, 256, e->stream, tb, rx, e->d_nres.p));
       CU_TRY(e, launch_chained(k_fold_mark, 1, 1, e->stream, rx));
       e->launches += 2;
       CU_TRY(e, cudaGetLastError());
@@ -1131,6 +1143,11 @@ int32_t grove_run_cycle(grove_engine_t* e, grove_cycle_stats_t* stats) {
       rounds = e->h_ctl.p[kRound] - 1;
     }
     rc = fold(); if (rc) return rc;   // everything is final now: the committed state and the final states of the outputs
+    if (e->holds_on) {   // the admitted owners' leftovers: the running gangs they replace are gone
+      k_hold_release<<<(G * 32 + 255) / 256, 256, 0, e->stream>>>(tb, rx, e->d_nres.p);
+      CU_TRY(e, cudaGetLastError());
+      e->launches += 1;
+    }
     e->last.evaluations = e->h_ctl.p[kEvals];
   }
   CU_TRY(e, cudaEventRecord(e->ev[3], e->stream));
@@ -1164,6 +1181,11 @@ int32_t grove_run_cycle(grove_engine_t* e, grove_cycle_stats_t* stats) {
   }
   if (stats) *stats = e->last;
   return GROVE_OK;
+}
+
+int32_t grove_run_cycle(grove_engine_t* e, grove_cycle_stats_t* stats) {
+  if (!e) return GROVE_ERR_INVALID_ARG;
+  return run_cycle(e, stats);
 }
 
 int32_t grove_get_placements(grove_engine_t* e, grove_placement_t* out, uint32_t cap, uint32_t* n_out) {
@@ -1400,6 +1422,80 @@ int32_t grove_get_victims(grove_engine_t* e, grove_victim_t* out, uint32_t cap, 
   if (cap < e->victims.size()) return fail(e, GROVE_ERR_LIMIT, "output buffer too small");
   std::memcpy(out, e->victims.data(), sizeof(grove_victim_t) * e->victims.size());
   return GROVE_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Reservation reuse (include/grove_place.h "reservation reuse"; DESIGN.md section 1).  The host validates the inputs and turns the
+// predecessors' holdings into one hold record per (replacement gang, node), in sorted node order; the ordinary cycle then runs with
+// the holds (relax.cuh k_hold_publish / k_fold / k_hold_release).
+// ---------------------------------------------------------------------------------------------
+int32_t grove_run_cycle_reuse(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs, const grove_running_gang_t* running,
+                              uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
+  if (!e || (n_gangs && !replaces) || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
+  if (!e->nodes_loaded) return fail(e, GROVE_ERR_STATE, "no node snapshot loaded");
+  if (!e->gangs_loaded) return fail(e, GROVE_ERR_STATE, "no gangs submitted");
+  if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
+  if (n_gangs != e->G) return fail(e, GROVE_ERR_INVALID_ARG, "replaces must have one entry per submitted gang");
+  for (uint32_t r = 0; r < n_running; ++r)
+    if (uint64_t(running[r].holding_off) + running[r].n_holdings > n_holdings) return fail(e, GROVE_ERR_INVALID_ARG, "running gang holdings out of range");
+  for (uint32_t h = 0; h < n_holdings; ++h)
+    if (holdings[h].node >= e->N) return fail(e, GROVE_ERR_INVALID_ARG, "holding on a node out of range");
+  std::vector<uint8_t> taken(n_running, 0);
+  for (uint32_t g = 0; g < n_gangs; ++g) {
+    const uint32_t r = replaces[g];
+    if (r == GROVE_NONE_U32) continue;
+    if (r >= n_running) return fail(e, GROVE_ERR_INVALID_ARG, "replaces names a running gang out of range");
+    if (taken[r]) return fail(e, GROVE_ERR_INVALID_ARG, "a running gang is replaced by more than one gang");
+    taken[r] = 1;
+  }
+  CU_TRY(e, cudaSetDevice(e->cfg.device));
+  // one record per (gang, node): x = sorted node, then cpu, mem, gpu, pods summed over the predecessor's holdings there
+  struct Rec { uint32_t node; uint64_t v[4]; };
+  std::vector<uint32_t> off(size_t(n_gangs) + 1, 0);
+  std::vector<Rec> recs;
+  for (uint32_t g = 0; g < n_gangs; ++g) {
+    off[g] = uint32_t(recs.size());
+    const uint32_t r = replaces[g];
+    if (r == GROVE_NONE_U32) continue;
+    const size_t first = recs.size();
+    for (uint32_t k = 0; k < running[r].n_holdings; ++k) {
+      const grove_holding_t& h = holdings[running[r].holding_off + k];
+      recs.push_back(Rec{e->inv[h.node], {h.cpu_milli, h.mem_mib, h.gpu, h.pods}});
+    }
+    std::sort(recs.begin() + first, recs.end(), [](const Rec& a, const Rec& b) { return a.node < b.node; });
+    size_t w = first;
+    for (size_t i = first; i < recs.size(); ++i) {
+      if (w > first && recs[w - 1].node == recs[i].node) { for (int k = 0; k < 4; ++k) recs[w - 1].v[k] += recs[i].v[k]; }
+      else recs[w++] = recs[i];
+    }
+    recs.resize(w);
+  }
+  off[n_gangs] = uint32_t(recs.size());
+  // the free table plus every hold must fit the node record's fields
+  if (!recs.empty()) {
+    std::vector<uint4> nres(e->Npad);
+    CU_TRY(e, cudaMemcpyAsync(nres.data(), e->d_nres.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToHost, e->stream));
+    CU_TRY(e, cudaStreamSynchronize(e->stream));
+    std::vector<Rec> tot(recs);
+    std::sort(tot.begin(), tot.end(), [](const Rec& a, const Rec& b) { return a.node < b.node; });
+    for (size_t i = 0; i < tot.size();) {
+      const uint32_t n = tot[i].node;
+      uint64_t v[4] = {nres[n].x, nres[n].y, nres[n].z & 0xFFFFu, nres[n].z >> 16};
+      for (; i < tot.size() && tot[i].node == n; ++i) for (int k = 0; k < 4; ++k) v[k] += tot[i].v[k];
+      if (v[0] > UINT32_MAX || v[1] > UINT32_MAX || v[2] > UINT16_MAX || v[3] > UINT16_MAX)
+        return fail(e, GROVE_ERR_INVALID_ARG, "free resources plus holdings overflow a field of a node record");
+    }
+  }
+  std::vector<uint4> hold(std::max<size_t>(recs.size(), 1));
+  for (size_t i = 0; i < recs.size(); ++i)
+    hold[i] = make_uint4(recs[i].node, uint32_t(recs[i].v[0]), uint32_t(recs[i].v[1]), uint32_t(recs[i].v[2]) | (uint32_t(recs[i].v[3]) << 16));
+  CU_TRY(e, e->d_hold_off.ensure(off.size())); CU_TRY(e, e->d_hold.ensure(hold.size()));
+  CU_TRY(e, cudaMemcpyAsync(e->d_hold_off.p, off.data(), sizeof(uint32_t) * off.size(), cudaMemcpyHostToDevice, e->stream));
+  CU_TRY(e, cudaMemcpyAsync(e->d_hold.p, hold.data(), sizeof(uint4) * hold.size(), cudaMemcpyHostToDevice, e->stream));
+  CU_TRY(e, cudaStreamSynchronize(e->stream));   // (pageable sources)
+  struct HoldsOn { grove_engine* e; ~HoldsOn() { e->holds_on = false; e->n_hold = 0; } } holds_guard{e};
+  e->holds_on = !recs.empty(); e->n_hold = uint32_t(recs.size());
+  return run_cycle(e, stats);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -485,13 +485,16 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
   if (auto e = chk(grove_submit_gangs(engine_, t.gangs.data(), uint32_t(t.gangs.size()), t.cliques.data(), uint32_t(t.cliques.size()),
                                       t.scopes.data(), uint32_t(t.scopes.size())), "grove_submit_gangs")) return e;
   grove_cycle_stats_t st{};
-  // running PodGangs -> the reclaim pass's tables (holdings on nodes that left the snapshot are dropped)
+  // running PodGangs -> the reclaim pass's / reservation reuse's tables (holdings on nodes that left the snapshot are dropped)
   std::vector<grove_running_gang_t> run; std::vector<grove_holding_t> held; std::vector<std::string> runNames;
-  bool preempt = false;
+  bool preempt = false, reuse = false;
+  std::vector<uint32_t> replaces;   // reservation reuse: per gang row, the running gang it is the new version of
   {
     std::lock_guard<std::mutex> l(mu_);
+    if (preemption_ && reuse_) return mkerr("ERR_SYNC_PODGANG", "RunCycle", "preemption and reservation reuse cannot both be on");
     preempt = preemption_ && !running_.empty();
-    if (preempt) {
+    reuse = reuse_ && !running_.empty();
+    if (preempt || reuse) {
       std::map<std::string, uint32_t> nodeIdx;
       for (uint32_t i = 0; i < nodes.size(); ++i) nodeIdx[nodes[i].Name] = i;
       for (const auto& kv : running_) {
@@ -505,8 +508,23 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
         run.push_back(r); runNames.push_back(kv.first);
       }
     }
+    if (reuse) {   // the minimum row of a PodGang whose ReuseReservationRef names a running PodGang; one new version per running gang
+      std::map<std::string, uint32_t> runIdx;
+      for (uint32_t r = 0; r < runNames.size(); ++r) runIdx[runNames[r]] = r;
+      std::vector<uint8_t> taken(run.size(), 0);
+      replaces.assign(t.gangs.size(), GROVE_NONE_U32);
+      for (uint32_t g = 0; g < t.gangs.size(); ++g) {
+        const PodGang& pg = snap.at(t.gangNames[g]);
+        if (t.remainder[g] || !pg.Spec.ReuseReservationRef) continue;
+        auto it = runIdx.find(pg.Spec.ReuseReservationRef->Namespace + "/" + pg.Spec.ReuseReservationRef->Name);
+        if (it == runIdx.end() || taken[it->second]) continue;
+        taken[it->second] = 1; replaces[g] = it->second;
+      }
+      reuse = std::any_of(replaces.begin(), replaces.end(), [](uint32_t r) { return r != GROVE_NONE_U32; });
+    }
   }
-  if (preempt) { if (auto e = chk(grove_run_cycle_preempt(engine_, run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_preempt")) return e; }
+  if (reuse) { if (auto e = chk(grove_run_cycle_reuse(engine_, replaces.data(), uint32_t(replaces.size()), run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_reuse")) return e; }
+  else if (preempt) { if (auto e = chk(grove_run_cycle_preempt(engine_, run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_preempt")) return e; }
   else if (auto e = chk(grove_run_cycle(engine_, &st), "grove_run_cycle")) return e;
   if (stats) *stats = st;
   std::vector<grove_placement_t> pl(st.pods_bound + 1);
@@ -559,6 +577,9 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
       running_.erase(runNames[vs[i].running]);
     }
   }
+  if (reuse)   // an admitted new version replaces its predecessor: the caller deletes the old pods, whose resources the cycle released
+    for (uint32_t i = 0; i < gs.size(); ++i)
+      if (gs[i].state == GROVE_GANG_ADMITTED && replaces[i] != GROVE_NONE_U32) running_.erase(runNames[replaces[i]]);
   for (uint32_t i = 0; i < gs.size(); ++i) {
     if (gs[i].state != GROVE_GANG_ADMITTED) continue;
     const std::string& key = t.gangNames[i];

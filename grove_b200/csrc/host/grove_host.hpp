@@ -243,6 +243,12 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   // rejects may evict running PodGangs of a lower priority.  Victims come back in `statuses` with DisruptionTarget set and
   // are forgotten here: the caller deletes their pods (the node snapshot of the next cycle shows the resources as free).
   void SetPreemption(bool on) { std::lock_guard<std::mutex> l(mu_); preemption_ = on; }
+  // Reservation reuse (ReuseReservationRef, podgang.go:65-71): with it on, a PodGang whose ReuseReservationRef names a running
+  // PodGang is that gang's new version and the cycle is grove_run_cycle_reuse -- it may use what its predecessor holds, nobody
+  // else may.  Once it is admitted the predecessor is forgotten as running (the caller deletes its pods; a later OnPodGangDelete
+  // of it releases nothing twice).  The anchor hint stays either way.  Off by default; a cycle with both this and preemption on
+  // fails.
+  void SetReservationReuse(bool on) { std::lock_guard<std::mutex> l(mu_); reuse_ = on; }
   size_t Running() const { std::lock_guard<std::mutex> l(mu_); return running_.size(); }
   // why a PodGang cannot be handed to the engine (limits of the packed tables), or empty.  SyncPodGang accepts every
   // PodGang -- the reference's reconciler would requeue forever on an error -- and RunCycle reports these as
@@ -271,6 +277,7 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   struct RunningGang { int32_t priority = 0; std::vector<Held> held; };
   std::map<std::string, RunningGang> running_;   // PodGangs scheduled by this backend and not deleted since
   bool preemption_ = false;
+  bool reuse_ = false;
   grove_engine_t* engine_ = nullptr;
   uint32_t engineLevels_ = 0;
   mutable std::mutex mu_;        // pending set, bindings, levels: everything SyncPodGang / OnPodGangDelete / SyncTopology touch

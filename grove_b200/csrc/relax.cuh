@@ -94,10 +94,11 @@ __device__ __forceinline__ void claim_remove(const Relax& rx, uint32_t n, uint32
   }
 }
 
-__device__ __forceinline__ void claim_add(const Relax& rx, uint32_t n, uint32_t rank, uint32_t cpu, uint32_t mem, uint32_t gpw) {
+// (rank: the claim's tag -- a rank, or rank | kHold for a hold; maxr: the rank that goes into cmaxr)
+__device__ __forceinline__ void claim_add(const Relax& rx, uint32_t n, uint32_t rank, uint32_t cpu, uint32_t mem, uint32_t gpw, uint32_t maxr) {
   uint32_t* line = reinterpret_cast<uint32_t*>(rx.claims + size_t(n) * kClaimSlots);
   ctot_add(rx, n, int(cpu), int(mem), gpw, +1);
-  atomicMax(rx.cmaxr + n, rank);
+  atomicMax(rx.cmaxr + n, maxr);
   for (int pass = 0; pass < 3; ++pass) {   // look first, then take; somebody else may win the slot: look again
     uint32_t freeb = 0;
 #pragma unroll
@@ -140,7 +141,72 @@ __device__ __forceinline__ uint32_t run_length(const uint32_t* node, const uint1
   return t;
 }
 
-// one warp per evaluated gang: publish a changed result
+// ---- holds (grove_run_cycle_reuse) ---------------------------------------------------------------------
+// A replacement gang's HOLD is what the running gang it replaces holds: added to the committed state when the cycle starts and
+// published as claims (tag rank | kHold) that every gang but the owner subtracts.  Holds never change during the relaxation, so
+// they leave no stamps; they leave the claim lines when their owner is folded.
+__device__ __forceinline__ bool has_hold(const Relax& rx, uint32_t g) { return rx.hold_off && rx.hold_off[g + 1] > rx.hold_off[g]; }
+
+// the hold of gang g on node n (zero where it holds nothing)
+__device__ __forceinline__ uint4 hold_at(const Relax& rx, uint32_t g, uint32_t n) {
+  for (uint32_t i = rx.hold_off[g], e = rx.hold_off[g + 1]; i < e; ++i) { const uint4 h = rx.hold[i]; if (h.x == n) return h; }
+  return make_uint4(n, 0u, 0u, 0u);
+}
+
+// The claim of the run at entry i (len pods of one clique on one node) of a hold owner's placement: the part its hold on the node
+// does not cover.  The runs on a node use the hold in entry order, so together they claim (U - H)+ per resource there.
+// -> cpu, mem, gpu | pods << 16
+__device__ uint3 owner_claim(const Tables& tb, const Relax& rx, uint32_t g, const uint32_t* node, const uint16_t* meta, uint32_t i, uint32_t len) {
+  const uint32_t n = node[i], coff = tb.gangs[g].clique_off;
+  uint32_t u[4] = {0u, 0u, 0u, 0u};   // what the entries before the run put on the node
+  for (uint32_t j = 0; j < i; ++j)
+    if (node[j] == n) { const grove_clique_t q = tb.cliques[coff + meta[j]]; u[0] += q.req_cpu_milli; u[1] += q.req_mem_mib; u[2] += q.req_gpu; u[3] += 1u; }
+  const grove_clique_t q = tb.cliques[coff + meta[i]];
+  const uint32_t r[4] = {len * q.req_cpu_milli, len * q.req_mem_mib, len * uint32_t(q.req_gpu), len};
+  const uint4 h = hold_at(rx, g, n);
+  const uint32_t hv[4] = {h.y, h.z, h.w & 0xFFFFu, h.w >> 16};
+  uint32_t c[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) c[k] = max(u[k] + r[k], hv[k]) - max(u[k], hv[k]);
+  return make_uint3(c[0], c[1], c[2] | (c[3] << 16));
+}
+
+// cycle start: every hold joins the committed state and is published as a claim of its owner.  One warp per gang.
+__global__ void __launch_bounds__(256) k_hold_publish(Tables tb, Relax rx, uint4* nres) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (g >= tb.G) return;
+  const uint32_t tag = tb.ginfo[g].order | kHold;
+  for (uint32_t i = rx.hold_off[g] + lane; i < rx.hold_off[g + 1]; i += 32) {
+    const uint4 h = rx.hold[i];
+    uint32_t* r = reinterpret_cast<uint32_t*>(nres + h.x);
+    atomicAdd(r + 0, h.y); atomicAdd(r + 1, h.z); atomicAdd(r + 2, h.w);   // (the host checked that no field overflows)
+    claim_add(rx, h.x, tag, h.y, h.z, h.w, tag & (kHold - 1u));   // cmaxr >= the owner's rank: the owner reads the line
+  }
+}
+
+// cycle end, after the last fold: an admitted owner gives back what it left of its hold, (H - U)+ per node.  One warp per gang.
+__global__ void __launch_bounds__(256) k_hold_release(Tables tb, Relax rx, uint4* nres) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (g >= tb.G || rx.state[g] != GROVE_GANG_ADMITTED) return;
+  const uint32_t po = tb.ginfo[g].pod_off, cnt = rx.cur_n[g], coff = tb.gangs[g].clique_off;
+  for (uint32_t i = rx.hold_off[g] + lane; i < rx.hold_off[g + 1]; i += 32) {
+    const uint4 h = rx.hold[i];
+    uint32_t u[4] = {0u, 0u, 0u, 0u};
+    for (uint32_t j = 0; j < cnt; ++j)
+      if (rx.ent_node[po + j] == h.x) { const grove_clique_t q = tb.cliques[coff + rx.ent_meta[po + j]]; u[0] += q.req_cpu_milli; u[1] += q.req_mem_mib; u[2] += q.req_gpu; u[3] += 1u; }
+    const uint32_t hv[4] = {h.y, h.z, h.w & 0xFFFFu, h.w >> 16};
+    uint32_t* r = reinterpret_cast<uint32_t*>(nres + h.x);
+    const uint32_t back[4] = {hv[0] - min(u[0], hv[0]), hv[1] - min(u[1], hv[1]), hv[2] - min(u[2], hv[2]), hv[3] - min(u[3], hv[3])};
+    if (back[0]) atomicAdd(r + 0, back[0]);
+    if (back[1]) atomicAdd(r + 1, back[1]);
+    if (back[2] | back[3]) atomicAdd(r + 2, back[2] | (back[3] << 16));
+  }
+}
+
+// one warp per evaluated gang: publish a changed result (kHolds: a cycle with holds)
+template <bool kHolds>
 __global__ void __launch_bounds__(256) k_apply(Tables tb, Relax rx) {
   cudaGridDependencySynchronize();   // (launched chained: engine.cu launch_chained)
   const uint32_t lane = threadIdx.x & 31;
@@ -176,6 +242,7 @@ __global__ void __launch_bounds__(256) k_apply(Tables tb, Relax rx) {
     if (lane == 0) rx.extent[g] = n_ext;   // what the LATEST evaluation read, changed result or not
     if (!diff) continue;
     const uint32_t stamp = make_stamp(round, rank);
+    const bool owner = kHolds && has_hold(rx, g);   // its claims are what its placement needs beyond its hold
     // withdraw the old claims
     for (uint32_t i = lane; i < on; i += 32) {
       if (!run_length(rx.ent_node + po, rx.ent_meta + po, i, on)) continue;
@@ -192,7 +259,8 @@ __global__ void __launch_bounds__(256) k_apply(Tables tb, Relax rx) {
       const uint32_t t = run_length(rx.nxt_node + po, rx.nxt_meta + po, i, nn);
       if (t) {
         const grove_clique_t q = tb.cliques[gg.clique_off + m];
-        claim_add(rx, n, rank, t * q.req_cpu_milli, t * q.req_mem_mib, t * uint32_t(q.req_gpu) | (t << 16));
+        if (owner) { const uint3 c = owner_claim(tb, rx, g, rx.nxt_node + po, rx.nxt_meta + po, i, t); claim_add(rx, n, rank, c.x, c.y, c.z, rank); }
+        else claim_add(rx, n, rank, t * q.req_cpu_milli, t * q.req_mem_mib, t * uint32_t(q.req_gpu) | (t << 16), rank);
         atomicMin(rx.add_stamp + n, stamp);
       }
     }
@@ -292,6 +360,7 @@ __global__ void __launch_bounds__(256) k_detect(Topo tp, Tables tb, Relax rx, ui
 // one warp per gang that became final since the last fold: its claims move into the committed state.  Not every round: the
 // claims of final gangs are as good as committed for everybody who ranks after them, so the fold runs before a capacity-table
 // rebuild (the tables are built from the committed state) and when the cycle ends; k_fold_mark then moves the marker.
+template <bool kHolds>
 __global__ void __launch_bounds__(256) k_fold(Tables tb, Relax rx, uint4* nres) {
   cudaGridDependencySynchronize();
   const uint32_t lane = threadIdx.x & 31;
@@ -301,6 +370,16 @@ __global__ void __launch_bounds__(256) k_fold(Tables tb, Relax rx, uint4* nres) 
     const uint32_t g = tb.by_rank[p];
     const uint32_t t = rx.tstate[g];
     if (lane == 0) rx.state[g] = uint8_t(t);
+    const bool owner = kHolds && has_hold(rx, g);
+    if (owner) {   // its hold leaves whole, whatever the result: an admitted owner's leftovers come back when the cycle ends (k_hold_release)
+      for (uint32_t i = rx.hold_off[g] + lane; i < rx.hold_off[g + 1]; i += 32) {
+        const uint4 h = rx.hold[i];
+        claim_remove(rx, h.x, p | kHold);
+        uint32_t* r = reinterpret_cast<uint32_t*>(nres + h.x);
+        atomicSub(r + 0, h.y); atomicSub(r + 1, h.z); atomicSub(r + 2, h.w);
+        atomicOr(rx.nlive + (h.x >> 2), kStale << ((h.x & 3u) * 8u));
+      }
+    }
     if (t != GROVE_GANG_ADMITTED) continue;
     const uint32_t po = tb.ginfo[g].pod_off, cnt = rx.cur_n[g], coff = tb.gangs[g].clique_off;
     for (uint32_t i = lane; i < cnt; i += 32) {
@@ -310,9 +389,14 @@ __global__ void __launch_bounds__(256) k_fold(Tables tb, Relax rx, uint4* nres) 
       const grove_clique_t q = tb.cliques[coff + rx.ent_meta[po + i]];
       claim_remove(rx, n, p);
       uint32_t* r = reinterpret_cast<uint32_t*>(nres + n);
-      if (q.req_cpu_milli) atomicSub(r + 0, len * q.req_cpu_milli);
-      if (q.req_mem_mib) atomicSub(r + 1, len * q.req_mem_mib);
-      atomicSub(r + 2, len * uint32_t(q.req_gpu) | (len << 16));
+      if (owner) {   // the claim it published (k_apply)
+        const uint3 c = owner_claim(tb, rx, g, rx.ent_node + po, rx.ent_meta + po, i, len);
+        atomicSub(r + 0, c.x); atomicSub(r + 1, c.y); atomicSub(r + 2, c.z);
+      } else {
+        if (q.req_cpu_milli) atomicSub(r + 0, len * q.req_cpu_milli);
+        if (q.req_mem_mib) atomicSub(r + 1, len * q.req_mem_mib);
+        atomicSub(r + 2, len * uint32_t(q.req_gpu) | (len << 16));
+      }
       atomicOr(rx.nlive + (n >> 2), kStale << ((n & 3u) * 8u));   // the capacity tables no longer describe this node
     }
   }

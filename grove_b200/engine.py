@@ -24,7 +24,7 @@ SYMBOLS = [
     "grove_abi_version", "grove_engine_create", "grove_engine_destroy", "grove_last_error",
     "grove_load_nodes", "grove_update_nodes", "grove_get_nodes", "grove_submit_gangs", "grove_run_cycle",
     "grove_get_placements", "grove_get_gang_status", "grove_get_scope_domains", "grove_load_nodes_device",
-    "grove_build_score_matrix", "grove_run_cycle_preempt", "grove_get_victims",
+    "grove_build_score_matrix", "grove_run_cycle_preempt", "grove_get_victims", "grove_run_cycle_reuse",
     "grove_shard_range", "grove_run_score_pass", "grove_shard_summary_device",
     "grove_debug_get_perm", "grove_debug_get_fit_row", "grove_debug_get_score_row",
 ]
@@ -137,6 +137,18 @@ class PlacementEngine:
         st = np.zeros(1, dtype=T.stats_dt)
         self._check(self.lib.grove_run_cycle_preempt(self.h, _p(running), C.c_uint32(len(running)), _p(holdings),
                                                      C.c_uint32(len(holdings)), _p(st)))
+        return {k: st[k][0].item() for k in T.stats_dt.names}
+
+    def run_cycle_reuse(self, replaces: np.ndarray, running: np.ndarray, holdings: np.ndarray) -> dict:
+        """the ordinary cycle in which gang g with replaces[g] = r != NONE_U32 is the new version of running gang r
+        (PodGangSpec.ReuseReservationRef): it may use what r holds (`running` T.running_dt, `holdings` T.holding_dt), nobody else
+        may, and when g is admitted r's leftovers return to the free table (include/grove_place.h "reservation reuse")"""
+        replaces = np.ascontiguousarray(replaces, dtype=np.uint32)
+        running = np.ascontiguousarray(running, dtype=T.running_dt)
+        holdings = np.ascontiguousarray(holdings, dtype=T.holding_dt)
+        st = np.zeros(1, dtype=T.stats_dt)
+        self._check(self.lib.grove_run_cycle_reuse(self.h, _p(replaces), C.c_uint32(len(replaces)), _p(running),
+                                                   C.c_uint32(len(running)), _p(holdings), C.c_uint32(len(holdings)), _p(st)))
         return {k: st[k][0].item() for k in T.stats_dt.names}
 
     def victims(self) -> np.ndarray:

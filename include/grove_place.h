@@ -248,6 +248,23 @@ int32_t grove_run_cycle_preempt(grove_engine_t* e, const grove_running_gang_t* r
                                 const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats);
 int32_t grove_get_victims(grove_engine_t* e, grove_victim_t* out, uint32_t cap, uint32_t* n_out);
 
+/* ---- reservation reuse ---------------------------------------------------------------------------
+ * The API names it (PodGangSpec.ReuseReservationRef, podgang.go:65-71: "During updates, an operator can suggest to reuse the
+ * reservation of the previous PodGang for a newer version of the PodGang resource"); the arithmetic is ours (DESIGN.md section
+ * 1, "Reservation reuse").  RUNNING gangs are handed in as for grove_run_cycle_preempt (the loaded node table does not include
+ * what they hold).  replaces[g] (one entry per submitted gang) is the running gang that gang g is the new version of, or
+ * GROVE_NONE_U32; a running gang is replaced by at most one gang.  The cycle is the ordinary sequential pass, except that a
+ * gang g with a predecessor is evaluated against free + H_g, where the hold H_g starts as the predecessor's holdings and no other
+ * gang ever sees it.  Admitted with usage U (per node and resource): free -= (U - H_g)+ and H_g = (H_g - U)+ -- the new version
+ * uses its own reservation first.  Rejected, GATED_SKIP or BASE_REJECTED: nothing changes, the predecessor keeps running.  When
+ * the pass ends every admitted replacement's predecessor is gone: free += H_g.  Outputs through the usual getters; the node
+ * table is the free table after all that.  GROVE_ERR_INVALID_ARG when n_gangs is not the submitted count, replaces[] names a
+ * running gang out of range or one twice, a holding lies on a node out of range, or free + all holds overflows a field of a
+ * node record.  No reclaim pass. */
+int32_t grove_run_cycle_reuse(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs,
+                              const grove_running_gang_t* running, uint32_t n_running,
+                              const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats);
+
 /* K2: the topology-distance score matrix T[clique][node] = fit ? 1 + levels shared with the gang's anchor : 0 (u8) over the
  * snapshot the last cycle started from -- what a scheduler's Score extension point would hand out.  The admission does
  * not read it (its visiting order comes from the anchor's domain ranges), so it is built on request; GROVE_TUNE_SCORE=1

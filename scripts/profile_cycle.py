@@ -104,7 +104,7 @@ def rounds_of(acts: list[dict]) -> list[dict]:
         n = a["name"]
         if n.startswith("k_eval"):
             evals.append(a)
-        elif n == "k_apply":
+        elif n.startswith("k_apply"):
             apply_ = a
         elif n == "k_detect" and evals and apply_ is not None:
             k3_s, k3_e = min(e["start"] for e in evals), max(e["end"] for e in evals)
