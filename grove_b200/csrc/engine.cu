@@ -222,6 +222,13 @@ struct grove_engine {
   DevBuf<uint4> d_hold;
   uint32_t n_hold = 0;
   bool holds_on = false;
+  // reclaim views of a grove_run_cycle_reuse_preempt (reclaim.cuh): the running gangs' holdings by sorted node, their
+  // priorities, the gone mask, the class's free table, the free table after the ordinary pass (restored on an error), and
+  // the row gather / patch buffers
+  DevBuf<uint32_t> d_rc_off, d_rc_idx, d_rc_bad;
+  DevBuf<uint4> d_rc_ent, d_rc_real, d_rc_base, d_rc_rows, d_rc_patch;
+  DevBuf<int32_t> d_rc_prio;
+  DevBuf<uint8_t> d_rc_gone;
 };
 
 
@@ -1261,6 +1268,10 @@ inline void give(grove_node_t& n, const grove_holding_t& h) {
 }
 }  // namespace
 
+static int32_t publish_reclaim(grove_engine* e, std::vector<grove_gang_status_t>& status, const std::vector<grove_placement_t>& place,
+                               const std::vector<std::vector<grove_placement_t>>& extra, const std::vector<grove_scope_status_t>& sstat,
+                               grove_cycle_stats_t st0, std::vector<grove_victim_t> victims, grove_cycle_stats_t* stats);
+
 int32_t grove_run_cycle_preempt(grove_engine_t* e, const grove_running_gang_t* running, uint32_t n_running,
                                 const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
   if (!e || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
@@ -1389,7 +1400,14 @@ int32_t grove_run_cycle_preempt(grove_engine_t* e, const grove_running_gang_t* r
     rc = grove_load_nodes(e, real.data(), N); if (rc) return rc;
     rc = grove_submit_gangs(e, gangs.data(), G, cliques.data(), Q, scopes.data(), S); if (rc) return rc;
   }
-  // merged outputs: placements grouped by gang in submission order
+  return publish_reclaim(e, status, place, extra, sstat, st0, std::move(victims), stats);
+}
+
+// the outputs of a cycle with a reclaim pass, merged: placements grouped by gang in submission order (a preemptor's from `extra`)
+static int32_t publish_reclaim(grove_engine* e, std::vector<grove_gang_status_t>& status, const std::vector<grove_placement_t>& place,
+                               const std::vector<std::vector<grove_placement_t>>& extra, const std::vector<grove_scope_status_t>& sstat,
+                               grove_cycle_stats_t st0, std::vector<grove_victim_t> victims, grove_cycle_stats_t* stats) {
+  const uint32_t G = e->G, S = e->S;
   CU_TRY(e, e->h_status.ensure(std::max<uint32_t>(G, 1))); CU_TRY(e, e->h_scope_status.ensure(std::max<uint32_t>(S, 1)));
   size_t total = 0;
   for (uint32_t g = 0; g < G; ++g) total += status[g].state == GROVE_GANG_ADMITTED ? status[g].n_pods : 0u;
@@ -1429,9 +1447,9 @@ int32_t grove_get_victims(grove_engine_t* e, grove_victim_t* out, uint32_t cap, 
 // predecessors' holdings into one hold record per (replacement gang, node), in sorted node order; the ordinary cycle then runs with
 // the holds (relax.cuh k_hold_publish / k_fold / k_hold_release).
 // ---------------------------------------------------------------------------------------------
-int32_t grove_run_cycle_reuse(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs, const grove_running_gang_t* running,
-                              uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
-  if (!e || (n_gangs && !replaces) || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
+// the inputs of a cycle with replacements (grove_run_cycle_reuse, grove_run_cycle_reuse_preempt)
+static int32_t check_reuse_inputs(grove_engine* e, const uint32_t* replaces, uint32_t n_gangs, const grove_running_gang_t* running,
+                                  uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings) {
   if (!e->nodes_loaded) return fail(e, GROVE_ERR_STATE, "no node snapshot loaded");
   if (!e->gangs_loaded) return fail(e, GROVE_ERR_STATE, "no gangs submitted");
   if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
@@ -1448,6 +1466,14 @@ int32_t grove_run_cycle_reuse(grove_engine_t* e, const uint32_t* replaces, uint3
     if (taken[r]) return fail(e, GROVE_ERR_INVALID_ARG, "a running gang is replaced by more than one gang");
     taken[r] = 1;
   }
+  return GROVE_OK;
+}
+
+// The cycle over the submitted gangs in which gang g with replaces[g] != GROVE_NONE_U32 holds what that running gang holds
+// (inputs checked by check_reuse_inputs).  check_fit: first make sure that free plus every hold fits the node record's fields.
+static int32_t run_cycle_holds(grove_engine* e, const uint32_t* replaces, const grove_running_gang_t* running, const grove_holding_t* holdings,
+                               bool check_fit, grove_cycle_stats_t* stats) {
+  const uint32_t n_gangs = e->G;
   CU_TRY(e, cudaSetDevice(e->cfg.device));
   // one record per (gang, node): x = sorted node, then cpu, mem, gpu, pods summed over the predecessor's holdings there
   struct Rec { uint32_t node; uint64_t v[4]; };
@@ -1472,7 +1498,7 @@ int32_t grove_run_cycle_reuse(grove_engine_t* e, const uint32_t* replaces, uint3
   }
   off[n_gangs] = uint32_t(recs.size());
   // the free table plus every hold must fit the node record's fields
-  if (!recs.empty()) {
+  if (check_fit && !recs.empty()) {
     std::vector<uint4> nres(e->Npad);
     CU_TRY(e, cudaMemcpyAsync(nres.data(), e->d_nres.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToHost, e->stream));
     CU_TRY(e, cudaStreamSynchronize(e->stream));
@@ -1496,6 +1522,262 @@ int32_t grove_run_cycle_reuse(grove_engine_t* e, const uint32_t* replaces, uint3
   struct HoldsOn { grove_engine* e; ~HoldsOn() { e->holds_on = false; e->n_hold = 0; } } holds_guard{e};
   e->holds_on = !recs.empty(); e->n_hold = uint32_t(recs.size());
   return run_cycle(e, stats);
+}
+
+int32_t grove_run_cycle_reuse(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs, const grove_running_gang_t* running,
+                              uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
+  if (!e || (n_gangs && !replaces) || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
+  const int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);
+  if (rc) return rc;
+  return run_cycle_holds(e, replaces, running, holdings, true, stats);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Reuse with reclaim (include/grove_place.h "reuse with reclaim"; DESIGN.md section 1).  The ordinary pass is the reuse cycle.
+// Then every priority class of the gangs it rejected is ONE cycle with holds (the members whose predecessor ranks at or above
+// the class hold what it holds) over the class view, which reclaim.cuh builds on the device from the running gangs' holdings:
+// the free table plus whatever the standing running gangs of a lower priority hold.  Victims are chosen on the host, gang by
+// gang in rank order, over the rows of the nodes the class's preemptors use; then the device takes the holdings of the running
+// gangs still standing off the table again, which leaves the free table.
+// ---------------------------------------------------------------------------------------------
+int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs, const grove_running_gang_t* running,
+                                      uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
+  if (!e || (n_gangs && !replaces) || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
+  int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);
+  if (rc) return rc;
+  CU_TRY(e, cudaSetDevice(e->cfg.device));
+  const uint32_t N = e->N, nblk = (N + 255) / 256;
+  // the holdings by sorted node, running gangs ascending within a row: uploaded once
+  std::vector<uint32_t> off(size_t(N) + 1, 0);
+  for (uint32_t r = 0; r < n_running; ++r)
+    for (uint32_t k = 0; k < running[r].n_holdings; ++k) ++off[e->inv[holdings[running[r].holding_off + k].node] + 1];
+  for (uint32_t n = 0; n < N; ++n) off[n + 1] += off[n];
+  std::vector<uint4> ent(std::max<uint32_t>(off[N], 1));
+  {
+    std::vector<uint32_t> cur(off.begin(), off.end() - 1);
+    for (uint32_t r = 0; r < n_running; ++r)
+      for (uint32_t k = 0; k < running[r].n_holdings; ++k) {
+        const grove_holding_t& h = holdings[running[r].holding_off + k];
+        ent[cur[e->inv[h.node]]++] = make_uint4(r, h.cpu_milli, h.mem_mib, uint32_t(h.gpu) | (uint32_t(h.pods) << 16));
+      }
+  }
+  std::vector<int32_t> prio(std::max<uint32_t>(n_running, 1), 0);
+  for (uint32_t r = 0; r < n_running; ++r) prio[r] = running[r].priority;
+  std::vector<uint8_t> gone(std::max<uint32_t>(n_running, 1), 0);   // released or evicted
+  CU_TRY(e, e->d_rc_off.ensure(off.size())); CU_TRY(e, e->d_rc_ent.ensure(ent.size())); CU_TRY(e, e->d_rc_bad.ensure(1));
+  CU_TRY(e, e->d_rc_prio.ensure(prio.size())); CU_TRY(e, e->d_rc_gone.ensure(gone.size()));
+  CU_TRY(e, e->d_rc_real.ensure(e->Npad)); CU_TRY(e, e->d_rc_base.ensure(e->Npad));
+  CU_TRY(e, cudaMemcpyAsync(e->d_rc_off.p, off.data(), sizeof(uint32_t) * off.size(), cudaMemcpyHostToDevice, e->stream));
+  CU_TRY(e, cudaMemcpyAsync(e->d_rc_ent.p, ent.data(), sizeof(uint4) * ent.size(), cudaMemcpyHostToDevice, e->stream));
+  CU_TRY(e, cudaMemcpyAsync(e->d_rc_prio.p, prio.data(), sizeof(int32_t) * prio.size(), cudaMemcpyHostToDevice, e->stream));
+  CU_TRY(e, cudaMemsetAsync(e->d_rc_bad.p, 0, sizeof(uint32_t), e->stream));
+  const ReclaimCsr csr{e->d_rc_off.p, e->d_rc_ent.p, e->d_rc_prio.p, e->d_rc_gone.p};
+  // free plus every running gang's holdings must fit the node record's fields: then so does every class view and every hold
+  k_reclaim_check<<<nblk, 256, 0, e->stream>>>(e->d_nres.p, csr, N, e->d_rc_bad.p);
+  CU_TRY(e, cudaGetLastError());
+  uint32_t bad = 0;
+  CU_TRY(e, cudaMemcpyAsync(&bad, e->d_rc_bad.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
+  CU_TRY(e, cudaStreamSynchronize(e->stream));
+  if (bad) return fail(e, GROVE_ERR_INVALID_ARG, "free resources plus holdings overflow a field of a node record");
+
+  // 1. the ordinary pass: the reuse cycle.  An admitted new version's predecessor is released.
+  grove_cycle_stats_t st0{};
+  rc = run_cycle_holds(e, replaces, running, holdings, false, &st0);
+  if (rc) return rc;
+  const uint32_t G = e->G, Q = e->Q, S = e->S;
+  std::vector<grove_gang_t> gangs(e->gangs.data(), e->gangs.data() + G);
+  std::vector<grove_clique_t> cliques(e->cliques.data(), e->cliques.data() + Q);
+  std::vector<grove_scope_t> scopes(e->scopes.data(), e->scopes.data() + S);
+  std::vector<grove_gang_status_t> status(e->h_status.p, e->h_status.p + G);
+  std::vector<grove_placement_t> place(e->h_out.p, e->h_out.p + e->n_out);
+  std::vector<grove_scope_status_t> sstat(std::max<uint32_t>(S, 1));
+  if (S) { rc = grove_get_scope_domains(e, sstat.data(), S); if (rc) return rc; }
+  for (uint32_t g = 0; g < G; ++g)
+    if (status[g].state == GROVE_GANG_ADMITTED && replaces[g] != GROVE_NONE_U32) gone[replaces[g]] = 1;
+  std::vector<int32_t> classes;
+  for (uint32_t g = 0; g < G; ++g) if (status[g].state == GROVE_GANG_REJECTED) classes.push_back(gangs[g].priority);
+  std::sort(classes.begin(), classes.end(), std::greater<int32_t>());
+  classes.erase(std::unique(classes.begin(), classes.end()), classes.end());
+  auto below = [&](int32_t p) {   // is E(p) -- the standing running gangs of a priority below p -- non-empty?
+    for (uint32_t r = 0; r < n_running; ++r) if (!gone[r] && prio[r] < p) return true;
+    return false;
+  };
+  std::vector<grove_victim_t> victims;
+  std::vector<std::vector<grove_placement_t>> extra(G);   // placements of the preemptors, by gang
+  if (!classes.empty() && below(classes.front())) {
+    // whatever goes wrong from here on, the handle goes back to the caller's submission on the free table the ordinary pass left
+    CU_TRY(e, cudaMemcpyAsync(e->d_rc_base.p, e->d_nres.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToDevice, e->stream));
+    struct Restore {
+      grove_engine* e; const std::vector<grove_gang_t>* g; const std::vector<grove_clique_t>* c; const std::vector<grove_scope_t>* s; bool armed = true;
+      ~Restore() {
+        if (!armed) return;
+        const std::string keep = e->err;
+        cudaMemcpyAsync(e->d_nres.p, e->d_rc_base.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToDevice, e->stream);
+        cudaStreamSynchronize(e->stream);
+        grove_submit_gangs(e, g->data(), uint32_t(g->size()), c->data(), uint32_t(c->size()), s->data(), uint32_t(s->size()));
+        e->err = keep;
+      }
+    };
+    Restore restore{e, &gangs, &cliques, &scopes};
+    // running gangs by node (caller order), for the victim choice
+    std::vector<uint32_t> at_off(size_t(N) + 1, 0), at_run(n_holdings);
+    for (uint32_t r = 0; r < n_running; ++r) for (uint32_t h = 0; h < running[r].n_holdings; ++h) ++at_off[holdings[running[r].holding_off + h].node + 1];
+    for (uint32_t n = 0; n < N; ++n) at_off[n + 1] += at_off[n];
+    { std::vector<uint32_t> cur(at_off.begin(), at_off.end() - 1);
+      for (uint32_t r = 0; r < n_running; ++r) for (uint32_t h = 0; h < running[r].n_holdings; ++h) at_run[cur[holdings[running[r].holding_off + h].node]++] = r; }
+    std::vector<int32_t> slot(N, -1);   // node (caller order) -> its row in `rows` while a class chooses its victims
+    for (int32_t p : classes) {
+      if (!below(p)) break;   // E(p) only shrinks from one class to the next
+      // 2. the class's rejected gangs as a submission of their own: anchors pinned to what the ordinary pass used, no gating.
+      // A member holds its predecessor's holdings when that one still stands at or above p; below p it is evictable instead.
+      std::vector<uint32_t> ids, sub_rep;
+      std::vector<grove_gang_t> sg; std::vector<grove_clique_t> sq; std::vector<grove_scope_t> ss;
+      for (uint32_t g = 0; g < G; ++g) {
+        if (status[g].state != GROVE_GANG_REJECTED || gangs[g].priority != p) continue;
+        grove_gang_t x = gangs[g];
+        if (x.anchor_node == GROVE_NONE_U32) x.anchor_node = e->perm[fmix32(g) % N];
+        x.base_gang = GROVE_NONE_U32;
+        x.clique_off = uint32_t(sq.size()); x.scope_off = uint32_t(ss.size());
+        sq.insert(sq.end(), cliques.begin() + gangs[g].clique_off, cliques.begin() + gangs[g].clique_off + gangs[g].n_cliques);
+        ss.insert(ss.end(), scopes.begin() + gangs[g].scope_off, scopes.begin() + gangs[g].scope_off + gangs[g].n_scopes);
+        const uint32_t r = replaces[g];
+        ids.push_back(g); sg.push_back(x);
+        sub_rep.push_back(r != GROVE_NONE_U32 && !gone[r] && prio[r] >= p ? r : GROVE_NONE_U32);
+      }
+      // the class view, on the device: free + the standing holdings of E(p); the free table itself is kept for the victim choice
+      CU_TRY(e, cudaMemcpyAsync(e->d_rc_gone.p, gone.data(), gone.size(), cudaMemcpyHostToDevice, e->stream));
+      k_reclaim_view<<<nblk, 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_real.p, csr, N, p, 1u);
+      CU_TRY(e, cudaGetLastError());
+      rc = grove_submit_gangs(e, sg.data(), uint32_t(sg.size()), sq.data(), uint32_t(sq.size()), ss.data(), uint32_t(ss.size())); if (rc) return rc;
+      grove_cycle_stats_t stp{};
+      rc = run_cycle_holds(e, sub_rep.data(), running, holdings, false, &stp); if (rc) return rc;
+      st0.rounds += stp.rounds; st0.evaluations += stp.evaluations; st0.kernel_launches += stp.kernel_launches + 2;   // (+ the two k_reclaim_view)
+      st0.ms_fit += stp.ms_fit; st0.ms_admit += stp.ms_admit; st0.ms_commit += stp.ms_commit; st0.ms_total += stp.ms_total;
+      std::vector<grove_scope_status_t> ssp(std::max<size_t>(ss.size(), 1));
+      if (!ss.empty()) { rc = grove_get_scope_domains(e, ssp.data(), uint32_t(ss.size())); if (rc) return rc; }
+      // the free-table rows of the nodes the class's preemptors use
+      std::vector<uint32_t> used;
+      for (uint32_t k = 0; k < ids.size(); ++k) {
+        const grove_gang_status_t& sp = e->h_status.p[k];
+        if (sp.state != GROVE_GANG_ADMITTED) continue;
+        for (uint32_t i = 0; i < sp.n_pods; ++i) used.push_back(e->h_out.p[sp.placement_off + i].node);
+      }
+      std::sort(used.begin(), used.end());
+      used.erase(std::unique(used.begin(), used.end()), used.end());
+      std::vector<Res> rows(used.size());
+      if (!used.empty()) {
+        std::vector<uint32_t> idx(used.size());
+        for (size_t i = 0; i < used.size(); ++i) { idx[i] = e->inv[used[i]]; slot[used[i]] = int32_t(i); }
+        std::vector<uint4> got(used.size());
+        CU_TRY(e, e->d_rc_idx.ensure(idx.size())); CU_TRY(e, e->d_rc_rows.ensure(idx.size()));
+        CU_TRY(e, cudaMemcpyAsync(e->d_rc_idx.p, idx.data(), sizeof(uint32_t) * idx.size(), cudaMemcpyHostToDevice, e->stream));
+        k_reclaim_rows<<<uint32_t((idx.size() + 255) / 256), 256, 0, e->stream>>>(e->d_rc_real.p, e->d_rc_idx.p, e->d_rc_rows.p, uint32_t(idx.size()));
+        CU_TRY(e, cudaGetLastError());
+        CU_TRY(e, cudaMemcpyAsync(got.data(), e->d_rc_rows.p, sizeof(uint4) * got.size(), cudaMemcpyDeviceToHost, e->stream));
+        CU_TRY(e, cudaStreamSynchronize(e->stream));
+        for (size_t i = 0; i < got.size(); ++i) rows[i] = Res{got[i].x, got[i].y, got[i].z & 0xFFFFu, got[i].z >> 16};
+        st0.kernel_launches += 1;
+      }
+      auto release = [&](uint32_t v) {   // everything v held returns to the free table (only the tracked rows matter here)
+        gone[v] = 1;
+        for (uint32_t h = 0; h < running[v].n_holdings; ++h) {
+          const grove_holding_t& x = holdings[running[v].holding_off + h];
+          if (slot[x.node] < 0) continue;
+          Res& q = rows[slot[x.node]];
+          q.cpu += x.cpu_milli; q.mem += x.mem_mib; q.gpu += x.gpu; q.pods += x.pods;
+        }
+      };
+      // 3. victims, gang by gang in rank order (sub-submission order == order rank: one priority)
+      std::vector<uint32_t> skipped;   // admitted by the class cycle after E(p) ran out: they stay REJECTED
+      for (uint32_t k = 0; k < ids.size(); ++k) {
+        const grove_gang_status_t& sp = e->h_status.p[k];
+        if (sp.state != GROVE_GANG_ADMITTED) continue;
+        if (!below(p)) { skipped.push_back(k); continue; }
+        const uint32_t g = ids[k], r = replaces[g];
+        const bool holds = sub_rep[k] != GROVE_NONE_U32;
+        if (r != GROVE_NONE_U32 && !holds && !gone[r]) release(r);   // its predecessor is in E(p): released first, not a victim
+        std::vector<uint32_t> order; std::vector<Res> use, own;
+        for (uint32_t i = 0; i < sp.n_pods; ++i) {
+          const grove_placement_t pl = e->h_out.p[sp.placement_off + i];
+          const grove_clique_t& q = sq[pl.clique];
+          size_t j = 0;
+          for (; j < order.size(); ++j) if (order[j] == pl.node) break;
+          if (j == order.size()) { order.push_back(pl.node); use.emplace_back(); own.emplace_back(); }
+          use[j].cpu += q.req_cpu_milli; use[j].mem += q.req_mem_mib; use[j].gpu += q.req_gpu; use[j].pods += 1;
+          extra[g].push_back(grove_placement_t{gangs[g].clique_off + (pl.clique - sg[k].clique_off), pl.node});
+        }
+        if (holds)   // what its predecessor holds on each of those nodes: used first
+          for (uint32_t h = 0; h < running[r].n_holdings; ++h) {
+            const grove_holding_t& x = holdings[running[r].holding_off + h];
+            for (size_t j = 0; j < order.size(); ++j)
+              if (order[j] == x.node) { own[j].cpu += x.cpu_milli; own[j].mem += x.mem_mib; own[j].gpu += x.gpu; own[j].pods += x.pods; }
+          }
+        for (size_t j = 0; j < order.size(); ++j) {
+          const uint32_t n = order[j];
+          const Res need{std::max<int64_t>(use[j].cpu - own[j].cpu, 0), std::max<int64_t>(use[j].mem - own[j].mem, 0),
+                         std::max<int64_t>(use[j].gpu - own[j].gpu, 0), std::max<int64_t>(use[j].pods - own[j].pods, 0)};
+          Res& have = rows[slot[n]];
+          while (!(have.cpu >= need.cpu && have.mem >= need.mem && have.gpu >= need.gpu && have.pods >= need.pods)) {
+            uint32_t v = GROVE_NONE_U32;   // lowest priority first, then the highest running index
+            for (uint32_t a = at_off[n]; a < at_off[n + 1]; ++a) {
+              const uint32_t x = at_run[a];
+              if (gone[x] || prio[x] >= p) continue;
+              if (v == GROVE_NONE_U32 || prio[x] < prio[v] || (prio[x] == prio[v] && x > v)) v = x;
+            }
+            if (v == GROVE_NONE_U32) return fail(e, GROVE_ERR_STATE, "reclaim pass: a preemptor's node cannot be freed");
+            release(v);
+            victims.push_back(grove_victim_t{v, g});
+          }
+          have.cpu -= need.cpu; have.mem -= need.mem; have.gpu -= need.gpu; have.pods -= need.pods;
+        }
+        if (holds) gone[r] = 1;   // released; its leftover came back when the class cycle ended (k_hold_release)
+        grove_gang_status_t o = sp;
+        o.reserved0 = GROVE_STATUS_PREEMPTOR;
+        status[g] = o;   // placement_off is assigned when the outputs are merged
+        for (uint32_t si = 0; si < gangs[g].n_scopes; ++si) sstat[gangs[g].scope_off + si] = ssp[sg[k].scope_off + si];
+        st0.gangs_admitted += 1; st0.gangs_rejected -= 1;
+      }
+      for (uint32_t n : used) slot[n] = -1;
+      if (!skipped.empty()) {   // give back what the class cycle committed for them: +U, and -H for a member with a hold
+        std::vector<std::pair<uint32_t, std::array<int64_t, 4>>> d;   // (sorted node, change)
+        for (uint32_t k : skipped) {
+          const grove_gang_status_t& sp = e->h_status.p[k];
+          for (uint32_t i = 0; i < sp.n_pods; ++i) {
+            const grove_placement_t pl = e->h_out.p[sp.placement_off + i];
+            const grove_clique_t& q = sq[pl.clique];
+            d.push_back({e->inv[pl.node], {int64_t(q.req_cpu_milli), int64_t(q.req_mem_mib), int64_t(q.req_gpu), 1}});
+          }
+          if (sub_rep[k] != GROVE_NONE_U32)
+            for (uint32_t h = 0; h < running[sub_rep[k]].n_holdings; ++h) {
+              const grove_holding_t& x = holdings[running[sub_rep[k]].holding_off + h];
+              d.push_back({e->inv[x.node], {-int64_t(x.cpu_milli), -int64_t(x.mem_mib), -int64_t(x.gpu), -int64_t(x.pods)}});
+            }
+        }
+        std::sort(d.begin(), d.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+        std::vector<uint4> patch;
+        for (size_t i = 0; i < d.size();) {
+          const uint32_t n = d[i].first;
+          int64_t v[4] = {0, 0, 0, 0};
+          for (; i < d.size() && d[i].first == n; ++i) for (int k = 0; k < 4; ++k) v[k] += d[i].second[k];
+          patch.push_back(make_uint4(n, uint32_t(v[0]), uint32_t(v[1]), uint32_t(v[2] + v[3] * 65536)));
+        }
+        CU_TRY(e, e->d_rc_patch.ensure(patch.size()));
+        CU_TRY(e, cudaMemcpyAsync(e->d_rc_patch.p, patch.data(), sizeof(uint4) * patch.size(), cudaMemcpyHostToDevice, e->stream));
+        k_reclaim_patch<<<uint32_t((patch.size() + 255) / 256), 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_patch.p, uint32_t(patch.size()));
+        CU_TRY(e, cudaGetLastError());
+        st0.kernel_launches += 1;
+      }
+      // back to the free table: take off what the running gangs of E(p) that still stand hold
+      CU_TRY(e, cudaMemcpyAsync(e->d_rc_gone.p, gone.data(), gone.size(), cudaMemcpyHostToDevice, e->stream));
+      k_reclaim_view<<<nblk, 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_real.p, csr, N, p, 0u);
+      CU_TRY(e, cudaGetLastError());
+    }
+    // the handle goes back to the caller's submission; the device table is the free table
+    restore.armed = false;
+    rc = grove_submit_gangs(e, gangs.data(), G, cliques.data(), Q, scopes.data(), S); if (rc) return rc;
+  }
+  st0.kernel_launches += 1;   // k_reclaim_check
+  return publish_reclaim(e, status, place, extra, sstat, st0, std::move(victims), stats);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -487,13 +487,14 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
   grove_cycle_stats_t st{};
   // running PodGangs -> the reclaim pass's / reservation reuse's tables (holdings on nodes that left the snapshot are dropped)
   std::vector<grove_running_gang_t> run; std::vector<grove_holding_t> held; std::vector<std::string> runNames;
-  bool preempt = false, reuse = false;
+  bool preempt = false, reuse = false, both = false;   // both: SetReclaimWithReuse, one grove_run_cycle_reuse_preempt
   std::vector<uint32_t> replaces;   // reservation reuse: per gang row, the running gang it is the new version of
   {
     std::lock_guard<std::mutex> l(mu_);
-    if (preemption_ && reuse_) return mkerr("ERR_SYNC_PODGANG", "RunCycle", "preemption and reservation reuse cannot both be on");
-    preempt = preemption_ && !running_.empty();
-    reuse = reuse_ && !running_.empty();
+    if (preemption_ && reuse_ && !reclaimReuse_) return mkerr("ERR_SYNC_PODGANG", "RunCycle", "preemption and reservation reuse cannot both be on");
+    both = reclaimReuse_ && !running_.empty();
+    preempt = (preemption_ || reclaimReuse_) && !running_.empty();
+    reuse = (reuse_ || reclaimReuse_) && !running_.empty();
     if (preempt || reuse) {
       std::map<std::string, uint32_t> nodeIdx;
       for (uint32_t i = 0; i < nodes.size(); ++i) nodeIdx[nodes[i].Name] = i;
@@ -523,7 +524,8 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
       reuse = std::any_of(replaces.begin(), replaces.end(), [](uint32_t r) { return r != GROVE_NONE_U32; });
     }
   }
-  if (reuse) { if (auto e = chk(grove_run_cycle_reuse(engine_, replaces.data(), uint32_t(replaces.size()), run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_reuse")) return e; }
+  if (both) { if (auto e = chk(grove_run_cycle_reuse_preempt(engine_, replaces.data(), uint32_t(replaces.size()), run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_reuse_preempt")) return e; }
+  else if (reuse) { if (auto e = chk(grove_run_cycle_reuse(engine_, replaces.data(), uint32_t(replaces.size()), run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_reuse")) return e; }
   else if (preempt) { if (auto e = chk(grove_run_cycle_preempt(engine_, run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_preempt")) return e; }
   else if (auto e = chk(grove_run_cycle(engine_, &st), "grove_run_cycle")) return e;
   if (stats) *stats = st;
@@ -577,7 +579,10 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
       running_.erase(runNames[vs[i].running]);
     }
   }
-  if (reuse)   // an admitted new version replaces its predecessor: the caller deletes the old pods, whose resources the cycle released
+  // an admitted new version replaces its predecessor: the caller deletes the old pods, whose resources the cycle released.  (With
+  // reclaim a predecessor that an earlier preemptor evicted is that one's victim and was forgotten above; it keeps its
+  // DisruptionTarget.  A released one is not disrupted.)
+  if (reuse && !replaces.empty())
     for (uint32_t i = 0; i < gs.size(); ++i)
       if (gs[i].state == GROVE_GANG_ADMITTED && replaces[i] != GROVE_NONE_U32) running_.erase(runNames[replaces[i]]);
   for (uint32_t i = 0; i < gs.size(); ++i) {

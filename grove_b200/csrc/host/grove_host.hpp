@@ -249,6 +249,12 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   // of it releases nothing twice).  The anchor hint stays either way.  Off by default; a cycle with both this and preemption on
   // fails.
   void SetReservationReuse(bool on) { std::lock_guard<std::mutex> l(mu_); reuse_ = on; }
+  // Reuse with reclaim: with it on, a cycle with running PodGangs is grove_run_cycle_reuse_preempt -- reservation reuse as
+  // above, then the reclaim pass, in which a rejected new version may also use its predecessor's reservation -- whatever
+  // SetPreemption and SetReservationReuse say.  Admitted new versions forget their predecessor (not disrupted); victims get
+  // DisruptionTarget naming their preemptor and are forgotten.  Off by default; with it off the other two switches work as
+  // before: either one alone, and both together fail.
+  void SetReclaimWithReuse(bool on) { std::lock_guard<std::mutex> l(mu_); reclaimReuse_ = on; }
   size_t Running() const { std::lock_guard<std::mutex> l(mu_); return running_.size(); }
   // why a PodGang cannot be handed to the engine (limits of the packed tables), or empty.  SyncPodGang accepts every
   // PodGang -- the reference's reconciler would requeue forever on an error -- and RunCycle reports these as
@@ -278,6 +284,7 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   std::map<std::string, RunningGang> running_;   // PodGangs scheduled by this backend and not deleted since
   bool preemption_ = false;
   bool reuse_ = false;
+  bool reclaimReuse_ = false;
   grove_engine_t* engine_ = nullptr;
   uint32_t engineLevels_ = 0;
   mutable std::mutex mu_;        // pending set, bindings, levels: everything SyncPodGang / OnPodGangDelete / SyncTopology touch

@@ -7,6 +7,7 @@
 //   admit.cuh    k_eval  K3  one gang against its view: all-or-nothing admission, warp-cooperative packing
 //   relax.cuh    k_select / k_apply / k_detect / k_fold    the relaxation that makes the evaluations of all gangs
 //                agree with the sequential, priority-ordered pass; k_fin_* / k_emit  outputs
+//   reclaim.cuh  k_reclaim_*  reclaim-class views over the running gangs' holdings (grove_run_cycle_reuse_preempt)
 //
 // Semantics are DESIGN.md "Placement semantics"; the reference contract they restate is cited in
 // include/grove_place.h.  Integer / compare work only: no tensor cores, no floating point.
@@ -17,3 +18,4 @@
 #include "score.cuh"
 #include "admit.cuh"
 #include "relax.cuh"
+#include "reclaim.cuh"

@@ -25,6 +25,7 @@ SYMBOLS = [
     "grove_load_nodes", "grove_update_nodes", "grove_get_nodes", "grove_submit_gangs", "grove_run_cycle",
     "grove_get_placements", "grove_get_gang_status", "grove_get_scope_domains", "grove_load_nodes_device",
     "grove_build_score_matrix", "grove_run_cycle_preempt", "grove_get_victims", "grove_run_cycle_reuse",
+    "grove_run_cycle_reuse_preempt",
     "grove_shard_range", "grove_run_score_pass", "grove_shard_summary_device",
     "grove_debug_get_perm", "grove_debug_get_fit_row", "grove_debug_get_score_row",
 ]
@@ -151,8 +152,21 @@ class PlacementEngine:
                                                    C.c_uint32(len(running)), _p(holdings), C.c_uint32(len(holdings)), _p(st)))
         return {k: st[k][0].item() for k in T.stats_dt.names}
 
+    def run_cycle_reuse_preempt(self, replaces: np.ndarray, running: np.ndarray, holdings: np.ndarray) -> dict:
+        """run_cycle_reuse, then the reclaim pass over the gangs it rejected: a rejected gang may evict running gangs of a lower
+        priority, and a rejected new version still holds what its predecessor holds when that one ranks at or above it
+        (include/grove_place.h "reuse with reclaim"); victims() lists the evictions"""
+        replaces = np.ascontiguousarray(replaces, dtype=np.uint32)
+        running = np.ascontiguousarray(running, dtype=T.running_dt)
+        holdings = np.ascontiguousarray(holdings, dtype=T.holding_dt)
+        st = np.zeros(1, dtype=T.stats_dt)
+        self._check(self.lib.grove_run_cycle_reuse_preempt(self.h, _p(replaces), C.c_uint32(len(replaces)), _p(running),
+                                                           C.c_uint32(len(running)), _p(holdings), C.c_uint32(len(holdings)), _p(st)))
+        return {k: st[k][0].item() for k in T.stats_dt.names}
+
     def victims(self) -> np.ndarray:
-        """(running gang, preemptor gang) pairs of the last run_cycle_preempt: the caller sets DisruptionTarget on them"""
+        """(running gang, preemptor gang) pairs of the last run_cycle_preempt / run_cycle_reuse_preempt: the caller sets
+        DisruptionTarget on them"""
         n = C.c_uint32(0)
         self._check(self.lib.grove_get_victims(self.h, None, C.c_uint32(0), C.byref(n)))
         out = np.zeros(max(n.value, 1), dtype=T.victim_dt)

@@ -265,6 +265,23 @@ int32_t grove_run_cycle_reuse(grove_engine_t* e, const uint32_t* replaces, uint3
                               const grove_running_gang_t* running, uint32_t n_running,
                               const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats);
 
+/* ---- reuse with reclaim ---------------------------------------------------------------------------
+ * Reservation reuse and the reclaim pass in one cycle (DESIGN.md section 1, "Reuse with reclaim").  Inputs as for
+ * grove_run_cycle_reuse.  The ordinary pass is grove_run_cycle_reuse; every predecessor of an admitted new version is then
+ * released and can never be a victim.  Every gang it left REJECTED is then reconsidered in order rank as by
+ * grove_run_cycle_preempt, against free + E(p) (what the standing running gangs of a priority below p hold), skipped while E(p)
+ * is empty.  A gang g with a predecessor r that still stands:
+ *   - r's priority >= p: g also sees r's holdings H_r, nobody else does; admitted, it uses H_r first on every node, then evicts;
+ *     r is released (not a victim) and (H_r - U)+ returns to the free table after the last gang of priority p;
+ *   - r's priority < p: r is an ordinary evictable gang; admitted, g releases r first (everything it held returns at once, r is
+ *     not a victim), then evicts as usual.
+ * Preemptors carry GROVE_STATUS_PREEMPTOR; grove_get_victims lists (running gang, preemptor) pairs.  GROVE_ERR_INVALID_ARG for
+ * the inputs grove_run_cycle_reuse rejects, with the same reasons; the overflow check covers free + the holdings of every
+ * running gang. */
+int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs,
+                                      const grove_running_gang_t* running, uint32_t n_running,
+                                      const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats);
+
 /* K2: the topology-distance score matrix T[clique][node] = fit ? 1 + levels shared with the gang's anchor : 0 (u8) over the
  * snapshot the last cycle started from -- what a scheduler's Score extension point would hand out.  The admission does
  * not read it (its visiting order comes from the anchor's domain ranges), so it is built on request; GROVE_TUNE_SCORE=1
