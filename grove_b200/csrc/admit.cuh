@@ -36,6 +36,7 @@ struct GangShared {
   grove_scope_t scopes[GROVE_MAX_GANG_SCOPES];
   uint32_t sig[GROVE_MAX_GANG_CLIQUES];    // fit-bitmap / capacity row of each clique
   uint32_t smask[GROVE_MAX_GANG_CLIQUES];  // class mask | need_depth << 16
+  // a wide cycle (kWide) keeps its entry stacks in global memory (Relax::wide_node) and this space for its own state: see wide_own
   uint32_t ent_node[GROVE_MAX_GANG_PODS];
   uint16_t ent_meta[GROVE_MAX_GANG_PODS];  // clique_rel
   uint32_t Hlo[GROVE_MAX_GANG_CLIQUES], Hhi[GROVE_MAX_GANG_CLIQUES];
@@ -44,6 +45,26 @@ struct GangShared {
   int8_t c_got[GROVE_MAX_GANG_CLIQUES];    // level each clique / scope was packed at (-1: the whole cluster)
   int8_t s_got[GROVE_MAX_GANG_SCOPES];
 };
+// kWide (a gang of up to GROVE_MAX_WIDE_GANG_PODS pods, up to that many replicas per clique): the space of the shared entry
+// stack holds Ev::own_word's scratch (int4[32] in ent_node, 16-aligned) and the 16-bit counts, which the packed clq word has no
+// room for (min | replicas << 16, uint32_t[32] in ent_meta).  The ordinary instantiations never see these views.
+__device__ __forceinline__ int4* wide_own(GangShared& sh) { return reinterpret_cast<int4*>(sh.ent_node); }
+__device__ __forceinline__ uint32_t* wide_cnt(GangShared& sh) { return reinterpret_cast<uint32_t*>(sh.ent_meta); }
+__device__ __forceinline__ const uint32_t* wide_cnt(const GangShared& sh) { return reinterpret_cast<const uint32_t*>(sh.ent_meta); }
+static_assert(sizeof(GangShared::ent_node) >= 32 * sizeof(int4) && offsetof(GangShared, ent_node) % alignof(int4) == 0 &&
+              sizeof(GangShared::ent_meta) >= GROVE_MAX_GANG_CLIQUES * 4 && offsetof(GangShared, ent_meta) % 4 == 0, "wide views");
+
+// MinReplicas / replicas of clique cr: the packed word, or (kWide) the 16-bit counts
+template <bool kWide>
+__device__ __forceinline__ uint32_t clq_min(const GangShared& sh, uint32_t cr) {
+  if constexpr (kWide) return wide_cnt(sh)[cr] & 0xFFFFu;
+  else return sh.clq[cr].w & 0xFFu;
+}
+template <bool kWide>
+__device__ __forceinline__ uint32_t clq_rep(const GangShared& sh, uint32_t cr) {
+  if constexpr (kWide) return wide_cnt(sh)[cr] >> 16;
+  else return (sh.clq[cr].w >> 8) & 0xFFu;
+}
 
 // Ordered pieces of [lo,hi): descending score, ties by ascending rotated index (n - anchor) mod N.
 // from == L: node granularity (ring l = anc_l \ anc_{l+1}, upper part then lower part);
@@ -115,14 +136,19 @@ __device__ __forceinline__ uint32_t cap_from(uint32_t cpu, uint32_t mem, uint32_
 // floor(x / d) for the staged evaluator, exact below 256 and >= 256 above (callers never ask for more than 255 pods);
 // r = 1.0f / d.  Branch-free so that the three resources -- and the nodes a lane handles -- overlap: the estimate is
 // within one of the quotient (relative error of the product < 2^-22, quotients < 257), one signed remainder fixes it.
+// kWide (asks of up to GROVE_MAX_WIDE_GANG_PODS pods): exact below 4096 and >= 4096 above.  The clamped estimate is below
+// 4097 and the product's relative error below 2^-22, so its absolute error is below 4097 * 2^-22 < 0.001: the truncated
+// estimate is still within one of the quotient and the same single fix-up makes it exact.
+template <bool kWide = false>
 __device__ __forceinline__ uint32_t div_rcp(uint32_t x, uint32_t d, float r) {
-  uint32_t q = __float2uint_rz(fminf(__uint2float_rz(x) * r, 256.0f));
+  uint32_t q = __float2uint_rz(fminf(__uint2float_rz(x) * r, kWide ? 4096.0f : 256.0f));
   const long long rem = (long long)x - (long long)((unsigned long long)q * d);
   q += uint32_t(rem >= (long long)d) - uint32_t(rem < 0);
   return d ? q : 0xFFFFu;
 }
+template <bool kWide = false>
 __device__ __forceinline__ uint32_t cap_from_rcp(uint32_t cpu, uint32_t mem, uint32_t gpu, uint32_t pods, const uint4& q, const float4& r) {
-  return min(min(div_rcp(cpu, q.x, r.x), div_rcp(mem, q.y, r.y)), min(div_rcp(gpu, q.z, r.z), pods));
+  return min(min(div_rcp<kWide>(cpu, q.x, r.x), div_rcp<kWide>(mem, q.y, r.y)), min(div_rcp<kWide>(gpu, q.z, r.z), pods));
 }
 
 // position of node n in the gang's node visiting order (descending closeness to the anchor, ties by ascending
@@ -142,20 +168,46 @@ __device__ __forceinline__ uint32_t visit_pos(const GangRegs& g, uint32_t n) {
 }
 
 // ---- the evaluator: the whole warp packs ONE candidate range ------------------------------------------
-template <bool kPref_, bool kHolds>
+template <bool kPref_, bool kHolds, bool kWide_ = false>
 struct Ev {
   static constexpr bool kPref = kPref_;
+  static constexpr bool kWide = kWide_;
   static constexpr bool kStaged = false;
   const Topo& tp; const Relax& rb; GangShared& sh; const GangRegs& g; uint32_t lane;
   uint32_t np;
   uint32_t tmask = 0;   // bit (n & 31) set for every node the gang has put a pod on: quick 'untouched' test
   uint32_t ext = 0;     // see the file comment
   uint32_t t_stage = 0, t_pre = 0, t_pack = 0, n_stage = 0;
+  // the entry stack: shared memory, or (kWide) the warp's own stack in global memory
+  uint32_t* wn = nullptr; uint16_t* wm = nullptr;
+  __device__ __forceinline__ uint32_t& en(uint32_t i) const { if constexpr (kWide) return wn[i]; else return sh.ent_node[i]; }
+  __device__ __forceinline__ uint16_t& em(uint32_t i) const { if constexpr (kWide) return wm[i]; else return sh.ent_meta[i]; }
   __device__ Ev(const Topo& t, const Relax& r, GangShared& s, const GangRegs& gr, uint32_t ln)
       : tp(t), rb(r), sh(s), g(gr), lane(ln), np(0) {}
 
-  // pods of clique cr that still fit on node n under the gang's view, after what the gang itself put there
-  __device__ __forceinline__ uint32_t cap_view(uint32_t cr, uint32_t n) const {
+  // kWide: what the gang itself has put on each node of the 32-node word at `base` (the lane's node), gathered by the warp in
+  // one pass over the entry stack -- np / 32 loads a lane, where a scan per lane and node would cost np.  Warp-collective; the
+  // callers skip it for a word whose fit nodes the gang has not touched (tmask & word == 0: every fit lane's usage is zero).
+  __device__ __forceinline__ int4 own_word(uint32_t base) const {
+    int4* own = wide_own(sh);
+    own[lane] = make_int4(0, 0, 0, 0);
+    __syncwarp();
+    for (uint32_t i = lane; i < np; i += 32) {
+      const uint32_t d = wn[i] - base;
+      if (d < 32u) {
+        const uint4 q = sh.clq[wm[i]];
+        int* o = reinterpret_cast<int*>(own + d);
+        atomicAdd(o + 0, int(q.x)); atomicAdd(o + 1, int(q.y)); atomicAdd(o + 2, int(q.z)); atomicAdd(o + 3, 1);
+      }
+    }
+    __syncwarp();
+    const int4 r = own[lane];
+    __syncwarp();
+    return r;
+  }
+
+  // pods of clique cr that still fit on node n under the gang's view, after what the gang itself put there (kWide: o, from own_word)
+  __device__ __forceinline__ uint32_t cap_view(uint32_t cr, uint32_t n, int4 o = int4{}) const {
     const uint32_t live = (__ldg(rb.nlive + (n >> 2)) >> ((n & 3u) * 8u)) & 0xFFu;
     const bool own = (tmask >> (n & 31u)) & 1u;
     if (!live && !own) {
@@ -186,15 +238,20 @@ struct Ev {
         }
       }
     }
-    if (own) {
-      for (uint32_t i = 0; i < np; ++i) {
-        if (sh.ent_node[i] == n) {
-          const uint4 o = sh.clq[sh.ent_meta[i]];
-          cpu -= int(o.x); mem -= int(o.y); gpu -= int(o.z); pods -= 1;
+    if constexpr (kWide) {
+      cpu -= o.x; mem -= o.y; gpu -= o.z; pods -= o.w;
+      return cap_from_rcp<true>(uint32_t(max(cpu, 0)), uint32_t(max(mem, 0)), uint32_t(max(gpu, 0)), uint32_t(max(pods, 0)), sh.clq[cr], sh.rcp[cr]);
+    } else {
+      if (own) {
+        for (uint32_t i = 0; i < np; ++i) {
+          if (sh.ent_node[i] == n) {
+            const uint4 o = sh.clq[sh.ent_meta[i]];
+            cpu -= int(o.x); mem -= int(o.y); gpu -= int(o.z); pods -= 1;
+          }
         }
       }
+      return cap_from(uint32_t(max(cpu, 0)), uint32_t(max(mem, 0)), uint32_t(max(gpu, 0)), uint32_t(max(pods, 0)), sh.clq[cr]);
     }
-    return cap_from(uint32_t(max(cpu, 0)), uint32_t(max(mem, 0)), uint32_t(max(gpu, 0)), uint32_t(max(pods, 0)), sh.clq[cr]);
   }
 
   __device__ __forceinline__ uint32_t scope_filter(const grove_scope_t&, uint32_t, uint32_t, bool, int) { return kFull; }   // staged evaluator only
@@ -216,14 +273,16 @@ struct Ev {
         last = min(base + 31u, b - 1u);
         if (!word) continue;   // no fit node when the tables were built: none now
         const uint32_t n = base + lane;
-        const uint32_t c = ((word >> lane) & 1u) ? cap_view(cr, n) : 0u;
+        int4 o{};
+        if constexpr (kWide) if (tmask & word) o = own_word(base);   // (warp-uniform)
+        const uint32_t c = ((word >> lane) & 1u) ? cap_view(cr, n, o) : 0u;
         const uint32_t incl = warp_incl_scan(c, lane), excl = incl - c, rem = want - placed;
         const uint32_t t = excl >= rem ? 0u : min(c, rem - excl);
         const uint32_t tincl = warp_incl_scan(t, lane);
         __syncwarp();  // every lane's scan of the entry stack is over before it grows
         if (t) {
           const uint32_t pos = np + tincl - t;
-          for (uint32_t j = 0; j < t; ++j) { sh.ent_node[pos + j] = n; sh.ent_meta[pos + j] = uint16_t(cr); }
+          for (uint32_t j = 0; j < t; ++j) { en(pos + j) = n; em(pos + j) = uint16_t(cr); }
         }
         const uint32_t tb = __ballot_sync(kFull, t != 0);
         const uint32_t tot = __shfl_sync(kFull, tincl, 31);
@@ -238,7 +297,7 @@ struct Ev {
   }
 
   __device__ bool fill_min(uint32_t cr, uint32_t lo, uint32_t hi) {
-    const uint32_t m = sh.clq[cr].w & 0xFFu;
+    const uint32_t m = clq_min<kWide>(sh, cr);
     const uint32_t mark = np;
     if (take(cr, lo, hi, m) < m) { rollback(mark); return false; }
     if (lane == 0) { sh.Hlo[cr] = lo; sh.Hhi[cr] = hi; }
@@ -249,7 +308,7 @@ struct Ev {
   // clique whose own Required level is a unit level (one node per domain, e.g. hostname):
   // first node of [lo,hi) in score order that takes all m pods
   __device__ GROVE_NI bool find_unit(uint32_t cr, uint32_t lo, uint32_t hi) {
-    const uint32_t m = sh.clq[cr].w & 0xFFu;
+    const uint32_t m = clq_min<kWide>(sh, cr);
     const uint32_t* Frow = rb.F + size_t(sh.sig[cr]) * tp.words;
     PieceIt pit; pit.init(g, lo, hi, g.L);
     uint32_t last = GROVE_NONE_U32;
@@ -261,12 +320,14 @@ struct Ev {
         last = min(base + 31u, b - 1u);
         if (!word) continue;
         const uint32_t n = base + lane;
-        const uint32_t c = ((word >> lane) & 1u) ? cap_view(cr, n) : 0u;
+        int4 o{};
+        if constexpr (kWide) if (tmask & word) o = own_word(base);   // (warp-uniform)
+        const uint32_t c = ((word >> lane) & 1u) ? cap_view(cr, n, o) : 0u;
         const uint32_t okb = __ballot_sync(kFull, c >= m && ((word >> lane) & 1u));
         __syncwarp();
         if (okb) {
           const uint32_t nn = base + (__ffs(okb) - 1);
-          for (uint32_t j = lane; j < m; j += 32) { sh.ent_node[np + j] = nn; sh.ent_meta[np + j] = uint16_t(cr); }
+          for (uint32_t j = lane; j < m; j += 32) { en(np + j) = nn; em(np + j) = uint16_t(cr); }
           if (lane == 0) { sh.Hlo[cr] = nn; sh.Hhi[cr] = nn + 1; }
           tmask |= 1u << (nn & 31u);
           np += m;
@@ -290,9 +351,10 @@ struct Ev {
 // instead of a chain of dependent L2 look-ups per 32 nodes.
 constexpr uint32_t kStageMax = 128;
 
-template <bool kPref_, bool kHolds>
+template <bool kPref_, bool kHolds, bool kWide_ = false>
 struct EvS {
   static constexpr bool kPref = kPref_;
+  static constexpr bool kWide = kWide_;
   static constexpr bool kStaged = true;   // node state in shared memory: an attempt costs less than the table look-ups that would skip it
   const Topo& tp; const Relax& rb; GangShared& sh; const GangRegs& g; uint32_t lane;
   int4* view;           // [kStageMax] cpu, mem, gpu, pods the gang may still take.  Signed: the claims of lower ranks may transiently exceed
@@ -306,6 +368,10 @@ struct EvS {
   uint32_t np;
   uint32_t tmask = 0;
   uint32_t ext = 0;
+  // the entry stack: shared memory, or (kWide) the warp's own stack in global memory
+  uint32_t* wn = nullptr; uint16_t* wm = nullptr;
+  __device__ __forceinline__ uint32_t& en(uint32_t i) const { if constexpr (kWide) return wn[i]; else return sh.ent_node[i]; }
+  __device__ __forceinline__ uint16_t& em(uint32_t i) const { if constexpr (kWide) return wm[i]; else return sh.ent_meta[i]; }
   __device__ EvS(const Topo& t, const Relax& r, GangShared& s, const GangRegs& gr, uint32_t ln, int4* v, uint32_t* vf, uint8_t* cv)
       : tp(t), rb(r), sh(s), g(gr), lane(ln), view(v), vflag(vf), rk(cv), np(0) {}
 
@@ -365,7 +431,7 @@ struct EvS {
     const uint32_t f = vflag[n - vlo];
     const uint32_t sm = sh.smask[cr];
     const bool usable = (f & GROVE_NODE_SCHEDULABLE) && ((sm >> ((f >> GROVE_NODE_CLASS_SHIFT) & 0xFu)) & 1u) && ((f >> 16) & 0xFu) >= (sm >> 16);
-    const uint32_t c = cap_from_rcp(uint32_t(max(v.x, 0)), uint32_t(max(v.y, 0)), uint32_t(max(v.z, 0)), uint32_t(max(v.w, 0)), sh.clq[cr], sh.rcp[cr]);
+    const uint32_t c = cap_from_rcp<kWide>(uint32_t(max(v.x, 0)), uint32_t(max(v.y, 0)), uint32_t(max(v.z, 0)), uint32_t(max(v.w, 0)), sh.clq[cr], sh.rcp[cr]);
     return usable ? c : 0u;
   }
 
@@ -386,7 +452,7 @@ struct EvS {
     for (uint32_t i = 0; i < s.n_cliques; ++i) {
       const uint32_t cr = s.first_clique + i;
       const uint32_t w = sh.clq[cr].w;
-      const uint32_t m = w & 0xFFu, ql = (w >> 16) & 0xFFu;
+      const uint32_t m = clq_min<kWide>(sh, cr), ql = (w >> 16) & 0xFFu;
       if (m == 0) continue;
       rsum[lane] = 0; rmax[lane] = 0;
       __syncwarp();
@@ -409,8 +475,8 @@ struct EvS {
   __device__ GROVE_NI void rollback(uint32_t mark) {
     __syncwarp();
     for (uint32_t i = mark + lane; i < np; i += 32) {
-      const uint4 q = sh.clq[sh.ent_meta[i]];
-      int* v = reinterpret_cast<int*>(view + (sh.ent_node[i] - vlo));
+      const uint4 q = sh.clq[em(i)];
+      int* v = reinterpret_cast<int*>(view + (en(i) - vlo));
       if (q.x) atomicAdd(v + 0, int(q.x));
       if (q.y) atomicAdd(v + 1, int(q.y));
       if (q.z) atomicAdd(v + 2, int(q.z));
@@ -435,7 +501,7 @@ struct EvS {
         const uint32_t tincl = warp_incl_scan(t, lane);
         if (t) {
           const uint32_t pos = np + tincl - t;
-          for (uint32_t j = 0; j < t; ++j) { sh.ent_node[pos + j] = n; sh.ent_meta[pos + j] = uint16_t(cr); }
+          for (uint32_t j = 0; j < t; ++j) { en(pos + j) = n; em(pos + j) = uint16_t(cr); }
           int4 v = view[n - vlo];
           v.x -= int(t * q.x); v.y -= int(t * q.y); v.z -= int(t * q.z); v.w -= int(t);
           view[n - vlo] = v;
@@ -449,7 +515,7 @@ struct EvS {
   }
 
   __device__ bool fill_min(uint32_t cr, uint32_t lo, uint32_t hi) {
-    const uint32_t m = sh.clq[cr].w & 0xFFu;
+    const uint32_t m = clq_min<kWide>(sh, cr);
     const uint32_t mark = np;
     if (take(cr, lo, hi, m) < m) { rollback(mark); return false; }
     if (lane == 0) { sh.Hlo[cr] = lo; sh.Hhi[cr] = hi; }
@@ -458,7 +524,7 @@ struct EvS {
   }
 
   __device__ GROVE_NI bool find_unit(uint32_t cr, uint32_t lo, uint32_t hi) {
-    const uint32_t m = sh.clq[cr].w & 0xFFu;
+    const uint32_t m = clq_min<kWide>(sh, cr);
     const uint4 q = sh.clq[cr];
     PieceIt pit; pit.init(g, lo, hi, g.L);
     for (uint32_t a, b; pit.next(g, a, b);) {
@@ -469,7 +535,7 @@ struct EvS {
         const uint32_t okb = __ballot_sync(kFull, in && c >= m);
         if (okb) {
           const uint32_t nn = base + (__ffs(okb) - 1);
-          for (uint32_t j = lane; j < m; j += 32) { sh.ent_node[np + j] = nn; sh.ent_meta[np + j] = uint16_t(cr); }
+          for (uint32_t j = lane; j < m; j += 32) { en(np + j) = nn; em(np + j) = uint16_t(cr); }
           if (lane == 0) {
             sh.Hlo[cr] = nn; sh.Hhi[cr] = nn + 1;
             int4 v = view[nn - vlo];
@@ -490,54 +556,70 @@ struct EvS {
 // (each clique alone must find MinReplicas worth of capacity in a domain it could be packed into, and
 // the cliques of a scope must find it inside one common scope domain).  Reads only the small
 // per-signature capacity tables.
+// kWide: a clique may ask for more than 255 pods, and a capacity byte of 255 is saturated (the node may take any number): such a
+// node counts as unbounded, and so does a domain whose capacity maximum is 255 -- its sum under-counts it.
+template <bool kWide = false>
 __device__ __forceinline__ bool clique_plausible(const Topo& tp, const Relax& rb, const GangShared& sh, uint32_t cr,
                                  uint32_t lo, uint32_t hi, int lvl, uint32_t dE) {
   const uint32_t w = sh.clq[cr].w;
-  const uint32_t m = w & 0xFFu, ql = (w >> 16) & 0xFFu;
+  const uint32_t m = clq_min<kWide>(sh, cr), ql = (w >> 16) & 0xFFu;
   if (m == 0) return true;
+  const uint32_t m8 = kWide ? min(m, 255u) : m;   // a single node's byte against the ask
   const size_t row = size_t(sh.sig[cr]);
   const bool tabled = lvl >= 0 && !tp.unit[lvl];
   if (ql != GROVE_LEVEL_NONE && int(ql) > lvl) {
     if (tp.unit[ql]) {  // all m pods on one node
-      if (tabled) return __ldg(rb.capmax + row * tp.cap_stride + tp.cap_off[lvl] + dE) >= m;
-      for (uint32_t n = lo; n < hi; ++n) if (__ldg(rb.cap8 + row * tp.npad + n) >= m) return true;
+      if (tabled) return __ldg(rb.capmax + row * tp.cap_stride + tp.cap_off[lvl] + dE) >= m8;
+      for (uint32_t n = lo; n < hi; ++n) if (__ldg(rb.cap8 + row * tp.npad + n) >= m8) return true;
       return false;
     }
     const uint32_t d0 = __ldg(tp.next_dom[ql] + lo), d1 = __ldg(tp.next_dom[ql] + hi);
     uint32_t any = 0;  // no early exit: the look-ups are independent and overlap
-    for (uint32_t d = d0; d < d1; ++d) any |= __ldg(rb.capsum + row * tp.cap_stride + tp.cap_off[ql] + d) >= m;
+    for (uint32_t d = d0; d < d1; ++d) {
+      any |= __ldg(rb.capsum + row * tp.cap_stride + tp.cap_off[ql] + d) >= m;
+      if constexpr (kWide) any |= __ldg(rb.capmax + row * tp.cap_stride + tp.cap_off[ql] + d) >= 255u;
+    }
     return any != 0;
   }
-  if (tabled) return __ldg(rb.capsum + row * tp.cap_stride + tp.cap_off[lvl] + dE) >= m;
+  if (tabled) {
+    if constexpr (kWide) if (__ldg(rb.capmax + row * tp.cap_stride + tp.cap_off[lvl] + dE) >= 255u) return true;
+    return __ldg(rb.capsum + row * tp.cap_stride + tp.cap_off[lvl] + dE) >= m;
+  }
   uint32_t sum = 0;
-  for (uint32_t n = lo; n < hi && sum < m; ++n) sum += __ldg(rb.cap8 + row * tp.npad + n);
+  for (uint32_t n = lo; n < hi && sum < m; ++n) {
+    const uint32_t c = __ldg(rb.cap8 + row * tp.npad + n);
+    sum += (kWide && c == 255u) ? m : c;
+  }
   return sum >= m;
 }
 
+template <bool kWide = false>
 __device__ __forceinline__ bool scope_plausible(const Topo& tp, const Relax& rb, const GangShared& sh, const grove_scope_t& s,
                                 uint32_t lo, uint32_t hi, int lvl, uint32_t dE) {
   uint32_t all = 1;
-  for (uint32_t i = 0; i < s.n_cliques; ++i) all &= clique_plausible(tp, rb, sh, s.first_clique + i, lo, hi, lvl, dE);
+  for (uint32_t i = 0; i < s.n_cliques; ++i) all &= clique_plausible<kWide>(tp, rb, sh, s.first_clique + i, lo, hi, lvl, dE);
   return all != 0;
 }
 
 // one scope of a gang inside the candidate [lo, hi) of level lvl
+template <bool kWide = false>
 __device__ __forceinline__ bool scope_ok(const Topo& tp, const Relax& rb, const GangShared& sh, const grove_scope_t& s,
                                          uint32_t lo, uint32_t hi, int lvl, uint32_t dD) {
   if (s.level != GROVE_LEVEL_NONE && int(s.level) > lvl) {
     const uint32_t d0 = __ldg(tp.next_dom[s.level] + lo), d1 = __ldg(tp.next_dom[s.level] + hi);
     uint32_t any = 0;  // no early exit: children are independent table look-ups
     for (uint32_t d = d0; d < d1; ++d)
-      any |= scope_plausible(tp, rb, sh, s, __ldg(tp.dom_lo[s.level] + d), __ldg(tp.dom_hi[s.level] + d), int(s.level), d);
+      any |= scope_plausible<kWide>(tp, rb, sh, s, __ldg(tp.dom_lo[s.level] + d), __ldg(tp.dom_hi[s.level] + d), int(s.level), d);
     return any != 0;
   }
-  return scope_plausible(tp, rb, sh, s, lo, hi, lvl, dD);
+  return scope_plausible<kWide>(tp, rb, sh, s, lo, hi, lvl, dD);
 }
 
+template <bool kWide = false>
 __device__ bool gang_plausible(const Topo& tp, const Relax& rb, const GangShared& sh, uint32_t n_scopes,
                                uint32_t lo, uint32_t hi, int lvl, uint32_t dD) {
   for (uint32_t si = 0; si < n_scopes; ++si)
-    if (!scope_ok(tp, rb, sh, sh.scopes[si], lo, hi, lvl, dD)) return false;
+    if (!scope_ok<kWide>(tp, rb, sh, sh.scopes[si], lo, hi, lvl, dD)) return false;
   return true;
 }
 
@@ -561,7 +643,7 @@ __device__ GROVE_NI bool place_scope(Ev& ev, const grove_scope_t& s, uint32_t lo
   for (uint32_t i = 0; i < s.n_cliques; ++i) {
     const uint32_t cr = s.first_clique + i;
     const uint32_t w = ev.sh.clq[cr].w;
-    const uint32_t m = w & 0xFFu;
+    const uint32_t m = clq_min<Ev::kWide>(ev.sh, cr);
     bool ok = false;
     int first;
     const int base = level_span<Ev::kPref>((w >> 16) & 0xFFu, w >> 24, lvl, first);
@@ -654,7 +736,7 @@ __device__ GROVE_NI bool place_in(Ev& ev, uint32_t n_scopes, uint32_t lo, uint32
             const long long tp0 = ev.rb.dbg ? clock64() : 0;
             if (d < d1) {
               el = __ldg(tp.dom_lo[sl] + d); eh = __ldg(tp.dom_hi[sl] + d);
-              plaus = scope_plausible(tp, ev.rb, ev.sh, s, el, eh, sl, d);
+              plaus = scope_plausible<Ev::kWide>(tp, ev.rb, ev.sh, s, el, eh, sl, d);
             }
             uint32_t todo = __ballot_sync(kFull, plaus);
             const long long tp1 = ev.rb.dbg ? clock64() : 0;
@@ -690,6 +772,7 @@ __device__ __forceinline__ void score_unit(uint32_t req, uint32_t pref, int got,
 // The candidate pre-filter per (gang shape, domain): a CTA per 32 domains of one level, FOUR threads per domain (they share the
 // gang's scopes: a base gang's scopes are independent chains of table look-ups), the shape's representative gang staged in
 // shared memory.  Runs after every capacity-table build; k_eval then reads one bit per candidate.
+template <bool kWide>
 __global__ void __launch_bounds__(128) k_shape_plaus(Topo tp, Tables tb, Relax rx, const uint32_t* __restrict__ shape_rep) {
   __shared__ GangShared sh;
   __shared__ uint32_t s_bits;
@@ -708,6 +791,7 @@ __global__ void __launch_bounds__(128) k_shape_plaus(Topo tp, Tables tb, Relax r
                            uint32_t(q.min_replicas) | (uint32_t(q.replicas) << 8) | (uint32_t(q.level) << 16) |
                                (GROVE_CLIQUE_PREFERRED(q.scope) << 24));
     sh.sig[c] = tb.cinfo[gg.clique_off + c].sig;
+    if constexpr (kWide) wide_cnt(sh)[c] = rx.ccount[gg.clique_off + c];
   }
   for (uint32_t si = threadIdx.x; si < gg.n_scopes; si += blockDim.x) sh.scopes[si] = tb.scopes[gg.scope_off + si];
   if (threadIdx.x == 0) s_bits = 0;
@@ -716,7 +800,7 @@ __global__ void __launch_bounds__(128) k_shape_plaus(Topo tp, Tables tb, Relax r
   bool plaus = d < tp.n_dom[l];
   if (plaus) {
     const uint32_t lo = __ldg(tp.dom_lo[l] + d), hi = __ldg(tp.dom_hi[l] + d);
-    for (uint32_t si = slot; si < gg.n_scopes && plaus; si += 4) plaus = scope_ok(tp, rx, sh, sh.scopes[si], lo, hi, int(l), d);
+    for (uint32_t si = slot; si < gg.n_scopes && plaus; si += 4) plaus = scope_ok<kWide>(tp, rx, sh, sh.scopes[si], lo, hi, int(l), d);
   }
   plaus = plaus & bool(__shfl_xor_sync(kFull, uint32_t(plaus), 1));
   plaus = plaus & bool(__shfl_xor_sync(kFull, uint32_t(plaus), 2));
@@ -755,7 +839,8 @@ __device__ __forceinline__ uint32_t eval_list_at(const Relax& rx, const Tables& 
 // cudaGridDependencySynchronize().
 constexpr uint32_t kEvalDeferred = 0xFFu;   // nxt_tstate: no result this round
 constexpr int kEvalWarps = 8;
-template <bool kPref, bool kHolds>
+// kWide: the instantiation of a wide cycle (16-bit counts; the entry stack of each warp in Relax::wide_node).
+template <bool kPref, bool kHolds, bool kWide>
 __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb, Relax rx, uint32_t max_att) {
   __shared__ GangShared shs[kEvalWarps];
   __shared__ int4 s_view[kEvalWarps][kStageMax];
@@ -775,6 +860,11 @@ __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb,
   const uint32_t grp = min(uint32_t(kEvalWarps), max(1u, (n_light + gridDim.x - 1u) / gridDim.x));   // light entries per item
   const uint32_t n_items = n_heavy + (n_light + grp - 1u) / grp;
   GangShared& sh = shs[warp];
+  uint32_t* wide_node = nullptr; uint16_t* wide_meta = nullptr;
+  if constexpr (kWide) {
+    const size_t w = size_t(blockIdx.x) * kEvalWarps + warp;
+    wide_node = rx.wide_node + w * rx.wide_cap; wide_meta = rx.wide_meta + w * rx.wide_cap;
+  }
   for (;;) {
     __syncthreads();   // the previous item's shared state is no longer read
     if (threadIdx.x == 0) s_item = atomicAdd(rx.ctl + kEvalNext, 1u);
@@ -796,6 +886,8 @@ __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb,
     const bool has_c = lane < gg.n_cliques, has_s = lane < gg.n_scopes;
     const grove_clique_t q0 = has_c ? tb.cliques[gg.clique_off + lane] : grove_clique_t{};
     const CliqueInfo ci0 = has_c ? tb.cinfo[gg.clique_off + lane] : CliqueInfo{};
+    uint32_t cnt0 = 0;
+    if constexpr (kWide) cnt0 = has_c ? rx.ccount[gg.clique_off + lane] : 0u;
     const grove_scope_t sc0 = has_s ? tb.scopes[gg.scope_off + lane] : grove_scope_t{};
     const uint32_t round_now = rx.ctl[kRound];
     const uint32_t le = rx.last_eval[gi], fu_word = rx.fail_upto[gi], ext_word = rx.extent[gi];
@@ -831,6 +923,7 @@ __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb,
                               q.req_gpu ? 1.0f / float(q.req_gpu) : 0.f, 0.f);
       sh.sig[c] = ci.sig; sh.smask[c] = uint32_t(q.class_mask) | (ci.need_depth << 16);
       sh.Hlo[c] = 0; sh.Hhi[c] = 0; sh.c_got[c] = -1;
+      if constexpr (kWide) wide_cnt(sh)[c] = cnt0;
     }
     if (has_s) { sh.scopes[lane] = sc0; sh.s_got[lane] = -1; sh.s_lo[lane] = 0; }
     if (tt == 0) { s_win[w0] = GROVE_NONE_U32; s_ext[w0] = 0; s_att[w0] = 0; s_npl[w0] = 0; }
@@ -839,8 +932,9 @@ __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb,
     // shrink otherwise (claims are added, settled claims move into the committed state).  So a re-evaluation skips the
     // candidates in front of its last answer that no withdrawal touched -- gangs that meet a nearly full cluster would
     // otherwise re-run dozens of failing attempts every round.  (Single candidate level only.)
-    Ev<kPref, kHolds> ev(tp, rx, sh, g, lane);                         // candidates of any size, node state from L2
-    EvS<kPref, kHolds> evs(tp, rx, sh, g, lane, s_view[warp], s_vflag[warp], s_rk[warp]);         // candidates of <= kStageMax nodes, node state staged in shared memory
+    Ev<kPref, kHolds, kWide> ev(tp, rx, sh, g, lane);                         // candidates of any size, node state from L2
+    EvS<kPref, kHolds, kWide> evs(tp, rx, sh, g, lane, s_view[warp], s_vflag[warp], s_rk[warp]);         // candidates of <= kStageMax nodes, node state staged in shared memory
+    if constexpr (kWide) { ev.wn = evs.wn = wide_node; ev.wm = evs.wm = wide_meta; }
     bool staged = false;  // the winning attempt ran on evs
     bool won = false;     // this warp holds the answer
     bool done = false;    // CTA-uniform
@@ -896,7 +990,7 @@ __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb,
                 const uint32_t bit = rx.pl_off[gl] + d;
                 plaus = (__ldg(rx.shape_bits + size_t(info.pad) * rx.pl_words + (bit >> 5)) >> (bit & 31u)) & 1u;
               } else {
-                plaus = gang_plausible(tp, rx, sh, gg.n_scopes, dl, dh, gl, d);
+                plaus = gang_plausible<kWide>(tp, rx, sh, gg.n_scopes, dl, dh, gl, d);
               }
               if (base == 0) { s_cl[w0 + c][lane] = dl; s_ch[w0 + c][lane] = dh; }   // (c < tw in the first chunk)
               if (plaus && k < fu) {   // failed last time: worth another attempt only if somebody withdrew a claim in there since
@@ -966,8 +1060,7 @@ __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb,
     if (!won) continue;   // warp-uniform: the winner finishes alone
     // surplus beyond MinReplicas (best effort, podgang.go:80-83), inside the domain each clique was packed into
     for (uint32_t cr = 0; cr < gg.n_cliques; ++cr) {
-      const uint32_t w = sh.clq[cr].w;
-      const uint32_t mn = w & 0xFFu, rp = (w >> 8) & 0xFFu;
+      const uint32_t mn = clq_min<kWide>(sh, cr), rp = clq_rep<kWide>(sh, cr);
       if (rp > mn) { if (staged) evs.take(cr, sh.Hlo[cr], sh.Hhi[cr], rp - mn); else ev.take(cr, sh.Hlo[cr], sh.Hhi[cr], rp - mn); }
     }
     __syncwarp();
@@ -987,8 +1080,8 @@ __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb,
     for (int o = 16; o; o >>= 1) { num += __shfl_xor_sync(kFull, num, o); den += __shfl_xor_sync(kFull, den, o); }
     if (den == 0) { num = 1; den = 1; }
     for (uint32_t i = lane; i < n_ent; i += 32) {
-      rx.nxt_node[info.pod_off + i] = sh.ent_node[i];
-      rx.nxt_meta[info.pod_off + i] = sh.ent_meta[i];
+      rx.nxt_node[info.pod_off + i] = ev.en(i);   // (ev and evs share the entry stack)
+      rx.nxt_meta[info.pod_off + i] = ev.em(i);
     }
     for (uint32_t si = lane; si < gg.n_scopes; si += 32) {
       const bool own = int(sh.s_got[si]) > g_got;   // a scope packed at the gang's own level has no domain of its own

@@ -158,6 +158,12 @@ struct Relax {
   const uint4* hold;
   uint32_t* dbg;            // [G][8] optional per-gang evaluation statistics
   uint32_t* live;           // [kLiveWords] host-mapped: progress words the host polls (null: not available)
+  // wide submissions (grove_submit_gangs_wide), read only by the kWide instantiations of k_eval / k_shape_plaus: the 16-bit counts
+  // of every clique, and one entry stack per k_eval warp (a gang of up to 2048 pods does not fit the shared-memory one)
+  const uint32_t* ccount;   // [Q] min_replicas | replicas << 16 (null: not a wide cycle)
+  uint32_t* wide_node;      // [k_eval CTAs * kEvalWarps][wide_cap]
+  uint16_t* wide_meta;      // [k_eval CTAs * kEvalWarps][wide_cap] clique_rel
+  uint32_t wide_cap;        // pods of the largest gang
 };
 
 __device__ __forceinline__ uint32_t warp_incl_scan(uint32_t v, uint32_t lane) {

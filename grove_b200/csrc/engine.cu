@@ -136,6 +136,8 @@ struct grove_engine {
   PinVec<grove_gang_t> gangs;
   PinVec<grove_clique_t> cliques;
   PinVec<grove_scope_t> scopes;
+  PinVec<uint32_t> ccount;         // [Q] min_replicas | replicas << 16: what the engine reads, whichever entry submitted
+  bool wide = false;               // some gang has more than GROVE_MAX_GANG_PODS pods or some clique more than 255 replicas
   PinBuf<uint8_t> h_state0;        // initial gang states of a cycle
   PinBuf<GangInfo> ginfo_pin;      // derived tables are built straight into pinned memory: their upload is a plain DMA
   PinBuf<CliqueInfo> cinfo_pin;
@@ -149,6 +151,9 @@ struct grove_engine {
   DevBuf<grove_gang_t> d_gangs;
   DevBuf<grove_clique_t> d_cliques;
   DevBuf<grove_scope_t> d_scopes;
+  DevBuf<uint32_t> d_ccount;           // uploaded for wide submissions (the kernels of an ordinary cycle read the clique records)
+  DevBuf<uint32_t> d_wide_node;        // wide cycles: one entry stack per k_eval warp (relax.cuh Relax::wide_node)
+  DevBuf<uint16_t> d_wide_meta;
   DevBuf<GangInfo> d_ginfo;
   DevBuf<CliqueInfo> d_cinfo;
   DevBuf<uint4> d_sigs;
@@ -242,6 +247,11 @@ struct grove_engine {
   } while (0)
 
 static int32_t fail(grove_engine* e, int32_t code, const char* msg) { e->err = msg; return code; }
+static int32_t refuse_wide(grove_engine* e, const char* entry) {
+  e->err = std::string(entry) + ": not supported for a wide submission (a gang of more than " + std::to_string(GROVE_MAX_GANG_PODS) +
+           " pods or a clique of more than 255 replicas)";
+  return GROVE_ERR_LIMIT;
+}
 
 // A kernel of the relaxation chain, launched as a programmatic dependent of the kernel before it on the stream: its CTAs are
 // launched and become resident while that kernel drains, and wait in cudaGridDependencySynchronize() -- the first statement of
@@ -394,6 +404,7 @@ static Relax make_relax(grove_engine* e) {
   r.hold_off = e->holds_on ? e->d_hold_off.p : nullptr; r.hold = e->d_hold.p;
   r.dbg = e->dbg_on ? e->d_dbg.p : nullptr;
   r.live = e->d_live;
+  r.ccount = e->wide ? e->d_ccount.p : nullptr; r.wide_node = e->d_wide_node.p; r.wide_meta = e->d_wide_meta.p; r.wide_cap = e->max_gang_pods;
   return r;
 }
 
@@ -558,8 +569,9 @@ int32_t grove_get_nodes(grove_engine_t* e, grove_node_t* out, uint32_t cap) {
 }
 
 // one gang; returns nullptr when it is well formed, else the reason (code through *code)
-static const char* validate_gang(const grove_engine* e, const grove_gang_t* gangs, uint32_t G, const grove_clique_t* cliques, uint32_t Q,
-                                 const grove_scope_t* scopes, uint32_t S, uint32_t gi, int32_t* code) {
+static const char* validate_gang(const grove_engine* e, const grove_gang_t* gangs, uint32_t G, const grove_clique_t* cliques,
+                                 const uint32_t* ccount, uint32_t Q, const grove_scope_t* scopes, uint32_t S, uint32_t gi,
+                                 uint32_t max_pods, int32_t* code) {
   const uint32_t L = e->L;
   const grove_gang_t& g = gangs[gi];
   *code = GROVE_ERR_LIMIT;
@@ -587,40 +599,44 @@ static const char* validate_gang(const grove_engine* e, const grove_gang_t* gang
       const uint32_t qp = GROVE_CLIQUE_PREFERRED(q.scope);
       if (qp != GROVE_LEVEL_NONE && (qp >= L || (q.level != GROVE_LEVEL_NONE && qp <= q.level)))
         return "clique preferred level must be a level deeper than the required one";
-      if (q.replicas < q.min_replicas) return "replicas < min_replicas";
-      pods += q.replicas;
+      const uint32_t c = ccount[g.clique_off + next + i];
+      if ((c >> 16) < (c & 0xFFFFu)) return "replicas < min_replicas";
+      pods += c >> 16;
     }
     next += s.n_cliques;
   }
   if (next != g.n_cliques) return "scopes do not cover the gang";
-  if (pods > GROVE_MAX_GANG_PODS) { *code = GROVE_ERR_LIMIT; return "gang exceeds GROVE_MAX_GANG_PODS"; }
+  if (pods > max_pods) {
+    *code = GROVE_ERR_LIMIT;
+    return max_pods == GROVE_MAX_GANG_PODS ? "gang exceeds GROVE_MAX_GANG_PODS" : "gang exceeds GROVE_MAX_WIDE_GANG_PODS";
+  }
   return nullptr;
 }
 
 // same structural rules as the PodGang admission webhook guarantees
 // (operator/internal/webhook/admission/pcs/validation/topologyconstraints.go:195-280); the first offending gang
 // (lowest index) is reported whatever the thread count
-static int32_t validate(grove_engine* e, const grove_gang_t* gangs, uint32_t G, const grove_clique_t* cliques, uint32_t Q,
-                        const grove_scope_t* scopes, uint32_t S) {
+static int32_t validate(grove_engine* e, const grove_gang_t* gangs, uint32_t G, const grove_clique_t* cliques, const uint32_t* ccount,
+                        uint32_t Q, const grove_scope_t* scopes, uint32_t S, uint32_t max_pods) {
   uint32_t first_bad = GROVE_NONE_U32;
   const int T = G >= 2048 ? host_threads() : 1;
 #pragma omp parallel for num_threads(T) schedule(static) reduction(min : first_bad)
   for (uint32_t gi = 0; gi < G; ++gi) {
     int32_t code;
-    if (gi < first_bad && validate_gang(e, gangs, G, cliques, Q, scopes, S, gi, &code)) first_bad = gi;
+    if (gi < first_bad && validate_gang(e, gangs, G, cliques, ccount, Q, scopes, S, gi, max_pods, &code)) first_bad = gi;
   }
   if (first_bad == GROVE_NONE_U32) return GROVE_OK;
   int32_t code = GROVE_ERR_INVALID_ARG;
-  const char* why = validate_gang(e, gangs, G, cliques, Q, scopes, S, first_bad, &code);
+  const char* why = validate_gang(e, gangs, G, cliques, ccount, Q, scopes, S, first_bad, max_pods, &code);
   return fail(e, code, why ? why : "malformed gang tables");
 }
 
-int32_t grove_submit_gangs(grove_engine_t* e, const grove_gang_t* gangs, uint32_t n_gangs, const grove_clique_t* cliques,
-                           uint32_t n_cliques, const grove_scope_t* scopes, uint32_t n_scopes) {
-  if (!e || (n_gangs && (!gangs || !cliques || !scopes))) return GROVE_ERR_INVALID_ARG;
+// both submit entries: ccount[q] = min_replicas | replicas << 16 of clique q, at most max_pods pods per gang
+static int32_t submit(grove_engine* e, const grove_gang_t* gangs, uint32_t n_gangs, const grove_clique_t* cliques,
+                      const std::vector<uint32_t>& ccount, uint32_t n_cliques, const grove_scope_t* scopes, uint32_t n_scopes, uint32_t max_pods) {
   if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
   if (n_gangs >= (1u << 24)) return fail(e, GROVE_ERR_LIMIT, "too many gangs");  // order rank + round tag share a stamp word
-  int32_t rc = validate(e, gangs, n_gangs, cliques, n_cliques, scopes, n_scopes);
+  int32_t rc = validate(e, gangs, n_gangs, cliques, ccount.data(), n_cliques, scopes, n_scopes, max_pods);
   if (rc) return rc;
   CU_TRY(e, cudaSetDevice(e->cfg.device));
   CU_TRY(e, cudaEventSynchronize(e->ev_tables_up));  // an earlier upload may still be reading the pinned tables
@@ -628,6 +644,18 @@ int32_t grove_submit_gangs(grove_engine_t* e, const grove_gang_t* gangs, uint32_
   CU_TRY(e, e->gangs.assign(gangs, n_gangs));
   CU_TRY(e, e->cliques.assign(cliques, n_cliques));
   CU_TRY(e, e->scopes.assign(scopes, n_scopes));
+  CU_TRY(e, e->ccount.assign(ccount.data(), n_cliques));
+  bool wide = false;
+  for (uint32_t i = 0; i < n_cliques && !wide; ++i) wide |= (ccount[i] >> 16) > 255u;
+  for (uint32_t g = 0; g < n_gangs && !wide; ++g)
+    for (uint32_t c = 0, pods = 0; c < gangs[g].n_cliques && !wide; ++c) wide |= (pods += ccount[gangs[g].clique_off + c] >> 16) > GROVE_MAX_GANG_PODS;
+  e->wide = wide;
+  if (!wide)   // the ordinary kernels read the clique records' own counts: a wide-entry submission within the old limits brings them in
+    for (uint32_t i = 0; i < n_cliques; ++i) { e->cliques[i].min_replicas = uint8_t(ccount[i]); e->cliques[i].replicas = uint8_t(ccount[i] >> 16); }
+  if (wide) {
+    CU_TRY(e, e->d_ccount.ensure(n_cliques));
+    CU_TRY(e, cudaMemcpyAsync(e->d_ccount.p, e->ccount.data(), sizeof(uint32_t) * n_cliques, cudaMemcpyHostToDevice, e->stream));
+  }
   e->gangs_loaded = true; e->ginfo_dirty = true; e->have_results = false; e->score_pass_valid = false;
   bool pref = false;
   for (uint32_t g = 0; g < n_gangs && !pref; ++g) pref |= gangs[g].preferred != GROVE_LEVEL_NONE;
@@ -640,6 +668,22 @@ int32_t grove_submit_gangs(grove_engine_t* e, const grove_gang_t* gangs, uint32_
   if (n_scopes) CU_TRY(e, cudaMemcpyAsync(e->d_scopes.p, e->scopes.data(), sizeof(grove_scope_t) * n_scopes, cudaMemcpyHostToDevice, e->stream));
   CU_TRY(e, cudaEventRecord(e->ev_tables_up, e->stream));
   return GROVE_OK;  // the uploads read engine-owned pinned memory: nothing of the caller's is referenced any more
+}
+
+int32_t grove_submit_gangs(grove_engine_t* e, const grove_gang_t* gangs, uint32_t n_gangs, const grove_clique_t* cliques,
+                           uint32_t n_cliques, const grove_scope_t* scopes, uint32_t n_scopes) {
+  if (!e || (n_gangs && (!gangs || !cliques || !scopes))) return GROVE_ERR_INVALID_ARG;
+  std::vector<uint32_t> ccount(n_cliques);
+  for (uint32_t i = 0; i < n_cliques; ++i) ccount[i] = uint32_t(cliques[i].min_replicas) | uint32_t(cliques[i].replicas) << 16;
+  return submit(e, gangs, n_gangs, cliques, ccount, n_cliques, scopes, n_scopes, GROVE_MAX_GANG_PODS);
+}
+
+int32_t grove_submit_gangs_wide(grove_engine_t* e, const grove_gang_t* gangs, uint32_t n_gangs, const grove_clique_t* cliques,
+                                const grove_clique_count_t* counts, uint32_t n_cliques, const grove_scope_t* scopes, uint32_t n_scopes) {
+  if (!e || (n_gangs && (!gangs || !cliques || !counts || !scopes))) return GROVE_ERR_INVALID_ARG;
+  std::vector<uint32_t> ccount(n_cliques);
+  for (uint32_t i = 0; i < n_cliques; ++i) ccount[i] = uint32_t(counts[i].min_replicas) | uint32_t(counts[i].replicas) << 16;
+  return submit(e, gangs, n_gangs, cliques, ccount, n_cliques, scopes, n_scopes, GROVE_MAX_WIDE_GANG_PODS);
 }
 
 
@@ -785,7 +829,7 @@ static int32_t build_ginfo(grove_engine* e) {
           if (q.level != GROVE_LEVEL_NONE) nd = std::max(nd, uint32_t(q.level) + 1);
           if (e->cinfo[qi].gang != GROVE_NONE_U32) shared_rows++;  // rows of different threads never overlap unless the tables are malformed
           e->cinfo[qi] = CliqueInfo{gi, nd, st.intern({q.req_cpu_milli, q.req_mem_mib, q.req_gpu, q.class_mask, nd}), uint32_t(t)};
-          pods += q.replicas;
+          pods += e->ccount[qi] >> 16;
         }
       }
       gang_pods[gi] = pods;
@@ -812,7 +856,7 @@ static int32_t build_ginfo(grove_engine* e) {
       uint64_t h = 0x9E3779B97F4A7C15ull ^ (uint64_t(g.n_cliques) << 32 | uint64_t(g.n_scopes) << 16 | uint64_t(g.level) << 8 | g.preferred);
       auto mix = [&h](uint64_t v) { h ^= v + 0x9E3779B97F4A7C15ull + (h << 6) + (h >> 2); };
       for (uint32_t si = 0; si < g.n_scopes; ++si) { const grove_scope_t& s = e->scopes[g.scope_off + si]; mix(uint64_t(s.first_clique) | uint64_t(s.n_cliques) << 16 | uint64_t(s.level) << 32 | uint64_t(s.preferred1) << 40); }
-      for (uint32_t c = 0; c < g.n_cliques; ++c) { const grove_clique_t& q = e->cliques[g.clique_off + c]; mix(uint64_t(e->cinfo[g.clique_off + c].sig) | uint64_t(q.min_replicas) << 32 | uint64_t(q.level) << 40 | uint64_t(q.scope) << 48); }
+      for (uint32_t c = 0; c < g.n_cliques; ++c) { const grove_clique_t& q = e->cliques[g.clique_off + c]; mix(uint64_t(e->cinfo[g.clique_off + c].sig) | uint64_t(e->ccount[g.clique_off + c] & 0xFFFFu) << 32 | uint64_t(q.level) << 40 | uint64_t(q.scope) << 48); }
       return h;
     };
     auto shape_equal = [e](uint32_t a, uint32_t b) {
@@ -824,7 +868,8 @@ static int32_t build_ginfo(grove_engine* e) {
       }
       for (uint32_t c = 0; c < x.n_cliques; ++c) {
         const grove_clique_t& q = e->cliques[x.clique_off + c]; const grove_clique_t& r = e->cliques[y.clique_off + c];
-        if (e->cinfo[x.clique_off + c].sig != e->cinfo[y.clique_off + c].sig || q.min_replicas != r.min_replicas || q.level != r.level || q.scope != r.scope) return false;
+        if (e->cinfo[x.clique_off + c].sig != e->cinfo[y.clique_off + c].sig || ((e->ccount[x.clique_off + c] ^ e->ccount[y.clique_off + c]) & 0xFFFFu) ||
+            q.level != r.level || q.scope != r.scope) return false;
       }
       return true;
     };
@@ -923,12 +968,18 @@ static int32_t build_cap_tables(grove_engine* e, const Topo& tp, const Tables& t
       const int first = g.preferred != GROVE_LEVEL_NONE && int(g.preferred) > base ? int(g.preferred) : base;
       for (int l = std::max(base, 0); l <= first && l < int(e->L); ++l) mx = std::max(mx, e->n_dom[l]);
     }
-    if (mx) CU_TRY(e, launch_chained(k_shape_plaus, dim3((mx + 31) / 32, e->n_shapes, e->L), 128, e->stream, tp, tb, rx, e->d_shape_rep.p));
+    if (mx) CU_TRY(e, launch_chained(e->wide ? k_shape_plaus<true> : k_shape_plaus<false>, dim3((mx + 31) / 32, e->n_shapes, e->L), 128, e->stream, tp, tb, rx, e->d_shape_rep.p));
     e->launches += 1;
   }
   CU_TRY(e, cudaGetLastError());
   e->launches += 3;
   return GROVE_OK;
+}
+
+// K3 CTAs: they take work items from a queue; by default as many as are resident at once (heavy gangs take whole CTAs)
+static uint32_t eval_ctas(const grove_engine* e) {
+  const uint32_t W = e->tune_window ? e->tune_window : std::max(e->G, 1u);
+  return std::max(1u, e->tune_eval_ctas ? e->tune_eval_ctas : std::min(W, e->n_sm * e->tune_heavy_ctas));
 }
 
 static int32_t cycle_begin(grove_engine* e) {
@@ -955,6 +1006,10 @@ static int32_t cycle_begin(grove_engine* e) {
   CU_TRY(e, e->d_add_stamp.ensure(N)); CU_TRY(e, e->d_rem_stamp.ensure(e->words)); CU_TRY(e, e->d_rem_round.ensure(e->words));
   CU_TRY(e, e->d_last_eval.ensure(g1)); CU_TRY(e, e->d_fail_upto.ensure(g1));
   CU_TRY(e, e->d_status.ensure(g1)); CU_TRY(e, e->d_scope_status.ensure(s1)); CU_TRY(e, e->d_out.ensure(p1));
+  if (e->wide) {   // the entry stacks of a wide cycle's evaluations: one per k_eval warp, as deep as the largest gang
+    const size_t ws = size_t(eval_ctas(e)) * kEvalWarps * e->max_gang_pods;
+    CU_TRY(e, e->d_wide_node.ensure(ws)); CU_TRY(e, e->d_wide_meta.ensure(ws));
+  }
   CU_TRY(e, e->h_status.ensure(g1)); CU_TRY(e, e->h_scope_status.ensure(s1)); CU_TRY(e, e->h_out.ensure(p1));
   CU_TRY(e, e->d_fin.ensure((G + kFinThreads - 1) / kFinThreads + 4)); CU_TRY(e, e->d_totals.ensure(4));
   // the S x N tables and the Q x N score matrix
@@ -1054,8 +1109,7 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
     }
     CU_TRY(e, cudaEventRecord(e->ev[2], e->stream));
     const uint32_t W = rx.window;
-    // K3: CTAs that take work items from a queue; by default as many as are resident at once (heavy gangs take whole CTAs)
-    const uint32_t eval_ctas = std::max(1u, e->tune_eval_ctas ? e->tune_eval_ctas : std::min(W, e->n_sm * e->tune_heavy_ctas));
+    const uint32_t n_eval_ctas = eval_ctas(e);
     const uint32_t warp_ctas = std::max(1u, std::min((W * 32 + 255) / 256, e->n_sm * e->tune_warp_ctas));
     // Rounds are enqueued `batch` at a time without waiting: every kernel returns at once when the cycle is over, so the
     // host only looks at the control words between batches (to rebuild the capacity tables when the settled prefix has
@@ -1068,7 +1122,11 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
         CU_TRY(e, cudaMemsetAsync(e->d_rem_stamp.p, 0xFF, sizeof(uint32_t) * e->words, e->stream));
       }
       // one stream-ordered chain: evaluate -> publish -> detect, each launched while the one before drains
-      CU_TRY(e, launch_chained(e->holds_on ? (e->any_preferred ? k_eval<true, true> : k_eval<false, true>) : (e->any_preferred ? k_eval<true, false> : k_eval<false, false>), eval_ctas, kEvalWarps * 32, e->stream, tp, tb, rx, e->tune_max_att));
+      // (a wide cycle never has holds: grove_run_cycle_reuse refuses wide submissions)
+      auto* k3 = e->wide ? (e->any_preferred ? k_eval<true, false, true> : k_eval<false, false, true>)
+                 : e->holds_on ? (e->any_preferred ? k_eval<true, true, false> : k_eval<false, true, false>)
+                               : (e->any_preferred ? k_eval<true, false, false> : k_eval<false, false, false>);
+      CU_TRY(e, launch_chained(k3, n_eval_ctas, kEvalWarps * 32, e->stream, tp, tb, rx, e->tune_max_att));
       CU_TRY(e, launch_chained(e->holds_on ? k_apply<true> : k_apply<false>, warp_ctas, 256, e->stream, tb, rx));
       CU_TRY(e, launch_chained(k_detect, warp_ctas, 256, e->stream, tp, tb, rx, e->tune_refresh));
       e->launches += 3;
@@ -1275,6 +1333,7 @@ static int32_t publish_reclaim(grove_engine* e, std::vector<grove_gang_status_t>
 int32_t grove_run_cycle_preempt(grove_engine_t* e, const grove_running_gang_t* running, uint32_t n_running,
                                 const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
   if (!e || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
+  if (e->wide) return refuse_wide(e, "grove_run_cycle_preempt");
   for (uint32_t r = 0; r < n_running; ++r)
     if (uint64_t(running[r].holding_off) + running[r].n_holdings > n_holdings) return fail(e, GROVE_ERR_INVALID_ARG, "running gang holdings out of range");
   if (e->nodes_loaded) for (uint32_t h = 0; h < n_holdings; ++h)
@@ -1527,6 +1586,7 @@ static int32_t run_cycle_holds(grove_engine* e, const uint32_t* replaces, const 
 int32_t grove_run_cycle_reuse(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs, const grove_running_gang_t* running,
                               uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
   if (!e || (n_gangs && !replaces) || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
+  if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse");
   const int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);
   if (rc) return rc;
   return run_cycle_holds(e, replaces, running, holdings, true, stats);
@@ -1543,6 +1603,7 @@ int32_t grove_run_cycle_reuse(grove_engine_t* e, const uint32_t* replaces, uint3
 int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs, const grove_running_gang_t* running,
                                       uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
   if (!e || (n_gangs && !replaces) || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
+  if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse_preempt");
   int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);
   if (rc) return rc;
   CU_TRY(e, cudaSetDevice(e->cfg.device));
@@ -1798,6 +1859,7 @@ int32_t grove_shard_range(grove_engine_t* e, uint32_t* lo, uint32_t* hi) {
 int32_t grove_run_score_pass(grove_engine_t* e, float* ms) {
   if (!e) return GROVE_ERR_INVALID_ARG;
   if (ms) *ms = 0.f;
+  if (e->wide) return refuse_wide(e, "grove_run_score_pass");
   int32_t rc = cycle_begin(e);   // allocations, derived gang tables, state resets: the pass leaves the handle ready for a cycle
   if (rc) return rc;
   CycleGuard guard{e};
@@ -1826,6 +1888,7 @@ int32_t grove_run_score_pass(grove_engine_t* e, float* ms) {
 
 int32_t grove_shard_summary_device(grove_engine_t* e, void* d_out, uint32_t cap_words) {
   if (!e || !d_out) return GROVE_ERR_INVALID_ARG;
+  if (e->wide) return refuse_wide(e, "grove_shard_summary_device");
   if (!e->score_pass_valid) return fail(e, GROVE_ERR_STATE, "no score pass over the loaded snapshot");
   if (cap_words < e->G + e->Q) return fail(e, GROVE_ERR_LIMIT, "output buffer too small");
   CU_TRY(e, cudaSetDevice(e->cfg.device));

@@ -16,8 +16,9 @@ namespace grove {
 constexpr int kFitTile = 4;     // signatures per CTA: the grid is (node tiles) x (signature tiles), every tile a short loop
 
 // min(x / d, 256) for d > 0, exactly, without the ~20-instruction integer division: quotients that matter are small
-// (a gang has at most GROVE_MAX_GANG_PODS pods; capacity bytes saturate at 255), so a float estimate is off by at most
-// one and is corrected with one multiply
+// (capacity bytes saturate at 255; the ordinary evaluator asks for at most GROVE_MAX_GANG_PODS pods, while a wide cycle's,
+// which asks for up to GROVE_MAX_WIDE_GANG_PODS, divides with admit.cuh div_rcp<true> and treats a byte of 255 as unbounded),
+// so a float estimate is off by at most one and is corrected with one multiply
 __device__ __forceinline__ uint32_t div_small(uint32_t x, uint32_t d) {
   if (x >= (uint64_t(d) << 8)) return 256u;
   uint32_t q = uint32_t(__fdividef(float(x), float(d)));   // x < 256 d: |error| <= 1

@@ -201,11 +201,15 @@ Err GpuBackend::ValidatePodCliqueSet(const PodCliqueSet& pcs) const {
     return mkerr("ERR_VALIDATE_PCS", "ValidatePodCliqueSet", errs[0].field + ": " + errs[0].message);
   std::vector<PodGangInfo> infos;
   if (auto e = ComputeExpectedPodGangs(pcs, levels_, true, &infos)) return e;
+  bool large;
+  { std::lock_guard<std::mutex> l(mu_); large = large_; }
+  const int maxPods = int(large ? GROVE_MAX_WIDE_GANG_PODS : GROVE_MAX_GANG_PODS);
   for (const auto& pg : infos) {
     int pods = 0;
     for (const auto& p : pg.pclqs) pods += p.replicas;
-    if (pg.pclqs.size() > GROVE_MAX_GANG_CLIQUES || pods > int(GROVE_MAX_GANG_PODS) || pg.pcsgTopologyConstraints.size() + 1 > GROVE_MAX_GANG_SCOPES)
-      return mkerr("ERR_VALIDATE_PCS", "ValidatePodCliqueSet", "PodGang " + pg.fqn + " exceeds the gpu-scheduler limits (32 PodCliques / 32 constraint groups / 128 pods per PodGang)");
+    if (pg.pclqs.size() > GROVE_MAX_GANG_CLIQUES || pods > maxPods || pg.pcsgTopologyConstraints.size() + 1 > GROVE_MAX_GANG_SCOPES)
+      return mkerr("ERR_VALIDATE_PCS", "ValidatePodCliqueSet", "PodGang " + pg.fqn + " exceeds the gpu-scheduler limits (32 PodCliques / 32 constraint groups / " +
+                                                                   std::to_string(maxPods) + " pods per PodGang)");
   }
   return std::nullopt;
 }
@@ -262,18 +266,21 @@ Err GpuBackend::OnPodGangDelete(const PodGang& podGang) {
   return std::nullopt;
 }
 
-std::string GpuBackend::WhyNotEncodable(const PodGang& pg) {
+std::string GpuBackend::WhyNotEncodable(const PodGang& pg) { return WhyNotEncodable(pg, false); }
+
+std::string GpuBackend::WhyNotEncodable(const PodGang& pg, bool large) {
+  const size_t maxRep = large ? GROVE_MAX_WIDE_GANG_PODS : 255u, maxPods = large ? GROVE_MAX_WIDE_GANG_PODS : GROVE_MAX_GANG_PODS;
   if (pg.Spec.PodGroups.empty()) return "spec.podgroups: a PodGang needs at least one PodGroup";
   if (pg.Spec.PodGroups.size() > GROVE_MAX_GANG_CLIQUES) return "spec.podgroups: more than " + std::to_string(GROVE_MAX_GANG_CLIQUES) + " PodGroups";
   if (pg.Spec.TopologyConstraintGroupConfigs.size() + 1 > GROVE_MAX_GANG_SCOPES) return "spec.topologyConstraintGroupConfigs: more than " + std::to_string(GROVE_MAX_GANG_SCOPES - 1) + " group configs";
   size_t pods = 0;
   for (const auto& p : pg.Spec.PodGroups) {
-    if (p.MinReplicas < 0 || p.MinReplicas > 255) return "spec.podgroups[" + p.Name + "].minReplicas: must be within 0..255";
-    if (p.PodReferences.size() > 255) return "spec.podgroups[" + p.Name + "].podReferences: more than 255 pods";
+    if (p.MinReplicas < 0 || size_t(p.MinReplicas) > maxRep) return "spec.podgroups[" + p.Name + "].minReplicas: must be within 0.." + std::to_string(maxRep);
+    if (p.PodReferences.size() > maxRep) return "spec.podgroups[" + p.Name + "].podReferences: more than " + std::to_string(maxRep) + " pods";
     if (size_t(p.MinReplicas) > p.PodReferences.size()) return "spec.podgroups[" + p.Name + "].minReplicas: exceeds the pods referenced";
     pods += p.PodReferences.size();
   }
-  if (pods > GROVE_MAX_GANG_PODS) return "spec.podgroups: more than " + std::to_string(GROVE_MAX_GANG_PODS) + " pods in one PodGang";
+  if (pods > maxPods) return "spec.podgroups: more than " + std::to_string(maxPods) + " pods in one PodGang";
   for (const auto& gc : pg.Spec.TopologyConstraintGroupConfigs)
     for (const auto& n : gc.PodGroupNames)
       if (std::none_of(pg.Spec.PodGroups.begin(), pg.Spec.PodGroups.end(), [&n](const PodGroup& p) { return p.Name == n; }))
@@ -353,7 +360,16 @@ Err GpuBackend::EncodeLocked(const std::vector<Node>& nodes, Tables* out) const 
   auto hasSurplus = [](const PodGang& pg) { for (const auto& p : pg.Spec.PodGroups) if (int64_t(p.PodReferences.size()) > p.MinReplicas) return true; return false; };
   // PodGangs the packed tables cannot hold are left out of the pass (and so is a scaled PodGang behind one); everybody else
   // is scheduled as usual
-  for (const auto& kv : pending_) { const std::string why = WhyNotEncodable(kv.second); if (!why.empty()) out->skipped[kv.first] = why; }
+  // (a large PodGang -- SetLargePodGangs -- only when no running-gang cycle may run: those take no wide submission)
+  const bool runningCycles = preemption_ || reuse_ || reclaimReuse_;
+  for (const auto& kv : pending_) {
+    std::string why = WhyNotEncodable(kv.second, large_);
+    if (why.empty() && large_ && runningCycles) {
+      const std::string narrow = WhyNotEncodable(kv.second, false);
+      if (!narrow.empty()) why = narrow + ": large PodGangs are not scheduled while preemption or reservation reuse is on";
+    }
+    if (!why.empty()) out->skipped[kv.first] = why;
+  }
   for (const auto& kv : pending_)
     if (!out->skipped.count(kv.first) && !kv.second.BasePodGangName.empty() && out->skipped.count(kv.second.Namespace + "/" + kv.second.BasePodGangName))
       out->skipped[kv.first] = "base PodGang " + kv.second.BasePodGangName + " cannot be scheduled: " + out->skipped[kv.second.Namespace + "/" + kv.second.BasePodGangName];
@@ -426,11 +442,14 @@ Err GpuBackend::EncodeLocked(const std::vector<Node>& nodes, Tables* out) const 
         PodGang::Requests rq;
         if (auto it = pg.PodGroupRequests.find(p.Name); it != pg.PodGroupRequests.end()) rq = it->second;
         c.req_cpu_milli = rq.cpu_milli; c.req_mem_mib = rq.mem_mib; c.req_gpu = rq.gpu;
-        if (p.MinReplicas < 0 || p.MinReplicas > 255 || p.PodReferences.size() > 255 || size_t(p.MinReplicas) > p.PodReferences.size())
+        const size_t maxRep = large_ ? GROVE_MAX_WIDE_GANG_PODS : 255u;
+        if (p.MinReplicas < 0 || size_t(p.MinReplicas) > maxRep || p.PodReferences.size() > maxRep || size_t(p.MinReplicas) > p.PodReferences.size())
           return mkerr("ERR_SYNC_PODGANG", "Encode", "PodGroup " + p.Name + ": MinReplicas / PodReferences out of range");
-        c.min_replicas = uint8_t(p.MinReplicas); c.replicas = uint8_t(p.PodReferences.size());
-        if (remainder) { c.min_replicas = 0; c.replicas = uint8_t(left(gi)); }
-        if (split) c.replicas = c.min_replicas;
+        grove_clique_count_t n{uint16_t(p.MinReplicas), uint16_t(p.PodReferences.size())};
+        if (remainder) { n.min_replicas = 0; n.replicas = uint16_t(left(gi)); }
+        if (split) n.replicas = n.min_replicas;
+        // the 8-bit fields are what grove_submit_gangs reads; grove_submit_gangs_wide reads the counts row
+        c.min_replicas = uint8_t(std::min<uint32_t>(n.min_replicas, 255u)); c.replicas = uint8_t(std::min<uint32_t>(n.replicas, 255u));
         uint8_t cpref;
         if (auto e = levelOf(p.Topology, &c.level, &cpref)) return e;
         c.scope = GROVE_CLIQUE_SCOPE_PREF(uint32_t(si), cpref);
@@ -445,12 +464,13 @@ Err GpuBackend::EncodeLocked(const std::vector<Node>& nodes, Tables* out) const 
         }
         c.class_mask = mask;
         out->cliques.push_back(c);
+        out->counts.push_back(n);
         out->cliqueOf.push_back({uint32_t(out->gangs.size()), gi});
         out->refBase.push_back(done ? (*done)[gi] : 0u);
-        pods += c.replicas; ++rel;
+        pods += n.replicas; ++rel;
       }
     }
-    if (rel == 0 || rel > GROVE_MAX_GANG_CLIQUES || scopes.size() > GROVE_MAX_GANG_SCOPES || pods > GROVE_MAX_GANG_PODS)
+    if (rel == 0 || rel > GROVE_MAX_GANG_CLIQUES || scopes.size() > GROVE_MAX_GANG_SCOPES || pods > (large_ ? GROVE_MAX_WIDE_GANG_PODS : GROVE_MAX_GANG_PODS))
       return mkerr("ERR_SYNC_PODGANG", "Encode", "PodGang " + key + " exceeds the gpu-scheduler limits");
     g.n_cliques = uint16_t(rel); g.n_scopes = uint16_t(scopes.size());
     out->gangs.push_back(g);
@@ -467,8 +487,10 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
   if (stats) *stats = grove_cycle_stats_t{};
   Tables t;
   std::map<std::string, PodGang> snap;            // the PodGangs of this pass: reconcilers may add / delete others meanwhile
+  bool large = false;
   {
     std::lock_guard<std::mutex> l(mu_);
+    large = large_;
     if (pending_.empty()) return std::nullopt;
     if (auto e = Init()) return e;
     if (!engine_) return mkerr("ERR_SYNC_PODGANG", "RunCycle", "no ClusterTopology synced");
@@ -482,8 +504,11 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
     return mkerr("ERR_SYNC_PODGANG", what, std::string(grove_last_error(engine_)) + " (" + std::to_string(rc) + ")");
   };
   if (auto e = chk(grove_load_nodes(engine_, t.nodes.data(), uint32_t(t.nodes.size())), "grove_load_nodes")) return e;
-  if (auto e = chk(grove_submit_gangs(engine_, t.gangs.data(), uint32_t(t.gangs.size()), t.cliques.data(), uint32_t(t.cliques.size()),
-                                      t.scopes.data(), uint32_t(t.scopes.size())), "grove_submit_gangs")) return e;
+  if (large) {
+    if (auto e = chk(grove_submit_gangs_wide(engine_, t.gangs.data(), uint32_t(t.gangs.size()), t.cliques.data(), t.counts.data(),
+                                             uint32_t(t.cliques.size()), t.scopes.data(), uint32_t(t.scopes.size())), "grove_submit_gangs_wide")) return e;
+  } else if (auto e = chk(grove_submit_gangs(engine_, t.gangs.data(), uint32_t(t.gangs.size()), t.cliques.data(), uint32_t(t.cliques.size()),
+                                             t.scopes.data(), uint32_t(t.scopes.size())), "grove_submit_gangs")) return e;
   grove_cycle_stats_t st{};
   // running PodGangs -> the reclaim pass's / reservation reuse's tables (holdings on nodes that left the snapshot are dropped)
   std::vector<grove_running_gang_t> run; std::vector<grove_holding_t> held; std::vector<std::string> runNames;

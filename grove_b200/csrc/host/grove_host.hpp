@@ -202,6 +202,7 @@ struct Tables {
   std::vector<grove_node_t> nodes;
   std::vector<grove_gang_t> gangs;
   std::vector<grove_clique_t> cliques;
+  std::vector<grove_clique_count_t> counts;             // clique row -> MinReplicas / replicas (what grove_submit_gangs_wide reads)
   std::vector<grove_scope_t> scopes;
   std::vector<std::string> gangNames;                 // row -> PodGang "<ns>/<name>"
   std::vector<std::pair<uint32_t, uint32_t>> cliqueOf; // clique row -> (gang row, PodGroup index in Spec.PodGroups)
@@ -255,11 +256,19 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   // DisruptionTarget naming their preemptor and are forgotten.  Off by default; with it off the other two switches work as
   // before: either one alone, and both together fail.
   void SetReclaimWithReuse(bool on) { std::lock_guard<std::mutex> l(mu_); reclaimReuse_ = on; }
+  // Large PodGangs: with it on, PodGangs of up to GROVE_MAX_WIDE_GANG_PODS pods (PodGroups of up to as many) are encoded and a
+  // cycle submits through grove_submit_gangs_wide; ValidatePodCliqueSet accepts base PodGangs of that size.  The running-gang
+  // cycles (preemption, reservation reuse, reuse with reclaim) do not take such PodGangs: while one of those switches is on too,
+  // a PodGang beyond GROVE_MAX_GANG_PODS pods or 255 replicas stays out of the pass, Unschedulable with a reason that says so.
+  // Off by default; off behaves exactly as before.
+  void SetLargePodGangs(bool on) { std::lock_guard<std::mutex> l(mu_); large_ = on; }
   size_t Running() const { std::lock_guard<std::mutex> l(mu_); return running_.size(); }
   // why a PodGang cannot be handed to the engine (limits of the packed tables), or empty.  SyncPodGang accepts every
   // PodGang -- the reference's reconciler would requeue forever on an error -- and RunCycle reports these as
   // Unschedulable with this message instead of failing the pass for everybody (ADVICE round 1).
   static std::string WhyNotEncodable(const PodGang& pg);
+  // the same under the limits of a large-PodGang backend (large = true: GROVE_MAX_WIDE_GANG_PODS pods per PodGang and PodGroup)
+  static std::string WhyNotEncodable(const PodGang& pg, bool large);
 
   // The cycle loop of the backend (INTEGRATION.md section 2): SyncPodGang / OnPodGangDelete are called concurrently by
   // the PodGang reconcilers (controller/podgang/register.go:34-36, MaxConcurrentReconciles) and only touch the pending
@@ -285,6 +294,7 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   bool preemption_ = false;
   bool reuse_ = false;
   bool reclaimReuse_ = false;
+  bool large_ = false;
   grove_engine_t* engine_ = nullptr;
   uint32_t engineLevels_ = 0;
   mutable std::mutex mu_;        // pending set, bindings, levels: everything SyncPodGang / OnPodGangDelete / SyncTopology touch

@@ -22,7 +22,7 @@ ERRORS = {0: "OK", -1: "INVALID_ARG", -2: "NO_DEVICE", -3: "CUDA", -4: "LIMIT", 
 # every symbol include/grove_place.h declares
 SYMBOLS = [
     "grove_abi_version", "grove_engine_create", "grove_engine_destroy", "grove_last_error",
-    "grove_load_nodes", "grove_update_nodes", "grove_get_nodes", "grove_submit_gangs", "grove_run_cycle",
+    "grove_load_nodes", "grove_update_nodes", "grove_get_nodes", "grove_submit_gangs", "grove_submit_gangs_wide", "grove_run_cycle",
     "grove_get_placements", "grove_get_gang_status", "grove_get_scope_domains", "grove_load_nodes_device",
     "grove_build_score_matrix", "grove_run_cycle_preempt", "grove_get_victims", "grove_run_cycle_reuse",
     "grove_run_cycle_reuse_preempt",
@@ -123,6 +123,20 @@ class PlacementEngine:
                                                 C.c_uint32(len(cliques)), _p(scopes), C.c_uint32(len(scopes))))
         self.G, self.Q, self.S = len(gangs), len(cliques), len(scopes)
         self._cap_pods = int(cliques["replicas"].astype(np.int64).sum()) if len(cliques) else 0
+
+    def submit_gangs_wide(self, gangs: np.ndarray, cliques: np.ndarray, counts: np.ndarray, scopes: np.ndarray):
+        """grove_submit_gangs_wide: `counts` (tables.clique_count_dt) holds every clique's MinReplicas / replicas, up to
+        tables.MAX_WIDE_GANG_PODS pods per gang; the 8-bit count fields of `cliques` are ignored."""
+        gangs = np.ascontiguousarray(gangs, dtype=T.gang_dt)
+        cliques = np.ascontiguousarray(cliques, dtype=T.clique_dt)
+        counts = np.ascontiguousarray(counts, dtype=T.clique_count_dt)
+        scopes = np.ascontiguousarray(scopes, dtype=T.scope_dt)
+        if len(counts) != len(cliques):
+            raise ValueError("one count record per clique")
+        self._check(self.lib.grove_submit_gangs_wide(self.h, _p(gangs), C.c_uint32(len(gangs)), _p(cliques), _p(counts),
+                                                     C.c_uint32(len(cliques)), _p(scopes), C.c_uint32(len(scopes))))
+        self.G, self.Q, self.S = len(gangs), len(cliques), len(scopes)
+        self._cap_pods = int(counts["replicas"].astype(np.int64).sum()) if len(cliques) else 0
 
     # ---- the cycle ----
     def run_cycle(self) -> dict:

@@ -192,6 +192,30 @@ def config_c4(n=50000, g=10000, seed=SEED_BASE + 4, max_used_pct=90):
     return dict(name="C4", n_levels=4, nodes=nodes, tables=b.build())
 
 
+def config_c4_large(n=50000, g=10000, n_large=24, seed=SEED_BASE + 44, max_used_pct=90):
+    """C4 (config_c4) plus `n_large` PodGangs of 256-2048 pods, for grove_submit_gangs_wide: a leader (Required host) and a
+    worker PodGroup of 255-2047 one-GPU pods under a Required zone with a Preferred block, priorities drawn from C4's three
+    classes so that they interleave with the ordinary gangs.  tables = (gangs, cliques, counts, scopes); `ordinary` = the C4
+    part alone, as grove_submit_gangs takes it."""
+    base = config_c4(n=n, g=g, seed=seed, max_used_pct=max_used_pct)
+    og, oc, os_ = base["tables"]
+    b = T.GangTableBuilder()
+    size = 256 + _rand_below(seed, 30, n_large, T.MAX_WIDE_GANG_PODS - 256 + 1)
+    pr = _rand_below(seed, 31, n_large, 3)
+    for i in range(n_large):
+        lead = dict(cpu=2000, mem=16384, gpu=1, min=1, level=3)
+        work = dict(cpu=1000, mem=8192, gpu=1, min=int(size[i]) - 1)
+        b.add_gang([(None, [lead, work])], level=0, preferred=1, priority=int(pr[i]))
+    lg, lc, lcnt, ls = b.build_wide()
+    lg["clique_off"] += len(oc)
+    lg["scope_off"] += len(os_)
+    counts = np.zeros(len(oc) + len(lc), dtype=T.clique_count_dt)
+    counts["min_replicas"][: len(oc)], counts["replicas"][: len(oc)] = oc["min_replicas"], oc["replicas"]
+    counts[len(oc):] = lcnt
+    tables = (np.concatenate([og, lg]), np.concatenate([oc, lc]), counts, np.concatenate([os_, ls]))
+    return dict(name="C4+large", n_levels=4, nodes=base["nodes"], tables=tables, ordinary=base["tables"])
+
+
 class ChurnC5:
     """BASELINE.json config 5: steady-state churn on the C4 cluster.  Every tick (100 ms of scheduler
     time) `arrivals` new PodGangs join the gangs still pending from earlier ticks, one cycle runs, and

@@ -31,6 +31,9 @@ clique_dt = np.dtype([
     ("req_cpu_milli", "<u4"), ("req_mem_mib", "<u4"), ("req_gpu", "<u2"), ("min_replicas", "u1"),
     ("replicas", "u1"), ("class_mask", "<u2"), ("level", "u1"), ("scope", "u1"),
 ])
+# grove_submit_gangs_wide: MinReplicas / replicas of one clique, up to GROVE_MAX_WIDE_GANG_PODS
+clique_count_dt = np.dtype([("min_replicas", "<u2"), ("replicas", "<u2")])
+MAX_GANG_PODS, MAX_WIDE_GANG_PODS = 128, 2048
 scope_dt = np.dtype([
     ("first_clique", "<u2"), ("n_cliques", "<u2"), ("level", "u1"), ("preferred1", "u1"), ("reserved", "u1", (2,)),
 ])
@@ -132,3 +135,15 @@ class GangTableBuilder:
         for i, s in enumerate(self.scopes):
             scopes["first_clique"][i], scopes["n_cliques"][i], scopes["level"][i], scopes["preferred1"][i] = s
         return gangs, cliques, scopes
+
+    def build_wide(self):
+        """The tables of grove_submit_gangs_wide: (gangs, cliques, counts, scopes).  `counts` carries every clique's MinReplicas
+        and replicas (up to MAX_WIDE_GANG_PODS); the clique records' 8-bit count fields, which that entry ignores, are zero."""
+        counts = np.zeros(len(self.cliques), dtype=clique_count_dt)
+        for i, c in enumerate(self.cliques):
+            counts["min_replicas"][i], counts["replicas"][i] = c[3], c[4]
+        narrow = GangTableBuilder()
+        narrow.gangs, narrow.scopes = self.gangs, self.scopes
+        narrow.cliques = [c[:3] + (0, 0) + c[5:] for c in self.cliques]
+        gangs, cliques, scopes = narrow.build()
+        return gangs, cliques, counts, scopes

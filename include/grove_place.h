@@ -54,6 +54,7 @@ extern "C" {
 #define GROVE_DOM_ABSENT 0xFFFFFFFFu /* node lacks the label of that level (GREP-244 README.md:65) */
 #define GROVE_NONE_U32 0xFFFFFFFFu
 #define GROVE_MAX_GANG_PODS 128u     /* sum of replicas over a gang's cliques */
+#define GROVE_MAX_WIDE_GANG_PODS 2048u /* sum of replicas over a gang's cliques, wide submissions (grove_submit_gangs_wide) */
 #define GROVE_MAX_GANG_CLIQUES 32u
 #define GROVE_MAX_GANG_SCOPES 32u
 #define GROVE_MAX_NODES (1u << 24)
@@ -209,6 +210,22 @@ int32_t grove_get_nodes(grove_engine_t* e, grove_node_t* out, uint32_t cap);
 int32_t grove_submit_gangs(grove_engine_t* e, const grove_gang_t* gangs, uint32_t n_gangs,
                            const grove_clique_t* cliques, uint32_t n_cliques,
                            const grove_scope_t* scopes, uint32_t n_scopes);
+
+/* ---- wide submissions: PodGangs of up to GROVE_MAX_WIDE_GANG_PODS pods ------------------------------------------
+ * counts[q] replaces the 8-bit min_replicas / replicas of clique q (those fields are ignored).  Everything else is
+ * validated as by grove_submit_gangs, with min_replicas <= replicas and at most GROVE_MAX_WIDE_GANG_PODS pods per gang.
+ * A submission is WIDE when some gang has more than GROVE_MAX_GANG_PODS pods or some clique more than 255 replicas;
+ * one within the old limits behaves exactly as if it had come through grove_submit_gangs.  A wide submission is
+ * scheduled by grove_run_cycle and read back by every getter and grove_build_score_matrix; grove_run_cycle_preempt,
+ * grove_run_cycle_reuse, grove_run_cycle_reuse_preempt, grove_run_score_pass and grove_shard_summary_device refuse it
+ * with GROVE_ERR_LIMIT. */
+typedef struct grove_clique_count {
+  uint16_t min_replicas;  /* PodGroup.MinReplicas */
+  uint16_t replicas;      /* len(PodReferences) >= min_replicas */
+} grove_clique_count_t;
+int32_t grove_submit_gangs_wide(grove_engine_t* e, const grove_gang_t* gangs, uint32_t n_gangs,
+                                const grove_clique_t* cliques, const grove_clique_count_t* counts, uint32_t n_cliques,
+                                const grove_scope_t* scopes, uint32_t n_scopes);
 
 /* blocking: fit -> score -> admit -> commit; on return every gang is decided */
 int32_t grove_run_cycle(grove_engine_t* e, grove_cycle_stats_t* stats);

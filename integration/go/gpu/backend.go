@@ -32,9 +32,10 @@ const SchedulerNameGPU configv1alpha1.SchedulerName = "gpu-scheduler"
 // engine limits (include/grove_place.h): PodGangs beyond them are reported Unschedulable, never an error from
 // SyncPodGang -- the reconciler would requeue for ever (podgang/reconciler.go:86-89)
 const (
-	maxGangPods    = 128
-	maxGangCliques = 32
-	maxLevels      = 4
+	maxGangPods     = 128
+	maxWideGangPods = 2048 // with largePodGangs: grove_submit_gangs_wide, 16-bit replica counts (GROVE_MAX_WIDE_GANG_PODS)
+	maxGangCliques  = 32
+	maxLevels       = 4
 )
 
 type schedulerBackend struct {
@@ -48,7 +49,11 @@ type schedulerBackend struct {
 	levels   []string                                    // ClusterTopology.Spec.Levels[].Key, broadest first
 	running  map[string]runningGang                      // PodGangs scheduled by this backend: priority + holdings (reclaim pass)
 	preempt  bool
-	eng      *engine
+	// largePodGangs: PodGangs of up to maxWideGangPods pods are encoded (a counts row per clique) and submitted through
+	// grove_submit_gangs_wide.  The reclaim pass takes no such PodGang: with preempt also on, one beyond maxGangPods pods or 255
+	// replicas is reported Unschedulable (GpuBackend::SetLargePodGangs in the C++ mirror).
+	largePodGangs bool
+	eng           *engine
 	stopLoop chan struct{}
 }
 
@@ -110,8 +115,12 @@ func (b *schedulerBackend) ValidatePodCliqueSet(_ context.Context, pcs *grovecor
 	for _, c := range pcs.Spec.Template.Cliques {
 		pods += c.Spec.Replicas
 	}
-	if pods > maxGangPods {
-		return fmt.Errorf("spec.template.cliques: %d pods in the base PodGang, the %s backend packs at most %d", pods, b.Name(), maxGangPods)
+	limit := int32(maxGangPods)
+	if b.largePodGangs {
+		limit = maxWideGangPods
+	}
+	if pods > limit {
+		return fmt.Errorf("spec.template.cliques: %d pods in the base PodGang, the %s backend packs at most %d", pods, b.Name(), limit)
 	}
 	return nil
 }
@@ -214,7 +223,7 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 	for _, pg := range b.pending {
 		snap = append(snap, pg)
 	}
-	levels, eng, preempt := b.levels, b.eng, b.preempt
+	levels, eng, preempt, large := b.levels, b.eng, b.preempt, b.largePodGangs
 	b.mu.Unlock()
 	sort.Slice(snap, func(i, j int) bool { return snap[i].CreationTimestamp.Before(&snap[j].CreationTimestamp) }) // submission order
 
@@ -229,14 +238,14 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 	t, nodeNames := encodeNodes(nodeList.Items, podList.Items, levels) // allocatable - requests of bound pods; dom[l] = interned label value
 	rows := make([]*groveschedulerv1alpha1.PodGang, 0, len(snap))
 	for _, pg := range snap {
-		if why := whyNotEncodable(pg); why != "" {
+		if why := whyNotEncodable(pg, large, preempt); why != "" { // large && preempt: within the old limits only
 			b.setUnschedulable(ctx, pg, why)
 			continue
 		}
 		b.encodeGang(t, pg, levels, podList.Items) // one grove_gang_t + its cliques / scopes; requests come from the pods
 		rows = append(rows, pg)
 	}
-	res, err := eng.cycle(t, preempt)
+	res, err := eng.cycle(t, preempt, large)
 	if err != nil {
 		return err
 	}

@@ -50,6 +50,7 @@ type tables struct {
 	nodes   []C.grove_node_t
 	gangs   []C.grove_gang_t
 	cliques []C.grove_clique_t
+	counts  []C.grove_clique_count_t // per clique: MinReplicas / replicas, read by grove_submit_gangs_wide (large PodGangs)
 	scopes  []C.grove_scope_t
 	// reclaim pass (optional): PodGangs this backend scheduled earlier and what they hold per node
 	running  []C.grove_running_gang_t
@@ -65,7 +66,7 @@ type result struct {
 
 // cycle runs one scheduling cycle.  All slices are Go memory: the library copies them before each call returns and
 // keeps no pointer (cgo pointer-passing rules); outputs are written into Go slices.
-func (e *engine) cycle(t *tables, preempt bool) (*result, error) {
+func (e *engine) cycle(t *tables, preempt, large bool) (*result, error) {
 	e.mu.Lock()
 	defer e.mu.Unlock()
 	if len(t.nodes) == 0 || len(t.gangs) == 0 {
@@ -74,7 +75,12 @@ func (e *engine) cycle(t *tables, preempt bool) (*result, error) {
 	if err := e.err(C.grove_load_nodes(e.h, &t.nodes[0], C.uint32_t(len(t.nodes)))); err != nil {
 		return nil, err
 	}
-	if err := e.err(C.grove_submit_gangs(e.h, &t.gangs[0], C.uint32_t(len(t.gangs)), &t.cliques[0],
+	if large {
+		if err := e.err(C.grove_submit_gangs_wide(e.h, &t.gangs[0], C.uint32_t(len(t.gangs)), &t.cliques[0], &t.counts[0],
+			C.uint32_t(len(t.cliques)), &t.scopes[0], C.uint32_t(len(t.scopes)))); err != nil {
+			return nil, err
+		}
+	} else if err := e.err(C.grove_submit_gangs(e.h, &t.gangs[0], C.uint32_t(len(t.gangs)), &t.cliques[0],
 		C.uint32_t(len(t.cliques)), &t.scopes[0], C.uint32_t(len(t.scopes)))); err != nil {
 		return nil, err
 	}
