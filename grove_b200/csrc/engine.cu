@@ -234,6 +234,15 @@ struct grove_engine {
   DevBuf<uint4> d_rc_ent, d_rc_real, d_rc_base, d_rc_rows, d_rc_patch;
   DevBuf<int32_t> d_rc_prio;
   DevBuf<uint8_t> d_rc_gone;
+  // grove_diagnose (diagnose.cuh): whether the outputs on the device describe an ordinary cycle over the current inputs, the
+  // per-node usage lists, the batch descriptors, the per-domain capacity sums and the records
+  enum Diag : uint8_t { kDiagNoCycle, kDiagReady, kDiagRunning, kDiagChanged } diag = kDiagNoCycle;
+  DevBuf<uint32_t> d_dg_cnt, d_dg_off, d_dg_cur, d_dg_minr;
+  DevBuf<uint4> d_dg_rec;
+  DevBuf<DiagGang> d_dg_gang;
+  DevBuf<unsigned long long> d_dg_col;
+  DevBuf<grove_gang_diag_t> d_dg_gout;
+  DevBuf<grove_clique_diag_t> d_dg_qout;
 };
 
 
@@ -482,6 +491,7 @@ void grove_engine_destroy(grove_engine_t* e) {
 static int32_t load_nodes_common(grove_engine* e, const grove_node_t* host_nodes, const void* dev_nodes, uint32_t n) {
   if (n == 0 || n > GROVE_MAX_NODES) return fail(e, GROVE_ERR_INVALID_ARG, "node count out of range");
   if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
+  if (e->diag == grove_engine::kDiagReady) e->diag = grove_engine::kDiagChanged;
   CU_TRY(e, cudaSetDevice(e->cfg.device));
   if (host_nodes) {
     CU_TRY(e, cudaEventSynchronize(e->ev_nodes_up));  // an earlier upload may still be reading the staging buffer
@@ -533,6 +543,7 @@ int32_t grove_update_nodes(grove_engine_t* e, const uint32_t* idx, const grove_n
   if (!e || (n && (!idx || !recs))) return GROVE_ERR_INVALID_ARG;
   if (!e->nodes_loaded) return fail(e, GROVE_ERR_STATE, "no node snapshot loaded");
   if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
+  if (e->diag == grove_engine::kDiagReady) e->diag = grove_engine::kDiagChanged;
   if (n == 0) return GROVE_OK;
   e->score_pass_valid = false;
   CU_TRY(e, cudaSetDevice(e->cfg.device));
@@ -635,6 +646,7 @@ static int32_t validate(grove_engine* e, const grove_gang_t* gangs, uint32_t G, 
 static int32_t submit(grove_engine* e, const grove_gang_t* gangs, uint32_t n_gangs, const grove_clique_t* cliques,
                       const std::vector<uint32_t>& ccount, uint32_t n_cliques, const grove_scope_t* scopes, uint32_t n_scopes, uint32_t max_pods) {
   if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
+  if (e->diag == grove_engine::kDiagReady) e->diag = grove_engine::kDiagChanged;
   if (n_gangs >= (1u << 24)) return fail(e, GROVE_ERR_LIMIT, "too many gangs");  // order rank + round tag share a stamp word
   int32_t rc = validate(e, gangs, n_gangs, cliques, ccount.data(), n_cliques, scopes, n_scopes, max_pods);
   if (rc) return rc;
@@ -1030,7 +1042,7 @@ static int32_t cycle_begin(grove_engine* e) {
     k_reset<<<e->n_sm * 4, 256, 0, e->stream>>>(make_relax(e), G, S, N, e->words, std::min(G, std::min(W, E)));
     CU_TRY(e, cudaGetLastError());
   }
-  e->launches = 0; e->in_cycle = true; e->have_results = false; e->have_scopes = false;
+  e->launches = 0; e->in_cycle = true; e->have_results = false; e->have_scopes = false; e->diag = grove_engine::kDiagNoCycle;
   e->victims.clear(); e->score_pass_valid = false;
   std::memset(&e->last, 0, sizeof(e->last));
   return GROVE_OK;
@@ -1250,8 +1262,16 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
 
 int32_t grove_run_cycle(grove_engine_t* e, grove_cycle_stats_t* stats) {
   if (!e) return GROVE_ERR_INVALID_ARG;
-  return run_cycle(e, stats);
+  const int32_t rc = run_cycle(e, stats);
+  if (rc == GROVE_OK) e->diag = grove_engine::kDiagReady;
+  return rc;
 }
+
+// the entries with running gangs judge their gangs against other views: grove_diagnose refuses their outputs
+struct NoDiagnosis {
+  grove_engine* e;
+  ~NoDiagnosis() { if (e) e->diag = grove_engine::kDiagRunning; }
+};
 
 int32_t grove_get_placements(grove_engine_t* e, grove_placement_t* out, uint32_t cap, uint32_t* n_out) {
   if (!e || !n_out) return GROVE_ERR_INVALID_ARG;
@@ -1282,6 +1302,79 @@ int32_t grove_get_scope_domains(grove_engine_t* e, grove_scope_status_t* out, ui
     e->have_scopes = true;
   }
   std::memcpy(out, e->h_scope_status.p, sizeof(grove_scope_status_t) * e->S);
+  return GROVE_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Diagnosis (include/grove_place.h "diagnosis of rejected gangs"; DESIGN.md section 1; kernels in diagnose.cuh).  Reads the
+// outputs of the last ordinary cycle on the device (committed table, placements, ranks) and writes only its own buffers.
+// ---------------------------------------------------------------------------------------------
+// Rejected gangs go through the kernels in batches whose per-(gang, clique, domain) capacity sums take at most this many
+// 8-byte columns (64 MB); a gang that needs more on its own (32 cliques x 262 144 domains) is a batch of its own.
+static constexpr size_t kDiagScratchCols = size_t(1) << 23;
+
+int32_t grove_diagnose(grove_engine_t* e, grove_gang_diag_t* gangs, uint32_t cap_g, grove_clique_diag_t* cliques, uint32_t cap_q) {
+  if (!e) return GROVE_ERR_INVALID_ARG;
+  switch (e->diag) {
+    case grove_engine::kDiagReady: break;
+    case grove_engine::kDiagNoCycle: return fail(e, GROVE_ERR_STATE, "grove_diagnose: no completed cycle");
+    case grove_engine::kDiagRunning:
+      return fail(e, GROVE_ERR_STATE, "grove_diagnose: the last cycle ran with running gangs (preempt / reuse); only grove_run_cycle is diagnosed");
+    default: return fail(e, GROVE_ERR_STATE, "grove_diagnose: nodes or gangs were loaded, updated or submitted since the last cycle");
+  }
+  const uint32_t G = e->G, Q = e->Q;
+  if ((G && !gangs) || (Q && !cliques)) return GROVE_ERR_INVALID_ARG;
+  if (cap_g < G || cap_q < Q) return fail(e, GROVE_ERR_LIMIT, "output buffer too small");
+  if (G) std::memset(gangs, 0, sizeof(grove_gang_diag_t) * G);
+  if (Q) std::memset(cliques, 0, sizeof(grove_clique_diag_t) * Q);
+  // the rejected gangs, in batches
+  std::vector<DiagGang> dg;
+  std::vector<uint32_t> batch_at{0};
+  std::vector<size_t> batch_cols{0};
+  for (uint32_t g = 0; g < G; ++g) {
+    if (e->h_status.p[g].state != GROVE_GANG_REJECTED) continue;
+    const grove_gang_t& x = e->gangs[g];
+    DiagGang d{};
+    d.gang = g; d.rank = e->ginfo[g].order; d.n_cliques = x.n_cliques; d.level = x.level;
+    d.ncol = x.level == GROVE_LEVEL_NONE ? 1u : e->n_dom[x.level];
+    const size_t need = size_t(x.n_cliques) * d.ncol;
+    const uint32_t in_batch = uint32_t(dg.size()) - batch_at.back();
+    if (in_batch && (batch_cols.back() + need > kDiagScratchCols || in_batch == 65535u)) { batch_at.push_back(uint32_t(dg.size())); batch_cols.push_back(0); }
+    d.col_off = uint32_t(batch_cols.back());
+    batch_cols.back() += need;
+    dg.push_back(d);
+  }
+  batch_at.push_back(uint32_t(dg.size()));
+  if (dg.empty()) return GROVE_OK;
+  CU_TRY(e, cudaSetDevice(e->cfg.device));
+  const uint32_t Np = e->Npad, n_out = e->n_out;
+  CU_TRY(e, e->d_dg_gout.ensure(G)); CU_TRY(e, e->d_dg_qout.ensure(Q)); CU_TRY(e, e->d_dg_minr.ensure(Q));
+  CU_TRY(e, e->d_dg_cnt.ensure(Np)); CU_TRY(e, e->d_dg_off.ensure(size_t(Np) + 1)); CU_TRY(e, e->d_dg_cur.ensure(Np));
+  CU_TRY(e, e->d_dg_rec.ensure(std::max<uint32_t>(n_out, 1))); CU_TRY(e, e->d_dg_gang.ensure(dg.size()));
+  CU_TRY(e, e->d_dg_col.ensure(std::max<size_t>(*std::max_element(batch_cols.begin(), batch_cols.end()), 1)));
+  CU_TRY(e, cudaMemsetAsync(e->d_dg_gout.p, 0, sizeof(grove_gang_diag_t) * G, e->stream));
+  CU_TRY(e, cudaMemsetAsync(e->d_dg_qout.p, 0, sizeof(grove_clique_diag_t) * Q, e->stream));
+  CU_TRY(e, cudaMemsetAsync(e->d_dg_cnt.p, 0, sizeof(uint32_t) * Np, e->stream));
+  CU_TRY(e, cudaMemcpyAsync(e->d_dg_minr.p, e->ccount.data(), sizeof(uint32_t) * Q, cudaMemcpyHostToDevice, e->stream));
+  CU_TRY(e, cudaMemcpyAsync(e->d_dg_gang.p, dg.data(), sizeof(DiagGang) * dg.size(), cudaMemcpyHostToDevice, e->stream));
+  const Topo tp = make_topo(e); const Tables tb = make_tables(e);
+  // the admitted gangs' usage per node, in rank order with suffix sums
+  if (n_out) k_diag_count<<<(n_out + 255) / 256, 256, 0, e->stream>>>(e->d_out.p, n_out, e->d_inv.p, e->d_dg_cnt.p);
+  k_diag_scan<<<1, 1024, 0, e->stream>>>(e->d_dg_cnt.p, e->d_dg_off.p, e->d_dg_cur.p, Np);
+  if (n_out) k_diag_fill<<<(n_out + 255) / 256, 256, 0, e->stream>>>(e->d_out.p, n_out, e->d_inv.p, tb, e->d_dg_off.p, e->d_dg_cur.p, e->d_dg_rec.p);
+  k_diag_suffix<<<(e->N + 255) / 256, 256, 0, e->stream>>>(e->d_dg_off.p, e->d_dg_rec.p, e->N);
+  CU_TRY(e, cudaGetLastError());
+  const DiagUse use{e->d_dg_off.p, e->d_dg_rec.p};
+  for (size_t b = 0; b + 1 < batch_at.size(); ++b) {
+    const uint32_t a = batch_at[b], nb = batch_at[b + 1] - a;
+    if (batch_cols[b]) CU_TRY(e, cudaMemsetAsync(e->d_dg_col.p, 0, sizeof(unsigned long long) * batch_cols[b], e->stream));
+    k_diag_fit<<<dim3(Np / 256, nb), 256, 0, e->stream>>>(tp, tb, use, e->d_dg_gang.p + a, e->d_dg_minr.p, e->d_dg_col.p, e->d_dg_qout.p);
+    k_diag_verdict<<<nb, 256, 0, e->stream>>>(tb, e->d_dg_gang.p + a, e->d_dg_minr.p, e->d_dg_col.p, e->d_dg_qout.p, e->d_dg_gout.p);
+    CU_TRY(e, cudaGetLastError());
+  }
+  CU_TRY(e, cudaMemcpyAsync(gangs, e->d_dg_gout.p, sizeof(grove_gang_diag_t) * G, cudaMemcpyDeviceToHost, e->stream));
+  CU_TRY(e, cudaMemcpyAsync(cliques, e->d_dg_qout.p, sizeof(grove_clique_diag_t) * Q, cudaMemcpyDeviceToHost, e->stream));
+  CU_TRY(e, cudaStreamSynchronize(e->stream));
   return GROVE_OK;
 }
 
@@ -1333,6 +1426,7 @@ static int32_t publish_reclaim(grove_engine* e, std::vector<grove_gang_status_t>
 int32_t grove_run_cycle_preempt(grove_engine_t* e, const grove_running_gang_t* running, uint32_t n_running,
                                 const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
   if (!e || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
+  NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_preempt");
   for (uint32_t r = 0; r < n_running; ++r)
     if (uint64_t(running[r].holding_off) + running[r].n_holdings > n_holdings) return fail(e, GROVE_ERR_INVALID_ARG, "running gang holdings out of range");
@@ -1586,6 +1680,7 @@ static int32_t run_cycle_holds(grove_engine* e, const uint32_t* replaces, const 
 int32_t grove_run_cycle_reuse(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs, const grove_running_gang_t* running,
                               uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
   if (!e || (n_gangs && !replaces) || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
+  NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse");
   const int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);
   if (rc) return rc;
@@ -1603,6 +1698,7 @@ int32_t grove_run_cycle_reuse(grove_engine_t* e, const uint32_t* replaces, uint3
 int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs, const grove_running_gang_t* running,
                                       uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
   if (!e || (n_gangs && !replaces) || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
+  NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse_preempt");
   int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);
   if (rc) return rc;

@@ -487,10 +487,11 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
   if (stats) *stats = grove_cycle_stats_t{};
   Tables t;
   std::map<std::string, PodGang> snap;            // the PodGangs of this pass: reconcilers may add / delete others meanwhile
-  bool large = false;
+  bool large = false, explain = false;
+  std::vector<TopologyLevel> levels;
   {
     std::lock_guard<std::mutex> l(mu_);
-    large = large_;
+    large = large_; explain = explain_; levels = levels_;
     if (pending_.empty()) return std::nullopt;
     if (auto e = Init()) return e;
     if (!engine_) return mkerr("ERR_SYNC_PODGANG", "RunCycle", "no ClusterTopology synced");
@@ -582,6 +583,17 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
     if (t.remainder[g] && statuses->count(t.gangNames[g])) continue;   // the minimum row of the same PodGang already spoke
     (*statuses)[t.gangNames[g]] = s;
   }
+  // why the rejected PodGangs did not fit (an ordinary cycle only: the running-gang cycles judge gangs against other views).  A
+  // failed diagnosis leaves the messages empty: it never costs the cycle its bindings.
+  if (explain && !both && !reuse && !preempt &&
+      std::any_of(gs.begin(), gs.end(), [](const grove_gang_status_t& x) { return x.state == GROVE_GANG_REJECTED; })) {
+    std::vector<grove_gang_diag_t> gd(gs.size());
+    std::vector<grove_clique_diag_t> qd(t.cliques.size());
+    if (grove_diagnose(engine_, gd.data(), uint32_t(gd.size()), qd.data(), uint32_t(qd.size())) == GROVE_OK)
+      for (uint32_t g = 0; g < gs.size(); ++g)
+        if (gs[g].state == GROVE_GANG_REJECTED && !t.remainder[g])
+          (*statuses)[t.gangNames[g]].ScheduledMessage = ExplainRejection(t, snap.at(t.gangNames[g]), g, gd[g], qd.data(), levels);
+  }
   // a scheduled PodGang leaves the pending set once every PodReference is bound; until then its unbound pods are retried
   // as a remainder (Encode).  Remember where gangs landed for ReuseReservationRef hints.
   auto constrained = [](const PodGang& pg) {
@@ -644,6 +656,38 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
     if (all) { pending_.erase(key); bound_.erase(key); }
   }
   return std::nullopt;
+}
+
+std::string GpuBackend::ExplainRejection(const Tables& t, const PodGang& pg, uint32_t row, const grove_gang_diag_t& gd,
+                                         const grove_clique_diag_t* cliques, const std::vector<TopologyLevel>& levels) {
+  const grove_gang_t& g = t.gangs[row];
+  auto levelName = [&](uint32_t l) { return l < levels.size() ? levels[l].Domain : "level " + std::to_string(l); };
+  if (gd.verdict == GROVE_DIAG_CLIQUE_SHORT) {
+    const uint32_t q = g.clique_off + gd.clique;
+    const grove_clique_diag_t& c = cliques[q];
+    const grove_clique_t& rec = t.cliques[q];
+    const grove_scope_t& sc = t.scopes[g.scope_off + GROVE_CLIQUE_SCOPE(rec.scope)];
+    int deepest = -1;   // the deepest Required level binding the PodGroup: the label a node must carry
+    for (uint32_t l : {uint32_t(g.level), uint32_t(sc.level), uint32_t(rec.level)}) if (l != GROVE_LEVEL_NONE) deepest = std::max(deepest, int(l));
+    const std::pair<uint32_t, std::string> why[] = {
+        {c.unschedulable, "unschedulable"}, {c.selector, "not matching the node selector"},
+        {c.labels, "without the " + (deepest >= 0 && uint32_t(deepest) < levels.size() ? levels[deepest].Key : std::string("topology")) + " label"},
+        {c.cpu, "insufficient cpu"}, {c.mem, "insufficient memory"}, {c.gpu, "insufficient nvidia.com/gpu"}, {c.pods, "too many pods"}};
+    std::string parts;
+    for (const auto& w : why) if (w.first) parts += (parts.empty() ? "" : ", ") + std::to_string(w.first) + " " + w.second;
+    const uint32_t nodes = c.nodes_fit + c.unschedulable + c.selector + c.labels + c.cpu + c.mem + c.gpu + c.pods;
+    return "PodGroup " + pg.Spec.PodGroups[t.cliqueOf[q].second].Name + ": " + std::to_string(c.nodes_fit) + "/" + std::to_string(nodes) +
+           " nodes fit" + (parts.empty() ? "" : " (" + parts + ")") + "; " + std::to_string(c.pods_fit) + " of " +
+           std::to_string(t.counts[q].min_replicas) + " pods fit in the cluster";
+  }
+  if (gd.verdict == GROVE_DIAG_NO_DOMAIN)
+    return "no " + levelName(gd.level) + " holds every PodGroup's MinReplicas (0 of " + std::to_string(gd.domains) + ")";
+  if (gd.verdict == GROVE_DIAG_NO_JOINT_FIT) {
+    if (gd.level == GROVE_LEVEL_NONE) return "the cluster holds each PodGroup's MinReplicas alone, but not all of them together";
+    return std::to_string(gd.domains_ok) + " of " + std::to_string(gd.domains) + " " + levelName(gd.level) +
+           "s hold each PodGroup's MinReplicas alone, but not all of them together";
+  }
+  return "";
 }
 
 Err GpuBackend::Start(SnapshotFn snapshot, BindFn bind, std::chrono::milliseconds period) {

@@ -262,6 +262,14 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   // a PodGang beyond GROVE_MAX_GANG_PODS pods or 255 replicas stays out of the pass, Unschedulable with a reason that says so.
   // Off by default; off behaves exactly as before.
   void SetLargePodGangs(bool on) { std::lock_guard<std::mutex> l(mu_); large_ = on; }
+  // Unschedulable messages: with it on, after an ordinary cycle (no running-gang cycle: no preemption, reservation reuse or
+  // reuse with reclaim) the ScheduledMessage of every rejected PodGang says why, from grove_diagnose: the first PodGroup that
+  // fits nowhere in the cluster with the nodes each predicate turned away, or how many domains of the PodGang's Required level
+  // hold each PodGroup's MinReplicas.  Off by default (the message stays empty, as before).
+  void SetExplainUnschedulable(bool on) { std::lock_guard<std::mutex> l(mu_); explain_ = on; }
+  // the message for one rejected PodGang row of `t` from its diagnosis records (levels: the ClusterTopology's, broadest first)
+  static std::string ExplainRejection(const Tables& t, const PodGang& pg, uint32_t row, const grove_gang_diag_t& gd,
+                                      const grove_clique_diag_t* cliques, const std::vector<TopologyLevel>& levels);
   size_t Running() const { std::lock_guard<std::mutex> l(mu_); return running_.size(); }
   // why a PodGang cannot be handed to the engine (limits of the packed tables), or empty.  SyncPodGang accepts every
   // PodGang -- the reference's reconciler would requeue forever on an error -- and RunCycle reports these as
@@ -295,6 +303,7 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   bool reuse_ = false;
   bool reclaimReuse_ = false;
   bool large_ = false;
+  bool explain_ = false;
   grove_engine_t* engine_ = nullptr;
   uint32_t engineLevels_ = 0;
   mutable std::mutex mu_;        // pending set, bindings, levels: everything SyncPodGang / OnPodGangDelete / SyncTopology touch

@@ -8,6 +8,7 @@
 //   relax.cuh    k_select / k_apply / k_detect / k_fold    the relaxation that makes the evaluations of all gangs
 //                agree with the sequential, priority-ordered pass; k_fin_* / k_emit  outputs
 //   reclaim.cuh  k_reclaim_*  reclaim-class views over the running gangs' holdings (grove_run_cycle_reuse_preempt)
+//   diagnose.cuh k_diag_*  why each rejected gang did not fit, after the cycle (grove_diagnose)
 //
 // Semantics are DESIGN.md "Placement semantics"; the reference contract they restate is cited in
 // include/grove_place.h.  Integer / compare work only: no tensor cores, no floating point.
@@ -19,3 +20,4 @@
 #include "admit.cuh"
 #include "relax.cuh"
 #include "reclaim.cuh"
+#include "diagnose.cuh"

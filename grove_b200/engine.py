@@ -25,7 +25,7 @@ SYMBOLS = [
     "grove_load_nodes", "grove_update_nodes", "grove_get_nodes", "grove_submit_gangs", "grove_submit_gangs_wide", "grove_run_cycle",
     "grove_get_placements", "grove_get_gang_status", "grove_get_scope_domains", "grove_load_nodes_device",
     "grove_build_score_matrix", "grove_run_cycle_preempt", "grove_get_victims", "grove_run_cycle_reuse",
-    "grove_run_cycle_reuse_preempt",
+    "grove_run_cycle_reuse_preempt", "grove_diagnose",
     "grove_shard_range", "grove_run_score_pass", "grove_shard_summary_device",
     "grove_debug_get_perm", "grove_debug_get_fit_row", "grove_debug_get_score_row",
 ]
@@ -211,6 +211,16 @@ class PlacementEngine:
         out = np.zeros(max(self.S, 1), dtype=T.scope_status_dt)
         self._check(self.lib.grove_get_scope_domains(self.h, _p(out), C.c_uint32(len(out))))
         return out[: self.S]
+
+    def diagnose(self) -> tuple[np.ndarray, np.ndarray]:
+        """Why each REJECTED gang of the last run_cycle did not fit: (tables.gang_diag_dt[G], tables.clique_diag_dt[Q]), computed
+        on the GPU against the node table each gang met at its turn (include/grove_place.h "diagnosis of rejected gangs").
+        Other gangs and their cliques get zero records.  Raises GroveError STATE after a running-gang cycle or when nodes or
+        gangs changed since the cycle."""
+        g = np.zeros(max(self.G, 1), dtype=T.gang_diag_dt)
+        q = np.zeros(max(self.Q, 1), dtype=T.clique_diag_dt)
+        self._check(self.lib.grove_diagnose(self.h, _p(g), C.c_uint32(self.G), _p(q), C.c_uint32(self.Q)))
+        return g[: self.G], q[: self.Q]
 
     def nodes(self) -> np.ndarray:
         out = np.zeros(self.n, dtype=T.node_dt)

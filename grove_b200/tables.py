@@ -63,10 +63,19 @@ stats_dt = np.dtype([
     ("pairs_evaluated", "<u8"), ("kernel_launches", "<u8"), ("evaluations", "<u8"), ("ms_fit", "<f4"), ("ms_score", "<f4"),
     ("ms_admit", "<f4"), ("ms_commit", "<f4"), ("ms_total", "<f4"), ("reserved", "<f4"),
 ])
+# grove_diagnose: why each REJECTED gang of the last grove_run_cycle did not fit (include/grove_place.h "diagnosis")
+DIAG_NONE, DIAG_CLIQUE_SHORT, DIAG_NO_DOMAIN, DIAG_NO_JOINT_FIT = 0, 1, 2, 3
+gang_diag_dt = np.dtype([
+    ("verdict", "u1"), ("level", "u1"), ("clique", "<u2"), ("domains", "<u4"), ("domains_ok", "<u4"), ("reserved", "<u4"),
+])
+# the failure counts in the order a node is charged: the first predicate of fit(q, n) it fails
+DIAG_FAILURES = ("unschedulable", "selector", "labels", "cpu", "mem", "gpu", "pods")
+clique_diag_dt = np.dtype([("nodes_fit", "<u4")] + [(f, "<u4") for f in DIAG_FAILURES] + [("pods_fit", "<u8")])
 
 assert node_dt.itemsize == 32 and clique_dt.itemsize == 16 and scope_dt.itemsize == 8
 assert gang_dt.itemsize == 32 and placement_dt.itemsize == 8 and status_dt.itemsize == 32 and scope_status_dt.itemsize == 8
 assert config_dt.itemsize == 32 and stats_dt.itemsize == 64
+assert gang_diag_dt.itemsize == 16 and clique_diag_dt.itemsize == 40
 
 
 def make_nodes(n: int) -> np.ndarray:

@@ -29,6 +29,8 @@
  *                                    scheduler/api/core/v1alpha1/podgang.go:141-150,182-190
  *   grove_get_scope_domains          the topology domain chosen for every TopologyConstraintGroupConfig
  *                                    (podgang.go:120-131) -- what a binder needs to explain a placement
+ *   grove_diagnose                   why a REJECTED gang did not fit: the message of the Unschedulable
+ *                                    PodScheduled condition a pending pod carries
  *
  * cgo rules honoured: plain pointers + sizes only, every input array is copied
  * before the call returns (no Go pointer is retained), outputs go to
@@ -298,6 +300,42 @@ int32_t grove_run_cycle_reuse(grove_engine_t* e, const uint32_t* replaces, uint3
 int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs,
                                       const grove_running_gang_t* running, uint32_t n_running,
                                       const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats);
+
+/* ---- diagnosis of rejected gangs ------------------------------------------------------------------
+ * Why each REJECTED gang of the last grove_run_cycle did not fit (DESIGN.md section 1, "Diagnosis"): the Unschedulable message
+ * Kubernetes schedulers give a pending pod.  Gang g is judged against V_g = the node table the cycle left plus the usage of
+ * every admitted gang ranked after g, i.e. the table the sequential pass evaluated g against.  Per clique q of g, over all N
+ * nodes of V_g: nodes_fit = nodes where K1 fit(q, n) holds; every other node is counted once, under the first predicate it
+ * fails in the order of the fields below; pods_fit = sum over the fit nodes of the pods of q that fit there, exactly
+ * (min over resources with a request of floor(free / request), and the free pod slots).  Per gang, at its Required level l
+ * (the whole cluster is one domain when it has none): domains = the level-l domains, domains_ok = those in which every clique
+ * with MinReplicas > 0 finds MinReplicas pods on its own, and the verdict.  Gangs in any other state, and their cliques, get
+ * all-zero records.  The cycle's outputs are not touched.  GROVE_ERR_STATE when there is no completed cycle, when the last
+ * cycle was grove_run_cycle_preempt / _reuse / _reuse_preempt, or when grove_load_nodes*, grove_update_nodes or
+ * grove_submit_gangs* was called since; GROVE_ERR_LIMIT when cap_g < gangs submitted or cap_q < cliques submitted. */
+#define GROVE_DIAG_NONE 0u          /* the gang was not REJECTED */
+#define GROVE_DIAG_CLIQUE_SHORT 1u  /* a clique's pods_fit < MinReplicas: it fits nowhere in the cluster (`clique` names it) */
+#define GROVE_DIAG_NO_DOMAIN 2u     /* every clique fits the cluster, but no level-l domain holds each clique's MinReplicas */
+#define GROVE_DIAG_NO_JOINT_FIT 3u  /* domains_ok > 0 (or no Required level), yet no placement holds all cliques together:
+                                       shared nodes, or the Required levels of scopes / cliques inside those domains */
+typedef struct grove_gang_diag {   /* 16 B */
+  uint8_t verdict;        /* GROVE_DIAG_* */
+  uint8_t level;          /* the gang's Required level, GROVE_LEVEL_NONE = none (0 when not REJECTED) */
+  uint16_t clique;        /* GROVE_DIAG_CLIQUE_SHORT: first short clique, relative to the gang's clique_off; else 0 */
+  uint32_t domains;       /* level-l domains (nodes lacking the label are in none); 1 without a Required level */
+  uint32_t domains_ok;    /* domains in which every clique with MinReplicas > 0 has MinReplicas pods fitting on its own */
+  uint32_t reserved;
+} grove_gang_diag_t;
+typedef struct grove_clique_diag {   /* 40 B */
+  uint32_t nodes_fit;     /* nodes where fit(q, n) holds */
+  uint32_t unschedulable; /* not schedulable */
+  uint32_t selector;      /* selector class not accepted by the clique's class_mask */
+  uint32_t labels;        /* lacks a label down to the deepest Required level binding the clique */
+  uint32_t cpu, mem, gpu; /* free < request */
+  uint32_t pods;          /* no free pod slot */
+  uint64_t pods_fit;      /* sum over nodes of the pods of the clique that fit */
+} grove_clique_diag_t;
+int32_t grove_diagnose(grove_engine_t* e, grove_gang_diag_t* gangs, uint32_t cap_g, grove_clique_diag_t* cliques, uint32_t cap_q);
 
 /* K2: the topology-distance score matrix T[clique][node] = fit ? 1 + levels shared with the gang's anchor : 0 (u8) over the
  * snapshot the last cycle started from -- what a scheduler's Score extension point would hand out.  The admission does

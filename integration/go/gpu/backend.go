@@ -8,6 +8,7 @@ import (
 	"context"
 	"fmt"
 	"sort"
+	"strings"
 	"sync"
 	"time"
 
@@ -53,7 +54,10 @@ type schedulerBackend struct {
 	// grove_submit_gangs_wide.  The reclaim pass takes no such PodGang: with preempt also on, one beyond maxGangPods pods or 255
 	// replicas is reported Unschedulable (GpuBackend::SetLargePodGangs in the C++ mirror).
 	largePodGangs bool
-	eng           *engine
+	// explainUnschedulable: after an ordinary cycle the Unschedulable message of a rejected PodGang says why, from
+	// grove_diagnose (GpuBackend::SetExplainUnschedulable in the C++ mirror); off, it is the fixed message of before.
+	explainUnschedulable bool
+	eng                  *engine
 	stopLoop chan struct{}
 }
 
@@ -223,7 +227,7 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 	for _, pg := range b.pending {
 		snap = append(snap, pg)
 	}
-	levels, eng, preempt, large := b.levels, b.eng, b.preempt, b.largePodGangs
+	levels, eng, preempt, large, explain := b.levels, b.eng, b.preempt, b.largePodGangs, b.explainUnschedulable
 	b.mu.Unlock()
 	sort.Slice(snap, func(i, j int) bool { return snap[i].CreationTimestamp.Before(&snap[j].CreationTimestamp) }) // submission order
 
@@ -245,7 +249,7 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 		b.encodeGang(t, pg, levels, podList.Items) // one grove_gang_t + its cliques / scopes; requests come from the pods
 		rows = append(rows, pg)
 	}
-	res, err := eng.cycle(t, preempt, large)
+	res, err := eng.cycle(t, preempt, large, explain)
 	if err != nil {
 		return err
 	}
@@ -270,7 +274,11 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 			meta.SetStatusCondition(&pg.Status.Conditions, metav1.Condition{Type: string(groveschedulerv1alpha1.PodGangConditionTypeScheduled),
 				Status: metav1.ConditionTrue, Reason: "Scheduled"})
 		case C.GROVE_GANG_REJECTED:
-			b.setUnschedulable(ctx, pg, "no topology domain holds the gang's MinReplicas")
+			why := "no topology domain holds the gang's MinReplicas"
+			if res.gangDiag != nil {
+				why = explainRejection(t, pg, gi, res.gangDiag[gi], res.cliqueDiag, levels)
+			}
+			b.setUnschedulable(ctx, pg, why)
 			continue
 		default: // BASE_REJECTED / GATED_SKIP: waits, like its gated pods do (pod/syncflow.go:319-358)
 			continue
@@ -283,4 +291,60 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 		b.markDisruptionTarget(ctx, int(v.running), rows[v.preemptor])
 	}
 	return nil
+}
+
+// explainRejection: the Unschedulable message of rejected gang row gi from its grove_diagnose records, as
+// GpuBackend::ExplainRejection words it.  levels are the ClusterTopology's label keys, broadest first.
+func explainRejection(t *tables, pg *groveschedulerv1alpha1.PodGang, gi int, gd C.grove_gang_diag_t, qd []C.grove_clique_diag_t, levels []string) string {
+	g := t.gangs[gi]
+	levelName := func(l int) string {
+		if l < len(levels) {
+			return levels[l]
+		}
+		return fmt.Sprintf("level %d", l)
+	}
+	switch gd.verdict {
+	case C.GROVE_DIAG_CLIQUE_SHORT:
+		q := int(g.clique_off) + int(gd.clique)
+		c := qd[q]
+		rec := t.cliques[q]
+		sc := t.scopes[int(g.scope_off)+int(rec.scope&0x1F)]
+		deepest := -1 // the deepest Required level binding the PodGroup: the label a node must carry
+		for _, l := range []int{int(g.level), int(sc.level), int(rec.level)} {
+			if l != C.GROVE_LEVEL_NONE && l > deepest {
+				deepest = l
+			}
+		}
+		label := "topology"
+		if deepest >= 0 {
+			label = levelName(deepest)
+		}
+		why := []struct {
+			n    C.uint32_t
+			what string
+		}{{c.unschedulable, "unschedulable"}, {c.selector, "not matching the node selector"}, {c.labels, "without the " + label + " label"},
+			{c.cpu, "insufficient cpu"}, {c.mem, "insufficient memory"}, {c.gpu, "insufficient nvidia.com/gpu"}, {c.pods, "too many pods"}}
+		parts := []string{}
+		nodes := c.nodes_fit
+		for _, w := range why {
+			nodes += w.n
+			if w.n > 0 {
+				parts = append(parts, fmt.Sprintf("%d %s", w.n, w.what))
+			}
+		}
+		_, pgi := cliqueOwner(t, q)
+		msg := fmt.Sprintf("PodGroup %s: %d/%d nodes fit", pg.Spec.PodGroups[pgi].Name, c.nodes_fit, nodes)
+		if len(parts) > 0 {
+			msg += " (" + strings.Join(parts, ", ") + ")"
+		}
+		return msg + fmt.Sprintf("; %d of %d pods fit in the cluster", uint64(c.pods_fit), pg.Spec.PodGroups[pgi].MinReplicas)
+	case C.GROVE_DIAG_NO_DOMAIN:
+		return fmt.Sprintf("no %s holds every PodGroup's MinReplicas (0 of %d)", levelName(int(gd.level)), gd.domains)
+	case C.GROVE_DIAG_NO_JOINT_FIT:
+		if gd.level == C.GROVE_LEVEL_NONE {
+			return "the cluster holds each PodGroup's MinReplicas alone, but not all of them together"
+		}
+		return fmt.Sprintf("%d of %d %ss hold each PodGroup's MinReplicas alone, but not all of them together", gd.domains_ok, gd.domains, levelName(int(gd.level)))
+	}
+	return "no topology domain holds the gang's MinReplicas"
 }

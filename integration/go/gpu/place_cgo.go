@@ -62,11 +62,14 @@ type result struct {
 	status     []C.grove_gang_status_t
 	victims    []C.grove_victim_t
 	stats      C.grove_cycle_stats_t
+	// explain, after an ordinary cycle with a rejected gang: why each rejected gang did not fit (grove_diagnose)
+	gangDiag   []C.grove_gang_diag_t
+	cliqueDiag []C.grove_clique_diag_t
 }
 
 // cycle runs one scheduling cycle.  All slices are Go memory: the library copies them before each call returns and
 // keeps no pointer (cgo pointer-passing rules); outputs are written into Go slices.
-func (e *engine) cycle(t *tables, preempt, large bool) (*result, error) {
+func (e *engine) cycle(t *tables, preempt, large, explain bool) (*result, error) {
 	e.mu.Lock()
 	defer e.mu.Unlock()
 	if len(t.nodes) == 0 || len(t.gangs) == 0 {
@@ -116,6 +119,20 @@ func (e *engine) cycle(t *tables, preempt, large bool) (*result, error) {
 	r.status = make([]C.grove_gang_status_t, len(t.gangs))
 	if err := e.err(C.grove_get_gang_status(e.h, &r.status[0], C.uint32_t(len(r.status)))); err != nil {
 		return nil, err
+	}
+	if explain && !(preempt && len(t.running) > 0) {
+		for _, st := range r.status {
+			if st.state != C.GROVE_GANG_REJECTED {
+				continue
+			}
+			gd := make([]C.grove_gang_diag_t, len(t.gangs))
+			qd := make([]C.grove_clique_diag_t, len(t.cliques))
+			// a failed diagnosis leaves the messages as they were: it never costs the cycle its bindings
+			if C.grove_diagnose(e.h, &gd[0], C.uint32_t(len(gd)), &qd[0], C.uint32_t(len(qd))) == C.GROVE_OK {
+				r.gangDiag, r.cliqueDiag = gd, qd
+			}
+			break
+		}
 	}
 	return r, nil
 }
