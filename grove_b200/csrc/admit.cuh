@@ -840,7 +840,9 @@ __device__ __forceinline__ uint32_t eval_list_at(const Relax& rx, const Tables& 
 constexpr uint32_t kEvalDeferred = 0xFFu;   // nxt_tstate: no result this round
 constexpr int kEvalWarps = 8;
 // kWide: the instantiation of a wide cycle (16-bit counts; the entry stack of each warp in Relax::wide_node).
-template <bool kPref, bool kHolds, bool kWide>
+// kSpread: the instantiation of a cycle with topology spread members (spread.cuh): a member's candidates are those whose
+// level-l_s domain is allowed (HARD, and the first walk of SOFT) or not allowed (the second walk of SOFT).
+template <bool kPref, bool kHolds, bool kWide, bool kSpread = false>
 __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb, Relax rx, uint32_t max_att) {
   __shared__ GangShared shs[kEvalWarps];
   __shared__ int4 s_view[kEvalWarps][kStageMax];
@@ -891,6 +893,8 @@ __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb,
     const grove_scope_t sc0 = has_s ? tb.scopes[gg.scope_off + lane] : grove_scope_t{};
     const uint32_t round_now = rx.ctl[kRound];
     const uint32_t le = rx.last_eval[gi], fu_word = rx.fail_upto[gi], ext_word = rx.extent[gi];
+    uint32_t sp_grp = kFull;
+    if constexpr (kSpread) sp_grp = rx.sp.group[gi];
     // ---- gangs that need no packing
     uint32_t trivial = 0;
     if (gg.flags & GROVE_GANG_GATED) trivial = GROVE_GANG_GATED_SKIP;
@@ -945,9 +949,19 @@ __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb,
     int gfirst;
     const int gbase = level_span<kPref>(gg.level, gg.preferred, -1, gfirst);
     int gl = gfirst;
-    const uint32_t fu = (le && gfirst == gbase && gfirst >= 0) ? fu_word : 0u;
+    // a spread member: its group's level and mode, its allowed row.  The shortcut over the candidates that failed last time does
+    // not hold for it: a candidate that was not allowed then may be now
+    uint32_t sp_lvl = 0, sp_mode = 0;
+    const uint32_t* sp_bits = nullptr;
+    if constexpr (kSpread) {
+      if (sp_grp != kFull) { const uint32_t w = rx.sp.info[sp_grp]; sp_lvl = w & 0xFFu; sp_mode = (w >> 8) & 0xFFu; sp_bits = rx.sp.allowed + rx.sp.row[gi]; }
+    }
+    const uint32_t fu = (!sp_mode && le && gfirst == gbase && gfirst >= 0) ? fu_word : 0u;
     uint32_t k_won = 0;
     bool gave_up = false;
+    bool sp_full = false;   // a SOFT member reached its second walk: its extent is the whole visiting order
+    for (uint32_t walk = 0;; ++walk) {
+    gl = gfirst;
     do {
       if (gl < 0) {
         staged = false;
@@ -993,6 +1007,12 @@ __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb,
                 plaus = gang_plausible<kWide>(tp, rx, sh, gg.n_scopes, dl, dh, gl, d);
               }
               if (base == 0) { s_cl[w0 + c][lane] = dl; s_ch[w0 + c][lane] = dh; }   // (c < tw in the first chunk)
+              if constexpr (kSpread) {
+                if (sp_mode && plaus) {   // the level-l_s domain of the candidate's first node: allowed in walk 0, not allowed in walk 1
+                  const uint32_t A = __ldg(reinterpret_cast<const uint32_t*>(tp.ndom) + size_t(dl) * 4u + sp_lvl);
+                  plaus = ((__ldg(sp_bits + (A >> 5)) >> (A & 31u)) & 1u) == (walk == 0 ? 1u : 0u);
+                }
+              }
               if (plaus && k < fu) {   // failed last time: worth another attempt only if somebody withdrew a claim in there since
                 bool again = false;
                 for (uint32_t w = dl >> 5; w <= (dh - 1u) >> 5; ++w) again |= __ldg(rx.rem_round + w) >= le;
@@ -1031,8 +1051,11 @@ __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb,
         }
       }
     } while (kPref && !done && !gave_up && --gl >= gbase);
+    if (!(kSpread && sp_mode == GROVE_SPREAD_SOFT && walk == 0 && !done && !gave_up)) break;
+    sp_full = true;
+    }
     // what any of the attempts may have read (attempts past the winner only widen it)
-    if (lane == 0) atomicMax(&s_ext[w0], max(max(ev.ext, evs.ext), fu ? ext_word : 0u));   // skipped candidates were read by the last evaluation
+    if (lane == 0) atomicMax(&s_ext[w0], max(max(max(ev.ext, evs.ext), fu ? ext_word : 0u), sp_full ? tp.n : 0u));   // skipped candidates were read by the last evaluation
     team_sync();
     if (tt == 0) rx.last_att[gi] = uint8_t(gave_up ? 255u : min(254u, s_att[w0]));
     if (gave_up) {   // no result this round: k_apply keeps the gang dirty

@@ -98,6 +98,26 @@ enum Ctl : uint32_t {
 // reading memory -- no blocking call, no idle GPU between batches of rounds.
 enum Live : uint32_t { kLiveRound = 0, kLiveFront, kLiveDone, kLiveRefresh, kLiveOvf, kLiveEvals, kLiveWords = 8 };
 
+// Topology spread (grove_set_spread; kernels in spread.cuh), read only by the kSpread instantiations.  Members are listed per group
+// in rank order; member j of the list has an allowed row of ceil(n_dom[l_s] / 32) words, one bit per level-l_s domain.
+struct Spread {
+  const uint32_t* group;    // [G] spread group of the gang, kFull = none
+  const uint32_t* row;      // [G] word offset of a member's allowed row in `allowed`
+  const uint32_t* info;     // [groups] level | mode << 8 | max_skew << 16
+  const uint32_t* mem_off;  // [groups + 1] the group's members in `mem`
+  const uint32_t* mem;      // members, by group, in rank order
+  const uint32_t* cls;      // [members] union of the class masks of the member's cliques (same order as `mem`)
+  const uint32_t* cnt_off;  // [groups] offset of the group's per-domain counts in `seed` / `cnt`
+  const uint32_t* seed;     // seeds per level-l_s domain
+  uint32_t* cnt;            // scratch: c(A) while k_spread walks a group
+  uint32_t* dcls;           // [sum over levels of n_dom] OR of the classes of the schedulable nodes of every domain
+  uint32_t dcls_off[GROVE_MAX_LEVELS];
+  uint32_t* allowed;        // allowed rows of the members
+  uint32_t* stamp;          // [groups] round tag | lowest rank of a member whose result changed this round (k_apply)
+  uint8_t* skewed;          // [G] after the cycle: a SOFT member admitted outside its allowed domains
+  uint32_t n_groups;
+};
+
 // Relaxation state.  A gang's tentative result ("cur") lives in its own slots of the entry arrays and becomes final
 // in place; "nxt" is the scratch an evaluation writes before k_apply compares and publishes it.
 struct Relax {
@@ -164,6 +184,7 @@ struct Relax {
   uint32_t* wide_node;      // [k_eval CTAs * kEvalWarps][wide_cap]
   uint16_t* wide_meta;      // [k_eval CTAs * kEvalWarps][wide_cap] clique_rel
   uint32_t wide_cap;        // pods of the largest gang
+  Spread sp;                // topology spread (the kSpread instantiations of k_eval / k_apply / k_detect)
 };
 
 __device__ __forceinline__ uint32_t warp_incl_scan(uint32_t v, uint32_t lane) {

@@ -236,13 +236,20 @@ struct grove_engine {
   DevBuf<uint8_t> d_rc_gone;
   // grove_diagnose (diagnose.cuh): whether the outputs on the device describe an ordinary cycle over the current inputs, the
   // per-node usage lists, the batch descriptors, the per-domain capacity sums and the records
-  enum Diag : uint8_t { kDiagNoCycle, kDiagReady, kDiagRunning, kDiagChanged } diag = kDiagNoCycle;
+  enum Diag : uint8_t { kDiagNoCycle, kDiagReady, kDiagRunning, kDiagChanged, kDiagSpread } diag = kDiagNoCycle;
   DevBuf<uint32_t> d_dg_cnt, d_dg_off, d_dg_cur, d_dg_minr;
   DevBuf<uint4> d_dg_rec;
   DevBuf<DiagGang> d_dg_gang;
   DevBuf<unsigned long long> d_dg_col;
   DevBuf<grove_gang_diag_t> d_dg_gout;
   DevBuf<grove_clique_diag_t> d_dg_qout;
+  // topology spread (grove_set_spread; spread.cuh): the set of the current submission; the spread kernels run only while it has
+  // members (sp_members > 0)
+  uint32_t sp_groups = 0, sp_members = 0, sp_cnt_words = 0, sp_dcls_words = 0, sp_dcls_off[GROVE_MAX_LEVELS]{};
+  DevBuf<uint32_t> d_sp_group, d_sp_row, d_sp_info, d_sp_mem_off, d_sp_mem, d_sp_cls, d_sp_cnt_off, d_sp_seed, d_sp_cnt, d_sp_dcls;
+  DevBuf<uint32_t> d_sp_allowed, d_sp_stamp;
+  DevBuf<uint8_t> d_sp_skewed;
+  PinBuf<uint8_t> h_sp_skewed;
 };
 
 
@@ -256,6 +263,10 @@ struct grove_engine {
   } while (0)
 
 static int32_t fail(grove_engine* e, int32_t code, const char* msg) { e->err = msg; return code; }
+static int32_t refuse_spread(grove_engine* e, const char* entry) {
+  e->err = std::string(entry) + ": not supported while a topology spread set with members is in place (grove_set_spread)";
+  return GROVE_ERR_STATE;
+}
 static int32_t refuse_wide(grove_engine* e, const char* entry) {
   e->err = std::string(entry) + ": not supported for a wide submission (a gang of more than " + std::to_string(GROVE_MAX_GANG_PODS) +
            " pods or a clique of more than 255 replicas)";
@@ -414,6 +425,13 @@ static Relax make_relax(grove_engine* e) {
   r.dbg = e->dbg_on ? e->d_dbg.p : nullptr;
   r.live = e->d_live;
   r.ccount = e->wide ? e->d_ccount.p : nullptr; r.wide_node = e->d_wide_node.p; r.wide_meta = e->d_wide_meta.p; r.wide_cap = e->max_gang_pods;
+  if (e->sp_members) {
+    Spread& sp = r.sp;
+    sp.group = e->d_sp_group.p; sp.row = e->d_sp_row.p; sp.info = e->d_sp_info.p; sp.mem_off = e->d_sp_mem_off.p; sp.mem = e->d_sp_mem.p;
+    sp.cls = e->d_sp_cls.p; sp.cnt_off = e->d_sp_cnt_off.p; sp.seed = e->d_sp_seed.p; sp.cnt = e->d_sp_cnt.p; sp.dcls = e->d_sp_dcls.p;
+    for (uint32_t l = 0; l < GROVE_MAX_LEVELS; ++l) sp.dcls_off[l] = e->sp_dcls_off[l];
+    sp.allowed = e->d_sp_allowed.p; sp.stamp = e->d_sp_stamp.p; sp.skewed = e->d_sp_skewed.p; sp.n_groups = e->sp_groups;
+  }
   return r;
 }
 
@@ -491,7 +509,8 @@ void grove_engine_destroy(grove_engine_t* e) {
 static int32_t load_nodes_common(grove_engine* e, const grove_node_t* host_nodes, const void* dev_nodes, uint32_t n) {
   if (n == 0 || n > GROVE_MAX_NODES) return fail(e, GROVE_ERR_INVALID_ARG, "node count out of range");
   if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
-  if (e->diag == grove_engine::kDiagReady) e->diag = grove_engine::kDiagChanged;
+  if (e->diag == grove_engine::kDiagReady || e->diag == grove_engine::kDiagSpread) e->diag = grove_engine::kDiagChanged;
+  e->sp_groups = e->sp_members = 0;   // a spread set belongs to the nodes and gangs it was validated against
   CU_TRY(e, cudaSetDevice(e->cfg.device));
   if (host_nodes) {
     CU_TRY(e, cudaEventSynchronize(e->ev_nodes_up));  // an earlier upload may still be reading the staging buffer
@@ -543,7 +562,7 @@ int32_t grove_update_nodes(grove_engine_t* e, const uint32_t* idx, const grove_n
   if (!e || (n && (!idx || !recs))) return GROVE_ERR_INVALID_ARG;
   if (!e->nodes_loaded) return fail(e, GROVE_ERR_STATE, "no node snapshot loaded");
   if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
-  if (e->diag == grove_engine::kDiagReady) e->diag = grove_engine::kDiagChanged;
+  if (e->diag == grove_engine::kDiagReady || e->diag == grove_engine::kDiagSpread) e->diag = grove_engine::kDiagChanged;
   if (n == 0) return GROVE_OK;
   e->score_pass_valid = false;
   CU_TRY(e, cudaSetDevice(e->cfg.device));
@@ -646,8 +665,9 @@ static int32_t validate(grove_engine* e, const grove_gang_t* gangs, uint32_t G, 
 static int32_t submit(grove_engine* e, const grove_gang_t* gangs, uint32_t n_gangs, const grove_clique_t* cliques,
                       const std::vector<uint32_t>& ccount, uint32_t n_cliques, const grove_scope_t* scopes, uint32_t n_scopes, uint32_t max_pods) {
   if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
-  if (e->diag == grove_engine::kDiagReady) e->diag = grove_engine::kDiagChanged;
+  if (e->diag == grove_engine::kDiagReady || e->diag == grove_engine::kDiagSpread) e->diag = grove_engine::kDiagChanged;
   if (n_gangs >= (1u << 24)) return fail(e, GROVE_ERR_LIMIT, "too many gangs");  // order rank + round tag share a stamp word
+  e->sp_groups = e->sp_members = 0;
   int32_t rc = validate(e, gangs, n_gangs, cliques, ccount.data(), n_cliques, scopes, n_scopes, max_pods);
   if (rc) return rc;
   CU_TRY(e, cudaSetDevice(e->cfg.device));
@@ -1034,6 +1054,10 @@ static int32_t cycle_begin(grove_engine* e) {
       return fail(e, GROVE_ERR_OOM, "fit / capacity / score matrices do not fit in device memory");
     }
   }
+  if (e->sp_members) {   // the spread set's per-cycle scratch: counts per domain, classes per domain, stamps per group, flags
+    CU_TRY(e, e->d_sp_cnt.ensure(std::max<uint32_t>(e->sp_cnt_words, 1))); CU_TRY(e, e->d_sp_dcls.ensure(std::max<uint32_t>(e->sp_dcls_words, 1)));
+    CU_TRY(e, e->d_sp_stamp.ensure(std::max<uint32_t>(e->sp_groups, 1))); CU_TRY(e, e->d_sp_skewed.ensure(g1)); CU_TRY(e, e->h_sp_skewed.ensure(g1));
+  }
   if (e->dbg_on) { CU_TRY(e, e->d_dbg.ensure(g1 * 8 + 8)); CU_TRY(e, cudaMemsetAsync(e->d_dbg.p, 0, g1 * 32 + 32, e->stream)); }
   {
     const uint32_t W = e->tune_window ? e->tune_window : std::max(G, 1u);
@@ -1099,6 +1123,14 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
     CU_TRY(e, cudaGetLastError());
     e->launches += 1;
   }
+  const bool spread = e->sp_members > 0;   // (the running-gang entries refuse a spread set: no holds here)
+  if (G && spread) {   // the classes of every domain's schedulable nodes, over the cycle-start table; no member's stamp
+    CU_TRY(e, cudaMemsetAsync(e->d_sp_dcls.p, 0, sizeof(uint32_t) * e->sp_dcls_words, e->stream));
+    CU_TRY(e, cudaMemsetAsync(e->d_sp_stamp.p, 0xFF, sizeof(uint32_t) * e->sp_groups, e->stream));
+    k_spread_classes<<<(e->N + 255) / 256, 256, 0, e->stream>>>(tp, rx);
+    CU_TRY(e, cudaGetLastError());
+    e->launches += 1;
+  }
   if (G) {
     // K1 + capacity tables over the cycle-start snapshot; K2 (score matrix) forks to the second stream
     CU_TRY(e, cudaEventRecord(e->ev[0], e->stream));
@@ -1132,6 +1164,17 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
       if (next_round > 1 && next_round % kTagRounds == 0) {   // the stamp tags wrap: forget the stamps of the epoch that ends
         CU_TRY(e, cudaMemsetAsync(e->d_add_stamp.p, 0xFF, sizeof(uint32_t) * e->Npad, e->stream));
         CU_TRY(e, cudaMemsetAsync(e->d_rem_stamp.p, 0xFF, sizeof(uint32_t) * e->words, e->stream));
+        if (spread) CU_TRY(e, cudaMemsetAsync(e->d_sp_stamp.p, 0xFF, sizeof(uint32_t) * e->sp_groups, e->stream));
+      }
+      if (spread) {   // a spread cycle: the members' allowed domains first, then its own instantiations of the round's kernels
+        CU_TRY(e, launch_chained(k_spread, e->sp_groups, 256, e->stream, tp, tb, rx, 0u));
+        CU_TRY(e, launch_chained(e->any_preferred ? k_eval<true, false, false, true> : k_eval<false, false, false, true>, n_eval_ctas,
+                                 kEvalWarps * 32, e->stream, tp, tb, rx, e->tune_max_att));
+        CU_TRY(e, launch_chained(k_apply<false, true>, warp_ctas, 256, e->stream, tb, rx));
+        CU_TRY(e, launch_chained(k_detect<true>, warp_ctas, 256, e->stream, tp, tb, rx, e->tune_refresh));
+        e->launches += 4;
+        ++next_round;
+        return GROVE_OK;
       }
       // one stream-ordered chain: evaluate -> publish -> detect, each launched while the one before drains
       // (a wide cycle never has holds: grove_run_cycle_reuse refuses wide submissions)
@@ -1140,7 +1183,7 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
                                : (e->any_preferred ? k_eval<true, false, false> : k_eval<false, false, false>);
       CU_TRY(e, launch_chained(k3, n_eval_ctas, kEvalWarps * 32, e->stream, tp, tb, rx, e->tune_max_att));
       CU_TRY(e, launch_chained(e->holds_on ? k_apply<true> : k_apply<false>, warp_ctas, 256, e->stream, tb, rx));
-      CU_TRY(e, launch_chained(k_detect, warp_ctas, 256, e->stream, tp, tb, rx, e->tune_refresh));
+      CU_TRY(e, launch_chained(k_detect<false>, warp_ctas, 256, e->stream, tp, tb, rx, e->tune_refresh));
       e->launches += 3;
       ++next_round;
       return GROVE_OK;
@@ -1225,12 +1268,22 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
       CU_TRY(e, cudaGetLastError());
       e->launches += 1;
     }
+    if (spread) {   // which SOFT members landed outside their allowed domains (read back with the statuses); k_spread writes the
+                    // members' bytes only, so every other gang reads 0
+      CU_TRY(e, cudaMemsetAsync(e->d_sp_skewed.p, 0, G, e->stream));
+      k_spread<<<e->sp_groups, 256, 0, e->stream>>>(tp, tb, rx, 1u);
+      CU_TRY(e, cudaGetLastError());
+      CU_TRY(e, cudaMemcpyAsync(e->h_sp_skewed.p, e->d_sp_skewed.p, G, cudaMemcpyDeviceToHost, e->stream));
+      e->launches += 1;
+    }
     e->last.evaluations = e->h_ctl.p[kEvals];
   }
   CU_TRY(e, cudaEventRecord(e->ev[3], e->stream));
   if (e->tune_score && e->tune_overlap && G && e->Q) CU_TRY(e, cudaStreamWaitEvent(e->stream, e->ev_score, 0));  // the cycle ends when K2 has too
   rc = finish_cycle(e);
   if (rc) return rc;
+  if (spread)   // (finish_cycle waited for the copy)
+    for (uint32_t g = 0; g < G; ++g) if (e->h_sp_skewed.p[g]) e->h_status.p[g].reserved0 |= GROVE_STATUS_SPREAD_SKEWED;
   CU_TRY(e, cudaEventRecord(e->ev[9], e->stream));
   CU_TRY(e, cudaEventSynchronize(e->ev[9]));
   guard.armed = false;
@@ -1262,8 +1315,9 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
 
 int32_t grove_run_cycle(grove_engine_t* e, grove_cycle_stats_t* stats) {
   if (!e) return GROVE_ERR_INVALID_ARG;
+  const bool spread = e->sp_members > 0;
   const int32_t rc = run_cycle(e, stats);
-  if (rc == GROVE_OK) e->diag = grove_engine::kDiagReady;
+  if (rc == GROVE_OK) e->diag = spread ? grove_engine::kDiagSpread : grove_engine::kDiagReady;
   return rc;
 }
 
@@ -1306,6 +1360,91 @@ int32_t grove_get_scope_domains(grove_engine_t* e, grove_scope_status_t* out, ui
 }
 
 // ---------------------------------------------------------------------------------------------
+// Topology spread (include/grove_place.h "topology spread"; DESIGN.md section 1; kernels in spread.cuh).  Validated against the
+// loaded nodes and the submission and uploaded here; the cycle only builds the per-domain classes and runs k_spread.
+// ---------------------------------------------------------------------------------------------
+int32_t grove_set_spread(grove_engine_t* e, const grove_spread_t* groups, uint32_t n_groups, const uint32_t* gang_group, uint32_t n_gangs,
+                         const grove_spread_seed_t* seeds, uint32_t n_seeds) {
+  if (!e) return GROVE_ERR_INVALID_ARG;
+  if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
+  if (!e->nodes_loaded || !e->gangs_loaded) return fail(e, GROVE_ERR_STATE, "grove_set_spread: load nodes and submit gangs first");
+  if ((n_groups && !groups) || (n_gangs && !gang_group) || (n_seeds && !seeds)) return GROVE_ERR_INVALID_ARG;
+  if (n_gangs != e->G) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_spread: n_gangs is not the number of submitted gangs");
+  if (e->wide) return refuse_wide(e, "grove_set_spread");
+  for (uint32_t s = 0; s < n_groups; ++s) {
+    if (groups[s].level >= e->L) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_spread: spread level out of range");
+    if (groups[s].mode != GROVE_SPREAD_HARD && groups[s].mode != GROVE_SPREAD_SOFT)
+      return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_spread: mode must be GROVE_SPREAD_HARD or GROVE_SPREAD_SOFT");
+    if (groups[s].max_skew == 0) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_spread: max_skew must be at least 1");
+  }
+  uint32_t members = 0;
+  for (uint32_t g = 0; g < n_gangs; ++g) {
+    const uint32_t s = gang_group[g];
+    if (s == GROVE_NONE_U32) continue;
+    if (s >= n_groups) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_spread: spread group out of range");
+    const grove_gang_t& gg = e->gangs[g];
+    if (gg.level == GROVE_LEVEL_NONE || gg.level < groups[s].level)
+      return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_spread: a member needs a gang Required level at or below its group's level");
+    bool need = false;
+    for (uint32_t c = 0; c < gg.n_cliques; ++c) need |= (e->ccount[gg.clique_off + c] & 0xFFFFu) > 0;
+    if (!need) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_spread: a member needs a clique with MinReplicas > 0");
+    ++members;
+  }
+  for (uint32_t i = 0; i < n_seeds; ++i) {
+    if (seeds[i].group >= n_groups) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_spread: seed group out of range");
+    if (seeds[i].node >= e->N) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_spread: seed node out of range");
+  }
+  e->sp_groups = e->sp_members = 0;
+  if (!members) return GROVE_OK;   // nothing to spread: the ordinary cycle
+  // members by group in rank order (priority desc, index asc); an allowed row and a count row per group's level
+  const uint32_t G = n_gangs;
+  std::vector<uint32_t> order(G);
+  std::iota(order.begin(), order.end(), 0u);
+  std::stable_sort(order.begin(), order.end(), [e](uint32_t a, uint32_t b) { return e->gangs[a].priority > e->gangs[b].priority; });
+  std::vector<uint32_t> mem_off(n_groups + 1, 0), cnt_off(n_groups, 0), info(n_groups), row(G, GROVE_NONE_U32), group(gang_group, gang_group + G);
+  for (uint32_t g = 0; g < G; ++g) if (group[g] != GROVE_NONE_U32) ++mem_off[group[g] + 1];
+  for (uint32_t s = 0; s < n_groups; ++s) mem_off[s + 1] += mem_off[s];
+  std::vector<uint32_t> mem(members), cls(members), fill(mem_off.begin(), mem_off.end() - 1);
+  for (uint32_t g : order) {
+    const uint32_t s = group[g];
+    if (s == GROVE_NONE_U32) continue;
+    const grove_gang_t& gg = e->gangs[g];
+    uint32_t m = 0;
+    for (uint32_t c = 0; c < gg.n_cliques; ++c) m |= e->cliques[gg.clique_off + c].class_mask;
+    mem[fill[s]] = g; cls[fill[s]] = m; ++fill[s];
+  }
+  uint64_t cnt_words = 0, row_words = 0;
+  for (uint32_t s = 0; s < n_groups; ++s) {
+    const uint32_t nd = e->n_dom[groups[s].level];
+    info[s] = uint32_t(groups[s].level) | uint32_t(groups[s].mode) << 8 | uint32_t(groups[s].max_skew) << 16;
+    cnt_off[s] = uint32_t(cnt_words); cnt_words += nd;
+    for (uint32_t j = mem_off[s]; j < mem_off[s + 1]; ++j) { row[mem[j]] = uint32_t(row_words); row_words += (nd + 31u) / 32u; }
+  }
+  // members x domains of their level, one bit each (DESIGN.md section 2): refused beyond 1 GB
+  if (row_words > (uint64_t(1) << 28) || cnt_words > (uint64_t(1) << 28))
+    return fail(e, GROVE_ERR_LIMIT, "grove_set_spread: the allowed-domain rows (members x domains of their level) exceed 1 GB");
+  std::vector<uint32_t> seed(std::max<uint64_t>(cnt_words, 1), 0u);
+  for (uint32_t i = 0; i < n_seeds; ++i) {
+    const uint32_t s = seeds[i].group, d = e->tdom[size_t(e->inv[seeds[i].node]) * GROVE_MAX_LEVELS + groups[s].level];
+    if (d != GROVE_DOM_ABSENT) seed[cnt_off[s] + d] += 1u;   // a node without the level's label is in no domain of it
+  }
+  uint32_t dw = 0;
+  for (uint32_t l = 0; l < GROVE_MAX_LEVELS; ++l) { e->sp_dcls_off[l] = dw; if (l < e->L) dw += e->n_dom[l]; }
+  CU_TRY(e, cudaSetDevice(e->cfg.device));
+  auto up = [e](DevBuf<uint32_t>& d, const std::vector<uint32_t>& h) -> cudaError_t {
+    cudaError_t c = d.ensure(std::max<size_t>(h.size(), 1));
+    if (c == cudaSuccess && !h.empty()) c = cudaMemcpyAsync(d.p, h.data(), sizeof(uint32_t) * h.size(), cudaMemcpyHostToDevice, e->stream);
+    return c;
+  };
+  CU_TRY(e, up(e->d_sp_group, group)); CU_TRY(e, up(e->d_sp_row, row)); CU_TRY(e, up(e->d_sp_info, info)); CU_TRY(e, up(e->d_sp_mem_off, mem_off));
+  CU_TRY(e, up(e->d_sp_mem, mem)); CU_TRY(e, up(e->d_sp_cls, cls)); CU_TRY(e, up(e->d_sp_cnt_off, cnt_off)); CU_TRY(e, up(e->d_sp_seed, seed));
+  CU_TRY(e, e->d_sp_allowed.ensure(std::max<uint64_t>(row_words, 1)));
+  CU_TRY(e, cudaStreamSynchronize(e->stream));   // (the host vectors go out of scope)
+  e->sp_groups = n_groups; e->sp_members = members; e->sp_cnt_words = uint32_t(cnt_words); e->sp_dcls_words = dw;
+  return GROVE_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
 // Diagnosis (include/grove_place.h "diagnosis of rejected gangs"; DESIGN.md section 1; kernels in diagnose.cuh).  Reads the
 // outputs of the last ordinary cycle on the device (committed table, placements, ranks) and writes only its own buffers.
 // ---------------------------------------------------------------------------------------------
@@ -1320,6 +1459,8 @@ int32_t grove_diagnose(grove_engine_t* e, grove_gang_diag_t* gangs, uint32_t cap
     case grove_engine::kDiagNoCycle: return fail(e, GROVE_ERR_STATE, "grove_diagnose: no completed cycle");
     case grove_engine::kDiagRunning:
       return fail(e, GROVE_ERR_STATE, "grove_diagnose: the last cycle ran with running gangs (preempt / reuse); only grove_run_cycle is diagnosed");
+    case grove_engine::kDiagSpread:
+      return fail(e, GROVE_ERR_STATE, "grove_diagnose: the last cycle had topology spread members, which the diagnosis does not model");
     default: return fail(e, GROVE_ERR_STATE, "grove_diagnose: nodes or gangs were loaded, updated or submitted since the last cycle");
   }
   const uint32_t G = e->G, Q = e->Q;
@@ -1426,6 +1567,7 @@ static int32_t publish_reclaim(grove_engine* e, std::vector<grove_gang_status_t>
 int32_t grove_run_cycle_preempt(grove_engine_t* e, const grove_running_gang_t* running, uint32_t n_running,
                                 const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
   if (!e || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
+  if (e->sp_members) return refuse_spread(e, "grove_run_cycle_preempt");
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_preempt");
   for (uint32_t r = 0; r < n_running; ++r)
@@ -1680,6 +1822,7 @@ static int32_t run_cycle_holds(grove_engine* e, const uint32_t* replaces, const 
 int32_t grove_run_cycle_reuse(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs, const grove_running_gang_t* running,
                               uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
   if (!e || (n_gangs && !replaces) || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
+  if (e->sp_members) return refuse_spread(e, "grove_run_cycle_reuse");
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse");
   const int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);
@@ -1698,6 +1841,7 @@ int32_t grove_run_cycle_reuse(grove_engine_t* e, const uint32_t* replaces, uint3
 int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs, const grove_running_gang_t* running,
                                       uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
   if (!e || (n_gangs && !replaces) || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
+  if (e->sp_members) return refuse_spread(e, "grove_run_cycle_reuse_preempt");
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse_preempt");
   int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);

@@ -262,7 +262,18 @@ Err CheckPodSchedulingGate(bool podHasGate, bool podListedInPodGang, const std::
 Err GpuBackend::OnPodGangDelete(const PodGang& podGang) {
   std::lock_guard<std::mutex> l(mu_);
   const std::string key = podGang.Namespace + "/" + podGang.Name;
-  pending_.erase(key); bound_.erase(key); running_.erase(key);
+  pending_.erase(key); bound_.erase(key); running_.erase(key); setOf_.erase(key);
+  return std::nullopt;
+}
+
+Err GpuBackend::SetTopologySpread(const std::string& pcsName, std::optional<TopologySpread> spread) {
+  std::lock_guard<std::mutex> l(mu_);
+  if (!spread) { spread_.erase(pcsName); return std::nullopt; }
+  if (spread->LevelKey.empty()) return mkerr("ERR_SYNC_PODGANG", "SetTopologySpread", "topology spread of " + pcsName + ": no level key");
+  if (spread->MaxSkew < 1 || spread->MaxSkew > 0xFFFF) return mkerr("ERR_SYNC_PODGANG", "SetTopologySpread", "topology spread of " + pcsName + ": maxSkew out of range");
+  if (spread->WhenUnsatisfiable != "DoNotSchedule" && spread->WhenUnsatisfiable != "ScheduleAnyway")
+    return mkerr("ERR_SYNC_PODGANG", "SetTopologySpread", "topology spread of " + pcsName + ": whenUnsatisfiable must be DoNotSchedule or ScheduleAnyway");
+  spread_[pcsName] = *spread;
   return std::nullopt;
 }
 
@@ -370,6 +381,24 @@ Err GpuBackend::EncodeLocked(const std::vector<Node>& nodes, Tables* out) const 
     }
     if (!why.empty()) out->skipped[kv.first] = why;
   }
+  // topology spread: the base PodGangs of a set with a spread.  The running-gang cycles and wide submissions take no spread set:
+  // while one of them may run, the members stay out of the pass
+  auto spreadSetOf = [this](const PodGang& pg) -> const TopologySpread* {
+    if (!pg.BasePodGangName.empty()) return nullptr;
+    auto it = pg.Labels.find(kPartOfLabel);
+    if (it == pg.Labels.end()) return nullptr;
+    auto sp = spread_.find(it->second);
+    return sp == spread_.end() ? nullptr : &sp->second;
+  };
+  if (!spread_.empty()) {
+    bool wideAny = false;
+    if (large_) for (const auto& kv : pending_) wideAny |= !out->skipped.count(kv.first) && !WhyNotEncodable(kv.second, false).empty();
+    if (runningCycles || wideAny)
+      for (const auto& kv : pending_)
+        if (!out->skipped.count(kv.first) && spreadSetOf(kv.second))
+          out->skipped[kv.first] = runningCycles ? "topology spread is not applied while preemption or reservation reuse is on"
+                                                 : "topology spread is not applied in a pass with PodGangs beyond the ordinary limits";
+  }
   for (const auto& kv : pending_)
     if (!out->skipped.count(kv.first) && !kv.second.BasePodGangName.empty() && out->skipped.count(kv.second.Namespace + "/" + kv.second.BasePodGangName))
       out->skipped[kv.first] = "base PodGang " + kv.second.BasePodGangName + " cannot be scheduled: " + out->skipped[kv.second.Namespace + "/" + kv.second.BasePodGangName];
@@ -385,6 +414,19 @@ Err GpuBackend::EncodeLocked(const std::vector<Node>& nodes, Tables* out) const 
   for (size_t i = 0; i < nFull; ++i) row.emplace(*order[i], uint32_t(i));
   std::map<std::string, uint32_t> nodeIndex;
   for (size_t i = 0; i < nodes.size(); ++i) nodeIndex[nodes[i].Name] = uint32_t(i);
+  std::map<std::string, uint32_t> groupOf;   // "<ns>/<PodCliqueSet>" -> spread group
+  auto spreadGroup = [&](const std::string& ns, const std::string& pcs, const TopologySpread& sp) -> uint32_t {
+    uint8_t lvl = GROVE_LEVEL_NONE;
+    for (size_t l = 0; l < levels_.size(); ++l) if (levels_[l].Key == sp.LevelKey) lvl = uint8_t(l);
+    if (lvl == GROVE_LEVEL_NONE) return GROVE_NONE_U32;   // not a level of the synced ClusterTopology: dropped, as a pack domain is
+    auto [it, fresh] = groupOf.emplace(ns + "/" + pcs, uint32_t(out->spreadGroups.size()));
+    if (fresh) {
+      grove_spread_t g{}; g.level = lvl; g.max_skew = uint16_t(sp.MaxSkew);
+      g.mode = sp.WhenUnsatisfiable == "ScheduleAnyway" ? GROVE_SPREAD_SOFT : GROVE_SPREAD_HARD;
+      out->spreadGroups.push_back(g); out->spreadSet.push_back(it->first);
+    }
+    return it->second;
+  };
   for (size_t oi = 0; oi < order.size(); ++oi) {
     const std::string& key = *order[oi];
     const PodGang& pg = pending_.at(key);
@@ -473,10 +515,27 @@ Err GpuBackend::EncodeLocked(const std::vector<Node>& nodes, Tables* out) const 
     if (rel == 0 || rel > GROVE_MAX_GANG_CLIQUES || scopes.size() > GROVE_MAX_GANG_SCOPES || pods > (large_ ? GROVE_MAX_WIDE_GANG_PODS : GROVE_MAX_GANG_PODS))
       return mkerr("ERR_SYNC_PODGANG", "Encode", "PodGang " + key + " exceeds the gpu-scheduler limits");
     g.n_cliques = uint16_t(rel); g.n_scopes = uint16_t(scopes.size());
+    uint32_t grp = GROVE_NONE_U32;
+    if (const TopologySpread* sp = remainder ? nullptr : spreadSetOf(pg)) {
+      bool need = false;
+      for (size_t k = out->counts.size() - rel; k < out->counts.size(); ++k) need |= out->counts[k].min_replicas > 0;
+      const uint32_t s = spreadGroup(pg.Namespace, pg.Labels.at(kPartOfLabel), *sp);
+      if (s != GROVE_NONE_U32 && need && g.level != GROVE_LEVEL_NONE && g.level >= out->spreadGroups[s].level) grp = s;
+    }
+    out->spreadOf.push_back(grp);
     out->gangs.push_back(g);
     out->gangNames.push_back(key);
     out->remainder.push_back(remainder ? 1 : 0);
   }
+  // the running replicas of the sets being spread: where the base PodGangs this backend scheduled landed
+  if (std::any_of(out->spreadOf.begin(), out->spreadOf.end(), [](uint32_t x) { return x != GROVE_NONE_U32; }))
+    for (const auto& [key, set] : setOf_) {
+      auto gi = groupOf.find(set);
+      auto ln = lastNode_.find(key);
+      if (gi == groupOf.end() || ln == lastNode_.end() || row.count(key)) continue;
+      if (auto nt = nodeIndex.find(ln->second); nt != nodeIndex.end()) out->spreadSeeds.push_back(grove_spread_seed_t{gi->second, nt->second});
+    }
+  else { out->spreadGroups.clear(); out->spreadSet.clear(); }
   return std::nullopt;
 }
 
@@ -510,6 +569,10 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
                                              uint32_t(t.cliques.size()), t.scopes.data(), uint32_t(t.scopes.size())), "grove_submit_gangs_wide")) return e;
   } else if (auto e = chk(grove_submit_gangs(engine_, t.gangs.data(), uint32_t(t.gangs.size()), t.cliques.data(), uint32_t(t.cliques.size()),
                                              t.scopes.data(), uint32_t(t.scopes.size())), "grove_submit_gangs")) return e;
+  const bool spread = !t.spreadGroups.empty();   // (Encode keeps groups only when a row is a member)
+  if (spread)
+    if (auto e = chk(grove_set_spread(engine_, t.spreadGroups.data(), uint32_t(t.spreadGroups.size()), t.spreadOf.data(), uint32_t(t.spreadOf.size()),
+                                      t.spreadSeeds.data(), uint32_t(t.spreadSeeds.size())), "grove_set_spread")) return e;
   grove_cycle_stats_t st{};
   // running PodGangs -> the reclaim pass's / reservation reuse's tables (holdings on nodes that left the snapshot are dropped)
   std::vector<grove_running_gang_t> run; std::vector<grove_holding_t> held; std::vector<std::string> runNames;
@@ -583,6 +646,21 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
     if (t.remainder[g] && statuses->count(t.gangNames[g])) continue;   // the minimum row of the same PodGang already spoke
     (*statuses)[t.gangNames[g]] = s;
   }
+  // topology spread: a DoNotSchedule member that found no room in the domains it was allowed, a ScheduleAnyway member placed
+  // outside them (set after the diagnosis below, which refuses a spread cycle)
+  std::map<std::string, std::string> spreadMsg;
+  if (spread)
+    for (uint32_t g = 0; g < gs.size(); ++g) {
+      const uint32_t s = t.spreadOf[g];
+      if (s == GROVE_NONE_U32) continue;
+      const std::string key = levels[t.spreadGroups[s].level].Key, skew = std::to_string(t.spreadGroups[s].max_skew);
+      if (gs[g].state == GROVE_GANG_REJECTED && t.spreadGroups[s].mode == GROVE_SPREAD_HARD)
+        spreadMsg[t.gangNames[g]] = "topology spread of " + t.spreadSet[s] + " over " + key + " (maxSkew " + skew +
+                                    ", DoNotSchedule): no " + key + " domain within the skew had room for this replica";
+      if (gs[g].state == GROVE_GANG_ADMITTED && (gs[g].reserved0 & GROVE_STATUS_SPREAD_SKEWED))
+        spreadMsg[t.gangNames[g]] = "topology spread of " + t.spreadSet[s] + " over " + key + " (maxSkew " + skew +
+                                    ", ScheduleAnyway): no " + key + " domain within the skew had room; placed beyond it";
+    }
   // why the rejected PodGangs did not fit (an ordinary cycle only: the running-gang cycles judge gangs against other views).  A
   // failed diagnosis leaves the messages empty: it never costs the cycle its bindings.
   if (explain && !both && !reuse && !preempt &&
@@ -594,6 +672,7 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
         if (gs[g].state == GROVE_GANG_REJECTED && !t.remainder[g])
           (*statuses)[t.gangNames[g]].ScheduledMessage = ExplainRejection(t, snap.at(t.gangNames[g]), g, gd[g], qd.data(), levels);
   }
+  for (const auto& [key, msg] : spreadMsg) (*statuses)[key].ScheduledMessage = msg;
   // a scheduled PodGang leaves the pending set once every PodReference is bound; until then its unbound pods are retried
   // as a remainder (Encode).  Remember where gangs landed for ReuseReservationRef hints.
   auto constrained = [](const PodGang& pg) {
@@ -641,6 +720,8 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
       }
     }
     if (gs[i].n_pods && !lastNode_.count(key)) lastNode_[key] = nodes[pl[gs[i].placement_off].node].Name;
+    if (pg.BasePodGangName.empty())   // a replica of its PodCliqueSet from now on (topology spread counts it where it landed)
+      if (auto it = pg.Labels.find(kPartOfLabel); it != pg.Labels.end()) setOf_[key] = pg.Namespace + "/" + it->second;
     std::vector<uint32_t>& done = bound_[key];
     done.resize(pg.Spec.PodGroups.size(), 0u);
     for (uint32_t c = t.gangs[i].clique_off; c < t.gangs[i].clique_off + t.gangs[i].n_cliques; ++c) done[t.cliqueOf[c].second] += seen[c];

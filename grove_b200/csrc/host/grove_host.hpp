@@ -197,6 +197,13 @@ class TopologyAwareSchedBackend {                                               
   virtual std::pair<bool, std::string> CheckTopologyDrift(const std::vector<TopologyLevel>& levels) const = 0;
 };
 
+// a PodCliqueSet's topology spread (Kubernetes TopologySpreadConstraint at PodGang granularity; DESIGN.md section 1)
+struct TopologySpread {
+  std::string LevelKey;                               // a level of the ClusterTopology: the replicas spread over its domains
+  int32_t MaxSkew = 1;                                // >= 1
+  std::string WhenUnsatisfiable = "DoNotSchedule";    // or "ScheduleAnyway"
+};
+
 // packed tables of one cycle, as handed to libgrove_place.so
 struct Tables {
   std::vector<grove_node_t> nodes;
@@ -209,6 +216,11 @@ struct Tables {
   std::vector<uint8_t> remainder;                       // gang row -> 1: unbound pods of an already scheduled PodGang (MinReplicas 0)
   std::vector<uint32_t> refBase;                        // clique row -> first PodReference its placement entries bind (remainders)
   std::map<std::string, std::string> skipped;           // PodGang "<ns>/<name>" -> why it was left out of this pass
+  // topology spread (SetTopologySpread): the groups, each gang row's group (GROVE_NONE_U32: none), the running replicas
+  std::vector<grove_spread_t> spreadGroups;
+  std::vector<uint32_t> spreadOf;
+  std::vector<grove_spread_seed_t> spreadSeeds;
+  std::vector<std::string> spreadSet;                   // group -> "<ns>/<PodCliqueSet>"
 };
 
 // The `gpu` scheduler backend: the third case of newBackendForProfile (manager/manager.go:35-52).
@@ -270,6 +282,16 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   // the message for one rejected PodGang row of `t` from its diagnosis records (levels: the ClusterTopology's, broadest first)
   static std::string ExplainRejection(const Tables& t, const PodGang& pg, uint32_t row, const grove_gang_diag_t& gd,
                                       const grove_clique_diag_t* cliques, const std::vector<TopologyLevel>& levels);
+  // Topology spread: the pending BASE PodGangs (no BasePodGangName) whose app.kubernetes.io/part-of label names the PodCliqueSet
+  // `pcsName` spread over the domains of `spread.LevelKey` (grove_set_spread); the running base PodGangs of the set that this
+  // backend scheduled count where they landed.  A member must have a Required level at or below that level and a PodGroup with
+  // MinReplicas > 0; other PodGangs of the set are packed as usual and not counted.  A DoNotSchedule member rejected at its turn
+  // gets a ScheduledMessage that names the spread; a ScheduleAnyway member placed outside the allowed domains is scheduled with a
+  // message that says so.  With preemption, reservation reuse or reuse with reclaim on, or in a pass with a PodGang beyond the
+  // ordinary limits (SetLargePodGangs), members stay out of the pass, Unschedulable with a reason.  nullopt removes the set's
+  // spread.  Off by default (no set has one).
+  Err SetTopologySpread(const std::string& pcsName, std::optional<TopologySpread> spread);
+  static constexpr const char* kPartOfLabel = "app.kubernetes.io/part-of";
   size_t Running() const { std::lock_guard<std::mutex> l(mu_); return running_.size(); }
   // why a PodGang cannot be handed to the engine (limits of the packed tables), or empty.  SyncPodGang accepts every
   // PodGang -- the reference's reconciler would requeue forever on an error -- and RunCycle reports these as
@@ -304,6 +326,8 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   bool reclaimReuse_ = false;
   bool large_ = false;
   bool explain_ = false;
+  std::map<std::string, TopologySpread> spread_;       // PodCliqueSet name -> its spread
+  std::map<std::string, std::string> setOf_;           // scheduled base PodGang -> "<ns>/<PodCliqueSet>" (its part-of label)
   grove_engine_t* engine_ = nullptr;
   uint32_t engineLevels_ = 0;
   mutable std::mutex mu_;        // pending set, bindings, levels: everything SyncPodGang / OnPodGangDelete / SyncTopology touch

@@ -9,6 +9,7 @@
 //                agree with the sequential, priority-ordered pass; k_fin_* / k_emit  outputs
 //   reclaim.cuh  k_reclaim_*  reclaim-class views over the running gangs' holdings (grove_run_cycle_reuse_preempt)
 //   diagnose.cuh k_diag_*  why each rejected gang did not fit, after the cycle (grove_diagnose)
+//   spread.cuh   k_spread_classes / k_spread  allowed level-l_s domains of the topology spread members (grove_set_spread)
 //
 // Semantics are DESIGN.md "Placement semantics"; the reference contract they restate is cited in
 // include/grove_place.h.  Integer / compare work only: no tensor cores, no floating point.
@@ -21,3 +22,4 @@
 #include "relax.cuh"
 #include "reclaim.cuh"
 #include "diagnose.cuh"
+#include "spread.cuh"

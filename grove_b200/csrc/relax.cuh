@@ -205,8 +205,9 @@ __global__ void __launch_bounds__(256) k_hold_release(Tables tb, Relax rx, uint4
   }
 }
 
-// one warp per evaluated gang: publish a changed result (kHolds: a cycle with holds)
-template <bool kHolds>
+// one warp per evaluated gang: publish a changed result (kHolds: a cycle with holds; kSpread: a cycle with spread members, whose
+// changed results leave a stamp per group)
+template <bool kHolds, bool kSpread = false>
 __global__ void __launch_bounds__(256) k_apply(Tables tb, Relax rx) {
   cudaGridDependencySynchronize();   // (launched chained: engine.cu launch_chained)
   const uint32_t lane = threadIdx.x & 31;
@@ -242,6 +243,10 @@ __global__ void __launch_bounds__(256) k_apply(Tables tb, Relax rx) {
     if (lane == 0) rx.extent[g] = n_ext;   // what the LATEST evaluation read, changed result or not
     if (!diff) continue;
     const uint32_t stamp = make_stamp(round, rank);
+    if constexpr (kSpread) {   // dirty rule (d): the members of its group ranked after it
+      const uint32_t s = rx.sp.group[g];
+      if (lane == 0 && s != kFull) atomicMin(rx.sp.stamp + s, stamp);
+    }
     const bool owner = kHolds && has_hold(rx, g);   // its claims are what its placement needs beyond its hold
     // withdraw the old claims
     for (uint32_t i = lane; i < on; i += 32) {
@@ -275,7 +280,9 @@ __global__ void __launch_bounds__(256) k_apply(Tables tb, Relax rx) {
   }
 }
 
-// one warp per gang of the window: did its view change this round?
+// one warp per gang of the window: did its view change this round?  (kSpread: or, for a spread member, the result of a member
+// of its group ranked before it)
+template <bool kSpread = false>
 __global__ void __launch_bounds__(256) k_detect(Topo tp, Tables tb, Relax rx, uint32_t refresh_every) {
   __shared__ bool s_last;
   cudaGridDependencySynchronize();
@@ -294,6 +301,10 @@ __global__ void __launch_bounds__(256) k_detect(Topo tp, Tables tb, Relax rx, ui
     const uint32_t first_node = (ts == GROVE_GANG_ADMITTED && lane < cnt) ? rx.ent_node[po + lane] : GROVE_NONE_U32;
     // its base gang's result changed
     if (base != GROVE_NONE_U32 && rx.chg_round[base] == round) dirty = true;
+    if constexpr (kSpread) {
+      const uint32_t s = rx.sp.group[g];
+      if (s != kFull && stamp_below(rx.sp.stamp[s], round, p)) dirty = true;
+    }
     // a lower rank newly claimed a node this gang uses
     if (ts == GROVE_GANG_ADMITTED) {
       if (first_node != GROVE_NONE_U32) dirty |= stamp_below(rx.add_stamp[first_node], round, p);

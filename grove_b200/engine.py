@@ -25,7 +25,7 @@ SYMBOLS = [
     "grove_load_nodes", "grove_update_nodes", "grove_get_nodes", "grove_submit_gangs", "grove_submit_gangs_wide", "grove_run_cycle",
     "grove_get_placements", "grove_get_gang_status", "grove_get_scope_domains", "grove_load_nodes_device",
     "grove_build_score_matrix", "grove_run_cycle_preempt", "grove_get_victims", "grove_run_cycle_reuse",
-    "grove_run_cycle_reuse_preempt", "grove_diagnose",
+    "grove_run_cycle_reuse_preempt", "grove_diagnose", "grove_set_spread",
     "grove_shard_range", "grove_run_score_pass", "grove_shard_summary_device",
     "grove_debug_get_perm", "grove_debug_get_fit_row", "grove_debug_get_score_row",
 ]
@@ -137,6 +137,16 @@ class PlacementEngine:
                                                      C.c_uint32(len(cliques)), _p(scopes), C.c_uint32(len(scopes))))
         self.G, self.Q, self.S = len(gangs), len(cliques), len(scopes)
         self._cap_pods = int(counts["replicas"].astype(np.int64).sum()) if len(cliques) else 0
+
+    def set_spread(self, groups: np.ndarray, gang_group: np.ndarray, seeds: np.ndarray | None = None):
+        """grove_set_spread: topology spread groups (tables.spread_dt), the group of every submitted gang (tables.NONE_U32 = none)
+        and the running replicas of each group (tables.spread_seed_dt, caller node indices).  Call after submit_gangs; the next
+        submit / load_nodes clears it (include/grove_place.h "topology spread")."""
+        groups = np.ascontiguousarray(groups, dtype=T.spread_dt)
+        gang_group = np.ascontiguousarray(gang_group, dtype=np.uint32)
+        seeds = np.ascontiguousarray(np.zeros(0, dtype=T.spread_seed_dt) if seeds is None else seeds, dtype=T.spread_seed_dt)
+        self._check(self.lib.grove_set_spread(self.h, _p(groups), C.c_uint32(len(groups)), _p(gang_group), C.c_uint32(len(gang_group)),
+                                              _p(seeds), C.c_uint32(len(seeds))))
 
     # ---- the cycle ----
     def run_cycle(self) -> dict:

@@ -192,6 +192,30 @@ def config_c4(n=50000, g=10000, seed=SEED_BASE + 4, max_used_pct=90):
     return dict(name="C4", n_levels=4, nodes=nodes, tables=b.build())
 
 
+def c4_spread_groups(gangs, cliques, size=8, level=0, mode=T.SPREAD_HARD, max_skew=1):
+    """Topology spread groups over a C4-style submission (grove_set_spread): its base gangs whose Required level is `level` or
+    deeper, in groups of `size` by (priority, template) -- the replicas of one PodCliqueSet.  -> (T.spread_dt groups, gang_group)"""
+    gang_group = np.full(len(gangs), T.NONE_U32, dtype=np.uint32)
+    by_key = {}
+    for g in range(len(gangs)):
+        if gangs["base_gang"][g] != T.NONE_U32 or gangs["level"][g] == T.LEVEL_NONE or gangs["level"][g] < level:
+            continue
+        co = int(gangs["clique_off"][g]); n = int(gangs["n_cliques"][g])
+        q = cliques[co: co + n]
+        key = (int(gangs["priority"][g]), n, tuple(q["req_cpu_milli"]), tuple(q["req_mem_mib"]), tuple(q["req_gpu"]),
+               tuple(q["min_replicas"]), tuple(q["class_mask"]), int(gangs["level"][g]))
+        by_key.setdefault(key, []).append(g)
+    n_groups = 0
+    for key in sorted(by_key):
+        members = by_key[key]
+        for i in range(0, len(members), size):
+            gang_group[members[i: i + size]] = n_groups
+            n_groups += 1
+    groups = np.zeros(n_groups, dtype=T.spread_dt)
+    groups["level"], groups["mode"], groups["max_skew"] = level, mode, max_skew
+    return groups, gang_group
+
+
 def config_c4_large(n=50000, g=10000, n_large=24, seed=SEED_BASE + 44, max_used_pct=90):
     """C4 (config_c4) plus `n_large` PodGangs of 256-2048 pods, for grove_submit_gangs_wide: a leader (Required host) and a
     worker PodGroup of 255-2047 one-GPU pods under a Required zone with a Preferred block, priorities drawn from C4's three

@@ -72,10 +72,17 @@ gang_diag_dt = np.dtype([
 DIAG_FAILURES = ("unschedulable", "selector", "labels", "cpu", "mem", "gpu", "pods")
 clique_diag_dt = np.dtype([("nodes_fit", "<u4")] + [(f, "<u4") for f in DIAG_FAILURES] + [("pods_fit", "<u8")])
 
+# topology spread (grove_set_spread, include/grove_place.h "topology spread")
+SPREAD_HARD, SPREAD_SOFT = 1, 2   # DoNotSchedule, ScheduleAnyway
+STATUS_SPREAD_SKEWED = 0x2        # status reserved0: a SOFT member placed outside its allowed domains
+spread_dt = np.dtype([("level", "u1"), ("mode", "u1"), ("max_skew", "<u2"), ("reserved", "<u4")])
+spread_seed_dt = np.dtype([("group", "<u4"), ("node", "<u4")])
+
 assert node_dt.itemsize == 32 and clique_dt.itemsize == 16 and scope_dt.itemsize == 8
 assert gang_dt.itemsize == 32 and placement_dt.itemsize == 8 and status_dt.itemsize == 32 and scope_status_dt.itemsize == 8
 assert config_dt.itemsize == 32 and stats_dt.itemsize == 64
 assert gang_diag_dt.itemsize == 16 and clique_diag_dt.itemsize == 40
+assert spread_dt.itemsize == 8 and spread_seed_dt.itemsize == 8
 
 
 def make_nodes(n: int) -> np.ndarray:

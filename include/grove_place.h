@@ -148,7 +148,8 @@ typedef struct grove_gang_status {
   uint8_t state;
   uint8_t level;           /* level of the domain the whole gang was packed into (its Required level, or the deeper
                               Preferred level that held), GROVE_LEVEL_NONE = the whole cluster / not admitted */
-  uint16_t reserved0;      /* flags: GROVE_STATUS_PREEMPTOR = admitted by the reclaim pass of grove_run_cycle_preempt; else 0 */
+  uint16_t reserved0;      /* flags: GROVE_STATUS_PREEMPTOR = admitted by the reclaim pass of grove_run_cycle_preempt,
+                              GROVE_STATUS_SPREAD_SKEWED = a SOFT spread member placed outside its allowed domains; else 0 */
   uint16_t score_num;      /* PlacementScore = score_num / score_den (podgang.go:187-189): over the gang, its scopes and
                               its cliques that carry a pack constraint, (levels honoured) / (levels asked for), where
                               asked = Preferred if set else Required; 1/1 when nothing was asked or everything held;
@@ -336,6 +337,42 @@ typedef struct grove_clique_diag {   /* 40 B */
   uint64_t pods_fit;      /* sum over nodes of the pods of the clique that fit */
 } grove_clique_diag_t;
 int32_t grove_diagnose(grove_engine_t* e, grove_gang_diag_t* gangs, uint32_t cap_g, grove_clique_diag_t* cliques, uint32_t cap_q);
+
+/* ---- topology spread ---------------------------------------------------------------------------------
+ * The replicas of one PodCliqueSet spread over topology domains (DESIGN.md section 1, "Topology spread"; Kubernetes
+ * TopologySpreadConstraint at PodGang granularity).  A spread group s has a level l_s, a max_skew >= 1 and a mode.  Each
+ * submitted gang belongs to at most one group (gang_group[g], or GROVE_NONE_U32); a member's gang Required level is l_s or
+ * deeper, so an admitted member lies in exactly one level-l_s domain A(g), and it has a clique with MinReplicas > 0.  Seeds
+ * are running replicas of a group, each counted in the level-l_s domain of its node (nowhere when the node lacks that label).
+ * At member g's turn in the sequential pass: c(A) = seeds in A + members of s ranked before g that were admitted into A;
+ * E_g = the level-l_s domains holding a schedulable node whose selector class some clique of g accepts; m = min over E_g of
+ * c(A); A is ALLOWED iff A is in E_g and c(A) + 1 - m <= max_skew.
+ *   GROVE_SPREAD_HARD (DoNotSchedule): a candidate domain outside every allowed A is infeasible; none feasible -> REJECTED.
+ *   GROVE_SPREAD_SOFT (ScheduleAnyway): the allowed candidates first (the usual order, Preferred levels included); if none
+ *   fits, the disallowed ones.  A gang admitted by that second walk carries GROVE_STATUS_SPREAD_SKEWED.
+ * Everything else is the ordinary pass.  Call after grove_submit_gangs and before grove_run_cycle; the next
+ * grove_submit_gangs* or grove_load_nodes* clears the set, grove_update_nodes keeps it.  GROVE_ERR_INVALID_ARG for a wrong
+ * n_gangs, a group index out of range, a level >= n_levels, a bad mode, max_skew 0, a member without a gang Required level at
+ * l_s or deeper, a member with no MinReplicas > 0, a seed on a node or group out of range; GROVE_ERR_LIMIT for a wide
+ * submission, and when the members' allowed-domain rows (one bit per member and domain of its group's level) would exceed 1 GB;
+ * GROVE_ERR_STATE before nodes are loaded and gangs submitted.  While a set with members is in place grove_run_cycle_preempt / _reuse / _reuse_preempt return
+ * GROVE_ERR_STATE, and grove_diagnose returns GROVE_ERR_STATE after such a cycle.  A set without members changes nothing. */
+#define GROVE_SPREAD_HARD 1u            /* DoNotSchedule */
+#define GROVE_SPREAD_SOFT 2u            /* ScheduleAnyway */
+#define GROVE_STATUS_SPREAD_SKEWED 0x2u /* grove_gang_status_t.reserved0: a SOFT member placed outside its allowed domains */
+typedef struct grove_spread {
+  uint8_t level;
+  uint8_t mode;           /* GROVE_SPREAD_HARD or GROVE_SPREAD_SOFT */
+  uint16_t max_skew;      /* >= 1 */
+  uint32_t reserved;
+} grove_spread_t;
+typedef struct grove_spread_seed {
+  uint32_t group;
+  uint32_t node;          /* caller's node index */
+} grove_spread_seed_t;
+int32_t grove_set_spread(grove_engine_t* e, const grove_spread_t* groups, uint32_t n_groups,
+                         const uint32_t* gang_group, uint32_t n_gangs,
+                         const grove_spread_seed_t* seeds, uint32_t n_seeds);
 
 /* K2: the topology-distance score matrix T[clique][node] = fit ? 1 + levels shared with the gang's anchor : 0 (u8) over the
  * snapshot the last cycle started from -- what a scheduler's Score extension point would hand out.  The admission does

@@ -57,8 +57,111 @@ type schedulerBackend struct {
 	// explainUnschedulable: after an ordinary cycle the Unschedulable message of a rejected PodGang says why, from
 	// grove_diagnose (GpuBackend::SetExplainUnschedulable in the C++ mirror); off, it is the fixed message of before.
 	explainUnschedulable bool
+	// spread: PodCliqueSet name -> its topology spread (SetTopologySpread); setOf: scheduled base PodGang -> its PodCliqueSet
+	spread map[string]TopologySpread
+	setOf  map[string]string
 	eng                  *engine
 	stopLoop chan struct{}
+}
+
+// TopologySpread spreads the base PodGangs of one PodCliqueSet over the domains of a level (GpuBackend::SetTopologySpread in the
+// C++ mirror; DESIGN.md section 1 "Topology spread").  WhenUnsatisfiable is "DoNotSchedule" or "ScheduleAnyway".
+type TopologySpread struct {
+	LevelKey          string
+	MaxSkew           int32
+	WhenUnsatisfiable string
+}
+
+// the label the producer puts on every PodGang of a PodCliqueSet (components/podgang/podgang.go:129), and the one that names the
+// base PodGang of a scaled one (api/common/labels.go:35-37)
+const (
+	labelPartOf      = "app.kubernetes.io/part-of"
+	labelBasePodGang  = "grove.io/base-podgang"
+)
+
+// SetTopologySpread sets (nil: removes) the topology spread of PodCliqueSet pcs.  Its pending base PodGangs with a Required level
+// at or below spread.LevelKey and a PodGroup with MinReplicas > 0 are members; the running ones this backend scheduled count
+// where they landed.  With preemption on, or in a pass with a large PodGang, members stay out of the pass, Unschedulable.
+func (b *schedulerBackend) SetTopologySpread(pcs string, spread *TopologySpread) error {
+	b.mu.Lock()
+	defer b.mu.Unlock()
+	if b.spread == nil {
+		b.spread, b.setOf = map[string]TopologySpread{}, map[string]string{}
+	}
+	if spread == nil {
+		delete(b.spread, pcs)
+		return nil
+	}
+	if spread.LevelKey == "" || spread.MaxSkew < 1 || spread.MaxSkew > 0xFFFF ||
+		(spread.WhenUnsatisfiable != "DoNotSchedule" && spread.WhenUnsatisfiable != "ScheduleAnyway") {
+		return fmt.Errorf("topology spread of %s: want a level key, maxSkew >= 1 and DoNotSchedule or ScheduleAnyway", pcs)
+	}
+	b.spread[pcs] = *spread
+	return nil
+}
+
+// spreadSet: the PodCliqueSet whose spread pg is a member of, or ""
+func (b *schedulerBackend) spreadSet(pg *groveschedulerv1alpha1.PodGang) string {
+	if _, scaled := pg.Labels[labelBasePodGang]; scaled {
+		return ""
+	}
+	if _, ok := b.spread[pg.Labels[labelPartOf]]; ok {
+		return pg.Labels[labelPartOf]
+	}
+	return ""
+}
+
+// encodeSpread fills the spread tables of t for gang rows `rows`: one group per PodCliqueSet with a member, its running
+// replicas as seeds.
+func (b *schedulerBackend) encodeSpread(t *tables, rows []*groveschedulerv1alpha1.PodGang, levels []string, nodeIdx map[string]int) {
+	groupOf := map[string]int{}
+	t.spreadOf = make([]C.uint32_t, len(rows))
+	members := 0
+	for gi, pg := range rows {
+		t.spreadOf[gi] = C.GROVE_NONE_U32
+		set := b.spreadSet(pg)
+		if set == "" {
+			continue
+		}
+		sp := b.spread[set]
+		lvl := levelIndex(levels, &sp.LevelKey)
+		g := t.gangs[gi]
+		need := false
+		for q := int(g.clique_off); q < int(g.clique_off)+int(g.n_cliques); q++ {
+			need = need || t.cliques[q].min_replicas > 0 // (a spread pass is never wide: the 8-bit counts hold)
+		}
+		if lvl == C.GROVE_LEVEL_NONE || g.level == C.GROVE_LEVEL_NONE || g.level < lvl || !need {
+			continue // packed as usual, not counted
+		}
+		s, ok := groupOf[pg.Namespace+"/"+set]
+		if !ok {
+			s = len(t.spreadGroups)
+			groupOf[pg.Namespace+"/"+set] = s
+			mode := C.uint8_t(C.GROVE_SPREAD_HARD)
+			if sp.WhenUnsatisfiable == "ScheduleAnyway" {
+				mode = C.GROVE_SPREAD_SOFT
+			}
+			t.spreadGroups = append(t.spreadGroups, C.grove_spread_t{level: lvl, mode: mode, max_skew: C.uint16_t(sp.MaxSkew)})
+		}
+		t.spreadOf[gi] = C.uint32_t(s)
+		members++
+	}
+	if members == 0 {
+		t.spreadGroups, t.spreadOf = nil, nil
+		return
+	}
+	for key, set := range b.setOf { // a running replica counts in the domain of a node it holds
+		s, ok := groupOf[set]
+		if !ok {
+			continue
+		}
+		for node := range b.running[key].held {
+			if n, ok := nodeIdx[node]; ok {
+				t.spreadSeeds = append(t.spreadSeeds, C.grove_spread_seed_t{group: C.uint32_t(s), node: C.uint32_t(n)})
+				break
+			}
+		}
+	}
 }
 
 type runningGang struct {
@@ -104,6 +207,7 @@ func (b *schedulerBackend) OnPodGangDelete(_ context.Context, pg *grovescheduler
 	key := pg.Namespace + "/" + pg.Name
 	delete(b.pending, key)
 	delete(b.running, key) // its pods' resources show up as free in the next node snapshot
+	delete(b.setOf, key)
 	return nil
 }
 
@@ -228,6 +332,7 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 		snap = append(snap, pg)
 	}
 	levels, eng, preempt, large, explain := b.levels, b.eng, b.preempt, b.largePodGangs, b.explainUnschedulable
+	spreadOn := len(b.spread) > 0
 	b.mu.Unlock()
 	sort.Slice(snap, func(i, j int) bool { return snap[i].CreationTimestamp.Before(&snap[j].CreationTimestamp) }) // submission order
 
@@ -241,13 +346,30 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 	}
 	t, nodeNames := encodeNodes(nodeList.Items, podList.Items, levels) // allocatable - requests of bound pods; dom[l] = interned label value
 	rows := make([]*groveschedulerv1alpha1.PodGang, 0, len(snap))
+	wideAny := false // a wide submission takes no spread set
+	for _, pg := range snap {
+		wideAny = wideAny || (large && whyNotEncodable(pg, false, false) != "")
+	}
 	for _, pg := range snap {
 		if why := whyNotEncodable(pg, large, preempt); why != "" { // large && preempt: within the old limits only
 			b.setUnschedulable(ctx, pg, why)
 			continue
 		}
+		if spreadOn && (preempt || wideAny) && b.spreadSet(pg) != "" {
+			b.setUnschedulable(ctx, pg, "topology spread is not applied while preemption is on or in a pass with large PodGangs")
+			continue
+		}
 		b.encodeGang(t, pg, levels, podList.Items) // one grove_gang_t + its cliques / scopes; requests come from the pods
 		rows = append(rows, pg)
+	}
+	if spreadOn && !preempt && !wideAny {
+		nodeIdx := make(map[string]int, len(nodeNames))
+		for i, n := range nodeNames {
+			nodeIdx[n] = i
+		}
+		b.mu.Lock()
+		b.encodeSpread(t, rows, levels, nodeIdx)
+		b.mu.Unlock()
 	}
 	res, err := eng.cycle(t, preempt, large, explain)
 	if err != nil {
@@ -271,12 +393,27 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 			score := float64(st.score_num) / float64(st.score_den)
 			pg.Status.Phase = groveschedulerv1alpha1.PodGangPhaseStarting
 			pg.Status.PlacementScore = &score // podgang.go:187-189
+			msg := ""
+			if st.reserved0&C.GROVE_STATUS_SPREAD_SKEWED != 0 {
+				msg = "topology spread (ScheduleAnyway): no domain within the skew had room; placed beyond it"
+			}
 			meta.SetStatusCondition(&pg.Status.Conditions, metav1.Condition{Type: string(groveschedulerv1alpha1.PodGangConditionTypeScheduled),
-				Status: metav1.ConditionTrue, Reason: "Scheduled"})
+				Status: metav1.ConditionTrue, Reason: "Scheduled", Message: msg})
+			if _, scaled := pg.Labels[labelBasePodGang]; !scaled && pg.Labels[labelPartOf] != "" {
+				b.mu.Lock()
+				if b.setOf == nil {
+					b.setOf = map[string]string{}
+				}
+				b.setOf[pg.Namespace+"/"+pg.Name] = pg.Namespace + "/" + pg.Labels[labelPartOf]
+				b.mu.Unlock()
+			}
 		case C.GROVE_GANG_REJECTED:
 			why := "no topology domain holds the gang's MinReplicas"
 			if res.gangDiag != nil {
 				why = explainRejection(t, pg, gi, res.gangDiag[gi], res.cliqueDiag, levels)
+			}
+			if len(t.spreadOf) > 0 && t.spreadOf[gi] != C.GROVE_NONE_U32 && t.spreadGroups[t.spreadOf[gi]].mode == C.GROVE_SPREAD_HARD {
+				why = "topology spread (DoNotSchedule): no domain within the skew had room for this replica"
 			}
 			b.setUnschedulable(ctx, pg, why)
 			continue

@@ -55,6 +55,11 @@ type tables struct {
 	// reclaim pass (optional): PodGangs this backend scheduled earlier and what they hold per node
 	running  []C.grove_running_gang_t
 	holdings []C.grove_holding_t
+	// topology spread (optional; never together with the reclaim pass): the groups, each gang row's group (GROVE_NONE_U32 =
+	// none) and the running replicas
+	spreadGroups []C.grove_spread_t
+	spreadOf     []C.uint32_t
+	spreadSeeds  []C.grove_spread_seed_t
 }
 
 type result struct {
@@ -86,6 +91,16 @@ func (e *engine) cycle(t *tables, preempt, large, explain bool) (*result, error)
 	} else if err := e.err(C.grove_submit_gangs(e.h, &t.gangs[0], C.uint32_t(len(t.gangs)), &t.cliques[0],
 		C.uint32_t(len(t.cliques)), &t.scopes[0], C.uint32_t(len(t.scopes)))); err != nil {
 		return nil, err
+	}
+	if len(t.spreadGroups) > 0 {
+		var sp *C.grove_spread_seed_t
+		if len(t.spreadSeeds) > 0 {
+			sp = &t.spreadSeeds[0]
+		}
+		if err := e.err(C.grove_set_spread(e.h, &t.spreadGroups[0], C.uint32_t(len(t.spreadGroups)), &t.spreadOf[0],
+			C.uint32_t(len(t.spreadOf)), sp, C.uint32_t(len(t.spreadSeeds)))); err != nil {
+			return nil, err
+		}
 	}
 	r := &result{}
 	if preempt && len(t.running) > 0 {
