@@ -168,13 +168,15 @@ __device__ __forceinline__ uint32_t visit_pos(const GangRegs& g, uint32_t n) {
 }
 
 // ---- the evaluator: the whole warp packs ONE candidate range ------------------------------------------
-template <bool kPref_, bool kHolds, bool kWide_ = false>
+// kFence: the nodes of the fences active for the gang (fm0 / fm1, common.cuh fenced) take no pod
+template <bool kPref_, bool kHolds, bool kWide_ = false, bool kFence = false>
 struct Ev {
   static constexpr bool kPref = kPref_;
   static constexpr bool kWide = kWide_;
   static constexpr bool kStaged = false;
   const Topo& tp; const Relax& rb; GangShared& sh; const GangRegs& g; uint32_t lane;
   uint32_t np;
+  uint32_t fm0 = 0, fm1 = 0;   // (kFence) the active fences
   uint32_t tmask = 0;   // bit (n & 31) set for every node the gang has put a pod on: quick 'untouched' test
   uint32_t ext = 0;     // see the file comment
   uint32_t t_stage = 0, t_pre = 0, t_pack = 0, n_stage = 0;
@@ -208,6 +210,7 @@ struct Ev {
 
   // pods of clique cr that still fit on node n under the gang's view, after what the gang itself put there (kWide: o, from own_word)
   __device__ __forceinline__ uint32_t cap_view(uint32_t cr, uint32_t n, int4 o = int4{}) const {
+    if constexpr (kFence) if (fenced(rb.fc, fm0, fm1, n)) return 0u;
     const uint32_t live = (__ldg(rb.nlive + (n >> 2)) >> ((n & 3u) * 8u)) & 0xFFu;
     const bool own = (tmask >> (n & 31u)) & 1u;
     if (!live && !own) {
@@ -351,7 +354,7 @@ struct Ev {
 // instead of a chain of dependent L2 look-ups per 32 nodes.
 constexpr uint32_t kStageMax = 128;
 
-template <bool kPref_, bool kHolds, bool kWide_ = false>
+template <bool kPref_, bool kHolds, bool kWide_ = false, bool kFence = false>
 struct EvS {
   static constexpr bool kPref = kPref_;
   static constexpr bool kWide = kWide_;
@@ -366,6 +369,7 @@ struct EvS {
   uint32_t t_st2 = 0, t_st3 = 0;                              // of the staging: claim lines, overflow chains
   uint32_t vlo = 0, vhi = 0;
   uint32_t np;
+  uint32_t fm0 = 0, fm1 = 0;   // (kFence) the active fences: their nodes are staged unschedulable
   uint32_t tmask = 0;
   uint32_t ext = 0;
   // the entry stack: shared memory, or (kWide) the warp's own stack in global memory
@@ -418,7 +422,9 @@ struct EvS {
         }
       }
       view[k * 32u + lane] = make_int4(cpu, mem, gpu, pods);
-      vflag[k * 32u + lane] = r[k].w;
+      uint32_t f = r[k].w;
+      if constexpr (kFence) if (n < dh && fenced(rb.fc, fm0, fm1, n)) f &= ~uint32_t(GROVE_NODE_SCHEDULABLE);
+      vflag[k * 32u + lane] = f;
     }
     __syncwarp();
     // the whole range has been read: it ends at the furthest position any of its nodes has in the visiting order
@@ -842,7 +848,10 @@ constexpr int kEvalWarps = 8;
 // kWide: the instantiation of a wide cycle (16-bit counts; the entry stack of each warp in Relax::wide_node).
 // kSpread: the instantiation of a cycle with topology spread members (spread.cuh): a member's candidates are those whose
 // level-l_s domain is allowed (HARD, and the first walk of SOFT) or not allowed (the second walk of SOFT).
-template <bool kPref, bool kHolds, bool kWide, bool kSpread = false>
+// kFence: the instantiation of a cycle with fences (fence.cuh): the nodes of an active fence of a gang ranked before the evaluated
+// one fail K1 fit in every view it forms (staged attempts, unstaged reads, the record - total fast path).  The capacity tables and
+// shape bits come from the committed table and stay upper bounds.
+template <bool kPref, bool kHolds, bool kWide, bool kSpread = false, bool kFence = false>
 __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb, Relax rx, uint32_t max_att) {
   __shared__ GangShared shs[kEvalWarps];
   __shared__ int4 s_view[kEvalWarps][kStageMax];
@@ -936,9 +945,15 @@ __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb,
     // shrink otherwise (claims are added, settled claims move into the committed state).  So a re-evaluation skips the
     // candidates in front of its last answer that no withdrawal touched -- gangs that meet a nearly full cluster would
     // otherwise re-run dozens of failing attempts every round.  (Single candidate level only.)
-    Ev<kPref, kHolds, kWide> ev(tp, rx, sh, g, lane);                         // candidates of any size, node state from L2
-    EvS<kPref, kHolds, kWide> evs(tp, rx, sh, g, lane, s_view[warp], s_vflag[warp], s_rk[warp]);         // candidates of <= kStageMax nodes, node state staged in shared memory
+    Ev<kPref, kHolds, kWide, kFence> ev(tp, rx, sh, g, lane);                         // candidates of any size, node state from L2
+    EvS<kPref, kHolds, kWide, kFence> evs(tp, rx, sh, g, lane, s_view[warp], s_vflag[warp], s_rk[warp]);         // candidates of <= kStageMax nodes, node state staged in shared memory
     if constexpr (kWide) { ev.wn = evs.wn = wide_node; ev.wm = evs.wm = wide_meta; }
+    if constexpr (kFence) {   // the fences active for this gang: a lane per entry (at most 64), fixed for the round (k_apply writes tstate)
+      bool a0 = false, a1 = false;
+      if (lane < rx.fc.n) { const uint4 f = rx.fc.list[lane]; a0 = f.x != kFull && f.z < g.rank && rx.tstate[f.w] == GROVE_GANG_REJECTED; }
+      if (lane + 32u < rx.fc.n) { const uint4 f = rx.fc.list[lane + 32u]; a1 = f.x != kFull && f.z < g.rank && rx.tstate[f.w] == GROVE_GANG_REJECTED; }
+      ev.fm0 = evs.fm0 = __ballot_sync(kFull, a0); ev.fm1 = evs.fm1 = __ballot_sync(kFull, a1);
+    }
     bool staged = false;  // the winning attempt ran on evs
     bool won = false;     // this warp holds the answer
     bool done = false;    // CTA-uniform

@@ -118,6 +118,14 @@ struct Spread {
   uint32_t n_groups;
 };
 
+// Fences (grove_set_fences; kernels in fence.cuh), read only by the kFence instantiations.  The picks are ranges of sorted nodes
+// (a level-l domain is contiguous), sorted by their first node; a fencing gang without a pick has lo = hi = kFull (last).
+struct Fence {
+  const uint4* list;        // [n] lo, hi, rank, gang of the fencing gang
+  const uint32_t* slot;     // [G] entry of `list` of a fencing gang, kFull = none
+  uint32_t n;
+};
+
 // Relaxation state.  A gang's tentative result ("cur") lives in its own slots of the entry arrays and becomes final
 // in place; "nxt" is the scratch an evaluation writes before k_apply compares and publishes it.
 struct Relax {
@@ -185,7 +193,22 @@ struct Relax {
   uint16_t* wide_meta;      // [k_eval CTAs * kEvalWarps][wide_cap] clique_rel
   uint32_t wide_cap;        // pods of the largest gang
   Spread sp;                // topology spread (the kSpread instantiations of k_eval / k_apply / k_detect)
+  Fence fc;                 // fences (the kFence instantiations of k_eval / k_apply)
 };
+
+// Is sorted node n inside a fence that is active for the evaluating gang?  m0 / m1: bit j of the 64 entries of `fc.list` is set
+// when entry j belongs to a gang ranked before it that is tentatively REJECTED.  Entries are disjoint and sorted by lo.
+__device__ __forceinline__ bool fenced(const Fence& fc, uint32_t m0, uint32_t m1, uint32_t n) {
+  if (!(m0 | m1)) return false;
+  uint32_t lo = 0, hi = fc.n;   // -> the first entry that starts after n
+  while (lo < hi) {
+    const uint32_t m = (lo + hi) >> 1;
+    if (__ldg(&fc.list[m].x) <= n) lo = m + 1; else hi = m;
+  }
+  if (lo == 0) return false;
+  const uint32_t j = lo - 1;
+  return n < __ldg(&fc.list[j].y) && (((j < 32 ? m0 : m1) >> (j & 31u)) & 1u);
+}
 
 __device__ __forceinline__ uint32_t warp_incl_scan(uint32_t v, uint32_t lane) {
 #pragma unroll

@@ -101,6 +101,35 @@ __device__ __forceinline__ uint4 diag_view(const uint4* nres, DiagUse u, uint32_
   return r;
 }
 
+// the level-`level` domain of sorted node n (GROVE_LEVEL_NONE: the whole cluster is domain 0)
+__device__ __forceinline__ uint32_t diag_domain(const Topo& tp, uint32_t n, uint32_t level) {
+  if (level == GROVE_LEVEL_NONE) return 0;
+  const uint4 dm = tp.ndom[n];
+  return level == 0 ? dm.x : level == 1 ? dm.y : level == 2 ? dm.z : dm.w;
+}
+
+// K1 fit of clique q on a node with record r, exactly (k_diag_fit's predicates and capacity; k_diag_fit keeps its own copy of
+// them: written through this function it needs 32 registers instead of 30): 0 = fits, 1..7 = the first predicate it fails (the order of
+// grove_clique_diag_t), and the pods that fit (cap, left 0 unless it fits), by integer division with no 255 cap
+__device__ __forceinline__ uint32_t diag_fit(const uint4& r, const grove_clique_t& q, uint32_t need_depth, uint32_t& cap) {
+  const uint32_t gpu = r.z & 0xFFFFu, pods = r.z >> 16, depth = (r.w >> 16) & 0xFu, cls = (r.w >> GROVE_NODE_CLASS_SHIFT) & 0xFu;
+  uint32_t cat;
+  if (!(r.w & GROVE_NODE_SCHEDULABLE)) cat = 1;
+  else if (!((q.class_mask >> cls) & 1u)) cat = 2;
+  else if (depth < need_depth) cat = 3;
+  else if (r.x < q.req_cpu_milli) cat = 4;
+  else if (r.y < q.req_mem_mib) cat = 5;
+  else if (gpu < q.req_gpu) cat = 6;
+  else if (pods < 1) cat = 7;
+  else {
+    cat = 0; cap = pods;
+    if (q.req_cpu_milli) cap = min(cap, r.x / q.req_cpu_milli);
+    if (q.req_mem_mib) cap = min(cap, r.y / q.req_mem_mib);
+    if (q.req_gpu) cap = min(cap, gpu / q.req_gpu);
+  }
+  return cat;
+}
+
 // grid = (npad / 256 node tiles, gangs of the batch).  Per clique of the gang: the node's failure class (0 = fits, 1..7 = the
 // first predicate it fails, in the order of grove_clique_diag_t) counted with one ballot per class, the exact capacity summed
 // over the warp into pods_fit, and -- for cliques with MinReplicas > 0 -- over the lanes that share the node's level-l domain
@@ -126,7 +155,7 @@ __global__ void __launch_bounds__(256) k_diag_fit(Topo tp, Tables tb, DiagUse us
     const uint32_t qi = g.clique_off + c;
     const grove_clique_t q = tb.cliques[qi];
     uint32_t cat = 8, cap = 0;   // 8: padding node, counted nowhere
-    if (valid) {
+    if (valid) {   // (diag_fit above restates this chain for fence.cuh: a change here goes there too)
       if (!(r.w & GROVE_NODE_SCHEDULABLE)) cat = 1;
       else if (!((q.class_mask >> cls) & 1u)) cat = 2;
       else if (depth < tb.cinfo[qi].need_depth) cat = 3;

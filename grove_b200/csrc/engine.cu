@@ -236,7 +236,7 @@ struct grove_engine {
   DevBuf<uint8_t> d_rc_gone;
   // grove_diagnose (diagnose.cuh): whether the outputs on the device describe an ordinary cycle over the current inputs, the
   // per-node usage lists, the batch descriptors, the per-domain capacity sums and the records
-  enum Diag : uint8_t { kDiagNoCycle, kDiagReady, kDiagRunning, kDiagChanged, kDiagSpread } diag = kDiagNoCycle;
+  enum Diag : uint8_t { kDiagNoCycle, kDiagReady, kDiagRunning, kDiagChanged, kDiagSpread, kDiagFence } diag = kDiagNoCycle;
   DevBuf<uint32_t> d_dg_cnt, d_dg_off, d_dg_cur, d_dg_minr;
   DevBuf<uint4> d_dg_rec;
   DevBuf<DiagGang> d_dg_gang;
@@ -250,6 +250,12 @@ struct grove_engine {
   DevBuf<uint32_t> d_sp_allowed, d_sp_stamp;
   DevBuf<uint8_t> d_sp_skewed;
   PinBuf<uint8_t> h_sp_skewed;
+  // fences (grove_set_fences; fence.cuh): the fencing gangs of the current submission in rank order; the fence kernels run only
+  // while there are some
+  std::vector<uint32_t> fc_gangs, fc_off;   // (fc_off: first word of each gang's per-clique, per-domain sums; fc_words in all.  The
+  size_t fc_words = 0;                      // labels, hence the domains, cannot change while the set is kept)
+  DevBuf<uint32_t> d_fc_gang, d_fc_off, d_fc_have, d_fc_slot;
+  DevBuf<uint4> d_fc_list;
 };
 
 
@@ -265,6 +271,10 @@ struct grove_engine {
 static int32_t fail(grove_engine* e, int32_t code, const char* msg) { e->err = msg; return code; }
 static int32_t refuse_spread(grove_engine* e, const char* entry) {
   e->err = std::string(entry) + ": not supported while a topology spread set with members is in place (grove_set_spread)";
+  return GROVE_ERR_STATE;
+}
+static int32_t refuse_fences(grove_engine* e, const char* entry) {
+  e->err = std::string(entry) + ": not supported while a fence set is in place (grove_set_fences)";
   return GROVE_ERR_STATE;
 }
 static int32_t refuse_wide(grove_engine* e, const char* entry) {
@@ -432,6 +442,7 @@ static Relax make_relax(grove_engine* e) {
     for (uint32_t l = 0; l < GROVE_MAX_LEVELS; ++l) sp.dcls_off[l] = e->sp_dcls_off[l];
     sp.allowed = e->d_sp_allowed.p; sp.stamp = e->d_sp_stamp.p; sp.skewed = e->d_sp_skewed.p; sp.n_groups = e->sp_groups;
   }
+  if (!e->fc_gangs.empty()) { r.fc.list = e->d_fc_list.p; r.fc.slot = e->d_fc_slot.p; r.fc.n = uint32_t(e->fc_gangs.size()); }
   return r;
 }
 
@@ -509,8 +520,9 @@ void grove_engine_destroy(grove_engine_t* e) {
 static int32_t load_nodes_common(grove_engine* e, const grove_node_t* host_nodes, const void* dev_nodes, uint32_t n) {
   if (n == 0 || n > GROVE_MAX_NODES) return fail(e, GROVE_ERR_INVALID_ARG, "node count out of range");
   if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
-  if (e->diag == grove_engine::kDiagReady || e->diag == grove_engine::kDiagSpread) e->diag = grove_engine::kDiagChanged;
+  if (e->diag == grove_engine::kDiagReady || e->diag == grove_engine::kDiagSpread || e->diag == grove_engine::kDiagFence) e->diag = grove_engine::kDiagChanged;
   e->sp_groups = e->sp_members = 0;   // a spread set belongs to the nodes and gangs it was validated against
+  e->fc_gangs.clear();                // (a fence set too)
   CU_TRY(e, cudaSetDevice(e->cfg.device));
   if (host_nodes) {
     CU_TRY(e, cudaEventSynchronize(e->ev_nodes_up));  // an earlier upload may still be reading the staging buffer
@@ -562,7 +574,7 @@ int32_t grove_update_nodes(grove_engine_t* e, const uint32_t* idx, const grove_n
   if (!e || (n && (!idx || !recs))) return GROVE_ERR_INVALID_ARG;
   if (!e->nodes_loaded) return fail(e, GROVE_ERR_STATE, "no node snapshot loaded");
   if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
-  if (e->diag == grove_engine::kDiagReady || e->diag == grove_engine::kDiagSpread) e->diag = grove_engine::kDiagChanged;
+  if (e->diag == grove_engine::kDiagReady || e->diag == grove_engine::kDiagSpread || e->diag == grove_engine::kDiagFence) e->diag = grove_engine::kDiagChanged;
   if (n == 0) return GROVE_OK;
   e->score_pass_valid = false;
   CU_TRY(e, cudaSetDevice(e->cfg.device));
@@ -665,9 +677,10 @@ static int32_t validate(grove_engine* e, const grove_gang_t* gangs, uint32_t G, 
 static int32_t submit(grove_engine* e, const grove_gang_t* gangs, uint32_t n_gangs, const grove_clique_t* cliques,
                       const std::vector<uint32_t>& ccount, uint32_t n_cliques, const grove_scope_t* scopes, uint32_t n_scopes, uint32_t max_pods) {
   if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
-  if (e->diag == grove_engine::kDiagReady || e->diag == grove_engine::kDiagSpread) e->diag = grove_engine::kDiagChanged;
+  if (e->diag == grove_engine::kDiagReady || e->diag == grove_engine::kDiagSpread || e->diag == grove_engine::kDiagFence) e->diag = grove_engine::kDiagChanged;
   if (n_gangs >= (1u << 24)) return fail(e, GROVE_ERR_LIMIT, "too many gangs");  // order rank + round tag share a stamp word
   e->sp_groups = e->sp_members = 0;
+  e->fc_gangs.clear();
   int32_t rc = validate(e, gangs, n_gangs, cliques, ccount.data(), n_cliques, scopes, n_scopes, max_pods);
   if (rc) return rc;
   CU_TRY(e, cudaSetDevice(e->cfg.device));
@@ -1058,6 +1071,10 @@ static int32_t cycle_begin(grove_engine* e) {
     CU_TRY(e, e->d_sp_cnt.ensure(std::max<uint32_t>(e->sp_cnt_words, 1))); CU_TRY(e, e->d_sp_dcls.ensure(std::max<uint32_t>(e->sp_dcls_words, 1)));
     CU_TRY(e, e->d_sp_stamp.ensure(std::max<uint32_t>(e->sp_groups, 1))); CU_TRY(e, e->d_sp_skewed.ensure(g1)); CU_TRY(e, e->h_sp_skewed.ensure(g1));
   }
+  if (!e->fc_gangs.empty()) {   // the fence set's buffers (make_relax hands their pointers to every kernel of the cycle)
+    const size_t nf = e->fc_gangs.size();
+    CU_TRY(e, e->d_fc_gang.ensure(nf)); CU_TRY(e, e->d_fc_off.ensure(nf)); CU_TRY(e, e->d_fc_list.ensure(nf)); CU_TRY(e, e->d_fc_slot.ensure(g1));
+  }
   if (e->dbg_on) { CU_TRY(e, e->d_dbg.ensure(g1 * 8 + 8)); CU_TRY(e, cudaMemsetAsync(e->d_dbg.p, 0, g1 * 32 + 32, e->stream)); }
   {
     const uint32_t W = e->tune_window ? e->tune_window : std::max(G, 1u);
@@ -1085,6 +1102,11 @@ static int32_t finish_cycle(grove_engine* e) {
     k_emit<<<(G * 32 + 255) / 256, 256, 0, e->stream>>>(tb, rx, e->d_perm.p, e->d_status.p, e->d_out.p, e->d_scope_status.p);
     CU_TRY(e, cudaGetLastError());
     e->launches += 4;
+    if (!e->fc_gangs.empty()) {   // the flag, level and domain of the rejected gangs whose fence held
+      k_fence_status<<<1, GROVE_MAX_FENCES, 0, e->stream>>>(tb, rx, e->d_perm.p, e->d_status.p);
+      CU_TRY(e, cudaGetLastError());
+      e->launches += 1;
+    }
     CU_TRY(e, cudaMemcpyAsync(e->h_ctl.p, e->d_totals.p, sizeof(uint32_t) * 4, cudaMemcpyDeviceToHost, e->stream));
     CU_TRY(e, cudaMemcpyAsync(e->h_status.p, e->d_status.p, sizeof(grove_gang_status_t) * G, cudaMemcpyDeviceToHost, e->stream));
     // the placement count is only known on the device: copy the upper bound's worth in the same breath when it is small,
@@ -1131,6 +1153,19 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
     CU_TRY(e, cudaGetLastError());
     e->launches += 1;
   }
+  const bool fences = !e->fc_gangs.empty();   // (the running-gang entries and spread cycles refuse a fence set)
+  if (G && fences) {   // the picks, over the cycle-start table
+    const uint32_t nf = uint32_t(e->fc_gangs.size());
+    CU_TRY(e, e->d_fc_have.ensure(std::max<size_t>(e->fc_words, 1)));
+    CU_TRY(e, cudaMemcpyAsync(e->d_fc_gang.p, e->fc_gangs.data(), sizeof(uint32_t) * nf, cudaMemcpyHostToDevice, e->stream));
+    CU_TRY(e, cudaMemcpyAsync(e->d_fc_off.p, e->fc_off.data(), sizeof(uint32_t) * nf, cudaMemcpyHostToDevice, e->stream));
+    CU_TRY(e, cudaMemsetAsync(e->d_fc_have.p, 0, sizeof(uint32_t) * e->fc_words, e->stream));
+    CU_TRY(e, cudaMemsetAsync(e->d_fc_slot.p, 0xFF, sizeof(uint32_t) * G, e->stream));
+    k_fence_have<<<dim3(e->Npad / 256, nf), 256, 0, e->stream>>>(tp, tb, e->d_fc_gang.p, e->d_fc_off.p, e->d_fc_have.p);
+    k_fence_pick<<<1, 1024, 0, e->stream>>>(tp, tb, e->d_fc_gang.p, e->d_fc_off.p, e->d_fc_have.p, nf, e->d_fc_list.p, e->d_fc_slot.p);
+    CU_TRY(e, cudaGetLastError());
+    e->launches += 2;
+  }
   if (G) {
     // K1 + capacity tables over the cycle-start snapshot; K2 (score matrix) forks to the second stream
     CU_TRY(e, cudaEventRecord(e->ev[0], e->stream));
@@ -1173,6 +1208,15 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
         CU_TRY(e, launch_chained(k_apply<false, true>, warp_ctas, 256, e->stream, tb, rx));
         CU_TRY(e, launch_chained(k_detect<true>, warp_ctas, 256, e->stream, tp, tb, rx, e->tune_refresh));
         e->launches += 4;
+        ++next_round;
+        return GROVE_OK;
+      }
+      if (fences) {   // a fenced cycle: its own instantiations of K3 and k_apply
+        CU_TRY(e, launch_chained(e->any_preferred ? k_eval<true, false, false, false, true> : k_eval<false, false, false, false, true>,
+                                 n_eval_ctas, kEvalWarps * 32, e->stream, tp, tb, rx, e->tune_max_att));
+        CU_TRY(e, launch_chained(k_apply<false, false, true>, warp_ctas, 256, e->stream, tb, rx));
+        CU_TRY(e, launch_chained(k_detect<false>, warp_ctas, 256, e->stream, tp, tb, rx, e->tune_refresh));
+        e->launches += 3;
         ++next_round;
         return GROVE_OK;
       }
@@ -1315,9 +1359,10 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
 
 int32_t grove_run_cycle(grove_engine_t* e, grove_cycle_stats_t* stats) {
   if (!e) return GROVE_ERR_INVALID_ARG;
-  const bool spread = e->sp_members > 0;
+  const bool spread = e->sp_members > 0, fences = !e->fc_gangs.empty();
+  if (spread && fences) return fail(e, GROVE_ERR_STATE, "grove_run_cycle: a spread set with members and a fence set together are not supported");
   const int32_t rc = run_cycle(e, stats);
-  if (rc == GROVE_OK) e->diag = spread ? grove_engine::kDiagSpread : grove_engine::kDiagReady;
+  if (rc == GROVE_OK) e->diag = spread ? grove_engine::kDiagSpread : fences ? grove_engine::kDiagFence : grove_engine::kDiagReady;
   return rc;
 }
 
@@ -1445,6 +1490,40 @@ int32_t grove_set_spread(grove_engine_t* e, const grove_spread_t* groups, uint32
 }
 
 // ---------------------------------------------------------------------------------------------
+// Fences (include/grove_place.h "fences"; DESIGN.md section 1; kernels in fence.cuh).  Validated against the submission; the
+// cycle makes the picks and runs the kFence instantiations.
+// ---------------------------------------------------------------------------------------------
+int32_t grove_set_fences(grove_engine_t* e, const uint32_t* gangs, uint32_t n) {
+  if (!e) return GROVE_ERR_INVALID_ARG;
+  if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
+  if (!e->nodes_loaded || !e->gangs_loaded) return fail(e, GROVE_ERR_STATE, "grove_set_fences: load nodes and submit gangs first");
+  if (n && !gangs) return GROVE_ERR_INVALID_ARG;
+  if (n > GROVE_MAX_FENCES) return fail(e, GROVE_ERR_LIMIT, "grove_set_fences: more than GROVE_MAX_FENCES fencing gangs");
+  if (e->wide) return refuse_wide(e, "grove_set_fences");
+  std::vector<uint32_t> v(gangs, gangs + n);
+  for (uint32_t k = 0; k < n; ++k) {
+    if (v[k] >= e->G) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_fences: gang index out of range");
+    if (e->gangs[v[k]].level == GROVE_LEVEL_NONE) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_fences: a fencing gang needs a gang Required level");
+  }
+  std::vector<uint32_t> sorted(v);
+  std::sort(sorted.begin(), sorted.end());
+  if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end()) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_fences: a gang is named twice");
+  std::stable_sort(v.begin(), v.end(), [e](uint32_t a, uint32_t b) {   // rank order: priority desc, index asc
+    return e->gangs[a].priority != e->gangs[b].priority ? e->gangs[a].priority > e->gangs[b].priority : a < b;
+  });
+  std::vector<uint32_t> off(n);
+  size_t words = 0;
+  for (uint32_t k = 0; k < n; ++k) {
+    const grove_gang_t& gg = e->gangs[v[k]];
+    off[k] = uint32_t(words); words += size_t(gg.n_cliques) * e->n_dom[gg.level];
+  }
+  if (words > (size_t(1) << 28))
+    return fail(e, GROVE_ERR_LIMIT, "grove_set_fences: the per-domain sums (fencing gangs x cliques x domains of their level) exceed 1 GB");
+  e->fc_gangs = std::move(v); e->fc_off = std::move(off); e->fc_words = words;
+  return GROVE_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
 // Diagnosis (include/grove_place.h "diagnosis of rejected gangs"; DESIGN.md section 1; kernels in diagnose.cuh).  Reads the
 // outputs of the last ordinary cycle on the device (committed table, placements, ranks) and writes only its own buffers.
 // ---------------------------------------------------------------------------------------------
@@ -1461,6 +1540,8 @@ int32_t grove_diagnose(grove_engine_t* e, grove_gang_diag_t* gangs, uint32_t cap
       return fail(e, GROVE_ERR_STATE, "grove_diagnose: the last cycle ran with running gangs (preempt / reuse); only grove_run_cycle is diagnosed");
     case grove_engine::kDiagSpread:
       return fail(e, GROVE_ERR_STATE, "grove_diagnose: the last cycle had topology spread members, which the diagnosis does not model");
+    case grove_engine::kDiagFence:
+      return fail(e, GROVE_ERR_STATE, "grove_diagnose: the last cycle had fences, which the diagnosis does not model");
     default: return fail(e, GROVE_ERR_STATE, "grove_diagnose: nodes or gangs were loaded, updated or submitted since the last cycle");
   }
   const uint32_t G = e->G, Q = e->Q;
@@ -1568,6 +1649,7 @@ int32_t grove_run_cycle_preempt(grove_engine_t* e, const grove_running_gang_t* r
                                 const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
   if (!e || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
   if (e->sp_members) return refuse_spread(e, "grove_run_cycle_preempt");
+  if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_preempt");
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_preempt");
   for (uint32_t r = 0; r < n_running; ++r)
@@ -1823,6 +1905,7 @@ int32_t grove_run_cycle_reuse(grove_engine_t* e, const uint32_t* replaces, uint3
                               uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
   if (!e || (n_gangs && !replaces) || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
   if (e->sp_members) return refuse_spread(e, "grove_run_cycle_reuse");
+  if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_reuse");
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse");
   const int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);
@@ -1842,6 +1925,7 @@ int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replace
                                       uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
   if (!e || (n_gangs && !replaces) || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
   if (e->sp_members) return refuse_spread(e, "grove_run_cycle_reuse_preempt");
+  if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_reuse_preempt");
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse_preempt");
   int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);

@@ -262,7 +262,15 @@ Err CheckPodSchedulingGate(bool podHasGate, bool podListedInPodGang, const std::
 Err GpuBackend::OnPodGangDelete(const PodGang& podGang) {
   std::lock_guard<std::mutex> l(mu_);
   const std::string key = podGang.Namespace + "/" + podGang.Name;
-  pending_.erase(key); bound_.erase(key); running_.erase(key); setOf_.erase(key);
+  pending_.erase(key); bound_.erase(key); running_.erase(key); setOf_.erase(key); rejectedFor_.erase(key);
+  return std::nullopt;
+}
+
+Err GpuBackend::SetStarvationGuard(uint32_t afterCycles, uint32_t maxGangs) {
+  std::lock_guard<std::mutex> l(mu_);
+  if (afterCycles < 1) return mkerr("ERR_SYNC_PODGANG", "SetStarvationGuard", "afterCycles must be at least 1");
+  if (maxGangs > GROVE_MAX_FENCES) return mkerr("ERR_SYNC_PODGANG", "SetStarvationGuard", "maxGangs exceeds GROVE_MAX_FENCES");
+  guardAfter_ = afterCycles; guardMax_ = maxGangs;
   return std::nullopt;
 }
 
@@ -547,10 +555,13 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
   Tables t;
   std::map<std::string, PodGang> snap;            // the PodGangs of this pass: reconcilers may add / delete others meanwhile
   bool large = false, explain = false;
+  uint32_t guardAfter = 1, guardMax = 0;
+  std::map<std::string, uint32_t> rejectedFor;
   std::vector<TopologyLevel> levels;
   {
     std::lock_guard<std::mutex> l(mu_);
     large = large_; explain = explain_; levels = levels_;
+    guardAfter = guardAfter_; guardMax = guardMax_; rejectedFor = rejectedFor_;
     if (pending_.empty()) return std::nullopt;
     if (auto e = Init()) return e;
     if (!engine_) return mkerr("ERR_SYNC_PODGANG", "RunCycle", "no ClusterTopology synced");
@@ -613,6 +624,30 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
       reuse = std::any_of(replaces.begin(), replaces.end(), [](uint32_t r) { return r != GROVE_NONE_U32; });
     }
   }
+  // the starvation guard: the highest-ranked rows (priority desc, row asc = the engine's rank) of the PodGangs rejected often
+  // enough, in an ordinary pass only
+  std::vector<uint32_t> fences;
+  if (guardMax && !both && !reuse && !preempt && !spread) {
+    bool wide = false;   // a row beyond the ordinary limits makes the submission wide, which takes no fence set
+    for (const grove_gang_t& g : t.gangs) {
+      uint32_t pods = 0;
+      for (uint32_t c = g.clique_off; c < g.clique_off + g.n_cliques; ++c) {
+        const uint32_t rep = large ? t.counts[c].replicas : t.cliques[c].replicas;
+        pods += rep; wide |= rep > 255u;
+      }
+      wide |= pods > GROVE_MAX_GANG_PODS;
+    }
+    std::vector<uint32_t> rows;
+    for (uint32_t g = 0; g < t.gangs.size() && !wide; ++g) {
+      auto it = rejectedFor.find(t.gangNames[g]);
+      if (!t.remainder[g] && t.gangs[g].level != GROVE_LEVEL_NONE && it != rejectedFor.end() && it->second >= guardAfter) rows.push_back(g);
+    }
+    std::stable_sort(rows.begin(), rows.end(), [&](uint32_t a, uint32_t b) { return t.gangs[a].priority > t.gangs[b].priority; });
+    if (rows.size() > guardMax) rows.resize(guardMax);
+    fences = rows;
+    if (!fences.empty())
+      if (auto e = chk(grove_set_fences(engine_, fences.data(), uint32_t(fences.size())), "grove_set_fences")) return e;
+  }
   if (both) { if (auto e = chk(grove_run_cycle_reuse_preempt(engine_, replaces.data(), uint32_t(replaces.size()), run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_reuse_preempt")) return e; }
   else if (reuse) { if (auto e = chk(grove_run_cycle_reuse(engine_, replaces.data(), uint32_t(replaces.size()), run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_reuse")) return e; }
   else if (preempt) { if (auto e = chk(grove_run_cycle_preempt(engine_, run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_preempt")) return e; }
@@ -673,6 +708,16 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
           (*statuses)[t.gangNames[g]].ScheduledMessage = ExplainRejection(t, snap.at(t.gangNames[g]), g, gd[g], qd.data(), levels);
   }
   for (const auto& [key, msg] : spreadMsg) (*statuses)[key].ScheduledMessage = msg;
+  // the starvation guard's fences that held: the domain the PodGang keeps the PodGangs ranked after it out of
+  for (uint32_t g : fences) {
+    if (!(gs[g].reserved0 & GROVE_STATUS_FENCING) || gs[g].level >= levels.size()) continue;
+    const TopologyLevel& lv = levels[gs[g].level];
+    auto lab = nodes[gs[g].domain_node].Labels.find(lv.Key);
+    (*statuses)[t.gangNames[g]].ScheduledMessage =
+        "Unschedulable for " + std::to_string(rejectedFor.at(t.gangNames[g]) + 1) + " cycles in a row: " + lv.Domain + " " +
+        (lab == nodes[gs[g].domain_node].Labels.end() ? std::string("?") : lab->second) +
+        " is held for this PodGang; PodGangs ranked after it are kept out of it until it is scheduled";
+  }
   // a scheduled PodGang leaves the pending set once every PodReference is bound; until then its unbound pods are retried
   // as a remainder (Encode).  Remember where gangs landed for ReuseReservationRef hints.
   auto constrained = [](const PodGang& pg) {
@@ -683,6 +728,12 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
     return false;
   };
   std::lock_guard<std::mutex> l(mu_);
+  // the starvation guard's counts: consecutive Unschedulable cycles; a gated or base-not-scheduled cycle changes nothing
+  for (uint32_t g = 0; g < gs.size(); ++g) {
+    if (t.remainder[g] || !pending_.count(t.gangNames[g])) continue;
+    if (gs[g].state == GROVE_GANG_REJECTED) ++rejectedFor_[t.gangNames[g]];
+    else if (gs[g].state == GROVE_GANG_ADMITTED) rejectedFor_.erase(t.gangNames[g]);
+  }
   if (preempt) {   // victims: DisruptionTarget on the PodGang (podgang.go:166-170), forgotten as running
     uint32_t nv = 0;
     if (auto e = chk(grove_get_victims(engine_, nullptr, 0, &nv), "grove_get_victims")) return e;

@@ -291,6 +291,15 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   // ordinary limits (SetLargePodGangs), members stay out of the pass, Unschedulable with a reason.  nullopt removes the set's
   // spread.  Off by default (no set has one).
   Err SetTopologySpread(const std::string& pcsName, std::optional<TopologySpread> spread);
+  // Starvation guard (grove_set_fences; DESIGN.md section 1 "Fences"): counts, per pending PodGang, the consecutive cycles it came
+  // back Unschedulable (REJECTED; a gated or base-not-scheduled cycle neither counts nor resets, a scheduled one resets).  Each
+  // cycle the <= maxGangs highest-ranked PodGangs with a Required level that were rejected at least afterCycles times fence a
+  // domain: while one of them stays rejected, the PodGangs ranked after it are kept out of the domain of its Required level that
+  // was closest to fitting it, so that the nodes freed there accumulate for it.  A fencing PodGang's ScheduledMessage names the
+  // level and the label value of that domain.  In a pass with preemption, reservation reuse or topology spread members, or with a
+  // PodGang beyond the ordinary limits (SetLargePodGangs), nothing is fenced (the counts go on).  maxGangs = 0 turns it off (the
+  // default); afterCycles >= 1, maxGangs <= GROVE_MAX_FENCES.
+  Err SetStarvationGuard(uint32_t afterCycles, uint32_t maxGangs);
   static constexpr const char* kPartOfLabel = "app.kubernetes.io/part-of";
   size_t Running() const { std::lock_guard<std::mutex> l(mu_); return running_.size(); }
   // why a PodGang cannot be handed to the engine (limits of the packed tables), or empty.  SyncPodGang accepts every
@@ -326,6 +335,8 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   bool reclaimReuse_ = false;
   bool large_ = false;
   bool explain_ = false;
+  uint32_t guardAfter_ = 1, guardMax_ = 0;             // starvation guard (off: guardMax_ == 0)
+  std::map<std::string, uint32_t> rejectedFor_;        // pending PodGang -> consecutive Unschedulable cycles
   std::map<std::string, TopologySpread> spread_;       // PodCliqueSet name -> its spread
   std::map<std::string, std::string> setOf_;           // scheduled base PodGang -> "<ns>/<PodCliqueSet>" (its part-of label)
   grove_engine_t* engine_ = nullptr;

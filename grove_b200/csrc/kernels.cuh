@@ -10,6 +10,7 @@
 //   reclaim.cuh  k_reclaim_*  reclaim-class views over the running gangs' holdings (grove_run_cycle_reuse_preempt)
 //   diagnose.cuh k_diag_*  why each rejected gang did not fit, after the cycle (grove_diagnose)
 //   spread.cuh   k_spread_classes / k_spread  allowed level-l_s domains of the topology spread members (grove_set_spread)
+//   fence.cuh    k_fence_have / k_fence_pick / k_fence_status  the domain each fencing gang fences (grove_set_fences)
 //
 // Semantics are DESIGN.md "Placement semantics"; the reference contract they restate is cited in
 // include/grove_place.h.  Integer / compare work only: no tensor cores, no floating point.
@@ -23,3 +24,4 @@
 #include "reclaim.cuh"
 #include "diagnose.cuh"
 #include "spread.cuh"
+#include "fence.cuh"

@@ -206,8 +206,8 @@ __global__ void __launch_bounds__(256) k_hold_release(Tables tb, Relax rx, uint4
 }
 
 // one warp per evaluated gang: publish a changed result (kHolds: a cycle with holds; kSpread: a cycle with spread members, whose
-// changed results leave a stamp per group)
-template <bool kHolds, bool kSpread = false>
+// changed results leave a stamp per group; kFence: a cycle with fences, whose gangs' flips to or from REJECTED stamp their fence)
+template <bool kHolds, bool kSpread = false, bool kFence = false>
 __global__ void __launch_bounds__(256) k_apply(Tables tb, Relax rx) {
   cudaGridDependencySynchronize();   // (launched chained: engine.cu launch_chained)
   const uint32_t lane = threadIdx.x & 31;
@@ -246,6 +246,20 @@ __global__ void __launch_bounds__(256) k_apply(Tables tb, Relax rx) {
     if constexpr (kSpread) {   // dirty rule (d): the members of its group ranked after it
       const uint32_t s = rx.sp.group[g];
       if (lane == 0 && s != kFull) atomicMin(rx.sp.stamp + s, stamp);
+    }
+    if constexpr (kFence) {   // a fence that turns on is a claim added on every node of its range (dirty rule (a)); one that turns
+                              // off is a withdrawal from every word of it (rule (b), and K3's skip of the candidates that failed)
+      const uint32_t j = rx.fc.slot[g];
+      const bool was = ot == GROVE_GANG_REJECTED, now = nt == GROVE_GANG_REJECTED;
+      const uint4 f = j != kFull ? rx.fc.list[j] : make_uint4(kFull, kFull, 0u, 0u);
+      if (f.x != kFull && was != now) {
+        if (now) {
+          for (uint32_t n = f.x + lane; n < f.y; n += 32) atomicMin(rx.add_stamp + n, stamp);
+        } else {
+          for (uint32_t w = (f.x >> 5) + lane; w <= (f.y - 1u) >> 5; w += 32) { atomicMin(rx.rem_stamp + w, stamp); atomicMax(rx.rem_round + w, round); }
+          if (lane == 0) atomicMin(rx.ctl + kRemAny, stamp);
+        }
+      }
     }
     const bool owner = kHolds && has_hold(rx, g);   // its claims are what its placement needs beyond its hold
     // withdraw the old claims

@@ -25,7 +25,7 @@ SYMBOLS = [
     "grove_load_nodes", "grove_update_nodes", "grove_get_nodes", "grove_submit_gangs", "grove_submit_gangs_wide", "grove_run_cycle",
     "grove_get_placements", "grove_get_gang_status", "grove_get_scope_domains", "grove_load_nodes_device",
     "grove_build_score_matrix", "grove_run_cycle_preempt", "grove_get_victims", "grove_run_cycle_reuse",
-    "grove_run_cycle_reuse_preempt", "grove_diagnose", "grove_set_spread",
+    "grove_run_cycle_reuse_preempt", "grove_diagnose", "grove_set_spread", "grove_set_fences",
     "grove_shard_range", "grove_run_score_pass", "grove_shard_summary_device",
     "grove_debug_get_perm", "grove_debug_get_fit_row", "grove_debug_get_score_row",
 ]
@@ -147,6 +147,14 @@ class PlacementEngine:
         seeds = np.ascontiguousarray(np.zeros(0, dtype=T.spread_seed_dt) if seeds is None else seeds, dtype=T.spread_seed_dt)
         self._check(self.lib.grove_set_spread(self.h, _p(groups), C.c_uint32(len(groups)), _p(gang_group), C.c_uint32(len(gang_group)),
                                               _p(seeds), C.c_uint32(len(seeds))))
+
+    def set_fences(self, gangs):
+        """grove_set_fences: the fencing gangs of the current submission (at most tables.MAX_FENCES, each with a gang Required
+        level).  While one of them is REJECTED, the gangs ranked after it see the domain it picked at cycle start as unschedulable;
+        its status then carries tables.STATUS_FENCING with that domain.  Call after submit_gangs; the next submit / load_nodes
+        clears it (include/grove_place.h "fences")."""
+        gangs = np.ascontiguousarray(gangs, dtype=np.uint32)
+        self._check(self.lib.grove_set_fences(self.h, _p(gangs), C.c_uint32(len(gangs))))
 
     # ---- the cycle ----
     def run_cycle(self) -> dict:

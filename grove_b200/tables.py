@@ -78,6 +78,10 @@ STATUS_SPREAD_SKEWED = 0x2        # status reserved0: a SOFT member placed outsi
 spread_dt = np.dtype([("level", "u1"), ("mode", "u1"), ("max_skew", "<u2"), ("reserved", "<u4")])
 spread_seed_dt = np.dtype([("group", "<u4"), ("node", "<u4")])
 
+# fences (grove_set_fences, include/grove_place.h "fences")
+MAX_FENCES = 64
+STATUS_FENCING = 0x4              # status reserved0: a REJECTED gang whose fence held (level, domain_node name the fenced domain)
+
 assert node_dt.itemsize == 32 and clique_dt.itemsize == 16 and scope_dt.itemsize == 8
 assert gang_dt.itemsize == 32 and placement_dt.itemsize == 8 and status_dt.itemsize == 32 and scope_status_dt.itemsize == 8
 assert config_dt.itemsize == 32 and stats_dt.itemsize == 64

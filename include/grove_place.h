@@ -149,7 +149,8 @@ typedef struct grove_gang_status {
   uint8_t level;           /* level of the domain the whole gang was packed into (its Required level, or the deeper
                               Preferred level that held), GROVE_LEVEL_NONE = the whole cluster / not admitted */
   uint16_t reserved0;      /* flags: GROVE_STATUS_PREEMPTOR = admitted by the reclaim pass of grove_run_cycle_preempt,
-                              GROVE_STATUS_SPREAD_SKEWED = a SOFT spread member placed outside its allowed domains; else 0 */
+                              GROVE_STATUS_SPREAD_SKEWED = a SOFT spread member placed outside its allowed domains,
+                              GROVE_STATUS_FENCING = a REJECTED fencing gang whose fence held (grove_set_fences); else 0 */
   uint16_t score_num;      /* PlacementScore = score_num / score_den (podgang.go:187-189): over the gang, its scopes and
                               its cliques that carry a pack constraint, (levels honoured) / (levels asked for), where
                               asked = Preferred if set else Required; 1/1 when nothing was asked or everything held;
@@ -373,6 +374,33 @@ typedef struct grove_spread_seed {
 int32_t grove_set_spread(grove_engine_t* e, const grove_spread_t* groups, uint32_t n_groups,
                          const uint32_t* gang_group, uint32_t n_gangs,
                          const grove_spread_seed_t* seeds, uint32_t n_seeds);
+
+/* ---- fences -------------------------------------------------------------------------------------------
+ * A rejected gang keeps the gangs ranked after it out of the domain closest to fitting it, so that a large gang is not starved
+ * by smaller ones that take every node freed (DESIGN.md section 1, "Fences"; the backfill-with-reservation of batch schedulers).
+ * `gangs` names the FENCING gangs of the current submission; each has a gang Required level l.  F0 is the node table the cycle
+ * starts from, rank = (priority desc, submission index asc).
+ *   Picks, fixed at cycle start, in rank order: for each level-l domain D (nodes lacking the label are in none) and each clique q
+ *   with MinReplicas > 0, have_q(D) = sum over n in D of min(cap(q, n), MinReplicas_q), cap = grove_diagnose's exact capacity on
+ *   F0 (0 where K1 fit fails); shortfall(D) = sum over q of max(0, MinReplicas_q - have_q(D)).  The gang picks the D of least
+ *   shortfall among the level-l domains that share no node with an earlier pick, ties by its candidate order at level l
+ *   (descending min(closeness(first node, anchor), l + 1), then ascending rotated index); none left: no pick.
+ *   The pass: the sequential pass, except that a gang sees every node of an ACTIVE fence of a gang ranked before it as
+ *   unschedulable (K1 fit fails).  A fence is active when its gang was evaluated and came out REJECTED; an admitted, gated or
+ *   BASE_REJECTED gang fences nothing.
+ *   Outputs: a REJECTED gang with an active fence carries GROVE_STATUS_FENCING in reserved0, level = l and domain_node = the
+ *   caller index of the fenced domain's first node.  Everything else is what the pass gives; fences leave no trace in the node
+ *   table.
+ * Call after grove_submit_gangs and before grove_run_cycle; the next grove_submit_gangs* or grove_load_nodes* clears the set,
+ * grove_update_nodes keeps it.  GROVE_ERR_INVALID_ARG for an index out of range, a duplicate, or a gang without a gang Required
+ * level; GROVE_ERR_LIMIT for more than GROVE_MAX_FENCES gangs, for a wide submission, and when the per-domain sums (fencing gangs x
+ * cliques x domains of their level, 4 B each) would exceed 1 GB; GROVE_ERR_STATE before nodes are loaded and gangs submitted.
+ * While a non-empty set is in place grove_run_cycle_preempt / _reuse / _reuse_preempt return GROVE_ERR_STATE, so does
+ * grove_run_cycle with a spread set with members, and grove_diagnose returns GROVE_ERR_STATE after a fenced cycle.  An empty set
+ * changes nothing. */
+#define GROVE_MAX_FENCES 64u
+#define GROVE_STATUS_FENCING 0x4u       /* grove_gang_status_t.reserved0: a REJECTED gang whose fence held at the end of the cycle */
+int32_t grove_set_fences(grove_engine_t* e, const uint32_t* gangs, uint32_t n);
 
 /* K2: the topology-distance score matrix T[clique][node] = fit ? 1 + levels shared with the gang's anchor : 0 (u8) over the
  * snapshot the last cycle started from -- what a scheduler's Score extension point would hand out.  The admission does

@@ -60,6 +60,9 @@ type schedulerBackend struct {
 	// spread: PodCliqueSet name -> its topology spread (SetTopologySpread); setOf: scheduled base PodGang -> its PodCliqueSet
 	spread map[string]TopologySpread
 	setOf  map[string]string
+	// starvation guard (SetStarvationGuard): off while guardMax == 0; rejectedFor: pending PodGang -> consecutive Unschedulable cycles
+	guardAfter, guardMax int
+	rejectedFor          map[string]int
 	eng                  *engine
 	stopLoop chan struct{}
 }
@@ -208,6 +211,22 @@ func (b *schedulerBackend) OnPodGangDelete(_ context.Context, pg *grovescheduler
 	delete(b.pending, key)
 	delete(b.running, key) // its pods' resources show up as free in the next node snapshot
 	delete(b.setOf, key)
+	delete(b.rejectedFor, key)
+	return nil
+}
+
+// SetStarvationGuard fences, each cycle, the <= maxGangs highest-ranked pending PodGangs with a Required level that came back
+// Unschedulable at least afterCycles cycles in a row (gated or base-not-scheduled cycles neither count nor reset): while one
+// stays rejected, the PodGangs ranked after it are kept out of the domain closest to fitting it (grove_set_fences;
+// GpuBackend::SetStarvationGuard in the C++ mirror).  Nothing is fenced with preemption on, with topology spread members or in a
+// pass with a large PodGang.  maxGangs = 0 turns it off (the default).
+func (b *schedulerBackend) SetStarvationGuard(afterCycles, maxGangs int) error {
+	if afterCycles < 1 || maxGangs < 0 || maxGangs > int(C.GROVE_MAX_FENCES) {
+		return fmt.Errorf("starvation guard: want afterCycles >= 1 and 0 <= maxGangs <= %d", int(C.GROVE_MAX_FENCES))
+	}
+	b.mu.Lock()
+	defer b.mu.Unlock()
+	b.guardAfter, b.guardMax = afterCycles, maxGangs
 	return nil
 }
 
@@ -371,10 +390,48 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 		b.encodeSpread(t, rows, levels, nodeIdx)
 		b.mu.Unlock()
 	}
+	b.mu.Lock()
+	if b.guardMax > 0 && !preempt && !wideAny && len(t.spreadGroups) == 0 { // the starvation guard, in an ordinary pass only
+		cand := []int{}
+		for gi, pg := range rows {
+			if t.gangs[gi].level != C.GROVE_LEVEL_NONE && b.rejectedFor[pg.Namespace+"/"+pg.Name] >= b.guardAfter {
+				cand = append(cand, gi)
+			}
+		}
+		sort.SliceStable(cand, func(i, j int) bool { return t.gangs[cand[i]].priority > t.gangs[cand[j]].priority }) // rank order
+		if len(cand) > b.guardMax {
+			cand = cand[:b.guardMax]
+		}
+		for _, gi := range cand {
+			t.fences = append(t.fences, C.uint32_t(gi))
+		}
+	}
+	rejectedFor := map[string]int{}
+	for k, v := range b.rejectedFor {
+		rejectedFor[k] = v
+	}
+	b.mu.Unlock()
 	res, err := eng.cycle(t, preempt, large, explain)
 	if err != nil {
 		return err
 	}
+	nodeLabels := make(map[string]map[string]string, len(nodeList.Items))
+	for i := range nodeList.Items {
+		nodeLabels[nodeList.Items[i].Name] = nodeList.Items[i].Labels
+	}
+	b.mu.Lock()
+	if b.rejectedFor == nil {
+		b.rejectedFor = map[string]int{}
+	}
+	for gi, st := range res.status { // consecutive Unschedulable cycles; a gated or base-not-scheduled cycle changes nothing
+		key := rows[gi].Namespace + "/" + rows[gi].Name
+		if st.state == C.GROVE_GANG_REJECTED {
+			b.rejectedFor[key]++
+		} else if st.state == C.GROVE_GANG_ADMITTED {
+			delete(b.rejectedFor, key)
+		}
+	}
+	b.mu.Unlock()
 	seen := make([]int, len(t.cliques)) // the r-th entry of a clique binds its r-th PodReference
 	for _, pl := range res.placements {
 		gi, pgi := cliqueOwner(t, int(pl.clique))
@@ -414,6 +471,11 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 			}
 			if len(t.spreadOf) > 0 && t.spreadOf[gi] != C.GROVE_NONE_U32 && t.spreadGroups[t.spreadOf[gi]].mode == C.GROVE_SPREAD_HARD {
 				why = "topology spread (DoNotSchedule): no domain within the skew had room for this replica"
+			}
+			if st.reserved0&C.GROVE_STATUS_FENCING != 0 && int(st.level) < len(levels) { // the starvation guard's fence held
+				key := levels[st.level]
+				why = fmt.Sprintf("Unschedulable for %d cycles in a row: %s %s is held for this PodGang; PodGangs ranked after it are kept out of it until it is scheduled",
+					rejectedFor[pg.Namespace+"/"+pg.Name]+1, key, nodeLabels[nodeNames[st.domain_node]][key])
 			}
 			b.setUnschedulable(ctx, pg, why)
 			continue

@@ -60,6 +60,8 @@ type tables struct {
 	spreadGroups []C.grove_spread_t
 	spreadOf     []C.uint32_t
 	spreadSeeds  []C.grove_spread_seed_t
+	// fences (optional; ordinary passes only): the gang rows the starvation guard fences (grove_set_fences)
+	fences []C.uint32_t
 }
 
 type result struct {
@@ -99,6 +101,11 @@ func (e *engine) cycle(t *tables, preempt, large, explain bool) (*result, error)
 		}
 		if err := e.err(C.grove_set_spread(e.h, &t.spreadGroups[0], C.uint32_t(len(t.spreadGroups)), &t.spreadOf[0],
 			C.uint32_t(len(t.spreadOf)), sp, C.uint32_t(len(t.spreadSeeds)))); err != nil {
+			return nil, err
+		}
+	}
+	if len(t.fences) > 0 {
+		if err := e.err(C.grove_set_fences(e.h, &t.fences[0], C.uint32_t(len(t.fences)))); err != nil {
 			return nil, err
 		}
 	}
