@@ -256,6 +256,11 @@ struct grove_engine {
   size_t fc_words = 0;                      // labels, hence the domains, cannot change while the set is kept)
   DevBuf<uint32_t> d_fc_gang, d_fc_off, d_fc_have, d_fc_slot;
   DevBuf<uint4> d_fc_list;
+  // grove_run_cycle_consolidate (consolidate.cuh): the moves of the last such cycle, a target's view W, its per-domain capacity sums
+  // over F and W, the ranked try ranges and the (gang, offset) words k_fence_have reads
+  std::vector<grove_move_t> moves;
+  DevBuf<uint4> d_cs_view;
+  DevBuf<uint32_t> d_cs_have, d_cs_rank, d_cs_zero;
 };
 
 
@@ -1084,7 +1089,7 @@ static int32_t cycle_begin(grove_engine* e) {
     CU_TRY(e, cudaGetLastError());
   }
   e->launches = 0; e->in_cycle = true; e->have_results = false; e->have_scopes = false; e->diag = grove_engine::kDiagNoCycle;
-  e->victims.clear(); e->score_pass_valid = false;
+  e->victims.clear(); e->moves.clear(); e->score_pass_valid = false;
   std::memset(&e->last, 0, sizeof(e->last));
   return GROVE_OK;
 }
@@ -1696,7 +1701,9 @@ int32_t grove_run_cycle_preempt(grove_engine_t* e, const grove_running_gang_t* r
     Restore restore{e, &real0, &gangs, &cliques, &scopes};
     std::vector<uint8_t> evicted(n_running, 0);
     // running gangs by node (CSR), for the victim choice
-    std::vector<uint32_t> at_off(size_t(N) + 1, 0), at_run(n_holdings);
+    size_t n_held = 0;   // (ranges of running gangs may overlap: size by what the fill below writes)
+    for (uint32_t r = 0; r < n_running; ++r) n_held += running[r].n_holdings;
+    std::vector<uint32_t> at_off(size_t(N) + 1, 0), at_run(n_held);
     for (uint32_t r = 0; r < n_running; ++r) for (uint32_t h = 0; h < running[r].n_holdings; ++h) ++at_off[holdings[running[r].holding_off + h].node + 1];
     for (uint32_t n = 0; n < N; ++n) at_off[n + 1] += at_off[n];
     { std::vector<uint32_t> cur(at_off.begin(), at_off.end() - 1);
@@ -1780,7 +1787,8 @@ int32_t grove_run_cycle_preempt(grove_engine_t* e, const grove_running_gang_t* r
   return publish_reclaim(e, status, place, extra, sstat, st0, std::move(victims), stats);
 }
 
-// the outputs of a cycle with a reclaim pass, merged: placements grouped by gang in submission order (a preemptor's from `extra`)
+// the outputs of a cycle with a reclaim or consolidation pass, merged: placements grouped by gang in submission order (those of a
+// preemptor, a consolidated target or a moved spec row from `extra`)
 static int32_t publish_reclaim(grove_engine* e, std::vector<grove_gang_status_t>& status, const std::vector<grove_placement_t>& place,
                                const std::vector<std::vector<grove_placement_t>>& extra, const std::vector<grove_scope_status_t>& sstat,
                                grove_cycle_stats_t st0, std::vector<grove_victim_t> victims, grove_cycle_stats_t* stats) {
@@ -1793,7 +1801,7 @@ static int32_t publish_reclaim(grove_engine* e, std::vector<grove_gang_status_t>
   for (uint32_t g = 0; g < G; ++g) {
     if (status[g].state != GROVE_GANG_ADMITTED) continue;
     const uint32_t off = uint32_t(merged.size());
-    if (status[g].reserved0 & GROVE_STATUS_PREEMPTOR) merged.insert(merged.end(), extra[g].begin(), extra[g].end());
+    if (status[g].reserved0 & (GROVE_STATUS_PREEMPTOR | GROVE_STATUS_CONSOLIDATED | GROVE_STATUS_MOVED)) merged.insert(merged.end(), extra[g].begin(), extra[g].end());
     else merged.insert(merged.end(), place.begin() + status[g].placement_off, place.begin() + status[g].placement_off + status[g].n_pods);
     status[g].placement_off = off;
   }
@@ -1921,18 +1929,13 @@ int32_t grove_run_cycle_reuse(grove_engine_t* e, const uint32_t* replaces, uint3
 // gang in rank order, over the rows of the nodes the class's preemptors use; then the device takes the holdings of the running
 // gangs still standing off the table again, which leaves the free table.
 // ---------------------------------------------------------------------------------------------
-int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs, const grove_running_gang_t* running,
-                                      uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
-  if (!e || (n_gangs && !replaces) || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
-  if (e->sp_members) return refuse_spread(e, "grove_run_cycle_reuse_preempt");
-  if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_reuse_preempt");
-  NoDiagnosis no_diag{e};
-  if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse_preempt");
-  int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);
-  if (rc) return rc;
-  CU_TRY(e, cudaSetDevice(e->cfg.device));
+// The running gangs of grove_run_cycle_reuse_preempt / grove_run_cycle_consolidate on the device (reclaim.cuh): their holdings by
+// sorted node, running gangs ascending within a row, and their priorities, uploaded once; the gone mask (one byte per running gang)
+// is the caller's to upload.  Then the check that free plus every running gang's holdings fits the node record's fields: then so
+// does every view built from them.
+static int32_t upload_running(grove_engine* e, const grove_running_gang_t* running, uint32_t n_running, const grove_holding_t* holdings,
+                              ReclaimCsr* csr) {
   const uint32_t N = e->N, nblk = (N + 255) / 256;
-  // the holdings by sorted node, running gangs ascending within a row: uploaded once
   std::vector<uint32_t> off(size_t(N) + 1, 0);
   for (uint32_t r = 0; r < n_running; ++r)
     for (uint32_t k = 0; k < running[r].n_holdings; ++k) ++off[e->inv[holdings[running[r].holding_off + k].node] + 1];
@@ -1948,22 +1951,40 @@ int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replace
   }
   std::vector<int32_t> prio(std::max<uint32_t>(n_running, 1), 0);
   for (uint32_t r = 0; r < n_running; ++r) prio[r] = running[r].priority;
-  std::vector<uint8_t> gone(std::max<uint32_t>(n_running, 1), 0);   // released or evicted
   CU_TRY(e, e->d_rc_off.ensure(off.size())); CU_TRY(e, e->d_rc_ent.ensure(ent.size())); CU_TRY(e, e->d_rc_bad.ensure(1));
-  CU_TRY(e, e->d_rc_prio.ensure(prio.size())); CU_TRY(e, e->d_rc_gone.ensure(gone.size()));
+  CU_TRY(e, e->d_rc_prio.ensure(prio.size())); CU_TRY(e, e->d_rc_gone.ensure(prio.size()));
   CU_TRY(e, e->d_rc_real.ensure(e->Npad)); CU_TRY(e, e->d_rc_base.ensure(e->Npad));
   CU_TRY(e, cudaMemcpyAsync(e->d_rc_off.p, off.data(), sizeof(uint32_t) * off.size(), cudaMemcpyHostToDevice, e->stream));
   CU_TRY(e, cudaMemcpyAsync(e->d_rc_ent.p, ent.data(), sizeof(uint4) * ent.size(), cudaMemcpyHostToDevice, e->stream));
   CU_TRY(e, cudaMemcpyAsync(e->d_rc_prio.p, prio.data(), sizeof(int32_t) * prio.size(), cudaMemcpyHostToDevice, e->stream));
   CU_TRY(e, cudaMemsetAsync(e->d_rc_bad.p, 0, sizeof(uint32_t), e->stream));
-  const ReclaimCsr csr{e->d_rc_off.p, e->d_rc_ent.p, e->d_rc_prio.p, e->d_rc_gone.p};
-  // free plus every running gang's holdings must fit the node record's fields: then so does every class view and every hold
-  k_reclaim_check<<<nblk, 256, 0, e->stream>>>(e->d_nres.p, csr, N, e->d_rc_bad.p);
+  *csr = ReclaimCsr{e->d_rc_off.p, e->d_rc_ent.p, e->d_rc_prio.p, e->d_rc_gone.p};
+  k_reclaim_check<<<nblk, 256, 0, e->stream>>>(e->d_nres.p, *csr, N, e->d_rc_bad.p);
   CU_TRY(e, cudaGetLastError());
   uint32_t bad = 0;
   CU_TRY(e, cudaMemcpyAsync(&bad, e->d_rc_bad.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, e->stream));
-  CU_TRY(e, cudaStreamSynchronize(e->stream));
+  CU_TRY(e, cudaStreamSynchronize(e->stream));   // (pageable sources)
   if (bad) return fail(e, GROVE_ERR_INVALID_ARG, "free resources plus holdings overflow a field of a node record");
+  return GROVE_OK;
+}
+
+int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs, const grove_running_gang_t* running,
+                                      uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
+  if (!e || (n_gangs && !replaces) || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
+  if (e->sp_members) return refuse_spread(e, "grove_run_cycle_reuse_preempt");
+  if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_reuse_preempt");
+  NoDiagnosis no_diag{e};
+  if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse_preempt");
+  int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);
+  if (rc) return rc;
+  CU_TRY(e, cudaSetDevice(e->cfg.device));
+  const uint32_t N = e->N, nblk = (N + 255) / 256;
+  ReclaimCsr csr{};
+  rc = upload_running(e, running, n_running, holdings, &csr);
+  if (rc) return rc;
+  std::vector<int32_t> prio(std::max<uint32_t>(n_running, 1), 0);
+  for (uint32_t r = 0; r < n_running; ++r) prio[r] = running[r].priority;
+  std::vector<uint8_t> gone(std::max<uint32_t>(n_running, 1), 0);   // released or evicted
 
   // 1. the ordinary pass: the reuse cycle.  An admitted new version's predecessor is released.
   grove_cycle_stats_t st0{};
@@ -2005,7 +2026,9 @@ int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replace
     };
     Restore restore{e, &gangs, &cliques, &scopes};
     // running gangs by node (caller order), for the victim choice
-    std::vector<uint32_t> at_off(size_t(N) + 1, 0), at_run(n_holdings);
+    size_t n_held = 0;   // (ranges of running gangs may overlap: size by what the fill below writes)
+    for (uint32_t r = 0; r < n_running; ++r) n_held += running[r].n_holdings;
+    std::vector<uint32_t> at_off(size_t(N) + 1, 0), at_run(n_held);
     for (uint32_t r = 0; r < n_running; ++r) for (uint32_t h = 0; h < running[r].n_holdings; ++h) ++at_off[holdings[running[r].holding_off + h].node + 1];
     for (uint32_t n = 0; n < N; ++n) at_off[n + 1] += at_off[n];
     { std::vector<uint32_t> cur(at_off.begin(), at_off.end() - 1);
@@ -2163,6 +2186,303 @@ int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replace
   }
   st0.kernel_launches += 1;   // k_reclaim_check
   return publish_reclaim(e, status, place, extra, sstat, st0, std::move(victims), stats);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Consolidation (include/grove_place.h "consolidation"; DESIGN.md section 1; kernels in consolidate.cuh).  The ordinary pass, then
+// per target b: the device keeps F aside and builds W from the running gangs' CSR, sums b's capacities per domain over both
+// (k_fence_have) and ranks the qualifying domains (k_consol_rank).  A try is a one-gang cycle over the masked W; when b fits, the
+// rows of F at its nodes come back, the displaced set is chosen here, F' is patched in and X's spec rows run as one cycle.  The
+// node table stays on the device throughout: a rolled-back try is a copy of F back into place.
+// ---------------------------------------------------------------------------------------------
+int32_t grove_run_cycle_consolidate(grove_engine_t* e, const uint32_t* targets, uint32_t n_targets, const uint32_t* spec_of,
+                                    const grove_running_gang_t* running, uint32_t n_running, const grove_holding_t* holdings,
+                                    uint32_t n_holdings, grove_cycle_stats_t* stats) {
+  if (!e || (n_targets && !targets) || (n_running && (!running || !spec_of)) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
+  if (e->sp_members) return refuse_spread(e, "grove_run_cycle_consolidate");
+  if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_consolidate");
+  NoDiagnosis no_diag{e};
+  if (e->wide) return refuse_wide(e, "grove_run_cycle_consolidate");
+  if (n_targets > GROVE_MAX_CONSOLIDATE_TARGETS) return fail(e, GROVE_ERR_LIMIT, "grove_run_cycle_consolidate: more than GROVE_MAX_CONSOLIDATE_TARGETS targets");
+  if (!e->nodes_loaded) return fail(e, GROVE_ERR_STATE, "no node snapshot loaded");
+  if (!e->gangs_loaded) return fail(e, GROVE_ERR_STATE, "no gangs submitted");
+  if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
+  const uint32_t G = e->G, Q = e->Q, S = e->S, N = e->N, nblk = (N + 255) / 256;
+  std::vector<uint8_t> role(G, 0);   // 1: a target, 2: a spec row
+  for (uint32_t k = 0; k < n_targets; ++k) {
+    if (targets[k] >= G) return fail(e, GROVE_ERR_INVALID_ARG, "grove_run_cycle_consolidate: target out of range");
+    if (role[targets[k]]) return fail(e, GROVE_ERR_INVALID_ARG, "grove_run_cycle_consolidate: a target is named twice");
+    role[targets[k]] = 1;
+  }
+  for (uint32_t r = 0; r < n_running; ++r) {
+    const uint32_t s = spec_of[r];
+    if (s == GROVE_NONE_U32) continue;
+    if (s >= G) return fail(e, GROVE_ERR_INVALID_ARG, "grove_run_cycle_consolidate: spec row out of range");
+    if (role[s] == 1) return fail(e, GROVE_ERR_INVALID_ARG, "grove_run_cycle_consolidate: a spec row is also a target");
+    if (role[s] == 2) return fail(e, GROVE_ERR_INVALID_ARG, "grove_run_cycle_consolidate: a spec row is named twice");
+    if (!(e->gangs[s].flags & GROVE_GANG_GATED)) return fail(e, GROVE_ERR_INVALID_ARG, "grove_run_cycle_consolidate: a spec row must carry GROVE_GANG_GATED");
+    role[s] = 2;
+  }
+  for (uint32_t r = 0; r < n_running; ++r)
+    if (uint64_t(running[r].holding_off) + running[r].n_holdings > n_holdings) return fail(e, GROVE_ERR_INVALID_ARG, "running gang holdings out of range");
+  for (uint32_t h = 0; h < n_holdings; ++h)
+    if (holdings[h].node >= N) return fail(e, GROVE_ERR_INVALID_ARG, "holding on a node out of range");
+  CU_TRY(e, cudaSetDevice(e->cfg.device));
+  ReclaimCsr csr{};
+  int32_t rc = upload_running(e, running, n_running, holdings, &csr);
+  if (rc) return rc;
+
+  // 1. the ordinary pass
+  grove_cycle_stats_t st0{};
+  rc = grove_run_cycle(e, &st0);
+  if (rc) return rc;
+  std::vector<grove_gang_t> gangs(e->gangs.data(), e->gangs.data() + G);
+  std::vector<grove_clique_t> cliques(e->cliques.data(), e->cliques.data() + Q);
+  std::vector<grove_scope_t> scopes(e->scopes.data(), e->scopes.data() + S);
+  std::vector<grove_gang_status_t> status(e->h_status.p, e->h_status.p + G);
+  std::vector<grove_placement_t> place(e->h_out.p, e->h_out.p + e->n_out);
+  std::vector<grove_scope_status_t> sstat(std::max<uint32_t>(S, 1));
+  if (S) { rc = grove_get_scope_domains(e, sstat.data(), S); if (rc) return rc; }
+  std::vector<uint32_t> order(targets, targets + n_targets);
+  std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) {   // rank order: priority desc, index asc
+    return gangs[a].priority != gangs[b].priority ? gangs[a].priority > gangs[b].priority : a < b;
+  });
+  std::vector<uint8_t> gone(std::max<uint32_t>(n_running, 1), 1);   // not movable, or moved this cycle
+  for (uint32_t r = 0; r < n_running; ++r) gone[r] = spec_of[r] == GROVE_NONE_U32;
+  auto movable = [&](int32_t p) {   // is M (the standing movable gangs of priority <= p) non-empty?
+    for (uint32_t r = 0; r < n_running; ++r) if (!gone[r] && running[r].priority <= p) return true;
+    return false;
+  };
+  std::vector<grove_move_t> moves;
+  std::vector<std::vector<grove_placement_t>> extra(G);   // placements of the consolidated targets and the moved spec rows
+  bool any = false;
+  for (uint32_t b : order) any |= status[b].state == GROVE_GANG_REJECTED && movable(gangs[b].priority);
+  if (any) {
+    // whatever goes wrong from here on, the handle goes back to the caller's submission on the free table the ordinary pass left
+    CU_TRY(e, cudaMemcpyAsync(e->d_rc_base.p, e->d_nres.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToDevice, e->stream));
+    struct Restore {
+      grove_engine* e; const std::vector<grove_gang_t>* g; const std::vector<grove_clique_t>* c; const std::vector<grove_scope_t>* s; bool armed = true;
+      ~Restore() {
+        if (!armed) return;
+        const std::string keep = e->err;
+        cudaMemcpyAsync(e->d_nres.p, e->d_rc_base.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToDevice, e->stream);
+        cudaStreamSynchronize(e->stream);
+        grove_submit_gangs(e, g->data(), uint32_t(g->size()), c->data(), uint32_t(c->size()), s->data(), uint32_t(s->size()));
+        e->err = keep;
+      }
+    };
+    Restore restore{e, &gangs, &cliques, &scopes};
+    CU_TRY(e, e->d_cs_view.ensure(e->Npad)); CU_TRY(e, e->d_cs_rank.ensure(1 + 2 * kConsolTries)); CU_TRY(e, e->d_cs_zero.ensure(1));
+    CU_TRY(e, cudaMemsetAsync(e->d_cs_zero.p, 0, sizeof(uint32_t), e->stream));   // k_fence_have's gang index and offset: 0
+    // running gangs by node (caller order), for the choice of the displaced set
+    size_t n_held = 0;   // (ranges of running gangs may overlap: size by what the fill below writes)
+    for (uint32_t r = 0; r < n_running; ++r) n_held += running[r].n_holdings;
+    std::vector<uint32_t> at_off(size_t(N) + 1, 0), at_run(n_held);
+    for (uint32_t r = 0; r < n_running; ++r) for (uint32_t h = 0; h < running[r].n_holdings; ++h) ++at_off[holdings[running[r].holding_off + h].node + 1];
+    for (uint32_t n = 0; n < N; ++n) at_off[n + 1] += at_off[n];
+    { std::vector<uint32_t> cur(at_off.begin(), at_off.end() - 1);
+      for (uint32_t r = 0; r < n_running; ++r) for (uint32_t h = 0; h < running[r].n_holdings; ++h) at_run[cur[holdings[running[r].holding_off + h].node]++] = r; }
+    std::vector<int32_t> slot(N, -1);   // node (caller order) -> its row in `rows` during a try
+    auto accumulate = [&](grove_cycle_stats_t& s) {
+      st0.rounds += s.rounds; st0.evaluations += s.evaluations; st0.kernel_launches += s.kernel_launches;
+      st0.ms_fit += s.ms_fit; st0.ms_admit += s.ms_admit; st0.ms_commit += s.ms_commit; st0.ms_total += s.ms_total;
+    };
+    for (uint32_t b : order) {
+      const int32_t p = gangs[b].priority;
+      if (status[b].state != GROVE_GANG_REJECTED || !movable(p)) continue;
+      // 2. b as a submission of its own (anchor pinned to the ordinary pass's, no gating); F aside, W = F + what M holds
+      grove_gang_t x = gangs[b];
+      if (x.anchor_node == GROVE_NONE_U32) x.anchor_node = e->perm[fmix32(b) % N];
+      x.base_gang = GROVE_NONE_U32; x.clique_off = 0; x.scope_off = 0;
+      const grove_clique_t* bq = cliques.data() + gangs[b].clique_off;
+      const grove_scope_t* bs = scopes.data() + gangs[b].scope_off;
+      auto submit_b = [&]() { return grove_submit_gangs(e, &x, 1, bq, x.n_cliques, bs, x.n_scopes); };
+      rc = submit_b(); if (rc) return rc;
+      CU_TRY(e, cudaMemcpyAsync(e->d_rc_gone.p, gone.data(), gone.size(), cudaMemcpyHostToDevice, e->stream));
+      k_consol_view<<<nblk, 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_real.p, e->d_cs_view.p, csr, N, p);
+      CU_TRY(e, cudaGetLastError());
+      st0.kernel_launches += 1;
+      // 3. the candidate domains
+      std::vector<std::pair<uint32_t, uint32_t>> tries;
+      if (x.level == GROVE_LEVEL_NONE) {
+        tries.push_back({0u, N});
+      } else {
+        rc = build_ginfo(e); if (rc) return rc;
+        const size_t words = size_t(x.n_cliques) * e->n_dom[x.level];
+        CU_TRY(e, e->d_cs_have.ensure(std::max<size_t>(2 * words, 1)));
+        CU_TRY(e, cudaMemsetAsync(e->d_cs_have.p, 0, sizeof(uint32_t) * 2 * words, e->stream));
+        Topo tf = make_topo(e), tw = tf;
+        tw.nres = e->d_cs_view.p;
+        const Tables tb = make_tables(e);
+        k_fence_have<<<dim3(e->Npad / 256, 1), 256, 0, e->stream>>>(tf, tb, e->d_cs_zero.p, e->d_cs_zero.p, e->d_cs_have.p);
+        k_fence_have<<<dim3(e->Npad / 256, 1), 256, 0, e->stream>>>(tw, tb, e->d_cs_zero.p, e->d_cs_zero.p, e->d_cs_have.p + words);
+        k_consol_rank<<<1, 1024, 0, e->stream>>>(tf, tb, 0u, e->inv[x.anchor_node], e->d_cs_have.p, e->d_cs_have.p + words, e->d_cs_rank.p);
+        CU_TRY(e, cudaGetLastError());
+        st0.kernel_launches += 3;
+        uint32_t rk[1 + 2 * kConsolTries];
+        CU_TRY(e, cudaMemcpyAsync(rk, e->d_cs_rank.p, sizeof(rk), cudaMemcpyDeviceToHost, e->stream));
+        CU_TRY(e, cudaStreamSynchronize(e->stream));
+        for (uint32_t t = 0; t < rk[0]; ++t) tries.push_back({rk[1 + 2 * t], rk[2 + 2 * t]});
+      }
+      bool committed = false, b_loaded = true;
+      for (const auto& [lo, hi] : tries) {
+        // 4. evaluate b against W with every node outside D unschedulable
+        if (!b_loaded) { rc = submit_b(); if (rc) return rc; b_loaded = true; }
+        k_consol_mask<<<nblk, 256, 0, e->stream>>>(e->d_cs_view.p, e->d_nres.p, N, lo, hi);
+        CU_TRY(e, cudaGetLastError());
+        grove_cycle_stats_t stb{};
+        rc = grove_run_cycle(e, &stb); if (rc) return rc;
+        accumulate(stb); st0.kernel_launches += 1;
+        const grove_gang_status_t sb = e->h_status.p[0];
+        if (sb.state != GROVE_GANG_ADMITTED) continue;
+        std::vector<grove_scope_status_t> ssb(std::max<uint32_t>(x.n_scopes, 1));
+        if (x.n_scopes) { rc = grove_get_scope_domains(e, ssb.data(), x.n_scopes); if (rc) return rc; }
+        // b's usage, nodes in the order its placement first names them
+        std::vector<uint32_t> nodes_b; std::vector<Res> use;
+        std::vector<grove_placement_t> plb;
+        for (uint32_t i = 0; i < sb.n_pods; ++i) {
+          const grove_placement_t pl = e->h_out.p[sb.placement_off + i];
+          const grove_clique_t& q = bq[pl.clique];
+          if (slot[pl.node] < 0) { slot[pl.node] = int32_t(nodes_b.size()); nodes_b.push_back(pl.node); use.emplace_back(); }
+          Res& u = use[slot[pl.node]];
+          u.cpu += q.req_cpu_milli; u.mem += q.req_mem_mib; u.gpu += q.req_gpu; u.pods += 1;
+          plb.push_back(grove_placement_t{gangs[b].clique_off + pl.clique, pl.node});
+        }
+        // the rows of F at those nodes
+        std::vector<Res> rows(nodes_b.size());
+        if (!nodes_b.empty()) {
+          std::vector<uint32_t> idx(nodes_b.size());
+          for (size_t i = 0; i < nodes_b.size(); ++i) idx[i] = e->inv[nodes_b[i]];
+          std::vector<uint4> got(idx.size());
+          CU_TRY(e, e->d_rc_idx.ensure(idx.size())); CU_TRY(e, e->d_rc_rows.ensure(idx.size()));
+          CU_TRY(e, cudaMemcpyAsync(e->d_rc_idx.p, idx.data(), sizeof(uint32_t) * idx.size(), cudaMemcpyHostToDevice, e->stream));
+          k_reclaim_rows<<<uint32_t((idx.size() + 255) / 256), 256, 0, e->stream>>>(e->d_rc_real.p, e->d_rc_idx.p, e->d_rc_rows.p, uint32_t(idx.size()));
+          CU_TRY(e, cudaGetLastError());
+          CU_TRY(e, cudaMemcpyAsync(got.data(), e->d_rc_rows.p, sizeof(uint4) * got.size(), cudaMemcpyDeviceToHost, e->stream));
+          CU_TRY(e, cudaStreamSynchronize(e->stream));
+          for (size_t i = 0; i < got.size(); ++i) rows[i] = Res{got[i].x, got[i].y, got[i].z & 0xFFFFu, got[i].z >> 16};
+          st0.kernel_launches += 1;
+        }
+        // the displaced set: node by node, while F plus what X holds does not cover U, the victim rule of the reclaim pass over M
+        std::vector<uint32_t> X;
+        std::vector<uint8_t> in_x(std::max<uint32_t>(n_running, 1), 0);
+        for (size_t j = 0; j < nodes_b.size(); ++j) {
+          const uint32_t n = nodes_b[j];
+          const Res& u = use[j];
+          while (!(rows[j].cpu >= u.cpu && rows[j].mem >= u.mem && rows[j].gpu >= u.gpu && rows[j].pods >= u.pods)) {
+            uint32_t v = GROVE_NONE_U32;   // lowest priority first, then the highest running index
+            for (uint32_t a = at_off[n]; a < at_off[n + 1]; ++a) {
+              const uint32_t r = at_run[a];
+              if (gone[r] || in_x[r] || running[r].priority > p) continue;
+              if (v == GROVE_NONE_U32 || running[r].priority < running[v].priority || (running[r].priority == running[v].priority && r > v)) v = r;
+            }
+            if (v == GROVE_NONE_U32) return fail(e, GROVE_ERR_STATE, "consolidation: a target's node cannot be covered");
+            in_x[v] = 1; X.push_back(v);
+            for (uint32_t h = 0; h < running[v].n_holdings; ++h) {
+              const grove_holding_t& y = holdings[running[v].holding_off + h];
+              if (slot[y.node] < 0) continue;
+              Res& q = rows[slot[y.node]];
+              q.cpu += y.cpu_milli; q.mem += y.mem_mib; q.gpu += y.gpu; q.pods += y.pods;
+            }
+          }
+        }
+        for (uint32_t n : nodes_b) slot[n] = -1;
+        // F' = F + what X holds - U, patched into a copy of F
+        {
+          std::vector<std::pair<uint32_t, std::array<int64_t, 4>>> d;   // (sorted node, change)
+          for (size_t j = 0; j < nodes_b.size(); ++j) d.push_back({e->inv[nodes_b[j]], {-use[j].cpu, -use[j].mem, -use[j].gpu, -use[j].pods}});
+          for (uint32_t r : X)
+            for (uint32_t h = 0; h < running[r].n_holdings; ++h) {
+              const grove_holding_t& y = holdings[running[r].holding_off + h];
+              d.push_back({e->inv[y.node], {int64_t(y.cpu_milli), int64_t(y.mem_mib), int64_t(y.gpu), int64_t(y.pods)}});
+            }
+          std::sort(d.begin(), d.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+          std::vector<uint4> patch;
+          for (size_t i = 0; i < d.size();) {
+            const uint32_t n = d[i].first;
+            int64_t v[4] = {0, 0, 0, 0};
+            for (; i < d.size() && d[i].first == n; ++i) for (int k = 0; k < 4; ++k) v[k] += d[i].second[k];
+            patch.push_back(make_uint4(n, uint32_t(v[0]), uint32_t(v[1]), uint32_t(v[2] + v[3] * 65536)));
+          }
+          CU_TRY(e, cudaMemcpyAsync(e->d_nres.p, e->d_rc_real.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToDevice, e->stream));
+          if (!patch.empty()) {
+            CU_TRY(e, e->d_rc_patch.ensure(patch.size()));
+            CU_TRY(e, cudaMemcpyAsync(e->d_rc_patch.p, patch.data(), sizeof(uint4) * patch.size(), cudaMemcpyHostToDevice, e->stream));
+            k_reclaim_patch<<<uint32_t((patch.size() + 255) / 256), 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_patch.p, uint32_t(patch.size()));
+            CU_TRY(e, cudaGetLastError());
+            st0.kernel_launches += 1;
+          }
+        }
+        // relocate X: its spec rows as one sequential pass (running priority desc, running index asc), each with its own anchor
+        std::vector<uint32_t> xs(X);
+        std::sort(xs.begin(), xs.end(), [&](uint32_t a, uint32_t c) { return running[a].priority != running[c].priority ? running[a].priority > running[c].priority : a < c; });
+        std::vector<grove_gang_t> sg; std::vector<grove_clique_t> sq; std::vector<grove_scope_t> ss;
+        for (uint32_t r : xs) {
+          const uint32_t s = spec_of[r];
+          grove_gang_t y = gangs[s];
+          if (y.anchor_node == GROVE_NONE_U32) y.anchor_node = e->perm[fmix32(s) % N];
+          y.priority = running[r].priority; y.base_gang = GROVE_NONE_U32; y.flags &= uint16_t(~GROVE_GANG_GATED);
+          y.clique_off = uint32_t(sq.size()); y.scope_off = uint32_t(ss.size());
+          sq.insert(sq.end(), cliques.begin() + gangs[s].clique_off, cliques.begin() + gangs[s].clique_off + gangs[s].n_cliques);
+          ss.insert(ss.end(), scopes.begin() + gangs[s].scope_off, scopes.begin() + gangs[s].scope_off + gangs[s].n_scopes);
+          sg.push_back(y);
+        }
+        std::vector<grove_scope_status_t> ssx(std::max<size_t>(ss.size(), 1));
+        if (!xs.empty()) {
+          rc = grove_submit_gangs(e, sg.data(), uint32_t(sg.size()), sq.data(), uint32_t(sq.size()), ss.data(), uint32_t(ss.size())); if (rc) return rc;
+          b_loaded = false;
+          grove_cycle_stats_t stx{};
+          rc = grove_run_cycle(e, &stx); if (rc) return rc;
+          accumulate(stx);
+          bool all = true;
+          for (uint32_t k = 0; k < xs.size(); ++k) all &= e->h_status.p[k].state == GROVE_GANG_ADMITTED;
+          if (!all) continue;   // rolled back: the next try starts from the view again, and F is still aside
+          if (!ss.empty()) { rc = grove_get_scope_domains(e, ssx.data(), uint32_t(ss.size())); if (rc) return rc; }
+        }
+        // commit: the device table is F' minus the relocated gangs' usage
+        grove_gang_status_t ob = sb;
+        ob.reserved0 = GROVE_STATUS_CONSOLIDATED;
+        status[b] = ob; extra[b] = std::move(plb);
+        for (uint32_t si = 0; si < x.n_scopes; ++si) sstat[gangs[b].scope_off + si] = ssb[si];
+        for (uint32_t k = 0; k < xs.size(); ++k) {
+          const uint32_t s = spec_of[xs[k]];
+          grove_gang_status_t o = e->h_status.p[k];
+          for (uint32_t i = 0; i < o.n_pods; ++i) {
+            const grove_placement_t pl = e->h_out.p[o.placement_off + i];
+            extra[s].push_back(grove_placement_t{gangs[s].clique_off + (pl.clique - sg[k].clique_off), pl.node});
+          }
+          o.reserved0 = GROVE_STATUS_MOVED;
+          status[s] = o;
+          for (uint32_t si = 0; si < gangs[s].n_scopes; ++si) sstat[gangs[s].scope_off + si] = ssx[sg[k].scope_off + si];
+        }
+        for (uint32_t r : X) { gone[r] = 1; moves.push_back(grove_move_t{r, b}); }
+        st0.gangs_admitted += 1 + uint32_t(X.size()); st0.gangs_rejected -= 1;
+        committed = true;
+        break;
+      }
+      if (!committed) {   // every try rolled back: F back into place
+        CU_TRY(e, cudaMemcpyAsync(e->d_nres.p, e->d_rc_real.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToDevice, e->stream));
+      }
+    }
+    // the handle goes back to the caller's submission; the device table is F after every commit
+    restore.armed = false;
+    rc = grove_submit_gangs(e, gangs.data(), G, cliques.data(), Q, scopes.data(), S); if (rc) return rc;
+  }
+  st0.kernel_launches += 1;   // k_reclaim_check
+  rc = publish_reclaim(e, status, place, extra, sstat, st0, {}, stats);
+  if (rc) return rc;
+  e->moves = std::move(moves);
+  return GROVE_OK;
+}
+
+int32_t grove_get_moves(grove_engine_t* e, grove_move_t* out, uint32_t cap, uint32_t* n_out) {
+  if (!e || !n_out) return GROVE_ERR_INVALID_ARG;
+  if (!e->have_results) return fail(e, GROVE_ERR_STATE, "no completed cycle");
+  *n_out = uint32_t(e->moves.size());
+  if (!out) return GROVE_OK;
+  if (cap < e->moves.size()) return fail(e, GROVE_ERR_LIMIT, "output buffer too small");
+  std::memcpy(out, e->moves.data(), sizeof(grove_move_t) * e->moves.size());
+  return GROVE_OK;
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -263,6 +263,7 @@ Err GpuBackend::OnPodGangDelete(const PodGang& podGang) {
   std::lock_guard<std::mutex> l(mu_);
   const std::string key = podGang.Namespace + "/" + podGang.Name;
   pending_.erase(key); bound_.erase(key); running_.erase(key); setOf_.erase(key); rejectedFor_.erase(key);
+  specOf_.erase(key); moveAnchor_.erase(key);
   return std::nullopt;
 }
 
@@ -270,7 +271,17 @@ Err GpuBackend::SetStarvationGuard(uint32_t afterCycles, uint32_t maxGangs) {
   std::lock_guard<std::mutex> l(mu_);
   if (afterCycles < 1) return mkerr("ERR_SYNC_PODGANG", "SetStarvationGuard", "afterCycles must be at least 1");
   if (maxGangs > GROVE_MAX_FENCES) return mkerr("ERR_SYNC_PODGANG", "SetStarvationGuard", "maxGangs exceeds GROVE_MAX_FENCES");
+  if (maxGangs && consMax_) return mkerr("ERR_SYNC_PODGANG", "SetStarvationGuard", "the starvation guard and consolidation cannot both be on");
   guardAfter_ = afterCycles; guardMax_ = maxGangs;
+  return std::nullopt;
+}
+
+Err GpuBackend::SetConsolidation(uint32_t afterCycles, uint32_t maxTargets) {
+  std::lock_guard<std::mutex> l(mu_);
+  if (afterCycles < 1) return mkerr("ERR_SYNC_PODGANG", "SetConsolidation", "afterCycles must be at least 1");
+  if (maxTargets > GROVE_MAX_CONSOLIDATE_TARGETS) return mkerr("ERR_SYNC_PODGANG", "SetConsolidation", "maxTargets exceeds GROVE_MAX_CONSOLIDATE_TARGETS");
+  if (maxTargets && guardMax_) return mkerr("ERR_SYNC_PODGANG", "SetConsolidation", "the starvation guard and consolidation cannot both be on");
+  consAfter_ = afterCycles; consMax_ = maxTargets;
   return std::nullopt;
 }
 
@@ -312,7 +323,7 @@ Err GpuBackend::Encode(const std::vector<Node>& nodes, Tables* out) const {
   return EncodeLocked(nodes, out);
 }
 
-Err GpuBackend::EncodeLocked(const std::vector<Node>& nodes, Tables* out) const {
+Err GpuBackend::EncodeLocked(const std::vector<Node>& nodes, Tables* out, const std::vector<std::string>* restate) const {
   *out = Tables{};
   if (levels_.empty()) return mkerr("ERR_SYNC_PODGANG", "Encode", "no ClusterTopology levels synced");
   const uint32_t L = uint32_t(levels_.size());
@@ -435,11 +446,16 @@ Err GpuBackend::EncodeLocked(const std::vector<Node>& nodes, Tables* out) const 
     }
     return it->second;
   };
+  // consolidation: the running PodGangs to restate come last, as gated rows that bind all their pods (MinReplicas = replicas)
+  const size_t nRows = order.size();
+  if (restate) for (const std::string& key : *restate) order.push_back(&key);
+  out->specRow = uint32_t(nRows);
   for (size_t oi = 0; oi < order.size(); ++oi) {
     const std::string& key = *order[oi];
-    const PodGang& pg = pending_.at(key);
-    const bool remainder = oi >= nFull;
-    const bool split = !remainder && !constrained(pg) && hasSurplus(pg);          // this row carries the minimum only
+    const bool spec = oi >= nRows;
+    const PodGang& pg = spec ? specOf_.at(key) : pending_.at(key);
+    const bool remainder = !spec && oi >= nFull;
+    const bool split = !spec && !remainder && !constrained(pg) && hasSurplus(pg);  // this row carries the minimum only
     std::vector<uint32_t> minOnly;                                                 // surplus row of an unscheduled PodGang: its minimum is row `row[key]`
     const std::vector<uint32_t>* done = nullptr;                                   // pods covered elsewhere, per PodGroup
     if (remainder) {
@@ -449,14 +465,18 @@ Err GpuBackend::EncodeLocked(const std::vector<Node>& nodes, Tables* out) const 
     grove_gang_t g{};
     g.clique_off = uint32_t(out->cliques.size()); g.scope_off = uint32_t(out->scopes.size());
     g.anchor_node = GROVE_NONE_U32; g.base_gang = GROVE_NONE_U32; g.preferred = GROVE_LEVEL_NONE;
-    g.flags = pg.Gated ? GROVE_GANG_GATED : 0;
+    g.flags = pg.Gated || spec ? GROVE_GANG_GATED : 0;
     if (auto e = levelOf(pg.Spec.Topology, &g.level, &g.preferred)) return e;
     if (auto it = priorityClasses_.find(pg.Spec.PriorityClassName); it != priorityClasses_.end()) g.priority = it->second;
-    if (!remainder && !pg.BasePodGangName.empty())   // a base that is already scheduled gates nothing
+    if (!spec && !remainder && !pg.BasePodGangName.empty())   // a base that is already scheduled gates nothing
       if (auto it = row.find(pg.Namespace + "/" + pg.BasePodGangName); it != row.end()) g.base_gang = it->second;
     if (remainder && !minOnly.empty()) g.base_gang = row.at(key);   // surplus of a PodGang whose minimum is in this very pass
     if (remainder) {  // stay close to where the gang landed
       if (auto it = lastNode_.find(key); it != lastNode_.end()) if (auto nt = nodeIndex.find(it->second); nt != nodeIndex.end()) g.anchor_node = nt->second;
+    } else if (spec) {  // a restated running PodGang: anchored where it runs
+      if (auto it = lastNode_.find(key); it != lastNode_.end()) if (auto nt = nodeIndex.find(it->second); nt != nodeIndex.end()) g.anchor_node = nt->second;
+    } else if (auto mv = moveAnchor_.find(key); mv != moveAnchor_.end()) {   // moved by consolidation: where the cycle planned it
+      if (auto nt = nodeIndex.find(mv->second); nt != nodeIndex.end()) g.anchor_node = nt->second;
     } else if (pg.Spec.ReuseReservationRef) {  // locality hint: score distance against where that PodGang was placed
       auto it = lastNode_.find(pg.Spec.ReuseReservationRef->Namespace + "/" + pg.Spec.ReuseReservationRef->Name);
       if (it != lastNode_.end()) if (auto nt = nodeIndex.find(it->second); nt != nodeIndex.end()) g.anchor_node = nt->second;
@@ -498,6 +518,7 @@ Err GpuBackend::EncodeLocked(const std::vector<Node>& nodes, Tables* out) const 
         grove_clique_count_t n{uint16_t(p.MinReplicas), uint16_t(p.PodReferences.size())};
         if (remainder) { n.min_replicas = 0; n.replicas = uint16_t(left(gi)); }
         if (split) n.replicas = n.min_replicas;
+        if (spec) n.min_replicas = n.replicas;
         // the 8-bit fields are what grove_submit_gangs reads; grove_submit_gangs_wide reads the counts row
         c.min_replicas = uint8_t(std::min<uint32_t>(n.min_replicas, 255u)); c.replicas = uint8_t(std::min<uint32_t>(n.replicas, 255u));
         uint8_t cpref;
@@ -524,7 +545,7 @@ Err GpuBackend::EncodeLocked(const std::vector<Node>& nodes, Tables* out) const 
       return mkerr("ERR_SYNC_PODGANG", "Encode", "PodGang " + key + " exceeds the gpu-scheduler limits");
     g.n_cliques = uint16_t(rel); g.n_scopes = uint16_t(scopes.size());
     uint32_t grp = GROVE_NONE_U32;
-    if (const TopologySpread* sp = remainder ? nullptr : spreadSetOf(pg)) {
+    if (const TopologySpread* sp = remainder || spec ? nullptr : spreadSetOf(pg)) {
       bool need = false;
       for (size_t k = out->counts.size() - rel; k < out->counts.size(); ++k) need |= out->counts[k].min_replicas > 0;
       const uint32_t s = spreadGroup(pg.Namespace, pg.Labels.at(kPartOfLabel), *sp);
@@ -558,6 +579,9 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
   uint32_t guardAfter = 1, guardMax = 0;
   std::map<std::string, uint32_t> rejectedFor;
   std::vector<TopologyLevel> levels;
+  std::vector<std::string> restate;               // consolidation: the running PodGangs restated as gated spec rows
+  std::vector<grove_running_gang_t> crun; std::vector<grove_holding_t> cheld;
+  std::vector<uint32_t> targets, specOf;          // consolidation: target rows; spec row of each running gang of crun
   {
     std::lock_guard<std::mutex> l(mu_);
     large = large_; explain = explain_; levels = levels_;
@@ -565,9 +589,49 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
     if (pending_.empty()) return std::nullopt;
     if (auto e = Init()) return e;
     if (!engine_) return mkerr("ERR_SYNC_PODGANG", "RunCycle", "no ClusterTopology synced");
-    if (auto e = EncodeLocked(nodes, &t)) return e;
+    // consolidation runs in an ordinary pass only: every running PodGang scheduled whole is movable
+    const bool consOn = consMax_ && !preemption_ && !reuse_ && !reclaimReuse_;
+    if (consOn)
+      for (const auto& kv : running_)
+        if (!pending_.count(kv.first) && specOf_.count(kv.first) && WhyNotEncodable(specOf_.at(kv.first), false).empty()) restate.push_back(kv.first);
+    if (auto e = EncodeLocked(nodes, &t, consOn ? &restate : nullptr)) return e;
     snap = pending_;
+    if (t.specRow < t.gangs.size()) {   // the targets: as the starvation guard counts; none, or a pass that takes no consolidation: no spec rows
+      bool wide = false;
+      for (const grove_gang_t& g : t.gangs) {
+        uint32_t pods = 0;
+        for (uint32_t c = g.clique_off; c < g.clique_off + g.n_cliques; ++c) { const uint32_t rep = t.counts[c].replicas; pods += rep; wide |= rep > 255u; }
+        wide |= pods > GROVE_MAX_GANG_PODS;
+      }
+      if (!wide && t.spreadGroups.empty()) {
+        for (uint32_t g = 0; g < t.specRow; ++g) {
+          auto it = rejectedFor_.find(t.gangNames[g]);
+          if (!t.remainder[g] && it != rejectedFor_.end() && it->second >= consAfter_) targets.push_back(g);
+        }
+        std::stable_sort(targets.begin(), targets.end(), [&](uint32_t a, uint32_t b) { return t.gangs[a].priority > t.gangs[b].priority; });
+        if (targets.size() > consMax_) targets.resize(consMax_);
+      }
+      if (targets.empty()) {   // drop the spec rows (they come last)
+        const uint32_t r = t.specRow, q = t.gangs[r].clique_off, sc = t.gangs[r].scope_off;
+        t.gangs.resize(r); t.gangNames.resize(r); t.remainder.resize(r); t.spreadOf.resize(r);
+        t.cliques.resize(q); t.counts.resize(q); t.cliqueOf.resize(q); t.refBase.resize(q); t.scopes.resize(sc);
+      } else {   // the movable running PodGangs with what they hold (holdings on nodes that left the snapshot are dropped)
+        std::map<std::string, uint32_t> nodeIdx;
+        for (uint32_t i = 0; i < nodes.size(); ++i) nodeIdx[nodes[i].Name] = i;
+        for (uint32_t k = 0; k < restate.size(); ++k) {
+          const RunningGang& rg = running_.at(restate[k]);
+          grove_running_gang_t r{rg.priority, uint32_t(cheld.size()), 0u, 0u};
+          for (const auto& h : rg.held) {
+            auto it = nodeIdx.find(h.node);
+            if (it == nodeIdx.end()) continue;
+            cheld.push_back(grove_holding_t{it->second, h.cpu_milli, h.mem_mib, h.gpu, h.pods}); ++r.n_holdings;
+          }
+          crun.push_back(r); specOf.push_back(t.specRow + k);
+        }
+      }
+    }
   }
+  const bool consolidate = !targets.empty();
   for (const auto& kv : t.skipped) { PodGangStatus s; s.ScheduledReason = "Unschedulable"; s.ScheduledMessage = kv.second; (*statuses)[kv.first] = s; }
   if (t.gangs.empty()) return std::nullopt;
   auto chk = [this](int32_t rc, const char* what) -> Err {
@@ -651,6 +715,10 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
   if (both) { if (auto e = chk(grove_run_cycle_reuse_preempt(engine_, replaces.data(), uint32_t(replaces.size()), run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_reuse_preempt")) return e; }
   else if (reuse) { if (auto e = chk(grove_run_cycle_reuse(engine_, replaces.data(), uint32_t(replaces.size()), run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_reuse")) return e; }
   else if (preempt) { if (auto e = chk(grove_run_cycle_preempt(engine_, run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_preempt")) return e; }
+  else if (consolidate) {
+    if (auto e = chk(grove_run_cycle_consolidate(engine_, targets.data(), uint32_t(targets.size()), specOf.data(), crun.data(), uint32_t(crun.size()),
+                                                 cheld.data(), uint32_t(cheld.size()), &st), "grove_run_cycle_consolidate")) return e;
+  }
   else if (auto e = chk(grove_run_cycle(engine_, &st), "grove_run_cycle")) return e;
   if (stats) *stats = st;
   std::vector<grove_placement_t> pl(st.pods_bound + 1);
@@ -661,12 +729,13 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
   std::vector<uint32_t> seen(t.cliques.size(), 0);  // the r-th entry of a clique binds its r-th PodReference
   for (uint32_t i = 0; i < n; ++i) {
     const auto [grow, pgi] = t.cliqueOf[pl[i].clique];
+    if (grow >= t.specRow) continue;   // a moved PodGang: the caller deletes its pods, it is scheduled anew when synced again
     const PodGang& pg = snap.at(t.gangNames[grow]);
     const PodGroup& grp = pg.Spec.PodGroups[pgi];
     const NamespacedName& pod = grp.PodReferences[t.refBase[pl[i].clique] + seen[pl[i].clique]++];
     bindings->push_back({pod.Namespace, pod.Name, nodes[pl[i].node].Name});
   }
-  for (size_t g = 0; g < gs.size(); ++g) {
+  for (size_t g = 0; g < t.specRow; ++g) {
     PodGangStatus s;
     switch (gs[g].state) {
       case GROVE_GANG_ADMITTED:
@@ -698,7 +767,7 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
     }
   // why the rejected PodGangs did not fit (an ordinary cycle only: the running-gang cycles judge gangs against other views).  A
   // failed diagnosis leaves the messages empty: it never costs the cycle its bindings.
-  if (explain && !both && !reuse && !preempt &&
+  if (explain && !both && !reuse && !preempt && !consolidate &&
       std::any_of(gs.begin(), gs.end(), [](const grove_gang_status_t& x) { return x.state == GROVE_GANG_REJECTED; })) {
     std::vector<grove_gang_diag_t> gd(gs.size());
     std::vector<grove_clique_diag_t> qd(t.cliques.size());
@@ -708,6 +777,24 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
           (*statuses)[t.gangNames[g]].ScheduledMessage = ExplainRejection(t, snap.at(t.gangNames[g]), g, gd[g], qd.data(), levels);
   }
   for (const auto& [key, msg] : spreadMsg) (*statuses)[key].ScheduledMessage = msg;
+  // consolidation: a moved PodGang is disrupted (the caller deletes its pods); a consolidated one names the PodGangs it moved
+  std::vector<grove_move_t> moves;
+  if (consolidate) {
+    uint32_t nm = 0;
+    if (auto e = chk(grove_get_moves(engine_, nullptr, 0, &nm), "grove_get_moves")) return e;
+    moves.resize(nm + 1);
+    if (auto e = chk(grove_get_moves(engine_, moves.data(), uint32_t(moves.size()), &nm), "grove_get_moves")) return e;
+    moves.resize(nm);
+    std::map<uint32_t, std::string> names;
+    for (const grove_move_t& m : moves) {
+      const std::string& key = restate[m.running];
+      PodGangStatus s; s.Phase = PodGangPhase::Running; s.Scheduled = true;
+      s.DisruptionTarget = true; s.DisruptionMessage = "moved to make room for PodGang " + t.gangNames[m.target];
+      (*statuses)[key] = s;
+      names[m.target] += (names[m.target].empty() ? "" : ", ") + key;
+    }
+    for (const auto& [g, who] : names) (*statuses)[t.gangNames[g]].ScheduledMessage = "scheduled by moving PodGangs " + who;
+  }
   // the starvation guard's fences that held: the domain the PodGang keeps the PodGangs ranked after it out of
   for (uint32_t g : fences) {
     if (!(gs[g].reserved0 & GROVE_STATUS_FENCING) || gs[g].level >= levels.size()) continue;
@@ -729,7 +816,7 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
   };
   std::lock_guard<std::mutex> l(mu_);
   // the starvation guard's counts: consecutive Unschedulable cycles; a gated or base-not-scheduled cycle changes nothing
-  for (uint32_t g = 0; g < gs.size(); ++g) {
+  for (uint32_t g = 0; g < t.specRow; ++g) {
     if (t.remainder[g] || !pending_.count(t.gangNames[g])) continue;
     if (gs[g].state == GROVE_GANG_REJECTED) ++rejectedFor_[t.gangNames[g]];
     else if (gs[g].state == GROVE_GANG_ADMITTED) rejectedFor_.erase(t.gangNames[g]);
@@ -752,12 +839,19 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
   if (reuse && !replaces.empty())
     for (uint32_t i = 0; i < gs.size(); ++i)
       if (gs[i].state == GROVE_GANG_ADMITTED && replaces[i] != GROVE_NONE_U32) running_.erase(runNames[replaces[i]]);
-  for (uint32_t i = 0; i < gs.size(); ++i) {
+  for (const grove_move_t& m : moves) {   // forgotten as running; anchored where this cycle planned it when synced again
+    const std::string& key = restate[m.running];
+    const grove_gang_status_t& ms = gs[t.specRow + m.running];
+    running_.erase(key); specOf_.erase(key); lastNode_.erase(key);
+    if (ms.n_pods) moveAnchor_[key] = nodes[pl[ms.placement_off].node].Name;
+  }
+  for (uint32_t i = 0; i < t.specRow; ++i) {
     if (gs[i].state != GROVE_GANG_ADMITTED) continue;
     const std::string& key = t.gangNames[i];
     auto pit = pending_.find(key);
     if (pit == pending_.end()) continue;   // deleted while the cycle ran
     const PodGang& pg = pit->second;
+    specOf_[key] = pg; moveAnchor_.erase(key);
     {   // what the PodGang holds from now on (a remainder adds to what its minimum took)
       RunningGang& rg = running_[key];
       rg.priority = t.gangs[i].priority;

@@ -221,6 +221,9 @@ struct Tables {
   std::vector<uint32_t> spreadOf;
   std::vector<grove_spread_seed_t> spreadSeeds;
   std::vector<std::string> spreadSet;                   // group -> "<ns>/<PodCliqueSet>"
+  // consolidation (SetConsolidation): rows [specRow, gangs.size()) are gated rows restating running PodGangs, which makes them
+  // movable (grove_run_cycle_consolidate's spec rows); specRow == gangs.size() when there are none
+  uint32_t specRow = 0;
 };
 
 // The `gpu` scheduler backend: the third case of newBackendForProfile (manager/manager.go:35-52).
@@ -300,6 +303,17 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   // PodGang beyond the ordinary limits (SetLargePodGangs), nothing is fenced (the counts go on).  maxGangs = 0 turns it off (the
   // default); afterCycles >= 1, maxGangs <= GROVE_MAX_FENCES.
   Err SetStarvationGuard(uint32_t afterCycles, uint32_t maxGangs);
+  // Consolidation (grove_run_cycle_consolidate; DESIGN.md section 1 "Consolidation"): the spec of every PodGang this backend
+  // scheduled is remembered, and each running PodGang it scheduled whole (nothing left pending) is restated as a gated row, which
+  // makes it movable.  Each cycle the <= maxTargets highest-ranked pending PodGangs rejected at least afterCycles times in a row
+  // (counted as the starvation guard counts) are the targets: running PodGangs of their priority or below are relocated out of the
+  // domain closest to fitting one when every relocated PodGang is admitted elsewhere.  A moved PodGang comes back in `statuses`
+  // with DisruptionTarget set and a message naming the PodGang it made room for; it is forgotten as running (the caller deletes
+  // its pods), and when it is synced again it is anchored at the first node of the placement the cycle planned for it.  A
+  // consolidated PodGang's ScheduledMessage names the PodGangs that were moved.  Only in a pass without preemption, reservation
+  // reuse, topology spread members or PodGangs beyond the ordinary limits.  maxTargets = 0 turns it off (the default);
+  // afterCycles >= 1, maxTargets <= GROVE_MAX_CONSOLIDATE_TARGETS; it cannot be on together with the starvation guard.
+  Err SetConsolidation(uint32_t afterCycles, uint32_t maxTargets);
   static constexpr const char* kPartOfLabel = "app.kubernetes.io/part-of";
   size_t Running() const { std::lock_guard<std::mutex> l(mu_); return running_.size(); }
   // why a PodGang cannot be handed to the engine (limits of the packed tables), or empty.  SyncPodGang accepts every
@@ -337,6 +351,9 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   bool explain_ = false;
   uint32_t guardAfter_ = 1, guardMax_ = 0;             // starvation guard (off: guardMax_ == 0)
   std::map<std::string, uint32_t> rejectedFor_;        // pending PodGang -> consecutive Unschedulable cycles
+  uint32_t consAfter_ = 1, consMax_ = 0;               // consolidation (off: consMax_ == 0)
+  std::map<std::string, PodGang> specOf_;              // scheduled PodGang -> its spec (what a gated row restating it encodes)
+  std::map<std::string, std::string> moveAnchor_;      // moved PodGang -> the first node of its planned placement (anchor)
   std::map<std::string, TopologySpread> spread_;       // PodCliqueSet name -> its spread
   std::map<std::string, std::string> setOf_;           // scheduled base PodGang -> "<ns>/<PodCliqueSet>" (its part-of label)
   grove_engine_t* engine_ = nullptr;
@@ -347,7 +364,8 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   std::condition_variable cv_;
   bool stop_ = false;
   std::atomic<uint64_t> cycles_{0};
-  Err EncodeLocked(const std::vector<Node>& nodes, Tables* out) const;
+  // restate: running PodGangs to append as gated spec rows (consolidation), after every pending row
+  Err EncodeLocked(const std::vector<Node>& nodes, Tables* out, const std::vector<std::string>* restate = nullptr) const;
 };
 
 }  // namespace grove::host

@@ -11,6 +11,7 @@
 //   diagnose.cuh k_diag_*  why each rejected gang did not fit, after the cycle (grove_diagnose)
 //   spread.cuh   k_spread_classes / k_spread  allowed level-l_s domains of the topology spread members (grove_set_spread)
 //   fence.cuh    k_fence_have / k_fence_pick / k_fence_status  the domain each fencing gang fences (grove_set_fences)
+//   consolidate.cuh k_consol_view / k_consol_rank / k_consol_mask  the views of a consolidation try (grove_run_cycle_consolidate)
 //
 // Semantics are DESIGN.md "Placement semantics"; the reference contract they restate is cited in
 // include/grove_place.h.  Integer / compare work only: no tensor cores, no floating point.
@@ -25,3 +26,4 @@
 #include "diagnose.cuh"
 #include "spread.cuh"
 #include "fence.cuh"
+#include "consolidate.cuh"

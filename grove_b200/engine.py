@@ -26,6 +26,7 @@ SYMBOLS = [
     "grove_get_placements", "grove_get_gang_status", "grove_get_scope_domains", "grove_load_nodes_device",
     "grove_build_score_matrix", "grove_run_cycle_preempt", "grove_get_victims", "grove_run_cycle_reuse",
     "grove_run_cycle_reuse_preempt", "grove_diagnose", "grove_set_spread", "grove_set_fences",
+    "grove_run_cycle_consolidate", "grove_get_moves",
     "grove_shard_range", "grove_run_score_pass", "grove_shard_summary_device",
     "grove_debug_get_perm", "grove_debug_get_fit_row", "grove_debug_get_score_row",
 ]
@@ -203,6 +204,33 @@ class PlacementEngine:
         self._check(self.lib.grove_get_victims(self.h, None, C.c_uint32(0), C.byref(n)))
         out = np.zeros(max(n.value, 1), dtype=T.victim_dt)
         self._check(self.lib.grove_get_victims(self.h, _p(out), C.c_uint32(len(out)), C.byref(n)))
+        return out[: n.value]
+
+    def run_cycle_consolidate(self, targets, spec_of, running: np.ndarray, holdings: np.ndarray) -> dict:
+        """the ordinary cycle, then the consolidation pass: every REJECTED target (at most tables.MAX_CONSOLIDATE_TARGETS, tried in
+        rank order) may be admitted by relocating movable running gangs of its priority or below, and only when every relocated
+        gang is admitted elsewhere.  spec_of[r] is the gated row of the submission that restates running gang r (tables.NONE_U32:
+        not movable); `running` / `holdings` as for run_cycle_preempt.  Targets admitted this way carry
+        tables.STATUS_CONSOLIDATED, relocated spec rows tables.STATUS_MOVED; moves() lists the relocations
+        (include/grove_place.h "consolidation")"""
+        targets = np.ascontiguousarray(targets, dtype=np.uint32)
+        spec_of = np.ascontiguousarray(spec_of, dtype=np.uint32)
+        running = np.ascontiguousarray(running, dtype=T.running_dt)
+        holdings = np.ascontiguousarray(holdings, dtype=T.holding_dt)
+        if len(spec_of) != len(running):
+            raise ValueError("one spec_of entry per running gang")
+        st = np.zeros(1, dtype=T.stats_dt)
+        self._check(self.lib.grove_run_cycle_consolidate(self.h, _p(targets), C.c_uint32(len(targets)), _p(spec_of), _p(running),
+                                                         C.c_uint32(len(running)), _p(holdings), C.c_uint32(len(holdings)), _p(st)))
+        return {k: st[k][0].item() for k in T.stats_dt.names}
+
+    def moves(self) -> np.ndarray:
+        """(running gang, target gang) pairs of the last run_cycle_consolidate: the running gangs relocated to make room for each
+        consolidated target"""
+        n = C.c_uint32(0)
+        self._check(self.lib.grove_get_moves(self.h, None, C.c_uint32(0), C.byref(n)))
+        out = np.zeros(max(n.value, 1), dtype=T.move_dt)
+        self._check(self.lib.grove_get_moves(self.h, _p(out), C.c_uint32(len(out)), C.byref(n)))
         return out[: n.value]
 
     # ---- outputs ----

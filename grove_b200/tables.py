@@ -82,6 +82,13 @@ spread_seed_dt = np.dtype([("group", "<u4"), ("node", "<u4")])
 MAX_FENCES = 64
 STATUS_FENCING = 0x4              # status reserved0: a REJECTED gang whose fence held (level, domain_node name the fenced domain)
 
+# consolidation (grove_run_cycle_consolidate, include/grove_place.h "consolidation")
+MAX_CONSOLIDATE_TARGETS = 16
+CONSOLIDATE_TRIES = 4
+STATUS_CONSOLIDATED = 0x8         # status reserved0: a target admitted by the consolidation pass
+STATUS_MOVED = 0x10               # status reserved0: the spec row of a running gang that was relocated
+move_dt = np.dtype([("running", np.uint32), ("target", np.uint32)])
+
 assert node_dt.itemsize == 32 and clique_dt.itemsize == 16 and scope_dt.itemsize == 8
 assert gang_dt.itemsize == 32 and placement_dt.itemsize == 8 and status_dt.itemsize == 32 and scope_status_dt.itemsize == 8
 assert config_dt.itemsize == 32 and stats_dt.itemsize == 64

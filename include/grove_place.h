@@ -402,6 +402,44 @@ int32_t grove_set_spread(grove_engine_t* e, const grove_spread_t* groups, uint32
 #define GROVE_STATUS_FENCING 0x4u       /* grove_gang_status_t.reserved0: a REJECTED gang whose fence held at the end of the cycle */
 int32_t grove_set_fences(grove_engine_t* e, const uint32_t* gangs, uint32_t n);
 
+/* ---- consolidation ------------------------------------------------------------------------------------
+ * Running gangs are relocated so that a blocked gang fits, and only when every relocated gang finds a new place (DESIGN.md
+ * section 1, "Consolidation"; after KAI-Scheduler's consolidation action).  Running gangs and holdings are as for
+ * grove_run_cycle_preempt (the loaded node table does not include what they hold).  spec_of[r] (one entry per running gang) is
+ * the row of the current submission that restates running gang r's PodGang, which makes r MOVABLE, or GROVE_NONE_U32.  A spec row
+ * carries GROVE_GANG_GATED (so the ordinary pass skips it), its base_gang is ignored, it is named at most once and is not a
+ * target.  `targets` names up to GROVE_MAX_CONSOLIDATE_TARGETS submitted gangs.  F is the free table, rank = (priority desc,
+ * submission index asc).
+ *   1. The ordinary pass: grove_run_cycle on the submission; F is the table it leaves.
+ *   2. Every target b it left REJECTED, in rank order: M = the movable running gangs of priority <= p_b not moved this cycle
+ *      (empty: skip b), W = F + what the gangs of M hold.
+ *   3. Candidates: the level-l domains (l = b's gang Required level) in which every clique of b with MinReplicas m > 0 finds m pods
+ *      over W (grove_diagnose's exact capacities), in the order of their shortfall over F (as grove_set_fences computes it), ties
+ *      by the fences' candidate order; at most GROVE_CONSOLIDATE_TRIES of them.  Without a Required level: the whole cluster.
+ *   4. A try on D: b is evaluated with its ordinary-pass anchor against W with every node outside D unschedulable; it does not
+ *      fit: next D.  It fits with usage U: walking its nodes in the order its placement first names them, while F plus what X holds
+ *      does not cover U on the node, one more gang of M holding there joins the displaced set X (lowest priority first, then the
+ *      highest running index).  X's spec rows run as one sequential pass (rank = running priority desc, running index asc; each
+ *      keeps its own anchor) against F + what X holds - U.  All admitted: commit -- F is what that pass leaves, b is ADMITTED with
+ *      GROVE_STATUS_CONSOLIDATED, every spec row of X is ADMITTED with GROVE_STATUS_MOVED and its new placement and scope domains,
+ *      grove_get_moves lists (r, b) for each member; no more tries for b.  Otherwise nothing changes and the next D is tried.
+ * Outputs through the usual getters; the node table is F after all commits.  GROVE_ERR_LIMIT for a wide submission or more than
+ * GROVE_MAX_CONSOLIDATE_TARGETS targets; GROVE_ERR_STATE while a spread set with members or a non-empty fence set is in place;
+ * GROVE_ERR_INVALID_ARG for a target or spec row out of range or named twice, a spec row that is not gated or is a target, holdings
+ * out of range, or free + holdings overflowing a field of a node record.  grove_diagnose refuses the cycle that follows. */
+#define GROVE_MAX_CONSOLIDATE_TARGETS 16u
+#define GROVE_CONSOLIDATE_TRIES 4u
+#define GROVE_STATUS_CONSOLIDATED 0x8u  /* grove_gang_status_t.reserved0: a target admitted by the consolidation pass */
+#define GROVE_STATUS_MOVED 0x10u        /* grove_gang_status_t.reserved0: the spec row of a running gang that was relocated */
+typedef struct grove_move {
+  uint32_t running;       /* index into the running array */
+  uint32_t target;        /* gang index of the submission it made room for */
+} grove_move_t;
+int32_t grove_run_cycle_consolidate(grove_engine_t* e, const uint32_t* targets, uint32_t n_targets,
+                                    const uint32_t* spec_of, const grove_running_gang_t* running, uint32_t n_running,
+                                    const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats);
+int32_t grove_get_moves(grove_engine_t* e, grove_move_t* out, uint32_t cap, uint32_t* n_out);
+
 /* K2: the topology-distance score matrix T[clique][node] = fit ? 1 + levels shared with the gang's anchor : 0 (u8) over the
  * snapshot the last cycle started from -- what a scheduler's Score extension point would hand out.  The admission does
  * not read it (its visiting order comes from the anchor's domain ranges), so it is built on request; GROVE_TUNE_SCORE=1

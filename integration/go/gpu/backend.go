@@ -63,6 +63,11 @@ type schedulerBackend struct {
 	// starvation guard (SetStarvationGuard): off while guardMax == 0; rejectedFor: pending PodGang -> consecutive Unschedulable cycles
 	guardAfter, guardMax int
 	rejectedFor          map[string]int
+	// consolidation (SetConsolidation): off while consMax == 0; specOf: scheduled PodGang -> its spec (restated as a gated row to
+	// make it movable); moveAnchor: moved PodGang -> the first node of the placement the cycle planned for it
+	consAfter, consMax int
+	specOf             map[string]*groveschedulerv1alpha1.PodGang
+	moveAnchor         map[string]string
 	eng                  *engine
 	stopLoop chan struct{}
 }
@@ -212,6 +217,8 @@ func (b *schedulerBackend) OnPodGangDelete(_ context.Context, pg *grovescheduler
 	delete(b.running, key) // its pods' resources show up as free in the next node snapshot
 	delete(b.setOf, key)
 	delete(b.rejectedFor, key)
+	delete(b.specOf, key)
+	delete(b.moveAnchor, key)
 	return nil
 }
 
@@ -226,8 +233,44 @@ func (b *schedulerBackend) SetStarvationGuard(afterCycles, maxGangs int) error {
 	}
 	b.mu.Lock()
 	defer b.mu.Unlock()
+	if maxGangs > 0 && b.consMax > 0 {
+		return fmt.Errorf("starvation guard: the starvation guard and consolidation cannot both be on")
+	}
 	b.guardAfter, b.guardMax = afterCycles, maxGangs
 	return nil
+}
+
+// SetConsolidation makes, each cycle, the <= maxTargets highest-ranked pending PodGangs that came back Unschedulable at least
+// afterCycles cycles in a row (counted as the starvation guard counts) targets of grove_run_cycle_consolidate: running PodGangs
+// this backend scheduled, restated as gated rows, are relocated out of the domain closest to fitting a target when every one of
+// them is admitted elsewhere.  A moved PodGang gets DisruptionTarget naming the PodGang it made room for and is forgotten as
+// running; synced again, it is anchored at the first node of its planned placement.  A consolidated PodGang's Scheduled message
+// names the moved ones.  Only in a pass without preemption, topology spread members or large PodGangs; not together with the
+// starvation guard (GpuBackend::SetConsolidation in the C++ mirror).  maxTargets = 0 turns it off (the default).
+func (b *schedulerBackend) SetConsolidation(afterCycles, maxTargets int) error {
+	if afterCycles < 1 || maxTargets < 0 || maxTargets > int(C.GROVE_MAX_CONSOLIDATE_TARGETS) {
+		return fmt.Errorf("consolidation: want afterCycles >= 1 and 0 <= maxTargets <= %d", int(C.GROVE_MAX_CONSOLIDATE_TARGETS))
+	}
+	b.mu.Lock()
+	defer b.mu.Unlock()
+	if maxTargets > 0 && b.guardMax > 0 {
+		return fmt.Errorf("consolidation: the starvation guard and consolidation cannot both be on")
+	}
+	b.consAfter, b.consMax = afterCycles, maxTargets
+	return nil
+}
+
+// markMoved sets DisruptionTarget on a PodGang consolidation relocated (podgang.go:166-170); the caller's controllers delete its
+// pods, and the PodGang is synced and scheduled again at its planned place.
+func (b *schedulerBackend) markMoved(ctx context.Context, key string, target *groveschedulerv1alpha1.PodGang) {
+	ns, name, _ := strings.Cut(key, "/")
+	var pg groveschedulerv1alpha1.PodGang
+	if err := b.client.Get(ctx, client.ObjectKey{Namespace: ns, Name: name}, &pg); err != nil {
+		return
+	}
+	meta.SetStatusCondition(&pg.Status.Conditions, metav1.Condition{Type: string(groveschedulerv1alpha1.PodGangConditionTypeDisruptionTarget),
+		Status: metav1.ConditionTrue, Reason: "Consolidated", Message: "moved to make room for PodGang " + target.Namespace + "/" + target.Name})
+	_ = b.client.Status().Update(ctx, &pg)
 }
 
 // PreparePod keeps kube-scheduler away from the pod, as kai/backend.go:72-75 does.
@@ -381,11 +424,20 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 		b.encodeGang(t, pg, levels, podList.Items) // one grove_gang_t + its cliques / scopes; requests come from the pods
 		rows = append(rows, pg)
 	}
-	if spreadOn && !preempt && !wideAny {
-		nodeIdx := make(map[string]int, len(nodeNames))
-		for i, n := range nodeNames {
-			nodeIdx[n] = i
+	nodeIdx := make(map[string]int, len(nodeNames))
+	for i, n := range nodeNames {
+		nodeIdx[n] = i
+	}
+	b.mu.Lock()
+	for gi, pg := range rows { // moved by consolidation: anchored where the cycle planned it
+		if n, ok := b.moveAnchor[pg.Namespace+"/"+pg.Name]; ok {
+			if i, ok := nodeIdx[n]; ok {
+				t.gangs[gi].anchor_node = C.uint32_t(i)
+			}
 		}
+	}
+	b.mu.Unlock()
+	if spreadOn && !preempt && !wideAny {
 		b.mu.Lock()
 		b.encodeSpread(t, rows, levels, nodeIdx)
 		b.mu.Unlock()
@@ -406,6 +458,47 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 			t.fences = append(t.fences, C.uint32_t(gi))
 		}
 	}
+	// consolidation, in an ordinary pass only: the targets as the starvation guard counts, and every running PodGang this backend
+	// scheduled whole restated as a gated row after the pending ones (all its pods: MinReplicas = replicas)
+	var moved []string // running gang of t.running -> PodGang key
+	if b.consMax > 0 && !preempt && !wideAny && len(t.spreadGroups) == 0 {
+		for gi, pg := range rows {
+			if b.rejectedFor[pg.Namespace+"/"+pg.Name] >= b.consAfter {
+				t.targets = append(t.targets, C.uint32_t(gi))
+			}
+		}
+		sort.SliceStable(t.targets, func(i, j int) bool { return t.gangs[t.targets[i]].priority > t.gangs[t.targets[j]].priority })
+		if len(t.targets) > b.consMax {
+			t.targets = t.targets[:b.consMax]
+		}
+		for key, rg := range b.running {
+			spec, ok := b.specOf[key]
+			if _, pending := b.pending[key]; len(t.targets) == 0 || pending || !ok || whyNotEncodable(spec, false, false) != "" {
+				continue
+			}
+			row := len(t.gangs)
+			b.encodeGang(t, spec, levels, podList.Items)
+			t.gangs[row].flags |= C.GROVE_GANG_GATED
+			for c := int(t.gangs[row].clique_off); c < int(t.gangs[row].clique_off)+int(t.gangs[row].n_cliques); c++ {
+				t.cliques[c].min_replicas = t.cliques[c].replicas
+				t.counts[c].min_replicas = t.counts[c].replicas
+			}
+			r := C.grove_running_gang_t{priority: C.int32_t(rg.priority), holding_off: C.uint32_t(len(t.holdings))}
+			for node, h := range rg.held {
+				if i, ok := nodeIdx[node]; ok { // holdings on nodes that left the snapshot are dropped
+					t.holdings = append(t.holdings, C.grove_holding_t{node: C.uint32_t(i), cpu_milli: C.uint32_t(h.cpuMilli),
+						mem_mib: C.uint32_t(h.memMiB), gpu: C.uint16_t(h.gpu), pods: C.uint16_t(h.pods)})
+					r.n_holdings++
+				}
+			}
+			t.running = append(t.running, r)
+			t.specOf = append(t.specOf, C.uint32_t(row))
+			moved = append(moved, key)
+		}
+		if len(moved) == 0 {
+			t.targets = nil
+		}
+	}
 	rejectedFor := map[string]int{}
 	for k, v := range b.rejectedFor {
 		rejectedFor[k] = v
@@ -423,7 +516,7 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 	if b.rejectedFor == nil {
 		b.rejectedFor = map[string]int{}
 	}
-	for gi, st := range res.status { // consecutive Unschedulable cycles; a gated or base-not-scheduled cycle changes nothing
+	for gi, st := range res.status[:len(rows)] { // consecutive Unschedulable cycles; a gated or base-not-scheduled cycle changes nothing
 		key := rows[gi].Namespace + "/" + rows[gi].Name
 		if st.state == C.GROVE_GANG_REJECTED {
 			b.rejectedFor[key]++
@@ -431,10 +524,27 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 			delete(b.rejectedFor, key)
 		}
 	}
+	movedFor := map[int][]string{} // consolidated target row -> the PodGangs moved for it
+	for _, m := range res.moves {  // forgotten as running; anchored where this cycle planned it when synced again
+		key := moved[m.running]
+		st := res.status[t.specOf[m.running]]
+		delete(b.running, key)
+		delete(b.specOf, key)
+		if st.n_pods > 0 {
+			if b.moveAnchor == nil {
+				b.moveAnchor = map[string]string{}
+			}
+			b.moveAnchor[key] = nodeNames[res.placements[st.placement_off].node]
+		}
+		movedFor[int(m.target)] = append(movedFor[int(m.target)], key)
+	}
 	b.mu.Unlock()
 	seen := make([]int, len(t.cliques)) // the r-th entry of a clique binds its r-th PodReference
 	for _, pl := range res.placements {
 		gi, pgi := cliqueOwner(t, int(pl.clique))
+		if gi >= len(rows) { // a moved PodGang: its pods are deleted and it is scheduled anew when synced again
+			continue
+		}
 		ref := rows[gi].Spec.PodGroups[pgi].PodReferences[seen[pl.clique]]
 		seen[pl.clique]++
 		binding := &corev1.Binding{ObjectMeta: metav1.ObjectMeta{Namespace: ref.Namespace, Name: ref.Name},
@@ -443,7 +553,7 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 			return err
 		}
 	}
-	for gi, st := range res.status {
+	for gi, st := range res.status[:len(rows)] {
 		pg := rows[gi]
 		switch st.state {
 		case C.GROVE_GANG_ADMITTED:
@@ -454,6 +564,16 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 			if st.reserved0&C.GROVE_STATUS_SPREAD_SKEWED != 0 {
 				msg = "topology spread (ScheduleAnyway): no domain within the skew had room; placed beyond it"
 			}
+			if st.reserved0&C.GROVE_STATUS_CONSOLIDATED != 0 {
+				msg = "scheduled by moving PodGangs " + strings.Join(movedFor[gi], ", ")
+			}
+			b.mu.Lock()
+			if b.specOf == nil {
+				b.specOf = map[string]*groveschedulerv1alpha1.PodGang{}
+			}
+			b.specOf[pg.Namespace+"/"+pg.Name] = pg.DeepCopy()
+			delete(b.moveAnchor, pg.Namespace+"/"+pg.Name)
+			b.mu.Unlock()
 			meta.SetStatusCondition(&pg.Status.Conditions, metav1.Condition{Type: string(groveschedulerv1alpha1.PodGangConditionTypeScheduled),
 				Status: metav1.ConditionTrue, Reason: "Scheduled", Message: msg})
 			if _, scaled := pg.Labels[labelBasePodGang]; !scaled && pg.Labels[labelPartOf] != "" {
@@ -488,6 +608,9 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 	}
 	for _, v := range res.victims { // podgang.go:166-170, reason 1
 		b.markDisruptionTarget(ctx, int(v.running), rows[v.preemptor])
+	}
+	for _, m := range res.moves {
+		b.markMoved(ctx, moved[m.running], rows[m.target])
 	}
 	return nil
 }

@@ -62,12 +62,17 @@ type tables struct {
 	spreadSeeds  []C.grove_spread_seed_t
 	// fences (optional; ordinary passes only): the gang rows the starvation guard fences (grove_set_fences)
 	fences []C.uint32_t
+	// consolidation (optional; ordinary passes only, never with fences): the target rows, and for each running gang of `running`
+	// the gated row that restates it (grove_run_cycle_consolidate)
+	targets []C.uint32_t
+	specOf  []C.uint32_t
 }
 
 type result struct {
 	placements []C.grove_placement_t
 	status     []C.grove_gang_status_t
 	victims    []C.grove_victim_t
+	moves      []C.grove_move_t // consolidation: (running gang, target row) per relocated gang
 	stats      C.grove_cycle_stats_t
 	// explain, after an ordinary cycle with a rejected gang: why each rejected gang did not fit (grove_diagnose)
 	gangDiag   []C.grove_gang_diag_t
@@ -129,6 +134,25 @@ func (e *engine) cycle(t *tables, preempt, large, explain bool) (*result, error)
 				return nil, err
 			}
 		}
+	} else if len(t.targets) > 0 && len(t.running) > 0 {
+		var hp *C.grove_holding_t
+		if len(t.holdings) > 0 {
+			hp = &t.holdings[0]
+		}
+		if err := e.err(C.grove_run_cycle_consolidate(e.h, &t.targets[0], C.uint32_t(len(t.targets)), &t.specOf[0], &t.running[0],
+			C.uint32_t(len(t.running)), hp, C.uint32_t(len(t.holdings)), &r.stats)); err != nil {
+			return nil, err
+		}
+		var n C.uint32_t
+		if err := e.err(C.grove_get_moves(e.h, nil, 0, &n)); err != nil {
+			return nil, err
+		}
+		if n > 0 {
+			r.moves = make([]C.grove_move_t, int(n))
+			if err := e.err(C.grove_get_moves(e.h, &r.moves[0], n, &n)); err != nil {
+				return nil, err
+			}
+		}
 	} else if err := e.err(C.grove_run_cycle(e.h, &r.stats)); err != nil {
 		return nil, err
 	}
@@ -142,7 +166,7 @@ func (e *engine) cycle(t *tables, preempt, large, explain bool) (*result, error)
 	if err := e.err(C.grove_get_gang_status(e.h, &r.status[0], C.uint32_t(len(r.status)))); err != nil {
 		return nil, err
 	}
-	if explain && !(preempt && len(t.running) > 0) {
+	if explain && len(t.running) == 0 { // the running-gang cycles judge gangs against other views: grove_diagnose refuses them
 		for _, st := range r.status {
 			if st.state != C.GROVE_GANG_REJECTED {
 				continue
