@@ -851,7 +851,9 @@ constexpr int kEvalWarps = 8;
 // kFence: the instantiation of a cycle with fences (fence.cuh): the nodes of an active fence of a gang ranked before the evaluated
 // one fail K1 fit in every view it forms (staged attempts, unstaged reads, the record - total fast path).  The capacity tables and
 // shape bits come from the committed table and stay upper bounds.
-template <bool kPref, bool kHolds, bool kWide, bool kSpread = false, bool kFence = false>
+// kQueue: the instantiation of a cycle with queue members (queue.cuh): a member whose gate is closed is REJECTED without evaluation,
+// and an admitted member packs each clique's surplus up to the replicas k_queue_gate allows.
+template <bool kPref, bool kHolds, bool kWide, bool kSpread = false, bool kFence = false, bool kQueue = false>
 __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb, Relax rx, uint32_t max_att) {
   __shared__ GangShared shs[kEvalWarps];
   __shared__ int4 s_view[kEvalWarps][kStageMax];
@@ -904,6 +906,8 @@ __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb,
     const uint32_t le = rx.last_eval[gi], fu_word = rx.fail_upto[gi], ext_word = rx.extent[gi];
     uint32_t sp_grp = kFull;
     if constexpr (kSpread) sp_grp = rx.sp.group[gi];
+    uint32_t q_slot = kFull;
+    if constexpr (kQueue) q_slot = rx.qu.slot[gi];
     // ---- gangs that need no packing
     uint32_t trivial = 0;
     if (gg.flags & GROVE_GANG_GATED) trivial = GROVE_GANG_GATED_SKIP;
@@ -914,6 +918,7 @@ __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb,
       if (brank < info.order) bs = rx.tstate[gg.base_gang];   // final for ranks below the front; 0 (not evaluated yet) counts as not admitted: its first result marks us dirty
       if (bs != GROVE_GANG_ADMITTED) trivial = GROVE_GANG_BASE_REJECTED;
     }
+    if constexpr (kQueue) if (!trivial && q_slot != kFull && rx.qu.gate[q_slot]) trivial = GROVE_GANG_REJECTED;   // its queue chain has no room
     if (trivial) {
       if (tt == 0) {
         rx.nxt_tstate[gi] = uint8_t(trivial); rx.nxt_n[gi] = 0; rx.nxt_info[gi] = 0xFFu; rx.nxt_glo[gi] = GROVE_NONE_U32; rx.nxt_extent[gi] = 0;
@@ -1098,7 +1103,9 @@ __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb,
     if (!won) continue;   // warp-uniform: the winner finishes alone
     // surplus beyond MinReplicas (best effort, podgang.go:80-83), inside the domain each clique was packed into
     for (uint32_t cr = 0; cr < gg.n_cliques; ++cr) {
-      const uint32_t mn = clq_min<kWide>(sh, cr), rp = clq_rep<kWide>(sh, cr);
+      const uint32_t mn = clq_min<kWide>(sh, cr);
+      uint32_t rp = clq_rep<kWide>(sh, cr);
+      if constexpr (kQueue) if (q_slot != kFull) rp = rx.qu.cap[gg.clique_off + cr];
       if (rp > mn) { if (staged) evs.take(cr, sh.Hlo[cr], sh.Hhi[cr], rp - mn); else ev.take(cr, sh.Hlo[cr], sh.Hhi[cr], rp - mn); }
     }
     __syncwarp();

@@ -126,6 +126,24 @@ struct Fence {
   uint32_t n;
 };
 
+// Queue limits (grove_set_queues; kernels in queue.cuh), read only by the kQueue instantiations.  Only the queues with a finite
+// limit are kept ("scanned queues"); a (queue, member) pair per scanned queue of the member's chain, sorted by (queue, rank).
+struct Queue {
+  const uint32_t* slot;       // [G] member index of the gang (members in rank order), kFull = none
+  const uint32_t* mem;        // [M] gang of each member
+  const uint4* mem_pair;      // [M] the member's pairs, one per scanned queue of its chain (kFull = none)
+  const uint32_t* mem_fin;    // [M] 3 bits per pair of mem_pair: which resources of that queue have a finite limit
+  const long long* rmin;      // [M][3] R_min
+  const uint32_t* q_off;      // [scanned + 1] the queue's pairs
+  const long long* q_base;    // [scanned][3] limit - load (clamped to +-2^62)
+  const uint4* pr;            // [pairs] gang, member index, rank of the pair's member, in rank order within the queue
+  long long* head;            // [pairs][3] H_Q at the pair's member's turn (k_queue_scan)
+  unsigned long long* use;    // [M][3] U of the member's current tentative result (k_apply)
+  uint8_t* gate;              // [M] 1 = the gate is closed (k_queue_gate)
+  uint8_t* cap;               // [Q] MinReplicas + s_q of every clique of a member (k_queue_gate)
+  uint32_t n_mem;
+};
+
 // Relaxation state.  A gang's tentative result ("cur") lives in its own slots of the entry arrays and becomes final
 // in place; "nxt" is the scratch an evaluation writes before k_apply compares and publishes it.
 struct Relax {
@@ -194,6 +212,7 @@ struct Relax {
   uint32_t wide_cap;        // pods of the largest gang
   Spread sp;                // topology spread (the kSpread instantiations of k_eval / k_apply / k_detect)
   Fence fc;                 // fences (the kFence instantiations of k_eval / k_apply)
+  Queue qu;                 // queue limits (the kQueue instantiations of k_eval / k_apply)
 };
 
 // Is sorted node n inside a fence that is active for the evaluating gang?  m0 / m1: bit j of the 64 entries of `fc.list` is set

@@ -261,6 +261,14 @@ struct grove_engine {
   std::vector<grove_move_t> moves;
   DevBuf<uint4> d_cs_view;
   DevBuf<uint32_t> d_cs_have, d_cs_rank, d_cs_zero;
+  // queue limits (grove_set_queues; queue.cuh): the tables of the current submission's members; the queue kernels run only while
+  // there are some (qu_members > 0)
+  uint32_t qu_members = 0, qu_scanned = 0;
+  DevBuf<uint32_t> d_qu_slot, d_qu_mem, d_qu_mem_fin, d_qu_q_off;
+  DevBuf<uint4> d_qu_mem_pair, d_qu_pr;
+  DevBuf<long long> d_qu_rmin, d_qu_q_base, d_qu_head;
+  DevBuf<unsigned long long> d_qu_use;
+  DevBuf<uint8_t> d_qu_gate, d_qu_cap;
 };
 
 
@@ -280,6 +288,10 @@ static int32_t refuse_spread(grove_engine* e, const char* entry) {
 }
 static int32_t refuse_fences(grove_engine* e, const char* entry) {
   e->err = std::string(entry) + ": not supported while a fence set is in place (grove_set_fences)";
+  return GROVE_ERR_STATE;
+}
+static int32_t refuse_queues(grove_engine* e, const char* entry) {
+  e->err = std::string(entry) + ": not supported while a queue set with members is in place (grove_set_queues)";
   return GROVE_ERR_STATE;
 }
 static int32_t refuse_wide(grove_engine* e, const char* entry) {
@@ -448,6 +460,12 @@ static Relax make_relax(grove_engine* e) {
     sp.allowed = e->d_sp_allowed.p; sp.stamp = e->d_sp_stamp.p; sp.skewed = e->d_sp_skewed.p; sp.n_groups = e->sp_groups;
   }
   if (!e->fc_gangs.empty()) { r.fc.list = e->d_fc_list.p; r.fc.slot = e->d_fc_slot.p; r.fc.n = uint32_t(e->fc_gangs.size()); }
+  if (e->qu_members) {
+    Queue& qu = r.qu;
+    qu.slot = e->d_qu_slot.p; qu.mem = e->d_qu_mem.p; qu.mem_pair = e->d_qu_mem_pair.p; qu.mem_fin = e->d_qu_mem_fin.p; qu.rmin = e->d_qu_rmin.p;
+    qu.q_off = e->d_qu_q_off.p; qu.q_base = e->d_qu_q_base.p; qu.pr = e->d_qu_pr.p; qu.head = e->d_qu_head.p; qu.use = e->d_qu_use.p;
+    qu.gate = e->d_qu_gate.p; qu.cap = e->d_qu_cap.p; qu.n_mem = e->qu_members;
+  }
   return r;
 }
 
@@ -528,6 +546,7 @@ static int32_t load_nodes_common(grove_engine* e, const grove_node_t* host_nodes
   if (e->diag == grove_engine::kDiagReady || e->diag == grove_engine::kDiagSpread || e->diag == grove_engine::kDiagFence) e->diag = grove_engine::kDiagChanged;
   e->sp_groups = e->sp_members = 0;   // a spread set belongs to the nodes and gangs it was validated against
   e->fc_gangs.clear();                // (a fence set too)
+  e->qu_members = 0;                  // (and a queue set)
   CU_TRY(e, cudaSetDevice(e->cfg.device));
   if (host_nodes) {
     CU_TRY(e, cudaEventSynchronize(e->ev_nodes_up));  // an earlier upload may still be reading the staging buffer
@@ -686,6 +705,7 @@ static int32_t submit(grove_engine* e, const grove_gang_t* gangs, uint32_t n_gan
   if (n_gangs >= (1u << 24)) return fail(e, GROVE_ERR_LIMIT, "too many gangs");  // order rank + round tag share a stamp word
   e->sp_groups = e->sp_members = 0;
   e->fc_gangs.clear();
+  e->qu_members = 0;
   int32_t rc = validate(e, gangs, n_gangs, cliques, ccount.data(), n_cliques, scopes, n_scopes, max_pods);
   if (rc) return rc;
   CU_TRY(e, cudaSetDevice(e->cfg.device));
@@ -1112,6 +1132,12 @@ static int32_t finish_cycle(grove_engine* e) {
       CU_TRY(e, cudaGetLastError());
       e->launches += 1;
     }
+    if (e->qu_members) {   // the members' flags, from the headroom over the final states
+      k_queue_scan<<<e->qu_scanned, 256, 0, e->stream>>>(tb, rx, 1u);
+      k_queue_gate<<<(e->qu_members + 255) / 256, 256, 0, e->stream>>>(tb, rx, 2u, e->d_status.p);
+      CU_TRY(e, cudaGetLastError());
+      e->launches += 2;
+    }
     CU_TRY(e, cudaMemcpyAsync(e->h_ctl.p, e->d_totals.p, sizeof(uint32_t) * 4, cudaMemcpyDeviceToHost, e->stream));
     CU_TRY(e, cudaMemcpyAsync(e->h_status.p, e->d_status.p, sizeof(grove_gang_status_t) * G, cudaMemcpyDeviceToHost, e->stream));
     // the placement count is only known on the device: copy the upper bound's worth in the same breath when it is small,
@@ -1159,6 +1185,13 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
     e->launches += 1;
   }
   const bool fences = !e->fc_gangs.empty();   // (the running-gang entries and spread cycles refuse a fence set)
+  const bool queues = e->qu_members > 0;   // (the running-gang entries, spread and fenced cycles refuse a queue set)
+  if (G && queues) {   // the members' gates and caps before round 1: no member holds anything yet, H_Q = limit - load
+    k_queue_scan<<<e->qu_scanned, 256, 0, e->stream>>>(tb, rx, 0u);
+    k_queue_gate<<<(e->qu_members + 255) / 256, 256, 0, e->stream>>>(tb, rx, 0u, nullptr);
+    CU_TRY(e, cudaGetLastError());
+    e->launches += 2;
+  }
   if (G && fences) {   // the picks, over the cycle-start table
     const uint32_t nf = uint32_t(e->fc_gangs.size());
     CU_TRY(e, e->d_fc_have.ensure(std::max<size_t>(e->fc_words, 1)));
@@ -1222,6 +1255,17 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
         CU_TRY(e, launch_chained(k_apply<false, false, true>, warp_ctas, 256, e->stream, tb, rx));
         CU_TRY(e, launch_chained(k_detect<false>, warp_ctas, 256, e->stream, tp, tb, rx, e->tune_refresh));
         e->launches += 3;
+        ++next_round;
+        return GROVE_OK;
+      }
+      if (queues) {   // a queue cycle: its own instantiations of K3 and k_apply, then the headroom and the gates before k_detect
+        CU_TRY(e, launch_chained(e->any_preferred ? k_eval<true, false, false, false, false, true> : k_eval<false, false, false, false, false, true>,
+                                 n_eval_ctas, kEvalWarps * 32, e->stream, tp, tb, rx, e->tune_max_att));
+        CU_TRY(e, launch_chained(k_apply<false, false, false, true>, warp_ctas, 256, e->stream, tb, rx));
+        CU_TRY(e, launch_chained(k_queue_scan, e->qu_scanned, 256, e->stream, tb, rx, 0u));
+        CU_TRY(e, launch_chained(k_queue_gate, (e->qu_members + 255) / 256, 256, e->stream, tb, rx, 1u, (grove_gang_status_t*)nullptr));
+        CU_TRY(e, launch_chained(k_detect<false>, warp_ctas, 256, e->stream, tp, tb, rx, e->tune_refresh));
+        e->launches += 5;
         ++next_round;
         return GROVE_OK;
       }
@@ -1366,6 +1410,8 @@ int32_t grove_run_cycle(grove_engine_t* e, grove_cycle_stats_t* stats) {
   if (!e) return GROVE_ERR_INVALID_ARG;
   const bool spread = e->sp_members > 0, fences = !e->fc_gangs.empty();
   if (spread && fences) return fail(e, GROVE_ERR_STATE, "grove_run_cycle: a spread set with members and a fence set together are not supported");
+  if (e->qu_members && (spread || fences))
+    return fail(e, GROVE_ERR_STATE, "grove_run_cycle: a queue set with members together with a spread set with members or a fence set is not supported");
   const int32_t rc = run_cycle(e, stats);
   if (rc == GROVE_OK) e->diag = spread ? grove_engine::kDiagSpread : fences ? grove_engine::kDiagFence : grove_engine::kDiagReady;
   return rc;
@@ -1529,6 +1575,112 @@ int32_t grove_set_fences(grove_engine_t* e, const uint32_t* gangs, uint32_t n) {
 }
 
 // ---------------------------------------------------------------------------------------------
+// Queue limits (include/grove_place.h "queue limits"; DESIGN.md section 1; kernels in queue.cuh).  Validated against the submission;
+// the tables the kernels read are built here once: the members in rank order with their chains and R_min, the queues with a
+// finite limit with limit - load, and the (queue, member) pairs sorted by (queue, rank).
+// ---------------------------------------------------------------------------------------------
+int32_t grove_set_queues(grove_engine_t* e, const grove_queue_t* queues, uint32_t n_queues, const uint32_t* gang_queue, uint32_t n_gangs) {
+  if (!e) return GROVE_ERR_INVALID_ARG;
+  if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
+  if (!e->nodes_loaded || !e->gangs_loaded) return fail(e, GROVE_ERR_STATE, "grove_set_queues: load nodes and submit gangs first");
+  if ((n_queues && !queues) || (n_gangs && !gang_queue)) return GROVE_ERR_INVALID_ARG;
+  if (n_gangs != e->G) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_queues: n_gangs is not the number of submitted gangs");
+  if (n_queues > GROVE_MAX_QUEUES) return fail(e, GROVE_ERR_LIMIT, "grove_set_queues: more than GROVE_MAX_QUEUES queues");
+  if (e->wide) return refuse_wide(e, "grove_set_queues");
+  std::vector<uint32_t> depth(n_queues, 1);
+  for (uint32_t q = 0; q < n_queues; ++q) {
+    const uint32_t p = queues[q].parent;
+    if (p == GROVE_NONE_U32) continue;
+    if (p >= q) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_queues: a parent must come before its queue");
+    depth[q] = depth[p] + 1;
+    if (depth[q] > GROVE_MAX_QUEUE_DEPTH) return fail(e, GROVE_ERR_LIMIT, "grove_set_queues: a chain deeper than GROVE_MAX_QUEUE_DEPTH");
+  }
+  for (uint32_t g = 0; g < n_gangs; ++g)
+    if (gang_queue[g] != GROVE_NONE_U32 && gang_queue[g] >= n_queues) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_queues: queue index out of range");
+  e->qu_members = e->qu_scanned = 0;
+  // load = own used + the descendants' (parents come first: one pass from the back), saturating; limit - load in signed 64 bits,
+  // both clamped to 2^62 (no gang asks for that much, so no decision changes)
+  constexpr uint64_t kClamp = uint64_t(1) << 62;
+  std::vector<uint64_t> load(size_t(n_queues) * 3);
+  for (uint32_t q = 0; q < n_queues; ++q) for (int r = 0; r < 3; ++r) load[q * 3 + r] = std::min(queues[q].used[r], kClamp);
+  for (uint32_t q = n_queues; q-- > 0;)
+    if (queues[q].parent != GROVE_NONE_U32)
+      for (int r = 0; r < 3; ++r) load[queues[q].parent * 3 + r] = std::min(load[queues[q].parent * 3 + r] + load[q * 3 + r], kClamp);
+  std::vector<uint32_t> scan_id(n_queues, GROVE_NONE_U32);   // the queues with a finite limit, renumbered
+  std::vector<long long> q_base;
+  uint32_t scanned = 0;
+  for (uint32_t q = 0; q < n_queues; ++q) {
+    bool fin = false;
+    for (int r = 0; r < 3; ++r) fin |= queues[q].limit[r] != GROVE_QUEUE_UNLIMITED;
+    if (!fin) continue;
+    scan_id[q] = scanned++;
+    for (int r = 0; r < 3; ++r)
+      q_base.push_back(queues[q].limit[r] == GROVE_QUEUE_UNLIMITED ? 0ll : (long long)std::min(queues[q].limit[r], kClamp) - (long long)load[q * 3 + r]);
+  }
+  // members in rank order; a gang whose chain has no finite limit is not one (it would behave as a non-member anyway)
+  const uint32_t G = n_gangs;
+  std::vector<uint32_t> order(G);
+  std::iota(order.begin(), order.end(), 0u);
+  std::stable_sort(order.begin(), order.end(), [e](uint32_t a, uint32_t b) { return e->gangs[a].priority > e->gangs[b].priority; });
+  std::vector<uint32_t> slot(G, GROVE_NONE_U32), mem, mem_fin, chains, q_off(scanned + 1, 0);
+  std::vector<long long> rmin;
+  for (uint32_t g : order) {
+    if (gang_queue[g] == GROVE_NONE_U32) continue;
+    uint32_t chain[GROVE_MAX_QUEUE_DEPTH] = {GROVE_NONE_U32, GROVE_NONE_U32, GROVE_NONE_U32, GROVE_NONE_U32}, n = 0, fin = 0;
+    for (uint32_t q = gang_queue[g]; q != GROVE_NONE_U32; q = queues[q].parent) {
+      if (scan_id[q] == GROVE_NONE_U32) continue;
+      for (int r = 0; r < 3; ++r) if (queues[q].limit[r] != GROVE_QUEUE_UNLIMITED) fin |= 1u << (3 * n + r);
+      ++q_off[scan_id[q] + 1];
+      chain[n++] = scan_id[q];
+    }
+    if (!n) continue;
+    slot[g] = uint32_t(mem.size()); mem.push_back(g); mem_fin.push_back(fin);
+    chains.insert(chains.end(), chain, chain + GROVE_MAX_QUEUE_DEPTH);
+    const grove_gang_t& gg = e->gangs[g];
+    long long R[3] = {0, 0, 0};
+    for (uint32_t c = 0; c < gg.n_cliques; ++c) {
+      const grove_clique_t& q = e->cliques[gg.clique_off + c];
+      R[0] += (long long)q.min_replicas * q.req_cpu_milli; R[1] += (long long)q.min_replicas * q.req_mem_mib; R[2] += (long long)q.min_replicas * q.req_gpu;
+    }
+    rmin.insert(rmin.end(), R, R + 3);
+  }
+  if (mem.empty()) return GROVE_OK;   // nothing to limit: the ordinary cycle
+  for (uint32_t q = 0; q < scanned; ++q) q_off[q + 1] += q_off[q];
+  // the pairs: members are taken in rank order, so each queue's pairs come out in rank order
+  std::vector<uint32_t> fill(q_off.begin(), q_off.end() - 1);
+  // the rank of every gang.  GangInfo::order is only built when the cycle starts (build_ginfo); it is the same order --
+  // priority desc, then submission index asc, which this stable sort over the submission gives -- and k_queue_scan's bound test
+  // (pr.z) and k_queue_gate's (GangInfo::order) rely on the two being equal
+  std::vector<uint32_t> rank_of(G);
+  for (uint32_t k = 0; k < G; ++k) rank_of[order[k]] = k;
+  std::vector<uint4> pr_list(q_off[scanned]);
+  std::vector<uint4> mem_pair(mem.size());
+  for (size_t j = 0; j < mem.size(); ++j) {
+    uint32_t pr[GROVE_MAX_QUEUE_DEPTH];
+    for (uint32_t k = 0; k < GROVE_MAX_QUEUE_DEPTH; ++k) {
+      const uint32_t q = chains[j * GROVE_MAX_QUEUE_DEPTH + k];
+      pr[k] = q == GROVE_NONE_U32 ? GROVE_NONE_U32 : fill[q]++;
+      if (q != GROVE_NONE_U32) pr_list[pr[k]] = make_uint4(mem[j], uint32_t(j), rank_of[mem[j]], 0u);
+    }
+    mem_pair[j] = make_uint4(pr[0], pr[1], pr[2], pr[3]);
+  }
+  const uint32_t M = uint32_t(mem.size()), P = q_off[scanned];
+  CU_TRY(e, cudaSetDevice(e->cfg.device));
+  auto up = [e](auto& d, const auto& h) -> cudaError_t {
+    cudaError_t c = d.ensure(std::max<size_t>(h.size(), 1));
+    if (c == cudaSuccess && !h.empty()) c = cudaMemcpyAsync(d.p, h.data(), sizeof(h[0]) * h.size(), cudaMemcpyHostToDevice, e->stream);
+    return c;
+  };
+  CU_TRY(e, up(e->d_qu_slot, slot)); CU_TRY(e, up(e->d_qu_mem, mem)); CU_TRY(e, up(e->d_qu_mem_pair, mem_pair)); CU_TRY(e, up(e->d_qu_mem_fin, mem_fin));
+  CU_TRY(e, up(e->d_qu_rmin, rmin)); CU_TRY(e, up(e->d_qu_q_off, q_off)); CU_TRY(e, up(e->d_qu_q_base, q_base)); CU_TRY(e, up(e->d_qu_pr, pr_list));
+  CU_TRY(e, e->d_qu_head.ensure(size_t(P) * 3)); CU_TRY(e, e->d_qu_use.ensure(size_t(M) * 3));
+  CU_TRY(e, e->d_qu_gate.ensure(M)); CU_TRY(e, e->d_qu_cap.ensure(std::max<uint32_t>(e->Q, 1)));
+  CU_TRY(e, cudaStreamSynchronize(e->stream));   // (the host vectors go out of scope)
+  e->qu_members = M; e->qu_scanned = scanned;
+  return GROVE_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
 // Diagnosis (include/grove_place.h "diagnosis of rejected gangs"; DESIGN.md section 1; kernels in diagnose.cuh).  Reads the
 // outputs of the last ordinary cycle on the device (committed table, placements, ranks) and writes only its own buffers.
 // ---------------------------------------------------------------------------------------------
@@ -1559,7 +1711,7 @@ int32_t grove_diagnose(grove_engine_t* e, grove_gang_diag_t* gangs, uint32_t cap
   std::vector<uint32_t> batch_at{0};
   std::vector<size_t> batch_cols{0};
   for (uint32_t g = 0; g < G; ++g) {
-    if (e->h_status.p[g].state != GROVE_GANG_REJECTED) continue;
+    if (e->h_status.p[g].state != GROVE_GANG_REJECTED || (e->h_status.p[g].reserved0 & GROVE_STATUS_OVER_LIMIT)) continue;
     const grove_gang_t& x = e->gangs[g];
     DiagGang d{};
     d.gang = g; d.rank = e->ginfo[g].order; d.n_cliques = x.n_cliques; d.level = x.level;
@@ -1654,6 +1806,7 @@ int32_t grove_run_cycle_preempt(grove_engine_t* e, const grove_running_gang_t* r
                                 const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
   if (!e || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
   if (e->sp_members) return refuse_spread(e, "grove_run_cycle_preempt");
+  if (e->qu_members) return refuse_queues(e, "grove_run_cycle_preempt");
   if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_preempt");
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_preempt");
@@ -1913,6 +2066,7 @@ int32_t grove_run_cycle_reuse(grove_engine_t* e, const uint32_t* replaces, uint3
                               uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
   if (!e || (n_gangs && !replaces) || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
   if (e->sp_members) return refuse_spread(e, "grove_run_cycle_reuse");
+  if (e->qu_members) return refuse_queues(e, "grove_run_cycle_reuse");
   if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_reuse");
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse");
@@ -1972,6 +2126,7 @@ int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replace
                                       uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
   if (!e || (n_gangs && !replaces) || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
   if (e->sp_members) return refuse_spread(e, "grove_run_cycle_reuse_preempt");
+  if (e->qu_members) return refuse_queues(e, "grove_run_cycle_reuse_preempt");
   if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_reuse_preempt");
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse_preempt");
@@ -2200,6 +2355,7 @@ int32_t grove_run_cycle_consolidate(grove_engine_t* e, const uint32_t* targets, 
                                     uint32_t n_holdings, grove_cycle_stats_t* stats) {
   if (!e || (n_targets && !targets) || (n_running && (!running || !spec_of)) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
   if (e->sp_members) return refuse_spread(e, "grove_run_cycle_consolidate");
+  if (e->qu_members) return refuse_queues(e, "grove_run_cycle_consolidate");
   if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_consolidate");
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_consolidate");

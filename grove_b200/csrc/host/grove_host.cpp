@@ -3,6 +3,8 @@
 #include "grove_host.hpp"
 
 #include <algorithm>
+#include <array>
+#include <cstdint>
 #include <set>
 
 namespace grove::host {
@@ -263,7 +265,30 @@ Err GpuBackend::OnPodGangDelete(const PodGang& podGang) {
   std::lock_guard<std::mutex> l(mu_);
   const std::string key = podGang.Namespace + "/" + podGang.Name;
   pending_.erase(key); bound_.erase(key); running_.erase(key); setOf_.erase(key); rejectedFor_.erase(key);
-  specOf_.erase(key); moveAnchor_.erase(key);
+  specOf_.erase(key); moveAnchor_.erase(key); queueOf_.erase(key);
+  return std::nullopt;
+}
+
+Err GpuBackend::SetQueue(const std::string& name, std::optional<Queue> queue) {
+  std::lock_guard<std::mutex> l(mu_);
+  if (name.empty()) return mkerr("ERR_SYNC_PODGANG", "SetQueue", "a queue needs a name");
+  if (!queue) {
+    for (const auto& [n, q] : queues_)
+      if (q.Parent == name) return mkerr("ERR_SYNC_PODGANG", "SetQueue", "queue " + name + " is the parent of queue " + n);
+    queues_.erase(name);
+    return std::nullopt;
+  }
+  uint32_t depth = 1;
+  for (std::string p = queue->Parent; !p.empty(); p = queues_.at(p).Parent) {
+    if (p == name) return mkerr("ERR_SYNC_PODGANG", "SetQueue", "queue " + name + " would be its own ancestor");
+    if (!queues_.count(p)) return mkerr("ERR_SYNC_PODGANG", "SetQueue", "queue " + name + ": parent queue " + p + " is not set");
+    if (++depth > GROVE_MAX_QUEUE_DEPTH) return mkerr("ERR_SYNC_PODGANG", "SetQueue", "queue " + name + ": chain deeper than GROVE_MAX_QUEUE_DEPTH");
+  }
+  for (const auto& [n, q] : queues_)   // a queue that is a parent keeps its place in the tree
+    if (q.Parent == name && queues_.at(name).Parent != queue->Parent)
+      return mkerr("ERR_SYNC_PODGANG", "SetQueue", "queue " + name + " is the parent of queue " + n + ": its parent cannot change");
+  if (!queues_.count(name) && queues_.size() >= GROVE_MAX_QUEUES) return mkerr("ERR_SYNC_PODGANG", "SetQueue", "more than GROVE_MAX_QUEUES queues");
+  queues_[name] = *queue;
   return std::nullopt;
 }
 
@@ -418,6 +443,28 @@ Err GpuBackend::EncodeLocked(const std::vector<Node>& nodes, Tables* out, const 
           out->skipped[kv.first] = runningCycles ? "topology spread is not applied while preemption or reservation reuse is on"
                                                  : "topology spread is not applied in a pass with PodGangs beyond the ordinary limits";
   }
+  // queue limits: the members of a known queue.  The running-gang cycles, consolidation, fences, spread sets and wide submissions
+  // take no queue set: while one of them may run, the members stay out of the pass
+  auto queueOfPg = [this](const PodGang& pg) -> std::string {
+    auto it = pg.Labels.find(kQueueLabel);
+    return it != pg.Labels.end() && queues_.count(it->second) ? it->second : std::string();
+  };
+  if (!queues_.empty()) {
+    bool wideAny = false, spreadAny = false;
+    for (const auto& kv : pending_) {
+      if (out->skipped.count(kv.first)) continue;
+      wideAny |= large_ && !WhyNotEncodable(kv.second, false).empty();
+      spreadAny |= spreadSetOf(kv.second) != nullptr;
+    }
+    const char* why = runningCycles ? "queue limits are not applied while preemption or reservation reuse is on"
+                      : consMax_ ? "queue limits are not applied while consolidation is on"
+                      : guardMax_ ? "queue limits are not applied while the starvation guard is on"
+                      : spreadAny ? "queue limits are not applied in a pass with topology spread members"
+                      : wideAny ? "queue limits are not applied in a pass with PodGangs beyond the ordinary limits" : nullptr;
+    if (why)
+      for (const auto& kv : pending_)
+        if (!out->skipped.count(kv.first) && !queueOfPg(kv.second).empty()) out->skipped[kv.first] = why;
+  }
   for (const auto& kv : pending_)
     if (!out->skipped.count(kv.first) && !kv.second.BasePodGangName.empty() && out->skipped.count(kv.second.Namespace + "/" + kv.second.BasePodGangName))
       out->skipped[kv.first] = "base PodGang " + kv.second.BasePodGangName + " cannot be scheduled: " + out->skipped[kv.second.Namespace + "/" + kv.second.BasePodGangName];
@@ -552,6 +599,8 @@ Err GpuBackend::EncodeLocked(const std::vector<Node>& nodes, Tables* out, const 
       if (s != GROVE_NONE_U32 && need && g.level != GROVE_LEVEL_NONE && g.level >= out->spreadGroups[s].level) grp = s;
     }
     out->spreadOf.push_back(grp);
+    const std::string qn = spec ? std::string() : queueOfPg(pg);   // (a gated spec row is never evaluated)
+    out->queueOf.push_back(qn.empty() ? GROVE_NONE_U32 : uint32_t(std::distance(queues_.begin(), queues_.find(qn))));
     out->gangs.push_back(g);
     out->gangNames.push_back(key);
     out->remainder.push_back(remainder ? 1 : 0);
@@ -565,6 +614,31 @@ Err GpuBackend::EncodeLocked(const std::vector<Node>& nodes, Tables* out, const 
       if (auto nt = nodeIndex.find(ln->second); nt != nodeIndex.end()) out->spreadSeeds.push_back(grove_spread_seed_t{gi->second, nt->second});
     }
   else { out->spreadGroups.clear(); out->spreadSet.clear(); }
+  // the queue table, parents first (ordered by depth, then name), with what the running PodGangs of each queue hold
+  if (std::any_of(out->queueOf.begin(), out->queueOf.end(), [](uint32_t x) { return x != GROVE_NONE_U32; })) {
+    auto depth = [this](const std::string& n) { uint32_t d = 0; for (std::string p = queues_.at(n).Parent; !p.empty(); p = queues_.at(p).Parent) ++d; return d; };
+    std::vector<std::string> names;
+    for (const auto& kv : queues_) names.push_back(kv.first);
+    std::stable_sort(names.begin(), names.end(), [&](const std::string& a, const std::string& b) { return depth(a) < depth(b); });
+    std::map<std::string, uint32_t> idx;
+    for (uint32_t i = 0; i < names.size(); ++i) idx[names[i]] = i;
+    for (const std::string& n : names) {
+      const Queue& q = queues_.at(n);
+      grove_queue_t r{};
+      r.parent = q.Parent.empty() ? GROVE_NONE_U32 : idx.at(q.Parent);
+      r.limit[0] = q.CpuMilli.value_or(GROVE_QUEUE_UNLIMITED); r.limit[1] = q.MemMiB.value_or(GROVE_QUEUE_UNLIMITED); r.limit[2] = q.Gpu.value_or(GROVE_QUEUE_UNLIMITED);
+      out->queues.push_back(r);
+    }
+    for (const auto& [key, qn] : queueOf_) {
+      auto it = idx.find(qn); auto rg = running_.find(key);
+      if (it == idx.end() || rg == running_.end()) continue;
+      for (const Held& h : rg->second.held) { out->queues[it->second].used[0] += h.cpu_milli; out->queues[it->second].used[1] += h.mem_mib; out->queues[it->second].used[2] += h.gpu; }
+    }
+    std::vector<uint32_t> byName(queues_.size());   // queueOf holds positions in queues_ (by name): renumber
+    { uint32_t k = 0; for (const auto& kv : queues_) byName[k++] = idx.at(kv.first); }
+    for (uint32_t& x : out->queueOf) if (x != GROVE_NONE_U32) x = byName[x];
+    out->queueNames = names;
+  } else out->queueOf.assign(out->queueOf.size(), GROVE_NONE_U32);
   return std::nullopt;
 }
 
@@ -613,7 +687,7 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
       }
       if (targets.empty()) {   // drop the spec rows (they come last)
         const uint32_t r = t.specRow, q = t.gangs[r].clique_off, sc = t.gangs[r].scope_off;
-        t.gangs.resize(r); t.gangNames.resize(r); t.remainder.resize(r); t.spreadOf.resize(r);
+        t.gangs.resize(r); t.gangNames.resize(r); t.remainder.resize(r); t.spreadOf.resize(r); t.queueOf.resize(r);
         t.cliques.resize(q); t.counts.resize(q); t.cliqueOf.resize(q); t.refBase.resize(q); t.scopes.resize(sc);
       } else {   // the movable running PodGangs with what they hold (holdings on nodes that left the snapshot are dropped)
         std::map<std::string, uint32_t> nodeIdx;
@@ -648,6 +722,8 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
   if (spread)
     if (auto e = chk(grove_set_spread(engine_, t.spreadGroups.data(), uint32_t(t.spreadGroups.size()), t.spreadOf.data(), uint32_t(t.spreadOf.size()),
                                       t.spreadSeeds.data(), uint32_t(t.spreadSeeds.size())), "grove_set_spread")) return e;
+  if (!t.queues.empty())   // (Encode keeps the queue table only when a row is a member, and only in a pass that takes one)
+    if (auto e = chk(grove_set_queues(engine_, t.queues.data(), uint32_t(t.queues.size()), t.queueOf.data(), uint32_t(t.queueOf.size())), "grove_set_queues")) return e;
   grove_cycle_stats_t st{};
   // running PodGangs -> the reclaim pass's / reservation reuse's tables (holdings on nodes that left the snapshot are dropped)
   std::vector<grove_running_gang_t> run; std::vector<grove_holding_t> held; std::vector<std::string> runNames;
@@ -777,6 +853,7 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
           (*statuses)[t.gangNames[g]].ScheduledMessage = ExplainRejection(t, snap.at(t.gangNames[g]), g, gd[g], qd.data(), levels);
   }
   for (const auto& [key, msg] : spreadMsg) (*statuses)[key].ScheduledMessage = msg;
+  for (const auto& [key, msg] : QueueMessages(t, gs, pl)) (*statuses)[key].ScheduledMessage = msg;
   // consolidation: a moved PodGang is disrupted (the caller deletes its pods); a consolidated one names the PodGangs it moved
   std::vector<grove_move_t> moves;
   if (consolidate) {
@@ -865,6 +942,7 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
       }
     }
     if (gs[i].n_pods && !lastNode_.count(key)) lastNode_[key] = nodes[pl[gs[i].placement_off].node].Name;
+    if (t.queueOf[i] != GROVE_NONE_U32) queueOf_[key] = t.queueNames[t.queueOf[i]];   // what it holds counts against its queue
     if (pg.BasePodGangName.empty())   // a replica of its PodCliqueSet from now on (topology spread counts it where it landed)
       if (auto it = pg.Labels.find(kPartOfLabel); it != pg.Labels.end()) setOf_[key] = pg.Namespace + "/" + it->second;
     std::vector<uint32_t>& done = bound_[key];
@@ -882,6 +960,71 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
     if (all) { pending_.erase(key); bound_.erase(key); }
   }
   return std::nullopt;
+}
+
+// The queue messages of a cycle, restated from its results in rank order (DESIGN.md section 1 "Queue limits"): the headroom each
+// member met, from the queues' limits and loads and what the admitted members ranked before it took.
+std::map<std::string, std::string> GpuBackend::QueueMessages(const Tables& t, const std::vector<grove_gang_status_t>& gs,
+                                                             const std::vector<grove_placement_t>& pl) {
+  std::map<std::string, std::string> msg;
+  if (t.queues.empty()) return msg;
+  static const char* kRes[3] = {"cpu (millicores)", "memory (MiB)", "GPUs"};
+  const size_t nq = t.queues.size();
+  std::vector<std::array<int64_t, 3>> load(nq);
+  for (size_t q = 0; q < nq; ++q) for (int r = 0; r < 3; ++r) load[q][r] = int64_t(t.queues[q].used[r]);
+  for (size_t q = nq; q-- > 0;)   // parents come first: a queue's load is its own and its descendants'
+    if (t.queues[q].parent != GROVE_NONE_U32) for (int r = 0; r < 3; ++r) load[t.queues[q].parent][r] += load[q][r];
+  std::vector<uint32_t> order;
+  for (uint32_t g = 0; g < t.queueOf.size(); ++g) if (t.queueOf[g] != GROVE_NONE_U32) order.push_back(g);
+  std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return t.gangs[a].priority > t.gangs[b].priority; });
+  auto finite = [&](size_t q, int r) { return t.queues[q].limit[r] != GROVE_QUEUE_UNLIMITED; };
+  for (uint32_t g : order) {
+    if (gs[g].state != GROVE_GANG_ADMITTED && gs[g].state != GROVE_GANG_REJECTED) continue;   // gated, or its base was not scheduled
+    const grove_gang_t& gg = t.gangs[g];
+    int64_t R[3] = {0, 0, 0};
+    for (uint32_t c = gg.clique_off; c < gg.clique_off + gg.n_cliques; ++c) {
+      const int64_t m = t.counts[c].min_replicas;
+      R[0] += m * t.cliques[c].req_cpu_milli; R[1] += m * t.cliques[c].req_mem_mib; R[2] += m * t.cliques[c].req_gpu;
+    }
+    std::vector<uint32_t> chain;
+    for (uint32_t q = t.queueOf[g]; q != GROVE_NONE_U32; q = t.queues[q].parent) chain.push_back(q);
+    if (gs[g].reserved0 & GROVE_STATUS_OVER_LIMIT) {   // the first queue of the chain, leaf first, and the resource without room
+      for (uint32_t q : chain) {
+        int r = 0;
+        while (r < 3 && !(finite(q, r) && R[r] > 0 && R[r] > int64_t(t.queues[q].limit[r]) - load[q][r])) ++r;
+        if (r == 3) continue;
+        msg[t.gangNames[g]] = "queue " + t.queueNames[q] + " has no room for this PodGang: " + kRes[r] + " limit " +
+                              std::to_string(t.queues[q].limit[r]) + ", load " + std::to_string(load[q][r]) + ", MinReplicas need " + std::to_string(R[r]);
+        break;
+      }
+      continue;
+    }
+    if (gs[g].state != GROVE_GANG_ADMITTED) continue;
+    if (gs[g].reserved0 & GROVE_STATUS_SURPLUS_CAPPED) {   // s_q clique by clique, as the engine caps the surplus
+      int64_t rem[3];
+      bool fin[3] = {false, false, false};
+      for (int r = 0; r < 3; ++r) {
+        rem[r] = INT64_MAX;
+        for (uint32_t q : chain) if (finite(q, r)) { fin[r] = true; rem[r] = std::min(rem[r], int64_t(t.queues[q].limit[r]) - load[q][r]); }
+        if (fin[r]) rem[r] -= R[r];
+      }
+      int64_t held = 0;
+      for (uint32_t c = gg.clique_off; c < gg.clique_off + gg.n_cliques; ++c) {
+        const int64_t extra = int64_t(t.counts[c].replicas) - t.counts[c].min_replicas;
+        const int64_t req[3] = {t.cliques[c].req_cpu_milli, t.cliques[c].req_mem_mib, t.cliques[c].req_gpu};
+        int64_t sq = extra;
+        for (int r = 0; r < 3; ++r) if (fin[r] && req[r] > 0) sq = rem[r] < 0 ? 0 : std::min(sq, rem[r] / req[r]);
+        for (int r = 0; r < 3; ++r) if (fin[r]) rem[r] -= sq * req[r];
+        held += extra - sq;
+      }
+      msg[t.gangNames[g]] = "queue limits held back " + std::to_string(held) + " best-effort pods of this PodGang";
+    }
+    for (uint32_t k = 0; k < gs[g].n_pods; ++k) {   // it charges what it took to every queue of its chain
+      const grove_clique_t& c = t.cliques[pl[gs[g].placement_off + k].clique];
+      for (uint32_t q : chain) { load[q][0] += c.req_cpu_milli; load[q][1] += c.req_mem_mib; load[q][2] += c.req_gpu; }
+    }
+  }
+  return msg;
 }
 
 std::string GpuBackend::ExplainRejection(const Tables& t, const PodGang& pg, uint32_t row, const grove_gang_diag_t& gd,

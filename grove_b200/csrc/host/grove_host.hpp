@@ -204,6 +204,13 @@ struct TopologySpread {
   std::string WhenUnsatisfiable = "DoNotSchedule";    // or "ScheduleAnyway"
 };
 
+// a KAI queue's hard limits (scheduling.run.ai/v2 Queue: spec.parentQueue, spec.resources.{cpu,memory,gpu}.limit; DESIGN.md
+// section 1 "Queue limits"), in the engine's units: millicores, MiB, GPUs.  nullopt = no limit (KAI's -1).
+struct Queue {
+  std::string Parent;                            // "" = a root queue; otherwise a queue set earlier
+  std::optional<uint64_t> CpuMilli, MemMiB, Gpu;
+};
+
 // packed tables of one cycle, as handed to libgrove_place.so
 struct Tables {
   std::vector<grove_node_t> nodes;
@@ -221,6 +228,11 @@ struct Tables {
   std::vector<uint32_t> spreadOf;
   std::vector<grove_spread_seed_t> spreadSeeds;
   std::vector<std::string> spreadSet;                   // group -> "<ns>/<PodCliqueSet>"
+  // queue limits (SetQueue): the queues (parents first) with what the running PodGangs of each hold, each gang row's queue
+  // (GROVE_NONE_U32: none)
+  std::vector<grove_queue_t> queues;
+  std::vector<std::string> queueNames;
+  std::vector<uint32_t> queueOf;
   // consolidation (SetConsolidation): rows [specRow, gangs.size()) are gated rows restating running PodGangs, which makes them
   // movable (grove_run_cycle_consolidate's spec rows); specRow == gangs.size() when there are none
   uint32_t specRow = 0;
@@ -314,6 +326,19 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   // reuse, topology spread members or PodGangs beyond the ordinary limits.  maxTargets = 0 turns it off (the default);
   // afterCycles >= 1, maxTargets <= GROVE_MAX_CONSOLIDATE_TARGETS; it cannot be on together with the starvation guard.
   Err SetConsolidation(uint32_t afterCycles, uint32_t maxTargets);
+  // Queue limits (grove_set_queues; DESIGN.md section 1 "Queue limits"): a pending PodGang whose kai.scheduler/queue label names
+  // a queue set here is a member of it (a label naming an unknown queue makes it a non-member); what the PodGangs this backend
+  // scheduled hold counts against their queue and its ancestors.  A member whose queue chain has no room for its MinReplicas is
+  // Unschedulable with a ScheduledMessage naming the first queue of its chain (leaf first) and the resource that had no room, with
+  // limit and load; a scheduled member whose best-effort pods the limits held back says how many.  With preemption, reservation
+  // reuse, reuse with reclaim, consolidation or the starvation guard on, or in a pass with topology spread members or a PodGang
+  // beyond the ordinary limits, members stay out of the pass, Unschedulable with a reason.  A parent must be set before its
+  // children, chains are at most GROVE_MAX_QUEUE_DEPTH deep; nullopt removes a queue (not one that is a parent).  Off by default.
+  Err SetQueue(const std::string& name, std::optional<Queue> queue);
+  // the ScheduledMessages of the queue members of one cycle of `t` (gs, pl: its statuses and placements)
+  static std::map<std::string, std::string> QueueMessages(const Tables& t, const std::vector<grove_gang_status_t>& gs,
+                                                          const std::vector<grove_placement_t>& pl);
+  static constexpr const char* kQueueLabel = "kai.scheduler/queue";
   static constexpr const char* kPartOfLabel = "app.kubernetes.io/part-of";
   size_t Running() const { std::lock_guard<std::mutex> l(mu_); return running_.size(); }
   // why a PodGang cannot be handed to the engine (limits of the packed tables), or empty.  SyncPodGang accepts every
@@ -356,6 +381,8 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   std::map<std::string, std::string> moveAnchor_;      // moved PodGang -> the first node of its planned placement (anchor)
   std::map<std::string, TopologySpread> spread_;       // PodCliqueSet name -> its spread
   std::map<std::string, std::string> setOf_;           // scheduled base PodGang -> "<ns>/<PodCliqueSet>" (its part-of label)
+  std::map<std::string, Queue> queues_;                // queue name -> its limits
+  std::map<std::string, std::string> queueOf_;         // scheduled PodGang -> its queue (kai.scheduler/queue label)
   grove_engine_t* engine_ = nullptr;
   uint32_t engineLevels_ = 0;
   mutable std::mutex mu_;        // pending set, bindings, levels: everything SyncPodGang / OnPodGangDelete / SyncTopology touch

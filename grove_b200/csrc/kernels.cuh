@@ -12,6 +12,7 @@
 //   spread.cuh   k_spread_classes / k_spread  allowed level-l_s domains of the topology spread members (grove_set_spread)
 //   fence.cuh    k_fence_have / k_fence_pick / k_fence_status  the domain each fencing gang fences (grove_set_fences)
 //   consolidate.cuh k_consol_view / k_consol_rank / k_consol_mask  the views of a consolidation try (grove_run_cycle_consolidate)
+//   queue.cuh    k_queue_scan / k_queue_gate  the headroom, gate and surplus caps of the queue members (grove_set_queues)
 //
 // Semantics are DESIGN.md "Placement semantics"; the reference contract they restate is cited in
 // include/grove_place.h.  Integer / compare work only: no tensor cores, no floating point.
@@ -27,3 +28,4 @@
 #include "spread.cuh"
 #include "fence.cuh"
 #include "consolidate.cuh"
+#include "queue.cuh"

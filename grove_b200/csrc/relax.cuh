@@ -206,8 +206,9 @@ __global__ void __launch_bounds__(256) k_hold_release(Tables tb, Relax rx, uint4
 }
 
 // one warp per evaluated gang: publish a changed result (kHolds: a cycle with holds; kSpread: a cycle with spread members, whose
-// changed results leave a stamp per group; kFence: a cycle with fences, whose gangs' flips to or from REJECTED stamp their fence)
-template <bool kHolds, bool kSpread = false, bool kFence = false>
+// changed results leave a stamp per group; kFence: a cycle with fences, whose gangs' flips to or from REJECTED stamp their fence;
+// kQueue: a cycle with queue members, whose changed results record their usage U for k_queue_scan)
+template <bool kHolds, bool kSpread = false, bool kFence = false, bool kQueue = false>
 __global__ void __launch_bounds__(256) k_apply(Tables tb, Relax rx) {
   cudaGridDependencySynchronize();   // (launched chained: engine.cu launch_chained)
   const uint32_t lane = threadIdx.x & 31;
@@ -273,15 +274,23 @@ __global__ void __launch_bounds__(256) k_apply(Tables tb, Relax rx) {
     if (on && lane == 0) atomicMin(rx.ctl + kRemAny, stamp);
     __syncwarp();
     // publish the new ones
+    unsigned long long u0 = 0, u1 = 0, u2 = 0;   // (kQueue) U, summed over the runs
     for (uint32_t i = lane; i < nn; i += 32) {
       const uint32_t n = rx.nxt_node[po + i]; const uint16_t m = rx.nxt_meta[po + i];
       const uint32_t t = run_length(rx.nxt_node + po, rx.nxt_meta + po, i, nn);
       if (t) {
         const grove_clique_t q = tb.cliques[gg.clique_off + m];
+        if constexpr (kQueue) { u0 += uint64_t(t) * q.req_cpu_milli; u1 += uint64_t(t) * q.req_mem_mib; u2 += uint64_t(t) * q.req_gpu; }
         if (owner) { const uint3 c = owner_claim(tb, rx, g, rx.nxt_node + po, rx.nxt_meta + po, i, t); claim_add(rx, n, rank, c.x, c.y, c.z, rank); }
         else claim_add(rx, n, rank, t * q.req_cpu_milli, t * q.req_mem_mib, t * uint32_t(q.req_gpu) | (t << 16), rank);
         atomicMin(rx.add_stamp + n, stamp);
       }
+    }
+    if constexpr (kQueue) {
+      const uint32_t j = rx.qu.slot[g];
+#pragma unroll
+      for (int o = 16; o; o >>= 1) { u0 += __shfl_xor_sync(kFull, u0, o); u1 += __shfl_xor_sync(kFull, u1, o); u2 += __shfl_xor_sync(kFull, u2, o); }
+      if (lane == 0 && j != kFull) { rx.qu.use[j * 3 + 0] = u0; rx.qu.use[j * 3 + 1] = u1; rx.qu.use[j * 3 + 2] = u2; }
     }
     __syncwarp();
     for (uint32_t i = lane; i < nn; i += 32) { rx.ent_node[po + i] = rx.nxt_node[po + i]; rx.ent_meta[po + i] = rx.nxt_meta[po + i]; }

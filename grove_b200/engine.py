@@ -25,7 +25,7 @@ SYMBOLS = [
     "grove_load_nodes", "grove_update_nodes", "grove_get_nodes", "grove_submit_gangs", "grove_submit_gangs_wide", "grove_run_cycle",
     "grove_get_placements", "grove_get_gang_status", "grove_get_scope_domains", "grove_load_nodes_device",
     "grove_build_score_matrix", "grove_run_cycle_preempt", "grove_get_victims", "grove_run_cycle_reuse",
-    "grove_run_cycle_reuse_preempt", "grove_diagnose", "grove_set_spread", "grove_set_fences",
+    "grove_run_cycle_reuse_preempt", "grove_diagnose", "grove_set_spread", "grove_set_fences", "grove_set_queues",
     "grove_run_cycle_consolidate", "grove_get_moves",
     "grove_shard_range", "grove_run_score_pass", "grove_shard_summary_device",
     "grove_debug_get_perm", "grove_debug_get_fit_row", "grove_debug_get_score_row",
@@ -156,6 +156,16 @@ class PlacementEngine:
         clears it (include/grove_place.h "fences")."""
         gangs = np.ascontiguousarray(gangs, dtype=np.uint32)
         self._check(self.lib.grove_set_fences(self.h, _p(gangs), C.c_uint32(len(gangs))))
+
+    def set_queues(self, queues: np.ndarray, gang_queue: np.ndarray):
+        """grove_set_queues: hierarchical queues (tables.queue_dt: parent, per-resource limit -- tables.QUEUE_UNLIMITED = none --
+        and what the running gangs of exactly that queue hold) and the queue of every submitted gang (tables.NONE_U32 = none).
+        A member is admitted only while its queue chain has room for its MinReplicas (else tables.STATUS_OVER_LIMIT), and its
+        best-effort pods are capped to what is left (tables.STATUS_SURPLUS_CAPPED).  Call after submit_gangs; the next submit /
+        load_nodes clears it (include/grove_place.h "queue limits")."""
+        queues = np.ascontiguousarray(queues, dtype=T.queue_dt)
+        gang_queue = np.ascontiguousarray(gang_queue, dtype=np.uint32)
+        self._check(self.lib.grove_set_queues(self.h, _p(queues), C.c_uint32(len(queues)), _p(gang_queue), C.c_uint32(len(gang_queue))))
 
     # ---- the cycle ----
     def run_cycle(self) -> dict:

@@ -15,6 +15,8 @@ counterpart used by tools and tests.
 from __future__ import annotations
 
 
+import numpy as np
+
 from . import tables as T
 
 from fractions import Fraction
@@ -219,6 +221,70 @@ def podgangs_from_pcs(pcs: dict, topology_levels, tas_enabled: bool = True):
                 name = f"{fqn}-{idx}"
                 gangs.append(manifest(name, pgs, tc)); base_of[name] = f"{pcs['name']}-{r}"
     return gangs, requests, base_of
+
+
+# ------------------------------------------------------------------------------------------------
+# KAI queues (scheduling.run.ai/v2 Queue) -> the queue table of grove_set_queues (DESIGN.md section 1 "Queue limits").
+# ------------------------------------------------------------------------------------------------
+QUEUE_LABEL = "kai.scheduler/queue"
+
+
+def podgroup_queues(podgangs, template_queue):
+    """PodGroup name -> queue name (or None): the kai.scheduler/queue label of the PodClique template each PodGroup was stamped
+    from.  template_queue: template name -> label value or None.  A PodGroup's name ends in "-<template name>"
+    (namegen.go:70-117); the longest template name that matches wins."""
+    names = sorted(template_queue, key=len, reverse=True)
+    out = {}
+    for pg in podgangs:
+        for grp in pg["spec"]["podgroups"]:
+            t = next((n for n in names if grp["name"].endswith("-" + n)), None)
+            out[grp["name"]] = template_queue[t] if t is not None else None
+    return out
+
+
+def _queue_limit(res, key, scale):
+    lim = ((res or {}).get(key) or {}).get("limit", -1)
+    if lim is None or float(lim) < 0:
+        return T.QUEUE_UNLIMITED
+    return int(_quantity(lim) * scale)
+
+
+def queues_from_manifests(queue_docs, podgangs, podgroup_queue, used=None):
+    """Queue manifests + PodGang manifests -> (tables.queue_dt[n], gang_queue[G] uint32, queue names in table order).
+
+    A Queue's spec.parentQueue names its parent; spec.resources.{cpu,memory,gpu}.limit is its hard limit, -1 (or absent) none.
+    KAI's source is not part of the reference, so the units are this repository's assumption (INTEGRATION.md): cpu in cores
+    (x 1000 -> millicores), memory in MiB, gpu in whole GPUs.  A PodGang's queue is the queue its PodGroups name
+    (podgroup_queue: PodGroup name -> queue or None); PodGroups of one PodGang that name different queues are an error, a queue
+    that is not among queue_docs makes the PodGang a non-member.  used: queue name -> (cpu milli, mem MiB, gpu) that its running
+    PodGangs hold.  Parents come before their children in the table."""
+    docs = {d["metadata"]["name"]: d for d in queue_docs if d and d.get("kind", "Queue") == "Queue"}
+    parent = {n: (d.get("spec") or {}).get("parentQueue") or None for n, d in docs.items()}
+    for n, p in parent.items():
+        if p is not None and p not in docs:
+            raise ValueError(f"Queue {n!r}: parent queue {p!r} does not exist")
+
+    def depth(n, seen=()):
+        if n in seen:
+            raise ValueError(f"Queue {n!r} is its own ancestor")
+        return 0 if parent[n] is None else 1 + depth(parent[n], seen + (n,))
+
+    names = sorted(docs, key=lambda n: (depth(n), n))
+    idx = {n: i for i, n in enumerate(names)}
+    q = np.zeros(len(names), dtype=T.queue_dt)
+    for n, i in idx.items():
+        res = (docs[n].get("spec") or {}).get("resources")
+        q["parent"][i] = T.NONE_U32 if parent[n] is None else idx[parent[n]]
+        q["limit"][i] = [_queue_limit(res, "cpu", 1000), _queue_limit(res, "memory", 1), _queue_limit(res, "gpu", 1)]
+        q["used"][i] = (used or {}).get(n, (0, 0, 0))
+    gq = np.full(len(podgangs), T.NONE_U32, dtype=np.uint32)
+    for g, pg in enumerate(podgangs):
+        named = {podgroup_queue.get(grp["name"]) for grp in pg["spec"]["podgroups"]} - {None}
+        if len(named) > 1:
+            raise ValueError(f"PodGang {pg['metadata']['name']!r}: its PodGroups name different queues {sorted(named)}")
+        if named and next(iter(named)) in idx:
+            gq[g] = idx[next(iter(named))]
+    return q, gq, names
 
 
 def tables_from_pcs(pcs: dict, topology_levels, tas_enabled: bool = True, class_mask=0xFFFF):

@@ -311,3 +311,25 @@ class ChurnC5:
 
 
 CONFIGS = {"C1": config_c1, "C2": config_c2, "C3": config_c3, "C4": config_c4}
+
+
+def c4_queues(gangs, cliques, share=0.3):
+    """eight leaf queues under two parents (queue indices 0-1 the parents, 2-9 the leaves) for the gangs of a C4 submission: a base
+    gang and its scaled gangs share a leaf (by base index mod 8).  Each leaf's GPU limit is `share` of its members' MinReplicas GPU
+    demand, each parent's 90 % of the sum of its leaves'; nothing runs yet -> (tables.queue_dt[10], gang_queue).  C4's cluster
+    admits about 60 % of the gangs by itself, so at one half no limit binds; at 0.3 the limits turn away about one gang in six."""
+    G = len(gangs)
+    base = gangs["base_gang"].astype(np.int64)
+    gq = (2 + np.where(base == T.NONE_U32, np.arange(G), base) % 8).astype(np.uint32)
+    gpu = cliques["min_replicas"].astype(np.int64) * cliques["req_gpu"].astype(np.int64)
+    per_gang = np.array([gpu[int(o): int(o) + int(n)].sum() for o, n in zip(gangs["clique_off"], gangs["n_cliques"])], dtype=np.int64)
+    need = np.bincount(gq, weights=per_gang, minlength=10)
+    q = np.zeros(10, dtype=T.queue_dt)
+    q["limit"] = T.QUEUE_UNLIMITED
+    q["parent"][:2] = T.NONE_U32
+    q["parent"][2:] = np.arange(8) // 4
+    q["limit"][2:, 2] = (share * need[2:]).astype(np.uint64)
+    q["limit"][0, 2] = int(share * need[2:6].sum() * 0.9)
+    q["limit"][1, 2] = int(share * need[6:10].sum() * 0.9)
+    return q, gq
+

@@ -88,12 +88,18 @@ CONSOLIDATE_TRIES = 4
 STATUS_CONSOLIDATED = 0x8         # status reserved0: a target admitted by the consolidation pass
 STATUS_MOVED = 0x10               # status reserved0: the spec row of a running gang that was relocated
 move_dt = np.dtype([("running", np.uint32), ("target", np.uint32)])
+MAX_QUEUES = 4096
+MAX_QUEUE_DEPTH = 4
+QUEUE_UNLIMITED = 0xFFFFFFFFFFFFFFFF   # a queue limit that is not set (KAI's -1)
+STATUS_OVER_LIMIT = 0x20          # status reserved0: REJECTED by its queue chain's headroom, not evaluated
+STATUS_SURPLUS_CAPPED = 0x40      # status reserved0: ADMITTED with fewer best-effort pods allowed than it asked for
+queue_dt = np.dtype([("parent", np.uint32), ("reserved", np.uint32), ("limit", "<u8", (3,)), ("used", "<u8", (3,))])
 
 assert node_dt.itemsize == 32 and clique_dt.itemsize == 16 and scope_dt.itemsize == 8
 assert gang_dt.itemsize == 32 and placement_dt.itemsize == 8 and status_dt.itemsize == 32 and scope_status_dt.itemsize == 8
 assert config_dt.itemsize == 32 and stats_dt.itemsize == 64
 assert gang_diag_dt.itemsize == 16 and clique_diag_dt.itemsize == 40
-assert spread_dt.itemsize == 8 and spread_seed_dt.itemsize == 8
+assert spread_dt.itemsize == 8 and spread_seed_dt.itemsize == 8 and queue_dt.itemsize == 56
 
 
 def make_nodes(n: int) -> np.ndarray:

@@ -150,7 +150,9 @@ typedef struct grove_gang_status {
                               Preferred level that held), GROVE_LEVEL_NONE = the whole cluster / not admitted */
   uint16_t reserved0;      /* flags: GROVE_STATUS_PREEMPTOR = admitted by the reclaim pass of grove_run_cycle_preempt,
                               GROVE_STATUS_SPREAD_SKEWED = a SOFT spread member placed outside its allowed domains,
-                              GROVE_STATUS_FENCING = a REJECTED fencing gang whose fence held (grove_set_fences); else 0 */
+                              GROVE_STATUS_FENCING = a REJECTED fencing gang whose fence held (grove_set_fences),
+                              GROVE_STATUS_OVER_LIMIT / GROVE_STATUS_SURPLUS_CAPPED = a queue member held back by its queue
+                              chain's limits (grove_set_queues); else 0 */
   uint16_t score_num;      /* PlacementScore = score_num / score_den (podgang.go:187-189): over the gang, its scopes and
                               its cliques that carry a pack constraint, (levels honoured) / (levels asked for), where
                               asked = Preferred if set else Required; 1/1 when nothing was asked or everything held;
@@ -439,6 +441,44 @@ int32_t grove_run_cycle_consolidate(grove_engine_t* e, const uint32_t* targets, 
                                     const uint32_t* spec_of, const grove_running_gang_t* running, uint32_t n_running,
                                     const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats);
 int32_t grove_get_moves(grove_engine_t* e, grove_move_t* out, uint32_t cap, uint32_t* n_out);
+
+/* ---- queue limits --------------------------------------------------------------------------------------
+ * Hierarchical queues bound what each tenant holds (DESIGN.md section 1, "Queue limits"; after KAI-Scheduler's Queue `limit`).
+ * Queue i has a parent (< i, or GROVE_NONE_U32; chains at most GROVE_MAX_QUEUE_DEPTH deep), limit[r] per resource r (cpu milli,
+ * mem MiB, gpu; GROVE_QUEUE_UNLIMITED = none) and used[r], what the running gangs of exactly this queue hold.  A queue's load is
+ * its own used plus that of all its descendants.  gang_queue[g] is the queue of submitted gang g, or GROVE_NONE_U32; chain(g) is
+ * that queue and its ancestors.  rank = (priority desc, submission index asc); R_min(g) = sum over g's cliques of MinReplicas *
+ * request; U(h) = the usage of h's placement, surplus included.
+ * The sequential pass is unchanged except at a member g, after the gating and base-gang rules, at its turn:
+ *   1. For each Q in chain(g): H_Q[r] = limit_Q[r] - load_Q[r] - sum of U(h)[r] over the members h ranked before g that were
+ *      admitted and have Q in chain(h) (signed 64-bit).
+ *   2. If R_min(g)[r] > H_Q[r] for some r with R_min(g)[r] > 0 and some Q in chain(g) with a finite limit_Q[r], g is REJECTED
+ *      without evaluation and carries GROVE_STATUS_OVER_LIMIT.
+ *   3. Otherwise H(g)[r] = min of H_Q[r] over chain(g) (finite limits only), rem = H(g) - R_min(g); clique by clique in order,
+ *      s_q = min(replicas_q - MinReplicas_q, floor(rem[r] / req_q[r]) over the r with req_q[r] > 0 and a finite limit), at least
+ *      0, rem -= s_q * req_q.  g is evaluated as always as if clique q had MinReplicas_q + s_q replicas.  Admitted with some
+ *      s_q < replicas_q - MinReplicas_q: GROVE_STATUS_SURPLUS_CAPPED.
+ *   4. An admitted member charges U(g) to every queue of its chain.
+ * Call after grove_submit_gangs and before grove_run_cycle; the next grove_submit_gangs* or grove_load_nodes* clears the set,
+ * grove_update_nodes keeps it.  A set without members changes nothing.  GROVE_ERR_INVALID_ARG for a wrong n_gangs, a parent at or
+ * after its own index, a queue index out of range; GROVE_ERR_LIMIT for more than GROVE_MAX_QUEUES queues, a chain deeper than
+ * GROVE_MAX_QUEUE_DEPTH, a wide submission; GROVE_ERR_STATE before nodes are loaded and gangs submitted.  While a set with members
+ * is in place grove_run_cycle_preempt / _reuse / _reuse_preempt / _consolidate return GROVE_ERR_STATE, and so does grove_run_cycle
+ * with a spread set with members or a fence set.  grove_diagnose accepts a queue cycle; a gang carrying GROVE_STATUS_OVER_LIMIT
+ * gets an all-zero record. */
+#define GROVE_MAX_QUEUES 4096u
+#define GROVE_MAX_QUEUE_DEPTH 4u
+#define GROVE_QUEUE_UNLIMITED 0xFFFFFFFFFFFFFFFFull
+#define GROVE_STATUS_OVER_LIMIT 0x20u      /* REJECTED by its queue chain's headroom, not evaluated */
+#define GROVE_STATUS_SURPLUS_CAPPED 0x40u  /* ADMITTED with fewer best-effort pods allowed than it asked for */
+typedef struct grove_queue {
+  uint32_t parent;                  /* < own index, or GROVE_NONE_U32 */
+  uint32_t reserved;
+  uint64_t limit[3];                /* cpu milli, mem MiB, gpu; GROVE_QUEUE_UNLIMITED = none */
+  uint64_t used[3];                 /* held by the running gangs of exactly this queue */
+} grove_queue_t;
+int32_t grove_set_queues(grove_engine_t* e, const grove_queue_t* queues, uint32_t n_queues,
+                         const uint32_t* gang_queue, uint32_t n_gangs);
 
 /* K2: the topology-distance score matrix T[clique][node] = fit ? 1 + levels shared with the gang's anchor : 0 (u8) over the
  * snapshot the last cycle started from -- what a scheduler's Score extension point would hand out.  The admission does

@@ -7,6 +7,7 @@ package gpu
 import (
 	"context"
 	"fmt"
+	"math"
 	"sort"
 	"strings"
 	"sync"
@@ -68,6 +69,9 @@ type schedulerBackend struct {
 	consAfter, consMax int
 	specOf             map[string]*groveschedulerv1alpha1.PodGang
 	moveAnchor         map[string]string
+	// queue limits (SetQueue): queue name -> its limits; queueOf: scheduled PodGang -> its queue (kai.scheduler/queue label)
+	queues  map[string]Queue
+	queueOf map[string]string
 	eng                  *engine
 	stopLoop chan struct{}
 }
@@ -172,6 +176,253 @@ func (b *schedulerBackend) encodeSpread(t *tables, rows []*groveschedulerv1alpha
 	}
 }
 
+// Queue is a KAI queue's hard limits in the engine's units (millicores, MiB, GPUs; nil = no limit, KAI's -1), and its parent
+// ("" = a root queue).  GpuBackend::SetQueue in the C++ mirror; DESIGN.md section 1 "Queue limits".
+type Queue struct {
+	Parent                string
+	CpuMilli, MemMiB, Gpu *uint64
+}
+
+const labelQueue = "kai.scheduler/queue"
+const queueUnlimited = ^uint64(0)
+
+// SetQueue sets (nil: removes) queue name.  A pending PodGang whose kai.scheduler/queue label names a set queue is a member: it is
+// admitted only while its queue chain has room for its MinReplicas, and its best-effort pods are capped to what is left.  A parent
+// is set before its children, chains are at most GROVE_MAX_QUEUE_DEPTH deep, a queue that is a parent is not removed.  With
+// preemption, the starvation guard or consolidation on, or in a pass with topology spread members or large PodGangs, members stay
+// out of the pass, Unschedulable with a reason.
+func (b *schedulerBackend) SetQueue(name string, q *Queue) error {
+	b.mu.Lock()
+	defer b.mu.Unlock()
+	if b.queues == nil {
+		b.queues, b.queueOf = map[string]Queue{}, map[string]string{}
+	}
+	if name == "" {
+		return fmt.Errorf("a queue needs a name")
+	}
+	if q == nil {
+		for n, x := range b.queues {
+			if x.Parent == name {
+				return fmt.Errorf("queue %s is the parent of queue %s", name, n)
+			}
+		}
+		delete(b.queues, name)
+		return nil
+	}
+	depth := 1
+	for p := q.Parent; p != ""; p = b.queues[p].Parent {
+		if p == name {
+			return fmt.Errorf("queue %s would be its own ancestor", name)
+		}
+		if _, ok := b.queues[p]; !ok {
+			return fmt.Errorf("queue %s: parent queue %s is not set", name, p)
+		}
+		if depth++; depth > C.GROVE_MAX_QUEUE_DEPTH {
+			return fmt.Errorf("queue %s: chain deeper than GROVE_MAX_QUEUE_DEPTH", name)
+		}
+	}
+	for n, x := range b.queues {
+		if old, ok := b.queues[name]; ok && x.Parent == name && old.Parent != q.Parent {
+			return fmt.Errorf("queue %s is the parent of queue %s: its parent cannot change", name, n)
+		}
+	}
+	if _, ok := b.queues[name]; !ok && len(b.queues) >= C.GROVE_MAX_QUEUES {
+		return fmt.Errorf("more than GROVE_MAX_QUEUES queues")
+	}
+	b.queues[name] = *q
+	return nil
+}
+
+// queueName: the set queue pg's label names, or ""
+func (b *schedulerBackend) queueName(pg *groveschedulerv1alpha1.PodGang) string {
+	if _, ok := b.queues[pg.Labels[labelQueue]]; ok {
+		return pg.Labels[labelQueue]
+	}
+	return ""
+}
+
+// encodeQueues fills the queue tables of t for gang rows `rows`: the queues parents first (by depth, then name) with what the
+// running PodGangs of each hold, and each row's queue.  Nothing when no row is a member.
+func (b *schedulerBackend) encodeQueues(t *tables, rows []*groveschedulerv1alpha1.PodGang) {
+	member := false
+	for _, pg := range rows {
+		member = member || b.queueName(pg) != ""
+	}
+	if !member {
+		return
+	}
+	depth := func(n string) int {
+		d := 0
+		for p := b.queues[n].Parent; p != ""; p = b.queues[p].Parent {
+			d++
+		}
+		return d
+	}
+	names := make([]string, 0, len(b.queues))
+	for n := range b.queues {
+		names = append(names, n)
+	}
+	sort.Slice(names, func(i, j int) bool {
+		if di, dj := depth(names[i]), depth(names[j]); di != dj {
+			return di < dj
+		}
+		return names[i] < names[j]
+	})
+	idx := make(map[string]int, len(names))
+	for i, n := range names {
+		idx[n] = i
+	}
+	lim := func(x *uint64) C.uint64_t {
+		if x == nil {
+			return C.uint64_t(queueUnlimited)
+		}
+		return C.uint64_t(*x)
+	}
+	for _, n := range names {
+		q := b.queues[n]
+		r := C.grove_queue_t{parent: C.GROVE_NONE_U32}
+		if q.Parent != "" {
+			r.parent = C.uint32_t(idx[q.Parent])
+		}
+		r.limit = [3]C.uint64_t{lim(q.CpuMilli), lim(q.MemMiB), lim(q.Gpu)}
+		t.queues = append(t.queues, r)
+	}
+	for key, qn := range b.queueOf {
+		i, ok := idx[qn]
+		rg, running := b.running[key]
+		if !ok || !running {
+			continue
+		}
+		for _, h := range rg.held {
+			t.queues[i].used[0] += C.uint64_t(h.cpuMilli)
+			t.queues[i].used[1] += C.uint64_t(h.memMiB)
+			t.queues[i].used[2] += C.uint64_t(h.gpu)
+		}
+	}
+	for _, pg := range rows {
+		if n := b.queueName(pg); n != "" {
+			t.queueOf = append(t.queueOf, C.uint32_t(idx[n]))
+		} else {
+			t.queueOf = append(t.queueOf, C.GROVE_NONE_U32)
+		}
+	}
+	t.queueNames = names
+}
+
+// queueMessages: the messages of the queue members of one cycle, restated from its results in rank order as
+// GpuBackend::QueueMessages words them.
+func queueMessages(t *tables, res *result, nRows int) map[int]string {
+	msg := map[int]string{}
+	if len(t.queues) == 0 {
+		return msg
+	}
+	kRes := [3]string{"cpu (millicores)", "memory (MiB)", "GPUs"}
+	load := make([][3]int64, len(t.queues))
+	for q := range t.queues {
+		for r := 0; r < 3; r++ {
+			load[q][r] = int64(t.queues[q].used[r])
+		}
+	}
+	for q := len(t.queues) - 1; q >= 0; q-- { // parents come first: a queue's load is its own and its descendants'
+		if p := t.queues[q].parent; p != C.GROVE_NONE_U32 {
+			for r := 0; r < 3; r++ {
+				load[p][r] += load[q][r]
+			}
+		}
+	}
+	finite := func(q, r int) bool { return uint64(t.queues[q].limit[r]) != queueUnlimited }
+	order := []int{}
+	for g := 0; g < nRows; g++ {
+		if t.queueOf[g] != C.GROVE_NONE_U32 {
+			order = append(order, g)
+		}
+	}
+	sort.SliceStable(order, func(i, j int) bool { return t.gangs[order[i]].priority > t.gangs[order[j]].priority }) // rank order
+	for _, g := range order {
+		st := res.status[g]
+		if st.state != C.GROVE_GANG_ADMITTED && st.state != C.GROVE_GANG_REJECTED {
+			continue
+		}
+		gg := t.gangs[g]
+		var R [3]int64
+		for c := int(gg.clique_off); c < int(gg.clique_off)+int(gg.n_cliques); c++ {
+			m := int64(t.counts[c].min_replicas)
+			R[0] += m * int64(t.cliques[c].req_cpu_milli)
+			R[1] += m * int64(t.cliques[c].req_mem_mib)
+			R[2] += m * int64(t.cliques[c].req_gpu)
+		}
+		chain := []int{}
+		for q := t.queueOf[g]; q != C.GROVE_NONE_U32; q = t.queues[q].parent {
+			chain = append(chain, int(q))
+		}
+		if st.reserved0&C.GROVE_STATUS_OVER_LIMIT != 0 { // the first queue of the chain, leaf first, and the resource without room
+		find:
+			for _, q := range chain {
+				for r := 0; r < 3; r++ {
+					if finite(q, r) && R[r] > 0 && R[r] > int64(t.queues[q].limit[r])-load[q][r] {
+						msg[g] = fmt.Sprintf("queue %s has no room for this PodGang: %s limit %d, load %d, MinReplicas need %d",
+							t.queueNames[q], kRes[r], uint64(t.queues[q].limit[r]), load[q][r], R[r])
+						break find
+					}
+				}
+			}
+			continue
+		}
+		if st.state != C.GROVE_GANG_ADMITTED {
+			continue
+		}
+		if st.reserved0&C.GROVE_STATUS_SURPLUS_CAPPED != 0 { // s_q clique by clique, as the engine caps the surplus
+			var rem [3]int64
+			var fin [3]bool
+			for r := 0; r < 3; r++ {
+				rem[r] = math.MaxInt64
+				for _, q := range chain {
+					if finite(q, r) {
+						fin[r] = true
+						if h := int64(t.queues[q].limit[r]) - load[q][r]; h < rem[r] {
+							rem[r] = h
+						}
+					}
+				}
+				if fin[r] {
+					rem[r] -= R[r]
+				}
+			}
+			var heldBack int64
+			for c := int(gg.clique_off); c < int(gg.clique_off)+int(gg.n_cliques); c++ {
+				extra := int64(t.counts[c].replicas) - int64(t.counts[c].min_replicas)
+				req := [3]int64{int64(t.cliques[c].req_cpu_milli), int64(t.cliques[c].req_mem_mib), int64(t.cliques[c].req_gpu)}
+				sq := extra
+				for r := 0; r < 3; r++ {
+					if fin[r] && req[r] > 0 {
+						if rem[r] < 0 {
+							sq = 0
+						} else if x := rem[r] / req[r]; x < sq {
+							sq = x
+						}
+					}
+				}
+				for r := 0; r < 3; r++ {
+					if fin[r] {
+						rem[r] -= sq * req[r]
+					}
+				}
+				heldBack += extra - sq
+			}
+			msg[g] = fmt.Sprintf("queue limits held back %d best-effort pods of this PodGang", heldBack)
+		}
+		for k := 0; k < int(st.n_pods); k++ { // it charges what it took to every queue of its chain
+			c := t.cliques[res.placements[int(st.placement_off)+k].clique]
+			for _, q := range chain {
+				load[q][0] += int64(c.req_cpu_milli)
+				load[q][1] += int64(c.req_mem_mib)
+				load[q][2] += int64(c.req_gpu)
+			}
+		}
+	}
+	return msg
+}
+
 type runningGang struct {
 	priority int32
 	held     map[string]held // node name -> resources
@@ -216,6 +467,7 @@ func (b *schedulerBackend) OnPodGangDelete(_ context.Context, pg *grovescheduler
 	delete(b.pending, key)
 	delete(b.running, key) // its pods' resources show up as free in the next node snapshot
 	delete(b.setOf, key)
+	delete(b.queueOf, key)
 	delete(b.rejectedFor, key)
 	delete(b.specOf, key)
 	delete(b.moveAnchor, key)
@@ -395,6 +647,16 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 	}
 	levels, eng, preempt, large, explain := b.levels, b.eng, b.preempt, b.largePodGangs, b.explainUnschedulable
 	spreadOn := len(b.spread) > 0
+	queuesOn := len(b.queues) > 0
+	queueWhy := "" // a pass that takes no queue set: its members stay out
+	switch {
+	case preempt:
+		queueWhy = "queue limits are not applied while preemption is on"
+	case b.consMax > 0:
+		queueWhy = "queue limits are not applied while consolidation is on"
+	case b.guardMax > 0:
+		queueWhy = "queue limits are not applied while the starvation guard is on"
+	}
 	b.mu.Unlock()
 	sort.Slice(snap, func(i, j int) bool { return snap[i].CreationTimestamp.Before(&snap[j].CreationTimestamp) }) // submission order
 
@@ -409,8 +671,20 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 	t, nodeNames := encodeNodes(nodeList.Items, podList.Items, levels) // allocatable - requests of bound pods; dom[l] = interned label value
 	rows := make([]*groveschedulerv1alpha1.PodGang, 0, len(snap))
 	wideAny := false // a wide submission takes no spread set
+	spreadAny := false // a pass with spread members takes no queue set
 	for _, pg := range snap {
 		wideAny = wideAny || (large && whyNotEncodable(pg, false, false) != "")
+		if spreadOn && !preempt {
+			b.mu.Lock()
+			spreadAny = spreadAny || b.spreadSet(pg) != ""
+			b.mu.Unlock()
+		}
+	}
+	if queueWhy == "" && spreadAny {
+		queueWhy = "queue limits are not applied in a pass with topology spread members"
+	}
+	if queueWhy == "" && wideAny {
+		queueWhy = "queue limits are not applied in a pass with large PodGangs"
 	}
 	for _, pg := range snap {
 		if why := whyNotEncodable(pg, large, preempt); why != "" { // large && preempt: within the old limits only
@@ -420,6 +694,15 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 		if spreadOn && (preempt || wideAny) && b.spreadSet(pg) != "" {
 			b.setUnschedulable(ctx, pg, "topology spread is not applied while preemption is on or in a pass with large PodGangs")
 			continue
+		}
+		if queuesOn && queueWhy != "" {
+			b.mu.Lock()
+			member := b.queueName(pg) != ""
+			b.mu.Unlock()
+			if member {
+				b.setUnschedulable(ctx, pg, queueWhy)
+				continue
+			}
 		}
 		b.encodeGang(t, pg, levels, podList.Items) // one grove_gang_t + its cliques / scopes; requests come from the pods
 		rows = append(rows, pg)
@@ -499,6 +782,9 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 			t.targets = nil
 		}
 	}
+	if queuesOn && queueWhy == "" {
+		b.encodeQueues(t, rows)
+	}
 	rejectedFor := map[string]int{}
 	for k, v := range b.rejectedFor {
 		rejectedFor[k] = v
@@ -524,6 +810,12 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 			delete(b.rejectedFor, key)
 		}
 	}
+	for gi, st := range res.status[:len(rows)] { // what an admitted member holds counts against its queue from now on
+		if st.state == C.GROVE_GANG_ADMITTED && len(t.queueOf) > 0 && t.queueOf[gi] != C.GROVE_NONE_U32 {
+			b.queueOf[rows[gi].Namespace+"/"+rows[gi].Name] = t.queueNames[t.queueOf[gi]]
+		}
+	}
+	queueMsg := queueMessages(t, res, len(rows))
 	movedFor := map[int][]string{} // consolidated target row -> the PodGangs moved for it
 	for _, m := range res.moves {  // forgotten as running; anchored where this cycle planned it when synced again
 		key := moved[m.running]
@@ -567,6 +859,9 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 			if st.reserved0&C.GROVE_STATUS_CONSOLIDATED != 0 {
 				msg = "scheduled by moving PodGangs " + strings.Join(movedFor[gi], ", ")
 			}
+			if m, ok := queueMsg[gi]; ok {
+				msg = m
+			}
 			b.mu.Lock()
 			if b.specOf == nil {
 				b.specOf = map[string]*groveschedulerv1alpha1.PodGang{}
@@ -591,6 +886,9 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 			}
 			if len(t.spreadOf) > 0 && t.spreadOf[gi] != C.GROVE_NONE_U32 && t.spreadGroups[t.spreadOf[gi]].mode == C.GROVE_SPREAD_HARD {
 				why = "topology spread (DoNotSchedule): no domain within the skew had room for this replica"
+			}
+			if m, ok := queueMsg[gi]; ok {
+				why = m
 			}
 			if st.reserved0&C.GROVE_STATUS_FENCING != 0 && int(st.level) < len(levels) { // the starvation guard's fence held
 				key := levels[st.level]

@@ -62,6 +62,11 @@ type tables struct {
 	spreadSeeds  []C.grove_spread_seed_t
 	// fences (optional; ordinary passes only): the gang rows the starvation guard fences (grove_set_fences)
 	fences []C.uint32_t
+	// queue limits (optional; ordinary passes only): the queues, parents first, each gang row's queue (GROVE_NONE_U32 = none) and
+	// the queue names in table order (grove_set_queues)
+	queues     []C.grove_queue_t
+	queueOf    []C.uint32_t
+	queueNames []string
 	// consolidation (optional; ordinary passes only, never with fences): the target rows, and for each running gang of `running`
 	// the gated row that restates it (grove_run_cycle_consolidate)
 	targets []C.uint32_t
@@ -111,6 +116,11 @@ func (e *engine) cycle(t *tables, preempt, large, explain bool) (*result, error)
 	}
 	if len(t.fences) > 0 {
 		if err := e.err(C.grove_set_fences(e.h, &t.fences[0], C.uint32_t(len(t.fences)))); err != nil {
+			return nil, err
+		}
+	}
+	if len(t.queues) > 0 {
+		if err := e.err(C.grove_set_queues(e.h, &t.queues[0], C.uint32_t(len(t.queues)), &t.queueOf[0], C.uint32_t(len(t.queueOf)))); err != nil {
 			return nil, err
 		}
 	}
