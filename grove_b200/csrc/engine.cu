@@ -264,6 +264,9 @@ struct grove_engine {
   // queue limits (grove_set_queues; queue.cuh): the tables of the current submission's members; the queue kernels run only while
   // there are some (qu_members > 0)
   uint32_t qu_members = 0, qu_scanned = 0;
+  bool qu_given = false;                   // a set was given for the current submission, members or not
+  std::vector<grove_queue_t> qu_queues;    // ... and what it was (grove_run_cycle_preempt_queues)
+  std::vector<uint32_t> qu_gang_queue;
   DevBuf<uint32_t> d_qu_slot, d_qu_mem, d_qu_mem_fin, d_qu_q_off;
   DevBuf<uint4> d_qu_mem_pair, d_qu_pr;
   DevBuf<long long> d_qu_rmin, d_qu_q_base, d_qu_head;
@@ -546,7 +549,7 @@ static int32_t load_nodes_common(grove_engine* e, const grove_node_t* host_nodes
   if (e->diag == grove_engine::kDiagReady || e->diag == grove_engine::kDiagSpread || e->diag == grove_engine::kDiagFence) e->diag = grove_engine::kDiagChanged;
   e->sp_groups = e->sp_members = 0;   // a spread set belongs to the nodes and gangs it was validated against
   e->fc_gangs.clear();                // (a fence set too)
-  e->qu_members = 0;                  // (and a queue set)
+  e->qu_members = 0; e->qu_given = false;   // (and a queue set)
   CU_TRY(e, cudaSetDevice(e->cfg.device));
   if (host_nodes) {
     CU_TRY(e, cudaEventSynchronize(e->ev_nodes_up));  // an earlier upload may still be reading the staging buffer
@@ -705,7 +708,7 @@ static int32_t submit(grove_engine* e, const grove_gang_t* gangs, uint32_t n_gan
   if (n_gangs >= (1u << 24)) return fail(e, GROVE_ERR_LIMIT, "too many gangs");  // order rank + round tag share a stamp word
   e->sp_groups = e->sp_members = 0;
   e->fc_gangs.clear();
-  e->qu_members = 0;
+  e->qu_members = 0; e->qu_given = false;
   int32_t rc = validate(e, gangs, n_gangs, cliques, ccount.data(), n_cliques, scopes, n_scopes, max_pods);
   if (rc) return rc;
   CU_TRY(e, cudaSetDevice(e->cfg.device));
@@ -1579,6 +1582,8 @@ int32_t grove_set_fences(grove_engine_t* e, const uint32_t* gangs, uint32_t n) {
 // the tables the kernels read are built here once: the members in rank order with their chains and R_min, the queues with a
 // finite limit with limit - load, and the (queue, member) pairs sorted by (queue, rank).
 // ---------------------------------------------------------------------------------------------
+static int32_t install_queues(grove_engine* e, const grove_queue_t* queues, uint32_t n_queues, const uint32_t* gang_queue);
+
 int32_t grove_set_queues(grove_engine_t* e, const grove_queue_t* queues, uint32_t n_queues, const uint32_t* gang_queue, uint32_t n_gangs) {
   if (!e) return GROVE_ERR_INVALID_ARG;
   if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
@@ -1597,6 +1602,18 @@ int32_t grove_set_queues(grove_engine_t* e, const grove_queue_t* queues, uint32_
   }
   for (uint32_t g = 0; g < n_gangs; ++g)
     if (gang_queue[g] != GROVE_NONE_U32 && gang_queue[g] >= n_queues) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_queues: queue index out of range");
+  e->qu_given = false;
+  const int32_t rc = install_queues(e, queues, n_queues, gang_queue);
+  if (rc) return rc;
+  e->qu_queues.assign(queues, queues + n_queues);
+  e->qu_gang_queue.assign(gang_queue, gang_queue + n_gangs);
+  e->qu_given = true;
+  return GROVE_OK;
+}
+
+// The tables of a queue set (checked by grove_set_queues) over the current submission; also the per-class sets of
+// grove_run_cycle_preempt_queues, whose `used` make the loads equal load'.
+static int32_t install_queues(grove_engine* e, const grove_queue_t* queues, uint32_t n_queues, const uint32_t* gang_queue) {
   e->qu_members = e->qu_scanned = 0;
   // load = own used + the descendants' (parents come first: one pass from the back), saturating; limit - load in signed 64 bits,
   // both clamped to 2^62 (no gang asks for that much, so no decision changes)
@@ -1618,7 +1635,7 @@ int32_t grove_set_queues(grove_engine_t* e, const grove_queue_t* queues, uint32_
       q_base.push_back(queues[q].limit[r] == GROVE_QUEUE_UNLIMITED ? 0ll : (long long)std::min(queues[q].limit[r], kClamp) - (long long)load[q * 3 + r]);
   }
   // members in rank order; a gang whose chain has no finite limit is not one (it would behave as a non-member anyway)
-  const uint32_t G = n_gangs;
+  const uint32_t G = e->G;
   std::vector<uint32_t> order(G);
   std::iota(order.begin(), order.end(), 0u);
   std::stable_sort(order.begin(), order.end(), [e](uint32_t a, uint32_t b) { return e->gangs[a].priority > e->gangs[b].priority; });
@@ -2122,6 +2139,24 @@ static int32_t upload_running(grove_engine* e, const grove_running_gang_t* runni
   return GROVE_OK;
 }
 
+// d = (sorted node, change) -> one record per node, added to the device's node table (reclaim.cuh k_reclaim_patch).  The give-back of
+// the members of a class admitted after E(p) ran out.
+static int32_t patch_nodes(grove_engine* e, std::vector<std::pair<uint32_t, std::array<int64_t, 4>>>& d) {
+  std::sort(d.begin(), d.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+  std::vector<uint4> patch;
+  for (size_t i = 0; i < d.size();) {
+    const uint32_t n = d[i].first;
+    int64_t v[4] = {0, 0, 0, 0};
+    for (; i < d.size() && d[i].first == n; ++i) for (int k = 0; k < 4; ++k) v[k] += d[i].second[k];
+    patch.push_back(make_uint4(n, uint32_t(v[0]), uint32_t(v[1]), uint32_t(v[2] + v[3] * 65536)));
+  }
+  CU_TRY(e, e->d_rc_patch.ensure(patch.size()));
+  CU_TRY(e, cudaMemcpyAsync(e->d_rc_patch.p, patch.data(), sizeof(uint4) * patch.size(), cudaMemcpyHostToDevice, e->stream));
+  k_reclaim_patch<<<uint32_t((patch.size() + 255) / 256), 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_patch.p, uint32_t(patch.size()));
+  CU_TRY(e, cudaGetLastError());
+  return GROVE_OK;
+}
+
 int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs, const grove_running_gang_t* running,
                                       uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
   if (!e || (n_gangs && !replaces) || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
@@ -2316,18 +2351,7 @@ int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replace
               d.push_back({e->inv[x.node], {-int64_t(x.cpu_milli), -int64_t(x.mem_mib), -int64_t(x.gpu), -int64_t(x.pods)}});
             }
         }
-        std::sort(d.begin(), d.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
-        std::vector<uint4> patch;
-        for (size_t i = 0; i < d.size();) {
-          const uint32_t n = d[i].first;
-          int64_t v[4] = {0, 0, 0, 0};
-          for (; i < d.size() && d[i].first == n; ++i) for (int k = 0; k < 4; ++k) v[k] += d[i].second[k];
-          patch.push_back(make_uint4(n, uint32_t(v[0]), uint32_t(v[1]), uint32_t(v[2] + v[3] * 65536)));
-        }
-        CU_TRY(e, e->d_rc_patch.ensure(patch.size()));
-        CU_TRY(e, cudaMemcpyAsync(e->d_rc_patch.p, patch.data(), sizeof(uint4) * patch.size(), cudaMemcpyHostToDevice, e->stream));
-        k_reclaim_patch<<<uint32_t((patch.size() + 255) / 256), 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_patch.p, uint32_t(patch.size()));
-        CU_TRY(e, cudaGetLastError());
+        rc = patch_nodes(e, d); if (rc) return rc;
         st0.kernel_launches += 1;
       }
       // back to the free table: take off what the running gangs of E(p) that still stand hold
@@ -2338,6 +2362,296 @@ int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replace
     // the handle goes back to the caller's submission; the device table is the free table
     restore.armed = false;
     rc = grove_submit_gangs(e, gangs.data(), G, cliques.data(), Q, scopes.data(), S); if (rc) return rc;
+  }
+  st0.kernel_launches += 1;   // k_reclaim_check
+  return publish_reclaim(e, status, place, extra, sstat, st0, std::move(victims), stats);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Reclaim within queue limits (include/grove_place.h "reclaim within queue limits"; DESIGN.md section 1).  The ordinary pass is the
+// queue cycle.  Every priority class of the gangs it rejected is then ONE queue cycle over the class view of
+// grove_run_cycle_reuse_preempt (free + what the standing running gangs of E(p) hold, built by reclaim.cuh) with a queue set of
+// its own, whose `used` leave out what the gangs of E(p) hold: its loads are load'.  Queue loads are followed here, between
+// classes; victims are chosen here, node step then queue step, gang by gang in rank order.
+// ---------------------------------------------------------------------------------------------
+int32_t grove_run_cycle_preempt_queues(grove_engine_t* e, const grove_running_gang_t* running, uint32_t n_running,
+                                       const grove_holding_t* holdings, uint32_t n_holdings, const uint32_t* running_queue,
+                                       grove_cycle_stats_t* stats) {
+  static const char* kEntry = "grove_run_cycle_preempt_queues";
+  if (!e || (n_running && (!running || !running_queue)) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
+  if (e->sp_members) return refuse_spread(e, kEntry);
+  if (!e->fc_gangs.empty()) return refuse_fences(e, kEntry);
+  if (!e->qu_given) return fail(e, GROVE_ERR_STATE, "grove_run_cycle_preempt_queues: no queue set given for the current submission (grove_set_queues)");
+  NoDiagnosis no_diag{e};
+  if (e->wide) return refuse_wide(e, kEntry);
+  if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
+  for (uint32_t r = 0; r < n_running; ++r)
+    if (uint64_t(running[r].holding_off) + running[r].n_holdings > n_holdings) return fail(e, GROVE_ERR_INVALID_ARG, "running gang holdings out of range");
+  for (uint32_t h = 0; h < n_holdings; ++h)
+    if (holdings[h].node >= e->N) return fail(e, GROVE_ERR_INVALID_ARG, "holding on a node out of range");
+  // the set of the current submission (the class cycles re-use the handle) and what each running gang holds
+  const std::vector<grove_queue_t> queues = e->qu_queues;
+  const std::vector<uint32_t> gang_queue = e->qu_gang_queue;
+  const uint32_t NQ = uint32_t(queues.size());
+  std::vector<std::array<int64_t, 3>> usage(n_running, {0, 0, 0});
+  std::vector<std::array<int64_t, 3>> own(NQ, {0, 0, 0});   // own used, then followed through the cycle
+  for (uint32_t q = 0; q < NQ; ++q) for (int k = 0; k < 3; ++k) own[q][k] = int64_t(std::min<uint64_t>(queues[q].used[k], uint64_t(1) << 62));
+  {
+    std::vector<std::array<int64_t, 3>> run_use(NQ, {0, 0, 0});
+    for (uint32_t r = 0; r < n_running; ++r) {
+      for (uint32_t h = 0; h < running[r].n_holdings; ++h) {
+        const grove_holding_t& x = holdings[running[r].holding_off + h];
+        usage[r][0] += x.cpu_milli; usage[r][1] += x.mem_mib; usage[r][2] += x.gpu;
+      }
+      const uint32_t q = running_queue[r];
+      if (q == GROVE_NONE_U32) continue;
+      if (q >= NQ) return fail(e, GROVE_ERR_INVALID_ARG, "grove_run_cycle_preempt_queues: running_queue names a queue out of range");
+      for (int k = 0; k < 3; ++k) run_use[q][k] += usage[r][k];
+    }
+    for (uint32_t q = 0; q < NQ; ++q)
+      for (int k = 0; k < 3; ++k)
+        if (uint64_t(run_use[q][k]) > queues[q].used[k])
+          return fail(e, GROVE_ERR_INVALID_ARG, "grove_run_cycle_preempt_queues: the running gangs of a queue hold more than its used");
+  }
+  CU_TRY(e, cudaSetDevice(e->cfg.device));
+  const uint32_t N = e->N, nblk = (N + 255) / 256;
+  ReclaimCsr csr{};
+  int32_t rc = upload_running(e, running, n_running, holdings, &csr);
+  if (rc) return rc;
+  std::vector<int32_t> prio(std::max<uint32_t>(n_running, 1), 0);
+  for (uint32_t r = 0; r < n_running; ++r) prio[r] = running[r].priority;
+  std::vector<uint8_t> gone(std::max<uint32_t>(n_running, 1), 0);   // evicted
+
+  // 1. the ordinary pass: the queue cycle
+  grove_cycle_stats_t st0{};
+  rc = run_cycle(e, &st0);
+  if (rc) return rc;
+  const uint32_t G = e->G, Q = e->Q, S = e->S;
+  std::vector<grove_gang_t> gangs(e->gangs.data(), e->gangs.data() + G);
+  std::vector<grove_clique_t> cliques(e->cliques.data(), e->cliques.data() + Q);
+  std::vector<grove_scope_t> scopes(e->scopes.data(), e->scopes.data() + S);
+  std::vector<grove_gang_status_t> status(e->h_status.p, e->h_status.p + G);
+  std::vector<grove_placement_t> place(e->h_out.p, e->h_out.p + e->n_out);
+  std::vector<grove_scope_status_t> sstat(std::max<uint32_t>(S, 1));
+  if (S) { rc = grove_get_scope_domains(e, sstat.data(), S); if (rc) return rc; }
+  // the loads: own used + the admitted members' usage, then every queue's own plus its descendants'
+  for (uint32_t g = 0; g < G; ++g) {
+    if (status[g].state != GROVE_GANG_ADMITTED || gang_queue[g] == GROVE_NONE_U32) continue;
+    int64_t u[3] = {0, 0, 0};
+    for (uint32_t i = 0; i < status[g].n_pods; ++i) {
+      const grove_clique_t& q = cliques[place[status[g].placement_off + i].clique];
+      u[0] += q.req_cpu_milli; u[1] += q.req_mem_mib; u[2] += q.req_gpu;
+    }
+    for (int k = 0; k < 3; ++k) own[gang_queue[g]][k] += u[k];
+  }
+  std::vector<std::array<int64_t, 3>> load(own);
+  for (uint32_t q = NQ; q-- > 0;)
+    if (queues[q].parent != GROVE_NONE_U32) for (int k = 0; k < 3; ++k) load[queues[q].parent][k] += load[q][k];
+  auto account = [&](uint32_t q, const int64_t* u, int64_t sign) {   // usage u joins (+1) or leaves (-1) queue q
+    for (int k = 0; k < 3; ++k) own[q][k] += sign * u[k];
+    for (; q != GROVE_NONE_U32; q = queues[q].parent) for (int k = 0; k < 3; ++k) load[q][k] += sign * u[k];
+  };
+  auto in_subtree = [&](uint32_t q, uint32_t Qx) {   // is Qx in chain(q)?
+    for (; q != GROVE_NONE_U32; q = queues[q].parent) if (q == Qx) return true;
+    return false;
+  };
+  std::vector<int32_t> classes;
+  for (uint32_t g = 0; g < G; ++g) if (status[g].state == GROVE_GANG_REJECTED) classes.push_back(gangs[g].priority);
+  std::sort(classes.begin(), classes.end(), std::greater<int32_t>());
+  classes.erase(std::unique(classes.begin(), classes.end()), classes.end());
+  auto below = [&](int32_t p) {   // is E(p) -- the standing running gangs of a priority below p -- non-empty?
+    for (uint32_t r = 0; r < n_running; ++r) if (!gone[r] && prio[r] < p) return true;
+    return false;
+  };
+  std::vector<grove_victim_t> victims;
+  std::vector<std::vector<grove_placement_t>> extra(G);   // placements of the preemptors, by gang
+  if (!classes.empty() && below(classes.front())) {
+    // whatever goes wrong from here on, the handle goes back to the caller's submission and queue set on the free table the
+    // ordinary pass left
+    CU_TRY(e, cudaMemcpyAsync(e->d_rc_base.p, e->d_nres.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToDevice, e->stream));
+    struct Restore {
+      grove_engine* e; const std::vector<grove_gang_t>* g; const std::vector<grove_clique_t>* c; const std::vector<grove_scope_t>* s;
+      const std::vector<grove_queue_t>* q; const std::vector<uint32_t>* gq; bool armed = true;
+      ~Restore() {
+        if (!armed) return;
+        const std::string keep = e->err;
+        cudaMemcpyAsync(e->d_nres.p, e->d_rc_base.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToDevice, e->stream);
+        cudaStreamSynchronize(e->stream);
+        if (grove_submit_gangs(e, g->data(), uint32_t(g->size()), c->data(), uint32_t(c->size()), s->data(), uint32_t(s->size())) == GROVE_OK &&
+            install_queues(e, q->data(), uint32_t(q->size()), gq->data()) == GROVE_OK) {
+          e->qu_queues = *q; e->qu_gang_queue = *gq; e->qu_given = true;
+        }
+        e->err = keep;
+      }
+    };
+    Restore restore{e, &gangs, &cliques, &scopes, &queues, &gang_queue};
+    // running gangs by node (caller order), for the victim choice
+    size_t n_held = 0;   // (ranges of running gangs may overlap: size by what the fill below writes)
+    for (uint32_t r = 0; r < n_running; ++r) n_held += running[r].n_holdings;
+    std::vector<uint32_t> at_off(size_t(N) + 1, 0), at_run(n_held);
+    for (uint32_t r = 0; r < n_running; ++r) for (uint32_t h = 0; h < running[r].n_holdings; ++h) ++at_off[holdings[running[r].holding_off + h].node + 1];
+    for (uint32_t n = 0; n < N; ++n) at_off[n + 1] += at_off[n];
+    { std::vector<uint32_t> cur(at_off.begin(), at_off.end() - 1);
+      for (uint32_t r = 0; r < n_running; ++r) for (uint32_t h = 0; h < running[r].n_holdings; ++h) at_run[cur[holdings[running[r].holding_off + h].node]++] = r; }
+    std::vector<int32_t> slot(N, -1);   // node (caller order) -> its row in `rows` while a class chooses its victims
+    for (int32_t p : classes) {
+      if (!below(p)) break;   // E(p) only shrinks from one class to the next
+      // 2. the class's rejected gangs as a submission of their own: anchors pinned to what the ordinary pass used, no gating
+      std::vector<uint32_t> ids, sub_queue;
+      std::vector<grove_gang_t> sg; std::vector<grove_clique_t> sq; std::vector<grove_scope_t> ss;
+      for (uint32_t g = 0; g < G; ++g) {
+        if (status[g].state != GROVE_GANG_REJECTED || gangs[g].priority != p) continue;
+        grove_gang_t x = gangs[g];
+        if (x.anchor_node == GROVE_NONE_U32) x.anchor_node = e->perm[fmix32(g) % N];
+        x.base_gang = GROVE_NONE_U32;
+        x.clique_off = uint32_t(sq.size()); x.scope_off = uint32_t(ss.size());
+        sq.insert(sq.end(), cliques.begin() + gangs[g].clique_off, cliques.begin() + gangs[g].clique_off + gangs[g].n_cliques);
+        ss.insert(ss.end(), scopes.begin() + gangs[g].scope_off, scopes.begin() + gangs[g].scope_off + gangs[g].n_scopes);
+        ids.push_back(g); sg.push_back(x); sub_queue.push_back(gang_queue[g]);
+      }
+      // the class view, on the device: free + the standing holdings of E(p); the free table itself is kept for the victim choice
+      CU_TRY(e, cudaMemcpyAsync(e->d_rc_gone.p, gone.data(), gone.size(), cudaMemcpyHostToDevice, e->stream));
+      k_reclaim_view<<<nblk, 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_real.p, csr, N, p, 1u);
+      CU_TRY(e, cudaGetLastError());
+      rc = grove_submit_gangs(e, sg.data(), uint32_t(sg.size()), sq.data(), uint32_t(sq.size()), ss.data(), uint32_t(ss.size())); if (rc) return rc;
+      // the class's queue set: own used without what the gangs of E(p) hold, so that its loads are load'
+      std::vector<grove_queue_t> cq(queues);
+      {
+        std::vector<std::array<int64_t, 3>> o(own);
+        for (uint32_t r = 0; r < n_running; ++r)
+          if (!gone[r] && prio[r] < p && running_queue[r] != GROVE_NONE_U32) for (int k = 0; k < 3; ++k) o[running_queue[r]][k] -= usage[r][k];
+        for (uint32_t q = 0; q < NQ; ++q) for (int k = 0; k < 3; ++k) cq[q].used[k] = uint64_t(o[q][k]);
+      }
+      rc = install_queues(e, cq.data(), NQ, sub_queue.data()); if (rc) return rc;
+      grove_cycle_stats_t stp{};
+      rc = run_cycle(e, &stp); if (rc) return rc;
+      st0.rounds += stp.rounds; st0.evaluations += stp.evaluations; st0.kernel_launches += stp.kernel_launches + 2;   // (+ the two k_reclaim_view)
+      st0.ms_fit += stp.ms_fit; st0.ms_admit += stp.ms_admit; st0.ms_commit += stp.ms_commit; st0.ms_total += stp.ms_total;
+      std::vector<grove_scope_status_t> ssp(std::max<size_t>(ss.size(), 1));
+      if (!ss.empty()) { rc = grove_get_scope_domains(e, ssp.data(), uint32_t(ss.size())); if (rc) return rc; }
+      // the free-table rows of the nodes the class's preemptors use
+      std::vector<uint32_t> used;
+      for (uint32_t k = 0; k < ids.size(); ++k) {
+        const grove_gang_status_t& sp = e->h_status.p[k];
+        if (sp.state != GROVE_GANG_ADMITTED) continue;
+        for (uint32_t i = 0; i < sp.n_pods; ++i) used.push_back(e->h_out.p[sp.placement_off + i].node);
+      }
+      std::sort(used.begin(), used.end());
+      used.erase(std::unique(used.begin(), used.end()), used.end());
+      std::vector<Res> rows(used.size());
+      if (!used.empty()) {
+        std::vector<uint32_t> idx(used.size());
+        for (size_t i = 0; i < used.size(); ++i) { idx[i] = e->inv[used[i]]; slot[used[i]] = int32_t(i); }
+        std::vector<uint4> got(used.size());
+        CU_TRY(e, e->d_rc_idx.ensure(idx.size())); CU_TRY(e, e->d_rc_rows.ensure(idx.size()));
+        CU_TRY(e, cudaMemcpyAsync(e->d_rc_idx.p, idx.data(), sizeof(uint32_t) * idx.size(), cudaMemcpyHostToDevice, e->stream));
+        k_reclaim_rows<<<uint32_t((idx.size() + 255) / 256), 256, 0, e->stream>>>(e->d_rc_real.p, e->d_rc_idx.p, e->d_rc_rows.p, uint32_t(idx.size()));
+        CU_TRY(e, cudaGetLastError());
+        CU_TRY(e, cudaMemcpyAsync(got.data(), e->d_rc_rows.p, sizeof(uint4) * got.size(), cudaMemcpyDeviceToHost, e->stream));
+        CU_TRY(e, cudaStreamSynchronize(e->stream));
+        for (size_t i = 0; i < got.size(); ++i) rows[i] = Res{got[i].x, got[i].y, got[i].z & 0xFFFFu, got[i].z >> 16};
+        st0.kernel_launches += 1;
+      }
+      auto evict = [&](uint32_t v, uint32_t g) {   // everything v held returns to the free table, its usage leaves its queues
+        gone[v] = 1;
+        for (uint32_t h = 0; h < running[v].n_holdings; ++h) {
+          const grove_holding_t& x = holdings[running[v].holding_off + h];
+          if (slot[x.node] < 0) continue;
+          Res& q = rows[slot[x.node]];
+          q.cpu += x.cpu_milli; q.mem += x.mem_mib; q.gpu += x.gpu; q.pods += x.pods;
+        }
+        if (running_queue[v] != GROVE_NONE_U32) account(running_queue[v], usage[v].data(), -1);
+        victims.push_back(grove_victim_t{v, g});
+      };
+      // 3. victims, gang by gang in rank order (sub-submission order == order rank: one priority)
+      std::vector<uint32_t> skipped;   // admitted by the class cycle after E(p) ran out: they stay as the ordinary pass left them
+      for (uint32_t k = 0; k < ids.size(); ++k) {
+        const grove_gang_status_t& sp = e->h_status.p[k];
+        if (sp.state != GROVE_GANG_ADMITTED) continue;
+        if (!below(p)) { skipped.push_back(k); continue; }
+        const uint32_t g = ids[k];
+        std::vector<uint32_t> order; std::vector<Res> use;
+        int64_t U[3] = {0, 0, 0};
+        for (uint32_t i = 0; i < sp.n_pods; ++i) {
+          const grove_placement_t pl = e->h_out.p[sp.placement_off + i];
+          const grove_clique_t& q = sq[pl.clique];
+          size_t j = 0;
+          for (; j < order.size(); ++j) if (order[j] == pl.node) break;
+          if (j == order.size()) { order.push_back(pl.node); use.emplace_back(); }
+          use[j].cpu += q.req_cpu_milli; use[j].mem += q.req_mem_mib; use[j].gpu += q.req_gpu; use[j].pods += 1;
+          U[0] += q.req_cpu_milli; U[1] += q.req_mem_mib; U[2] += q.req_gpu;
+          extra[g].push_back(grove_placement_t{gangs[g].clique_off + (pl.clique - sg[k].clique_off), pl.node});
+        }
+        // (a) the node step: the reclaim pass's rule
+        for (size_t j = 0; j < order.size(); ++j) {
+          const uint32_t n = order[j];
+          Res& have = rows[slot[n]];
+          const Res& need = use[j];
+          while (!(have.cpu >= need.cpu && have.mem >= need.mem && have.gpu >= need.gpu && have.pods >= need.pods)) {
+            uint32_t v = GROVE_NONE_U32;   // lowest priority first, then the highest running index
+            for (uint32_t a = at_off[n]; a < at_off[n + 1]; ++a) {
+              const uint32_t x = at_run[a];
+              if (gone[x] || prio[x] >= p) continue;
+              if (v == GROVE_NONE_U32 || prio[x] < prio[v] || (prio[x] == prio[v] && x > v)) v = x;
+            }
+            if (v == GROVE_NONE_U32) return fail(e, GROVE_ERR_STATE, "reclaim pass: a preemptor's node cannot be freed");
+            evict(v, g);
+          }
+          have.cpu -= need.cpu; have.mem -= need.mem; have.gpu -= need.gpu; have.pods -= need.pods;
+        }
+        // (b) the queue step: g's chain, leaf first, back within its limits on the resources g uses
+        const uint32_t gq = gang_queue[g];
+        if (gq != GROVE_NONE_U32) {
+          account(gq, U, 1);
+          for (uint32_t Qx = gq; Qx != GROVE_NONE_U32; Qx = queues[Qx].parent) {
+            for (;;) {
+              uint32_t over = 0;   // the resources g uses on which Qx is over its finite limit
+              for (int r = 0; r < 3; ++r)
+                if (U[r] > 0 && queues[Qx].limit[r] != GROVE_QUEUE_UNLIMITED && load[Qx][r] > 0 && uint64_t(load[Qx][r]) > queues[Qx].limit[r]) over |= 1u << r;
+              if (!over) break;
+              uint32_t v = GROVE_NONE_U32;   // a gang of E(p) in Qx's subtree holding some of it: lowest priority, then highest index
+              for (uint32_t x = 0; x < n_running; ++x) {
+                if (gone[x] || prio[x] >= p || running_queue[x] == GROVE_NONE_U32 || !in_subtree(running_queue[x], Qx)) continue;
+                bool holds = false;
+                for (int r = 0; r < 3; ++r) holds |= ((over >> r) & 1u) && usage[x][r] > 0;
+                if (!holds) continue;
+                if (v == GROVE_NONE_U32 || prio[x] < prio[v] || (prio[x] == prio[v] && x > v)) v = x;
+              }
+              if (v == GROVE_NONE_U32) return fail(e, GROVE_ERR_STATE, "reclaim pass: a preemptor's queue cannot be brought within its limit");
+              evict(v, g);
+            }
+          }
+        }
+        grove_gang_status_t o = sp;
+        o.reserved0 = uint16_t(GROVE_STATUS_PREEMPTOR | (sp.reserved0 & GROVE_STATUS_SURPLUS_CAPPED));
+        status[g] = o;   // placement_off is assigned when the outputs are merged
+        for (uint32_t si = 0; si < gangs[g].n_scopes; ++si) sstat[gangs[g].scope_off + si] = ssp[sg[k].scope_off + si];
+        st0.gangs_admitted += 1; st0.gangs_rejected -= 1;
+      }
+      for (uint32_t n : used) slot[n] = -1;
+      if (!skipped.empty()) {   // give back what the class cycle committed for them (their queue charge was never taken here)
+        std::vector<std::pair<uint32_t, std::array<int64_t, 4>>> d;   // (sorted node, change)
+        for (uint32_t k : skipped) {
+          const grove_gang_status_t& sp = e->h_status.p[k];
+          for (uint32_t i = 0; i < sp.n_pods; ++i) {
+            const grove_placement_t pl = e->h_out.p[sp.placement_off + i];
+            const grove_clique_t& q = sq[pl.clique];
+            d.push_back({e->inv[pl.node], {int64_t(q.req_cpu_milli), int64_t(q.req_mem_mib), int64_t(q.req_gpu), 1}});
+          }
+        }
+        rc = patch_nodes(e, d); if (rc) return rc;
+        st0.kernel_launches += 1;
+      }
+      // back to the free table: take off what the running gangs of E(p) that still stand hold
+      CU_TRY(e, cudaMemcpyAsync(e->d_rc_gone.p, gone.data(), gone.size(), cudaMemcpyHostToDevice, e->stream));
+      k_reclaim_view<<<nblk, 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_real.p, csr, N, p, 0u);
+      CU_TRY(e, cudaGetLastError());
+    }
+    // the handle goes back to the caller's submission and queue set; the device table is the free table
+    restore.armed = false;
+    rc = grove_submit_gangs(e, gangs.data(), G, cliques.data(), Q, scopes.data(), S); if (rc) return rc;
+    rc = install_queues(e, queues.data(), NQ, gang_queue.data()); if (rc) return rc;
+    e->qu_queues = queues; e->qu_gang_queue = gang_queue; e->qu_given = true;
   }
   st0.kernel_launches += 1;   // k_reclaim_check
   return publish_reclaim(e, status, place, extra, sstat, st0, std::move(victims), stats);

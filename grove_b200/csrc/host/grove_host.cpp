@@ -456,7 +456,8 @@ Err GpuBackend::EncodeLocked(const std::vector<Node>& nodes, Tables* out, const 
       wideAny |= large_ && !WhyNotEncodable(kv.second, false).empty();
       spreadAny |= spreadSetOf(kv.second) != nullptr;
     }
-    const char* why = runningCycles ? "queue limits are not applied while preemption or reservation reuse is on"
+    const bool withinQueues = preemptQueues_ && preemption_ && !reuse_ && !reclaimReuse_;   // grove_run_cycle_preempt_queues
+    const char* why = runningCycles && !withinQueues ? "queue limits are not applied while preemption or reservation reuse is on"
                       : consMax_ ? "queue limits are not applied while consolidation is on"
                       : guardMax_ ? "queue limits are not applied while the starvation guard is on"
                       : spreadAny ? "queue limits are not applied in a pass with topology spread members"
@@ -790,6 +791,17 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
   }
   if (both) { if (auto e = chk(grove_run_cycle_reuse_preempt(engine_, replaces.data(), uint32_t(replaces.size()), run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_reuse_preempt")) return e; }
   else if (reuse) { if (auto e = chk(grove_run_cycle_reuse(engine_, replaces.data(), uint32_t(replaces.size()), run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_reuse")) return e; }
+  else if (preempt && !t.queues.empty()) {   // (Encode keeps queue members in a pass with preemption only with SetPreemptionWithinQueues)
+    std::vector<uint32_t> runQueue(run.size(), GROVE_NONE_U32);   // the queue each running PodGang was scheduled in
+    {
+      std::lock_guard<std::mutex> l(mu_);
+      for (uint32_t r = 0; r < runNames.size(); ++r)
+        if (auto it = queueOf_.find(runNames[r]); it != queueOf_.end())
+          if (auto n = std::find(t.queueNames.begin(), t.queueNames.end(), it->second); n != t.queueNames.end()) runQueue[r] = uint32_t(n - t.queueNames.begin());
+    }
+    if (auto e = chk(grove_run_cycle_preempt_queues(engine_, run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), runQueue.data(), &st),
+                     "grove_run_cycle_preempt_queues")) return e;
+  }
   else if (preempt) { if (auto e = chk(grove_run_cycle_preempt(engine_, run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_preempt")) return e; }
   else if (consolidate) {
     if (auto e = chk(grove_run_cycle_consolidate(engine_, targets.data(), uint32_t(targets.size()), specOf.data(), crun.data(), uint32_t(crun.size()),

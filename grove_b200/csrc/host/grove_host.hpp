@@ -283,6 +283,11 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   // DisruptionTarget naming their preemptor and are forgotten.  Off by default; with it off the other two switches work as
   // before: either one alone, and both together fail.
   void SetReclaimWithReuse(bool on) { std::lock_guard<std::mutex> l(mu_); reclaimReuse_ = on; }
+  // Preemption within queue limits: with it and SetPreemption on (reservation reuse and reuse with reclaim off), queue members are
+  // no longer kept out of a pass with preemption; a pass with members is grove_run_cycle_preempt_queues, whose running gangs'
+  // queues are the ones their PodGangs were scheduled in.  A member its queue chain turns away may then evict lower-priority
+  // PodGangs of its own queues; victims get DisruptionTarget naming their preemptor, as with preemption.  Off by default.
+  void SetPreemptionWithinQueues(bool on) { std::lock_guard<std::mutex> l(mu_); preemptQueues_ = on; }
   // Large PodGangs: with it on, PodGangs of up to GROVE_MAX_WIDE_GANG_PODS pods (PodGroups of up to as many) are encoded and a
   // cycle submits through grove_submit_gangs_wide; ValidatePodCliqueSet accepts base PodGangs of that size.  The running-gang
   // cycles (preemption, reservation reuse, reuse with reclaim) do not take such PodGangs: while one of those switches is on too,
@@ -372,6 +377,7 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   bool preemption_ = false;
   bool reuse_ = false;
   bool reclaimReuse_ = false;
+  bool preemptQueues_ = false;
   bool large_ = false;
   bool explain_ = false;
   uint32_t guardAfter_ = 1, guardMax_ = 0;             // starvation guard (off: guardMax_ == 0)

@@ -26,7 +26,7 @@ SYMBOLS = [
     "grove_get_placements", "grove_get_gang_status", "grove_get_scope_domains", "grove_load_nodes_device",
     "grove_build_score_matrix", "grove_run_cycle_preempt", "grove_get_victims", "grove_run_cycle_reuse",
     "grove_run_cycle_reuse_preempt", "grove_diagnose", "grove_set_spread", "grove_set_fences", "grove_set_queues",
-    "grove_run_cycle_consolidate", "grove_get_moves",
+    "grove_run_cycle_consolidate", "grove_get_moves", "grove_run_cycle_preempt_queues",
     "grove_shard_range", "grove_run_score_pass", "grove_shard_summary_device",
     "grove_debug_get_perm", "grove_debug_get_fit_row", "grove_debug_get_score_row",
 ]
@@ -207,8 +207,25 @@ class PlacementEngine:
                                                            C.c_uint32(len(running)), _p(holdings), C.c_uint32(len(holdings)), _p(st)))
         return {k: st[k][0].item() for k in T.stats_dt.names}
 
+    def run_cycle_preempt_queues(self, running: np.ndarray, holdings: np.ndarray, running_queue: np.ndarray) -> dict:
+        """the queue cycle of the set_queues set, then the reclaim pass within queue limits: a gang it rejected (OVER_LIMIT ones
+        included) may evict running gangs of a lower priority, node by node and then from its own queues until they are within
+        their limits.  `running` / `holdings` as for run_cycle_preempt; running_queue[r] is the queue of running gang r
+        (tables.NONE_U32 = none), and what the running gangs of a queue hold must not exceed its `used`
+        (include/grove_place.h "reclaim within queue limits"); victims() lists the evictions"""
+        running = np.ascontiguousarray(running, dtype=T.running_dt)
+        holdings = np.ascontiguousarray(holdings, dtype=T.holding_dt)
+        running_queue = np.ascontiguousarray(running_queue, dtype=np.uint32)
+        if len(running_queue) != len(running):
+            raise ValueError("one running_queue entry per running gang")
+        st = np.zeros(1, dtype=T.stats_dt)
+        self._check(self.lib.grove_run_cycle_preempt_queues(self.h, _p(running), C.c_uint32(len(running)), _p(holdings),
+                                                            C.c_uint32(len(holdings)), _p(running_queue), _p(st)))
+        return {k: st[k][0].item() for k in T.stats_dt.names}
+
     def victims(self) -> np.ndarray:
-        """(running gang, preemptor gang) pairs of the last run_cycle_preempt / run_cycle_reuse_preempt: the caller sets
+        """(running gang, preemptor gang) pairs of the last run_cycle_preempt / run_cycle_reuse_preempt /
+        run_cycle_preempt_queues: the caller sets
         DisruptionTarget on them"""
         n = C.c_uint32(0)
         self._check(self.lib.grove_get_victims(self.h, None, C.c_uint32(0), C.byref(n)))

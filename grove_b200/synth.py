@@ -333,3 +333,44 @@ def c4_queues(gangs, cliques, share=0.3):
     q["limit"][1, 2] = int(share * need[6:10].sum() * 0.9)
     return q, gq
 
+
+
+def queue_running(tables, queues, gang_queue, placements, status, seed=0, boost=2, share=0.5):
+    """A running-gang layout for a queue set (synth.c4_queues): the gangs a queue cycle over `tables` admitted (its placements and
+    statuses) run in their queues at priorities 0-2, and the submission is the same gangs again at priorities 0-2, about `share` of
+    them (and every third base gang, with its scaled gangs) `boost` higher.  Each queue's `used` becomes what its running gangs
+    hold plus, at random, a little that is not handed in (0.5 cores, 1 GiB, one GPU).
+    -> (tables, queues, gang_queue, running, holdings, running_queue) for grove_run_cycle_preempt_queues"""
+    g, c, s = tables
+    rng = np.random.default_rng(seed)
+    run, hold, rq = [], [], []
+    for i in np.nonzero(status["state"] == T.GANG_ADMITTED)[0]:
+        per = {}
+        for e in placements[status["placement_off"][i]: status["placement_off"][i] + status["n_pods"][i]]:
+            q = c[int(e["clique"])]
+            u = per.setdefault(int(e["node"]), [0, 0, 0, 0])
+            u[0] += int(q["req_cpu_milli"]); u[1] += int(q["req_mem_mib"]); u[2] += int(q["req_gpu"]); u[3] += 1
+        run.append((int(rng.integers(0, 3)), len(hold), len(per), 0))
+        hold += [(n, *u) for n, u in per.items()]
+        rq.append(int(gang_queue[i]))
+    running = np.array(run, dtype=T.running_dt) if run else np.zeros(0, dtype=T.running_dt)
+    holdings = np.array(hold, dtype=T.holding_dt) if hold else np.zeros(0, dtype=T.holding_dt)
+    running_queue = np.array(rq, dtype=np.uint32)
+    q2 = np.asarray(queues, dtype=T.queue_dt).copy()
+    q2["used"] = 0
+    for r in range(len(running)):
+        if running_queue[r] != T.NONE_U32:
+            h = holdings[int(running["holding_off"][r]): int(running["holding_off"][r]) + int(running["n_holdings"][r])]
+            q2["used"][int(running_queue[r])] += np.array([h["cpu_milli"].astype(np.uint64).sum(), h["mem_mib"].astype(np.uint64).sum(),
+                                                           h["gpu"].astype(np.uint64).sum()], dtype=np.uint64)
+    q2["used"] += rng.integers(0, 2, (len(q2), 3)).astype(np.uint64) * np.array([500, 1024, 1], np.uint64)
+    g2 = g.copy()
+    for i in range(len(g2)):
+        b = int(g2["base_gang"][i])
+        root = i if b == T.NONE_U32 else b
+        g2["priority"][i] = int(rng.integers(0, 3)) + (boost if rng.random() < share or root % 3 == 0 else 0)
+    for i in range(len(g2)):   # a scaled gang keeps its base gang's priority
+        b = int(g2["base_gang"][i])
+        if b != T.NONE_U32:
+            g2["priority"][i] = g2["priority"][b]
+    return (g2, c, s), q2, np.asarray(gang_queue, dtype=np.uint32), running, holdings, running_queue

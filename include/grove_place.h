@@ -480,6 +480,30 @@ typedef struct grove_queue {
 int32_t grove_set_queues(grove_engine_t* e, const grove_queue_t* queues, uint32_t n_queues,
                          const uint32_t* gang_queue, uint32_t n_gangs);
 
+/* ---- reclaim within queue limits -----------------------------------------------------------------------
+ * The reclaim pass on a queue cycle: a gang its queue chain turns away can evict lower-priority gangs of the same queues
+ * (DESIGN.md section 1, "Reclaim within queue limits"; after KAI-Scheduler's preempt action).  Runs on the queue set that
+ * grove_set_queues gave the current submission (a set without members counts).  Running gangs and holdings are as for
+ * grove_run_cycle_preempt; running_queue[r] is the queue of running gang r, or GROVE_NONE_U32, and what the running gangs of queue
+ * q hold (cpu, mem, gpu summed over their holdings) must not exceed used(q).  E(p) = the standing running gangs of a priority below p.
+ *   1. The ordinary pass: grove_run_cycle with the queue set.  The load of each queue is then its starting load plus U of the
+ *      admitted members in its subtree.
+ *   2. Every gang it left REJECTED (OVER_LIMIT ones included) is reconsidered once, in rank order, while E(p) is non-empty: against
+ *      the node view free + what E(p) holds, and the queue limits with load'_Q = load_Q - what the gangs of E(p) whose queue lies in
+ *      Q's subtree hold.  Admitted: GROVE_STATUS_PREEMPTOR, ORed with GROVE_STATUS_SURPLUS_CAPPED; rejected again: its ordinary-pass
+ *      status, flags included.
+ *   3. Victims of an admitted g: (a) node by node, as grove_run_cycle_preempt evicts; (b) for each Q of chain(g), leaf first, while
+ *      load_Q[r] > limit_Q[r] for a resource r with U(g)[r] > 0 and a finite limit, one whole gang of E(p) in Q's subtree that holds
+ *      some of such a resource, lowest priority first, then highest running index.  An eviction returns the victim's holdings to the
+ *      free table and takes its usage off every queue of its chain.  grove_get_victims lists (victim, preemptor) in eviction order.
+ * Outputs through the usual getters; the queue set stays in place.  GROVE_ERR_STATE without a queue set given since the last
+ * submission, with a spread set with members or a non-empty fence set; GROVE_ERR_LIMIT for a wide submission; GROVE_ERR_INVALID_ARG
+ * for the inputs grove_run_cycle_preempt rejects, a running_queue entry out of range, or running usage of a queue above its used.
+ * grove_diagnose refuses the cycle that follows. */
+int32_t grove_run_cycle_preempt_queues(grove_engine_t* e, const grove_running_gang_t* running, uint32_t n_running,
+                                       const grove_holding_t* holdings, uint32_t n_holdings,
+                                       const uint32_t* running_queue, grove_cycle_stats_t* stats);
+
 /* K2: the topology-distance score matrix T[clique][node] = fit ? 1 + levels shared with the gang's anchor : 0 (u8) over the
  * snapshot the last cycle started from -- what a scheduler's Score extension point would hand out.  The admission does
  * not read it (its visiting order comes from the anchor's domain ranges), so it is built on request; GROVE_TUNE_SCORE=1

@@ -51,6 +51,9 @@ type schedulerBackend struct {
 	levels   []string                                    // ClusterTopology.Spec.Levels[].Key, broadest first
 	running  map[string]runningGang                      // PodGangs scheduled by this backend: priority + holdings (reclaim pass)
 	preempt  bool
+	// preemptQueues: with preempt also on, queue members stay in the pass and a pass with members is
+	// grove_run_cycle_preempt_queues (GpuBackend::SetPreemptionWithinQueues in the C++ mirror)
+	preemptQueues bool
 	// largePodGangs: PodGangs of up to maxWideGangPods pods are encoded (a counts row per clique) and submitted through
 	// grove_submit_gangs_wide.  The reclaim pass takes no such PodGang: with preempt also on, one beyond maxGangPods pods or 255
 	// replicas is reported Unschedulable (GpuBackend::SetLargePodGangs in the C++ mirror).
@@ -90,6 +93,16 @@ const (
 	labelPartOf      = "app.kubernetes.io/part-of"
 	labelBasePodGang  = "grove.io/base-podgang"
 )
+
+// SetPreemptionWithinQueues: with it and preemption on, queue members are no longer kept out of a pass with preemption, and a
+// pass with members runs grove_run_cycle_preempt_queues: a member its queue chain turns away may evict lower-priority PodGangs of
+// its own queues (DESIGN.md section 1 "Reclaim within queue limits").  The queue of each running PodGang is the one it was
+// scheduled in.  Off by default.
+func (b *schedulerBackend) SetPreemptionWithinQueues(on bool) {
+	b.mu.Lock()
+	defer b.mu.Unlock()
+	b.preemptQueues = on
+}
 
 // SetTopologySpread sets (nil: removes) the topology spread of PodCliqueSet pcs.  Its pending base PodGangs with a Required level
 // at or below spread.LevelKey and a PodGroup with MinReplicas > 0 are members; the running ones this backend scheduled count
@@ -650,7 +663,7 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 	queuesOn := len(b.queues) > 0
 	queueWhy := "" // a pass that takes no queue set: its members stay out
 	switch {
-	case preempt:
+	case preempt && !b.preemptQueues:
 		queueWhy = "queue limits are not applied while preemption is on"
 	case b.consMax > 0:
 		queueWhy = "queue limits are not applied while consolidation is on"
@@ -744,6 +757,7 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 	// consolidation, in an ordinary pass only: the targets as the starvation guard counts, and every running PodGang this backend
 	// scheduled whole restated as a gated row after the pending ones (all its pods: MinReplicas = replicas)
 	var moved []string // running gang of t.running -> PodGang key
+	var runningKeys []string // preemption: running gang of t.running -> PodGang key
 	if b.consMax > 0 && !preempt && !wideAny && len(t.spreadGroups) == 0 {
 		for gi, pg := range rows {
 			if b.rejectedFor[pg.Namespace+"/"+pg.Name] >= b.consAfter {
@@ -784,6 +798,19 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 	}
 	if queuesOn && queueWhy == "" {
 		b.encodeQueues(t, rows)
+		if preempt && len(t.queues) > 0 { // the queue of every running gang of t.running (runningKeys: its PodGang), or none
+			t.runningQueue = make([]C.uint32_t, len(t.running))
+			for r := range t.running {
+				t.runningQueue[r] = C.GROVE_NONE_U32
+				if r < len(runningKeys) {
+					for qi, n := range t.queueNames {
+						if n == b.queueOf[runningKeys[r]] {
+							t.runningQueue[r] = C.uint32_t(qi)
+						}
+					}
+				}
+			}
+		}
 	}
 	rejectedFor := map[string]int{}
 	for k, v := range b.rejectedFor {

@@ -66,6 +66,9 @@ type tables struct {
 	// the queue names in table order (grove_set_queues)
 	queues     []C.grove_queue_t
 	queueOf    []C.uint32_t
+	// reclaim within queue limits: the queue of each running gang of `running` (GROVE_NONE_U32: none); set only in a pass with
+	// preemption and queue members
+	runningQueue []C.uint32_t
 	queueNames []string
 	// consolidation (optional; ordinary passes only, never with fences): the target rows, and for each running gang of `running`
 	// the gated row that restates it (grove_run_cycle_consolidate)
@@ -130,7 +133,12 @@ func (e *engine) cycle(t *tables, preempt, large, explain bool) (*result, error)
 		if len(t.holdings) > 0 {
 			hp = &t.holdings[0]
 		}
-		if err := e.err(C.grove_run_cycle_preempt(e.h, &t.running[0], C.uint32_t(len(t.running)), hp,
+		if len(t.runningQueue) > 0 {
+			if err := e.err(C.grove_run_cycle_preempt_queues(e.h, &t.running[0], C.uint32_t(len(t.running)), hp,
+				C.uint32_t(len(t.holdings)), &t.runningQueue[0], &r.stats)); err != nil {
+				return nil, err
+			}
+		} else if err := e.err(C.grove_run_cycle_preempt(e.h, &t.running[0], C.uint32_t(len(t.running)), hp,
 			C.uint32_t(len(t.holdings)), &r.stats)); err != nil {
 			return nil, err
 		}
