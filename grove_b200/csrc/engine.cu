@@ -1055,10 +1055,16 @@ static uint32_t eval_ctas(const grove_engine* e) {
   return std::max(1u, e->tune_eval_ctas ? e->tune_eval_ctas : std::min(W, e->n_sm * e->tune_heavy_ctas));
 }
 
-static int32_t cycle_begin(grove_engine* e) {
+// a node snapshot loaded, gangs submitted, no cycle in flight
+static int32_t check_ready(grove_engine* e) {
   if (!e->nodes_loaded) return fail(e, GROVE_ERR_STATE, "no node snapshot loaded");
   if (!e->gangs_loaded) return fail(e, GROVE_ERR_STATE, "no gangs submitted");
   if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
+  return GROVE_OK;
+}
+
+static int32_t cycle_begin(grove_engine* e) {
+  if (int32_t rc = check_ready(e)) return rc;
   CU_TRY(e, cudaSetDevice(e->cfg.device));
   if (e->ginfo_dirty) { int32_t rc = build_ginfo(e); if (rc) return rc; }
   const uint32_t G = e->G, Q = e->Q, S = e->S, P = e->P, N = e->Npad;
@@ -1803,158 +1809,207 @@ int32_t grove_build_score_matrix(grove_engine_t* e, float* ms) {
 // device path: the gangs the ordinary pass rejected are re-submitted priority class by priority class (descending) against
 // the reclaim view of that class -- the evaluation of a gang does not depend on WHICH running gangs end up evicted, only on
 // what is free plus what is evictable, so a whole class is one ordinary cycle on the augmented node table; the victims
-// are then chosen gang by gang in order, exactly as the sequential statement says.
+// are then chosen gang by gang in order, exactly as the sequential statement says.  reclaim_cycle (below) runs that loop for
+// the three reclaim entries; consolidation runs its own over the same pieces, which come first.
 // ---------------------------------------------------------------------------------------------
 namespace {
-struct Res { int64_t cpu = 0, mem = 0, gpu = 0, pods = 0; };
-inline bool covers(const grove_node_t& n, const Res& r) {
-  return int64_t(n.free_cpu_milli) >= r.cpu && int64_t(n.free_mem_mib) >= r.mem && int64_t(n.free_gpu) >= r.gpu && int64_t(n.free_pods) >= r.pods;
-}
-inline void give(grove_node_t& n, const grove_holding_t& h) {
-  n.free_cpu_milli += h.cpu_milli; n.free_mem_mib += h.mem_mib; n.free_gpu = uint16_t(n.free_gpu + h.gpu); n.free_pods = uint16_t(n.free_pods + h.pods);
-}
+struct Res {   // resources on one node: a free-table row, a usage or a change
+  int64_t cpu = 0, mem = 0, gpu = 0, pods = 0;
+  bool covers(const Res& r) const { return cpu >= r.cpu && mem >= r.mem && gpu >= r.gpu && pods >= r.pods; }
+  void add(const Res& r, int64_t k = 1) { cpu += k * r.cpu; mem += k * r.mem; gpu += k * r.gpu; pods += k * r.pods; }
+};
+inline Res held(const grove_holding_t& h) { return Res{h.cpu_milli, h.mem_mib, h.gpu, h.pods}; }
+
+// the caller's submission and the outputs of the ordinary pass (the handle is re-used for the sub-cycles)
+struct Snapshot {
+  std::vector<grove_gang_t> gangs; std::vector<grove_clique_t> cliques; std::vector<grove_scope_t> scopes;
+  std::vector<grove_gang_status_t> status; std::vector<grove_placement_t> place; std::vector<grove_scope_status_t> sstat;
+};
+
+// Whatever goes wrong while armed, the handle goes back to the caller's submission, and queue set when one was given (queues
+// non-null), on the free table the ordinary pass left, kept in d_rc_base; the error of the failing call is what the caller sees.
+// put_back() alone is the normal end: the device table is then the free table as it is.
+struct Restore {
+  grove_engine* e; const Snapshot* s; const std::vector<grove_queue_t>* queues; const std::vector<uint32_t>* gang_queue;
+  bool armed = true;
+  int32_t put_back() const {
+    int32_t rc = grove_submit_gangs(e, s->gangs.data(), uint32_t(s->gangs.size()), s->cliques.data(), uint32_t(s->cliques.size()),
+                                    s->scopes.data(), uint32_t(s->scopes.size()));
+    if (rc || !queues) return rc;
+    // (after the submission, which clears the queue set)
+    rc = install_queues(e, queues->data(), uint32_t(queues->size()), gang_queue->data());
+    if (rc) return rc;
+    e->qu_queues = *queues; e->qu_gang_queue = *gang_queue; e->qu_given = true;
+    return GROVE_OK;
+  }
+  ~Restore() {
+    if (!armed) return;
+    const std::string keep = e->err;
+    cudaMemcpyAsync(e->d_nres.p, e->d_rc_base.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToDevice, e->stream);
+    cudaStreamSynchronize(e->stream);
+    put_back();
+    e->err = keep;
+  }
+};
+
+// a sub-submission of some of the caller's gangs: its gang k is the caller's ids[k]
+struct Sub {
+  std::vector<uint32_t> ids;
+  std::vector<grove_gang_t> gangs; std::vector<grove_clique_t> cliques; std::vector<grove_scope_t> scopes;
+};
+
+// the running gangs on each node (caller order) as a CSR: run[off[n] .. off[n + 1]), running gangs ascending
+struct RunningByNode { std::vector<uint32_t> off, run; };
 }  // namespace
 
-static int32_t publish_reclaim(grove_engine* e, std::vector<grove_gang_status_t>& status, const std::vector<grove_placement_t>& place,
-                               const std::vector<std::vector<grove_placement_t>>& extra, const std::vector<grove_scope_status_t>& sstat,
-                               grove_cycle_stats_t st0, std::vector<grove_victim_t> victims, grove_cycle_stats_t* stats);
-
-int32_t grove_run_cycle_preempt(grove_engine_t* e, const grove_running_gang_t* running, uint32_t n_running,
-                                const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
-  if (!e || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
-  if (e->sp_members) return refuse_spread(e, "grove_run_cycle_preempt");
-  if (e->qu_members) return refuse_queues(e, "grove_run_cycle_preempt");
-  if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_preempt");
-  NoDiagnosis no_diag{e};
-  if (e->wide) return refuse_wide(e, "grove_run_cycle_preempt");
+// the running gangs' inputs: every holding range inside `holdings`, every holding on a node of the snapshot
+static int32_t check_running(grove_engine* e, const grove_running_gang_t* running, uint32_t n_running, const grove_holding_t* holdings,
+                             uint32_t n_holdings) {
   for (uint32_t r = 0; r < n_running; ++r)
     if (uint64_t(running[r].holding_off) + running[r].n_holdings > n_holdings) return fail(e, GROVE_ERR_INVALID_ARG, "running gang holdings out of range");
-  if (e->nodes_loaded) for (uint32_t h = 0; h < n_holdings; ++h)
+  for (uint32_t h = 0; h < n_holdings; ++h)
     if (holdings[h].node >= e->N) return fail(e, GROVE_ERR_INVALID_ARG, "holding on a node out of range");
-  grove_cycle_stats_t st0{};
-  int32_t rc = grove_run_cycle(e, &st0);
-  if (rc) return rc;
-  const uint32_t G = e->G, Q = e->Q, S = e->S, N = e->N;
-  // the ordinary pass's outputs and the submission itself (the handle is re-used for the class cycles)
-  std::vector<grove_gang_t> gangs(e->gangs.data(), e->gangs.data() + G);
-  std::vector<grove_clique_t> cliques(e->cliques.data(), e->cliques.data() + Q);
-  std::vector<grove_scope_t> scopes(e->scopes.data(), e->scopes.data() + S);
-  std::vector<grove_gang_status_t> status(e->h_status.p, e->h_status.p + G);
-  std::vector<grove_placement_t> place(e->h_out.p, e->h_out.p + e->n_out);
-  std::vector<grove_scope_status_t> sstat(std::max<uint32_t>(S, 1));
-  if (S) { rc = grove_get_scope_domains(e, sstat.data(), S); if (rc) return rc; }
-  std::vector<int32_t> classes;
-  for (uint32_t g = 0; g < G; ++g) if (status[g].state == GROVE_GANG_REJECTED) classes.push_back(gangs[g].priority);
-  std::sort(classes.begin(), classes.end(), std::greater<int32_t>());
-  classes.erase(std::unique(classes.begin(), classes.end()), classes.end());
-  int32_t min_run = INT32_MAX;
-  for (uint32_t r = 0; r < n_running; ++r) min_run = std::min(min_run, running[r].priority);
-  std::vector<grove_victim_t> victims;
-  std::vector<std::vector<grove_placement_t>> extra(G);   // placements of the preemptors, by gang
-  if (!classes.empty() && n_running && classes.front() > min_run) {
-    std::vector<grove_node_t> real(N), view(N);
-    rc = grove_get_nodes(e, real.data(), N);
-    if (rc) return rc;
-    // whatever goes wrong from here on, the handle goes back to the caller's submission on the node table of the ordinary pass
-    // (its class cycles re-use the handle); the error of the failing call is what the caller sees
-    struct Restore {
-      grove_engine* e; const std::vector<grove_node_t>* nodes; const std::vector<grove_gang_t>* g; const std::vector<grove_clique_t>* c; const std::vector<grove_scope_t>* s; bool armed = true;
-      ~Restore() {
-        if (!armed) return;
-        const std::string keep = e->err;
-        grove_load_nodes(e, nodes->data(), uint32_t(nodes->size()));
-        grove_submit_gangs(e, g->data(), uint32_t(g->size()), c->data(), uint32_t(c->size()), s->data(), uint32_t(s->size()));
-        e->err = keep;
-      }
-    };
-    const std::vector<grove_node_t> real0 = real;
-    Restore restore{e, &real0, &gangs, &cliques, &scopes};
-    std::vector<uint8_t> evicted(n_running, 0);
-    // running gangs by node (CSR), for the victim choice
-    size_t n_held = 0;   // (ranges of running gangs may overlap: size by what the fill below writes)
-    for (uint32_t r = 0; r < n_running; ++r) n_held += running[r].n_holdings;
-    std::vector<uint32_t> at_off(size_t(N) + 1, 0), at_run(n_held);
-    for (uint32_t r = 0; r < n_running; ++r) for (uint32_t h = 0; h < running[r].n_holdings; ++h) ++at_off[holdings[running[r].holding_off + h].node + 1];
-    for (uint32_t n = 0; n < N; ++n) at_off[n + 1] += at_off[n];
-    { std::vector<uint32_t> cur(at_off.begin(), at_off.end() - 1);
-      for (uint32_t r = 0; r < n_running; ++r) for (uint32_t h = 0; h < running[r].n_holdings; ++h) at_run[cur[holdings[running[r].holding_off + h].node]++] = r; }
-    for (int32_t p : classes) {
-      bool any = false;
-      view = real;
-      for (uint32_t r = 0; r < n_running; ++r) {
-        if (evicted[r] || running[r].priority >= p) continue;
-        any = true;
-        for (uint32_t h = 0; h < running[r].n_holdings; ++h) give(view[holdings[running[r].holding_off + h].node], holdings[running[r].holding_off + h]);
-      }
-      if (!any) continue;   // nothing to reclaim for this class (nor for the lower ones)
-      // the class's rejected gangs as a submission of their own: anchors pinned to what the ordinary pass used, no gating
-      // (a rejected gang's base gang, if any, was admitted before it)
-      std::vector<uint32_t> ids;
-      std::vector<grove_gang_t> sg; std::vector<grove_clique_t> sq; std::vector<grove_scope_t> ss;
-      for (uint32_t g = 0; g < G; ++g) {
-        if (status[g].state != GROVE_GANG_REJECTED || gangs[g].priority != p) continue;
-        grove_gang_t x = gangs[g];
-        if (x.anchor_node == GROVE_NONE_U32) x.anchor_node = e->perm[fmix32(g) % N];
-        x.base_gang = GROVE_NONE_U32;
-        x.clique_off = uint32_t(sq.size()); x.scope_off = uint32_t(ss.size());
-        sq.insert(sq.end(), cliques.begin() + gangs[g].clique_off, cliques.begin() + gangs[g].clique_off + gangs[g].n_cliques);
-        ss.insert(ss.end(), scopes.begin() + gangs[g].scope_off, scopes.begin() + gangs[g].scope_off + gangs[g].n_scopes);
-        ids.push_back(g); sg.push_back(x);
-      }
-      if (ids.empty()) continue;
-      rc = grove_load_nodes(e, view.data(), N); if (rc) return rc;
-      rc = grove_submit_gangs(e, sg.data(), uint32_t(sg.size()), sq.data(), uint32_t(sq.size()), ss.data(), uint32_t(ss.size())); if (rc) return rc;
-      grove_cycle_stats_t stp{};
-      rc = grove_run_cycle(e, &stp); if (rc) return rc;
-      st0.rounds += stp.rounds; st0.evaluations += stp.evaluations; st0.kernel_launches += stp.kernel_launches;
-      st0.ms_fit += stp.ms_fit; st0.ms_admit += stp.ms_admit; st0.ms_commit += stp.ms_commit; st0.ms_total += stp.ms_total;
-      std::vector<grove_scope_status_t> ssp(std::max<size_t>(ss.size(), 1));
-      if (!ss.empty()) { rc = grove_get_scope_domains(e, ssp.data(), uint32_t(ss.size())); if (rc) return rc; }
-      for (uint32_t k = 0; k < ids.size(); ++k) {   // sub-submission order == order rank (one priority)
-        const grove_gang_status_t& sp = e->h_status.p[k];
-        if (sp.state != GROVE_GANG_ADMITTED) continue;
-        const uint32_t g = ids[k];
-        // what the gang puts on each node, nodes in the order its placement first names them
-        std::vector<uint32_t> order; std::vector<Res> use;
-        for (uint32_t i = 0; i < sp.n_pods; ++i) {
-          const grove_placement_t pl = e->h_out.p[sp.placement_off + i];
-          const grove_clique_t& q = sq[pl.clique];
-          size_t j = 0;
-          for (; j < order.size(); ++j) if (order[j] == pl.node) break;
-          if (j == order.size()) { order.push_back(pl.node); use.emplace_back(); }
-          use[j].cpu += q.req_cpu_milli; use[j].mem += q.req_mem_mib; use[j].gpu += q.req_gpu; use[j].pods += 1;
-          extra[g].push_back(grove_placement_t{gangs[g].clique_off + (pl.clique - sg[k].clique_off), pl.node});
-        }
-        for (size_t j = 0; j < order.size(); ++j) {
-          const uint32_t n = order[j];
-          while (!covers(real[n], use[j])) {
-            uint32_t v = GROVE_NONE_U32;   // lowest priority first, then the highest running index
-            for (uint32_t a = at_off[n]; a < at_off[n + 1]; ++a) {
-              const uint32_t r = at_run[a];
-              if (evicted[r] || running[r].priority >= p) continue;
-              if (v == GROVE_NONE_U32 || running[r].priority < running[v].priority || (running[r].priority == running[v].priority && r > v)) v = r;
-            }
-            if (v == GROVE_NONE_U32) return fail(e, GROVE_ERR_STATE, "reclaim pass: a preemptor's node cannot be freed");
-            evicted[v] = 1;
-            for (uint32_t h = 0; h < running[v].n_holdings; ++h) give(real[holdings[running[v].holding_off + h].node], holdings[running[v].holding_off + h]);
-            victims.push_back(grove_victim_t{v, g});
-          }
-          real[n].free_cpu_milli -= uint32_t(use[j].cpu); real[n].free_mem_mib -= uint32_t(use[j].mem);
-          real[n].free_gpu = uint16_t(real[n].free_gpu - use[j].gpu); real[n].free_pods = uint16_t(real[n].free_pods - use[j].pods);
-        }
-        grove_gang_status_t o = sp;
-        o.reserved0 = GROVE_STATUS_PREEMPTOR;
-        status[g] = o;   // placement_off is assigned when the outputs are merged
-        for (uint32_t si = 0; si < gangs[g].n_scopes; ++si) sstat[gangs[g].scope_off + si] = ssp[sg[k].scope_off + si];
-        st0.gangs_admitted += 1; st0.gangs_rejected -= 1;
-      }
-    }
-    // the handle goes back to the caller's submission, on the node table that is really free now
-    restore.armed = false;
-    rc = grove_load_nodes(e, real.data(), N); if (rc) return rc;
-    rc = grove_submit_gangs(e, gangs.data(), G, cliques.data(), Q, scopes.data(), S); if (rc) return rc;
+  return GROVE_OK;
+}
+
+// cpu, mem, gpu summed over a running gang's holdings
+static std::array<int64_t, 3> usage_of(const grove_running_gang_t& r, const grove_holding_t* holdings) {
+  std::array<int64_t, 3> u{0, 0, 0};
+  for (uint32_t h = 0; h < r.n_holdings; ++h) {
+    const grove_holding_t& x = holdings[r.holding_off + h];
+    u[0] += x.cpu_milli; u[1] += x.mem_mib; u[2] += x.gpu;
   }
-  return publish_reclaim(e, status, place, extra, sstat, st0, std::move(victims), stats);
+  return u;
+}
+
+static int32_t snapshot(grove_engine* e, Snapshot* s) {
+  const uint32_t G = e->G, Q = e->Q, S = e->S;
+  s->gangs.assign(e->gangs.data(), e->gangs.data() + G);
+  s->cliques.assign(e->cliques.data(), e->cliques.data() + Q);
+  s->scopes.assign(e->scopes.data(), e->scopes.data() + S);
+  s->status.assign(e->h_status.p, e->h_status.p + G);
+  s->place.assign(e->h_out.p, e->h_out.p + e->n_out);
+  s->sstat.assign(std::max<uint32_t>(S, 1), grove_scope_status_t{});
+  return S ? grove_get_scope_domains(e, s->sstat.data(), S) : GROVE_OK;
+}
+
+static RunningByNode running_by_node(uint32_t N, const grove_running_gang_t* running, uint32_t n_running, const grove_holding_t* holdings) {
+  RunningByNode at;
+  size_t n_held = 0;   // (ranges of running gangs may overlap: size by what the fill below writes)
+  for (uint32_t r = 0; r < n_running; ++r) n_held += running[r].n_holdings;
+  at.off.assign(size_t(N) + 1, 0); at.run.resize(n_held);
+  for (uint32_t r = 0; r < n_running; ++r) for (uint32_t h = 0; h < running[r].n_holdings; ++h) ++at.off[holdings[running[r].holding_off + h].node + 1];
+  for (uint32_t n = 0; n < N; ++n) at.off[n + 1] += at.off[n];
+  std::vector<uint32_t> cur(at.off.begin(), at.off.end() - 1);
+  for (uint32_t r = 0; r < n_running; ++r) for (uint32_t h = 0; h < running[r].n_holdings; ++h) at.run[cur[holdings[running[r].holding_off + h].node]++] = r;
+  return at;
+}
+
+// the victim rule: lowest priority first, then the highest running index.  Does running gang x go before v (GROVE_NONE_U32: none)?
+static bool evicted_before(const grove_running_gang_t* running, uint32_t x, uint32_t v) {
+  return v == GROVE_NONE_U32 || running[x].priority < running[v].priority || (running[x].priority == running[v].priority && x > v);
+}
+
+// the victim among the running gangs on node n that `eligible` admits, GROVE_NONE_U32 when there is none
+static uint32_t choose_victim(const RunningByNode& at, uint32_t n, const grove_running_gang_t* running,
+                              const std::function<bool(uint32_t)>& eligible) {
+  uint32_t v = GROVE_NONE_U32;
+  for (uint32_t a = at.off[n]; a < at.off[n + 1]; ++a)
+    if (eligible(at.run[a]) && evicted_before(running, at.run[a], v)) v = at.run[a];
+  return v;
+}
+
+// gang g of the caller's submission appended to a sub-submission: anchor pinned to the one the ordinary pass derived, no gating (a
+// rejected gang's base gang, if any, was admitted before it), cliques and scopes rebased -> the appended record
+static grove_gang_t& add_gang(grove_engine* e, const Snapshot& s, uint32_t g, Sub& sub) {
+  const grove_gang_t& o = s.gangs[g];
+  grove_gang_t x = o;
+  if (x.anchor_node == GROVE_NONE_U32) x.anchor_node = e->perm[fmix32(g) % e->N];
+  x.base_gang = GROVE_NONE_U32;
+  x.clique_off = uint32_t(sub.cliques.size()); x.scope_off = uint32_t(sub.scopes.size());
+  sub.cliques.insert(sub.cliques.end(), s.cliques.begin() + o.clique_off, s.cliques.begin() + o.clique_off + o.n_cliques);
+  sub.scopes.insert(sub.scopes.end(), s.scopes.begin() + o.scope_off, s.scopes.begin() + o.scope_off + o.n_scopes);
+  sub.ids.push_back(g); sub.gangs.push_back(x);
+  return sub.gangs.back();
+}
+
+static int32_t submit_sub(grove_engine* e, const Sub& sub) {
+  return grove_submit_gangs(e, sub.gangs.data(), uint32_t(sub.gangs.size()), sub.cliques.data(), uint32_t(sub.cliques.size()),
+                            sub.scopes.data(), uint32_t(sub.scopes.size()));
+}
+
+// the scope domains of the sub-cycle just run
+static int32_t sub_scope_domains(grove_engine* e, const Sub& sub, std::vector<grove_scope_status_t>& out) {
+  out.assign(std::max<size_t>(sub.scopes.size(), 1), grove_scope_status_t{});
+  return sub.scopes.empty() ? GROVE_OK : grove_get_scope_domains(e, out.data(), uint32_t(sub.scopes.size()));
+}
+
+// a sub-cycle's stats added to the call's
+static void accumulate(grove_cycle_stats_t& st0, const grove_cycle_stats_t& s) {
+  st0.rounds += s.rounds; st0.evaluations += s.evaluations; st0.kernel_launches += s.kernel_launches;
+  st0.ms_fit += s.ms_fit; st0.ms_admit += s.ms_admit; st0.ms_commit += s.ms_commit; st0.ms_total += s.ms_total;
+}
+
+// the rows of the free table kept aside in d_rc_real at these nodes (caller order)
+static int32_t read_rows(grove_engine* e, const std::vector<uint32_t>& nodes, std::vector<Res>& rows, grove_cycle_stats_t& st) {
+  rows.assign(nodes.size(), Res{});
+  if (nodes.empty()) return GROVE_OK;
+  std::vector<uint32_t> idx(nodes.size());
+  for (size_t i = 0; i < nodes.size(); ++i) idx[i] = e->inv[nodes[i]];
+  std::vector<uint4> got(idx.size());
+  CU_TRY(e, e->d_rc_idx.ensure(idx.size())); CU_TRY(e, e->d_rc_rows.ensure(idx.size()));
+  CU_TRY(e, cudaMemcpyAsync(e->d_rc_idx.p, idx.data(), sizeof(uint32_t) * idx.size(), cudaMemcpyHostToDevice, e->stream));
+  k_reclaim_rows<<<uint32_t((idx.size() + 255) / 256), 256, 0, e->stream>>>(e->d_rc_real.p, e->d_rc_idx.p, e->d_rc_rows.p, uint32_t(idx.size()));
+  CU_TRY(e, cudaGetLastError());
+  CU_TRY(e, cudaMemcpyAsync(got.data(), e->d_rc_rows.p, sizeof(uint4) * got.size(), cudaMemcpyDeviceToHost, e->stream));
+  CU_TRY(e, cudaStreamSynchronize(e->stream));
+  for (size_t i = 0; i < got.size(); ++i) rows[i] = Res{got[i].x, got[i].y, got[i].z & 0xFFFFu, got[i].z >> 16};
+  st.kernel_launches += 1;
+  return GROVE_OK;
+}
+
+// What the sub-cycle just run gave gang k of its sub-submission: its usage per node, nodes in the order its placement first names
+// them, and its placements with the cliques numbered as in the caller's submission (appended to pl).
+static void placed(grove_engine* e, const Snapshot& s, const Sub& sub, uint32_t k, std::vector<uint32_t>& nodes, std::vector<Res>& use,
+                   std::vector<grove_placement_t>& pl) {
+  const grove_gang_status_t& sp = e->h_status.p[k];
+  const uint32_t off = s.gangs[sub.ids[k]].clique_off;
+  for (uint32_t i = 0; i < sp.n_pods; ++i) {
+    const grove_placement_t x = e->h_out.p[sp.placement_off + i];
+    const grove_clique_t& q = sub.cliques[x.clique];
+    const size_t j = size_t(std::find(nodes.begin(), nodes.end(), x.node) - nodes.begin());
+    if (j == nodes.size()) { nodes.push_back(x.node); use.emplace_back(); }
+    use[j].add(Res{q.req_cpu_milli, q.req_mem_mib, q.req_gpu, 1});
+    pl.push_back(grove_placement_t{off + (x.clique - sub.gangs[k].clique_off), x.node});
+  }
+}
+
+// gang k of a sub-submission, admitted, into the outputs of the caller's gang sub.ids[k]: status o (placement_off is assigned when
+// the outputs are merged) and the scope domains ssp of the sub-cycle
+static void merge_gang(Snapshot& s, const Sub& sub, uint32_t k, const grove_gang_status_t& o, const std::vector<grove_scope_status_t>& ssp) {
+  const uint32_t g = sub.ids[k];
+  s.status[g] = o;
+  for (uint32_t si = 0; si < s.gangs[g].n_scopes; ++si) s.sstat[s.gangs[g].scope_off + si] = ssp[sub.gangs[k].scope_off + si];
+}
+
+// d = (sorted node, change) -> one record per node, added to the device's node table (reclaim.cuh k_reclaim_patch); nothing to do
+// for an empty d
+static int32_t patch_nodes(grove_engine* e, std::vector<std::pair<uint32_t, Res>>& d, grove_cycle_stats_t& st) {
+  if (d.empty()) return GROVE_OK;
+  std::sort(d.begin(), d.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+  std::vector<uint4> patch;
+  for (size_t i = 0; i < d.size();) {
+    const uint32_t n = d[i].first;
+    Res v;
+    for (; i < d.size() && d[i].first == n; ++i) v.add(d[i].second);
+    patch.push_back(make_uint4(n, uint32_t(v.cpu), uint32_t(v.mem), uint32_t(v.gpu + v.pods * 65536)));
+  }
+  CU_TRY(e, e->d_rc_patch.ensure(patch.size()));
+  CU_TRY(e, cudaMemcpyAsync(e->d_rc_patch.p, patch.data(), sizeof(uint4) * patch.size(), cudaMemcpyHostToDevice, e->stream));
+  k_reclaim_patch<<<uint32_t((patch.size() + 255) / 256), 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_patch.p, uint32_t(patch.size()));
+  CU_TRY(e, cudaGetLastError());
+  st.kernel_launches += 1;
+  return GROVE_OK;
 }
 
 // the outputs of a cycle with a reclaim or consolidation pass, merged: placements grouped by gang in submission order (those of a
@@ -2005,14 +2060,11 @@ int32_t grove_get_victims(grove_engine_t* e, grove_victim_t* out, uint32_t cap, 
 // the inputs of a cycle with replacements (grove_run_cycle_reuse, grove_run_cycle_reuse_preempt)
 static int32_t check_reuse_inputs(grove_engine* e, const uint32_t* replaces, uint32_t n_gangs, const grove_running_gang_t* running,
                                   uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings) {
-  if (!e->nodes_loaded) return fail(e, GROVE_ERR_STATE, "no node snapshot loaded");
-  if (!e->gangs_loaded) return fail(e, GROVE_ERR_STATE, "no gangs submitted");
-  if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
+  int32_t rc = check_ready(e);
+  if (rc) return rc;
   if (n_gangs != e->G) return fail(e, GROVE_ERR_INVALID_ARG, "replaces must have one entry per submitted gang");
-  for (uint32_t r = 0; r < n_running; ++r)
-    if (uint64_t(running[r].holding_off) + running[r].n_holdings > n_holdings) return fail(e, GROVE_ERR_INVALID_ARG, "running gang holdings out of range");
-  for (uint32_t h = 0; h < n_holdings; ++h)
-    if (holdings[h].node >= e->N) return fail(e, GROVE_ERR_INVALID_ARG, "holding on a node out of range");
+  rc = check_running(e, running, n_running, holdings, n_holdings);
+  if (rc) return rc;
   std::vector<uint8_t> taken(n_running, 0);
   for (uint32_t g = 0; g < n_gangs; ++g) {
     const uint32_t r = replaces[g];
@@ -2025,7 +2077,8 @@ static int32_t check_reuse_inputs(grove_engine* e, const uint32_t* replaces, uin
 }
 
 // The cycle over the submitted gangs in which gang g with replaces[g] != GROVE_NONE_U32 holds what that running gang holds
-// (inputs checked by check_reuse_inputs).  check_fit: first make sure that free plus every hold fits the node record's fields.
+// (inputs checked by check_reuse_inputs); with no hold at all, the ordinary cycle.  check_fit: first make sure that free plus every
+// hold fits the node record's fields.
 static int32_t run_cycle_holds(grove_engine* e, const uint32_t* replaces, const grove_running_gang_t* running, const grove_holding_t* holdings,
                                bool check_fit, grove_cycle_stats_t* stats) {
   const uint32_t n_gangs = e->G;
@@ -2051,9 +2104,10 @@ static int32_t run_cycle_holds(grove_engine* e, const uint32_t* replaces, const 
     }
     recs.resize(w);
   }
+  if (recs.empty()) return run_cycle(e, stats);
   off[n_gangs] = uint32_t(recs.size());
   // the free table plus every hold must fit the node record's fields
-  if (check_fit && !recs.empty()) {
+  if (check_fit) {
     std::vector<uint4> nres(e->Npad);
     CU_TRY(e, cudaMemcpyAsync(nres.data(), e->d_nres.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToHost, e->stream));
     CU_TRY(e, cudaStreamSynchronize(e->stream));
@@ -2067,7 +2121,7 @@ static int32_t run_cycle_holds(grove_engine* e, const uint32_t* replaces, const 
         return fail(e, GROVE_ERR_INVALID_ARG, "free resources plus holdings overflow a field of a node record");
     }
   }
-  std::vector<uint4> hold(std::max<size_t>(recs.size(), 1));
+  std::vector<uint4> hold(recs.size());
   for (size_t i = 0; i < recs.size(); ++i)
     hold[i] = make_uint4(recs[i].node, uint32_t(recs[i].v[0]), uint32_t(recs[i].v[1]), uint32_t(recs[i].v[2]) | (uint32_t(recs[i].v[3]) << 16));
   CU_TRY(e, e->d_hold_off.ensure(off.size())); CU_TRY(e, e->d_hold.ensure(hold.size()));
@@ -2075,7 +2129,7 @@ static int32_t run_cycle_holds(grove_engine* e, const uint32_t* replaces, const 
   CU_TRY(e, cudaMemcpyAsync(e->d_hold.p, hold.data(), sizeof(uint4) * hold.size(), cudaMemcpyHostToDevice, e->stream));
   CU_TRY(e, cudaStreamSynchronize(e->stream));   // (pageable sources)
   struct HoldsOn { grove_engine* e; ~HoldsOn() { e->holds_on = false; e->n_hold = 0; } } holds_guard{e};
-  e->holds_on = !recs.empty(); e->n_hold = uint32_t(recs.size());
+  e->holds_on = true; e->n_hold = uint32_t(recs.size());
   return run_cycle(e, stats);
 }
 
@@ -2093,14 +2147,17 @@ int32_t grove_run_cycle_reuse(grove_engine_t* e, const uint32_t* replaces, uint3
 }
 
 // ---------------------------------------------------------------------------------------------
-// Reuse with reclaim (include/grove_place.h "reuse with reclaim"; DESIGN.md section 1).  The ordinary pass is the reuse cycle.
-// Then every priority class of the gangs it rejected is ONE cycle with holds (the members whose predecessor ranks at or above
-// the class hold what it holds) over the class view, which reclaim.cuh builds on the device from the running gangs' holdings:
-// the free table plus whatever the standing running gangs of a lower priority hold.  Victims are chosen on the host, gang by
-// gang in rank order, over the rows of the nodes the class's preemptors use; then the device takes the holdings of the running
-// gangs still standing off the table again, which leaves the free table.
+// The reclaim loop of grove_run_cycle_preempt, grove_run_cycle_reuse_preempt and grove_run_cycle_preempt_queues (include/grove_place.h
+// "preemption / reclaim", "reuse with reclaim", "reclaim within queue limits"; DESIGN.md section 1).  The ordinary pass is the cycle
+// with holds.  Then every priority class of the gangs it rejected is ONE cycle with holds (the members whose predecessor ranks at
+// or above the class hold what it holds) over the class view, which reclaim.cuh builds on the device from the running gangs'
+// holdings: the free table plus whatever the standing running gangs of a lower priority hold.  Under a queue set the class cycle
+// is a queue cycle with a set of its own, whose `used` leave out what the gangs of E(p) hold: its loads are load'; queue loads are
+// followed here, between classes.  Victims are chosen on the host, gang by gang in rank order, over the rows of the nodes the
+// class's preemptors use: the node step, then for a queue member the queue step.  Then the device takes the holdings of the
+// running gangs still standing off the table again, which leaves the free table.
 // ---------------------------------------------------------------------------------------------
-// The running gangs of grove_run_cycle_reuse_preempt / grove_run_cycle_consolidate on the device (reclaim.cuh): their holdings by
+// The running gangs of the reclaim loop and grove_run_cycle_consolidate on the device (reclaim.cuh): their holdings by
 // sorted node, running gangs ascending within a row, and their priorities, uploaded once; the gone mask (one byte per running gang)
 // is the caller's to upload.  Then the check that free plus every running gang's holdings fits the node record's fields: then so
 // does every view built from them.
@@ -2139,310 +2196,46 @@ static int32_t upload_running(grove_engine* e, const grove_running_gang_t* runni
   return GROVE_OK;
 }
 
-// d = (sorted node, change) -> one record per node, added to the device's node table (reclaim.cuh k_reclaim_patch).  The give-back of
-// the members of a class admitted after E(p) ran out.
-static int32_t patch_nodes(grove_engine* e, std::vector<std::pair<uint32_t, std::array<int64_t, 4>>>& d) {
-  std::sort(d.begin(), d.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
-  std::vector<uint4> patch;
-  for (size_t i = 0; i < d.size();) {
-    const uint32_t n = d[i].first;
-    int64_t v[4] = {0, 0, 0, 0};
-    for (; i < d.size() && d[i].first == n; ++i) for (int k = 0; k < 4; ++k) v[k] += d[i].second[k];
-    patch.push_back(make_uint4(n, uint32_t(v[0]), uint32_t(v[1]), uint32_t(v[2] + v[3] * 65536)));
-  }
-  CU_TRY(e, e->d_rc_patch.ensure(patch.size()));
-  CU_TRY(e, cudaMemcpyAsync(e->d_rc_patch.p, patch.data(), sizeof(uint4) * patch.size(), cudaMemcpyHostToDevice, e->stream));
-  k_reclaim_patch<<<uint32_t((patch.size() + 255) / 256), 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_patch.p, uint32_t(patch.size()));
-  CU_TRY(e, cudaGetLastError());
-  return GROVE_OK;
-}
-
-int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs, const grove_running_gang_t* running,
-                                      uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
-  if (!e || (n_gangs && !replaces) || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
-  if (e->sp_members) return refuse_spread(e, "grove_run_cycle_reuse_preempt");
-  if (e->qu_members) return refuse_queues(e, "grove_run_cycle_reuse_preempt");
-  if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_reuse_preempt");
-  NoDiagnosis no_diag{e};
-  if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse_preempt");
-  int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);
-  if (rc) return rc;
+// replaces (null: no gang replaces a running gang) as for grove_run_cycle_reuse; running_queue (null: no queue set) the queue of each
+// running gang in the queue set of the current submission.  Inputs checked by the entry.
+static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const grove_running_gang_t* running, uint32_t n_running,
+                             const grove_holding_t* holdings, const uint32_t* running_queue, grove_cycle_stats_t* stats) {
   CU_TRY(e, cudaSetDevice(e->cfg.device));
-  const uint32_t N = e->N, nblk = (N + 255) / 256;
-  ReclaimCsr csr{};
-  rc = upload_running(e, running, n_running, holdings, &csr);
-  if (rc) return rc;
-  std::vector<int32_t> prio(std::max<uint32_t>(n_running, 1), 0);
-  for (uint32_t r = 0; r < n_running; ++r) prio[r] = running[r].priority;
-  std::vector<uint8_t> gone(std::max<uint32_t>(n_running, 1), 0);   // released or evicted
-
-  // 1. the ordinary pass: the reuse cycle.  An admitted new version's predecessor is released.
-  grove_cycle_stats_t st0{};
-  rc = run_cycle_holds(e, replaces, running, holdings, false, &st0);
-  if (rc) return rc;
-  const uint32_t G = e->G, Q = e->Q, S = e->S;
-  std::vector<grove_gang_t> gangs(e->gangs.data(), e->gangs.data() + G);
-  std::vector<grove_clique_t> cliques(e->cliques.data(), e->cliques.data() + Q);
-  std::vector<grove_scope_t> scopes(e->scopes.data(), e->scopes.data() + S);
-  std::vector<grove_gang_status_t> status(e->h_status.p, e->h_status.p + G);
-  std::vector<grove_placement_t> place(e->h_out.p, e->h_out.p + e->n_out);
-  std::vector<grove_scope_status_t> sstat(std::max<uint32_t>(S, 1));
-  if (S) { rc = grove_get_scope_domains(e, sstat.data(), S); if (rc) return rc; }
-  for (uint32_t g = 0; g < G; ++g)
-    if (status[g].state == GROVE_GANG_ADMITTED && replaces[g] != GROVE_NONE_U32) gone[replaces[g]] = 1;
-  std::vector<int32_t> classes;
-  for (uint32_t g = 0; g < G; ++g) if (status[g].state == GROVE_GANG_REJECTED) classes.push_back(gangs[g].priority);
-  std::sort(classes.begin(), classes.end(), std::greater<int32_t>());
-  classes.erase(std::unique(classes.begin(), classes.end()), classes.end());
-  auto below = [&](int32_t p) {   // is E(p) -- the standing running gangs of a priority below p -- non-empty?
-    for (uint32_t r = 0; r < n_running; ++r) if (!gone[r] && prio[r] < p) return true;
-    return false;
-  };
-  std::vector<grove_victim_t> victims;
-  std::vector<std::vector<grove_placement_t>> extra(G);   // placements of the preemptors, by gang
-  if (!classes.empty() && below(classes.front())) {
-    // whatever goes wrong from here on, the handle goes back to the caller's submission on the free table the ordinary pass left
-    CU_TRY(e, cudaMemcpyAsync(e->d_rc_base.p, e->d_nres.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToDevice, e->stream));
-    struct Restore {
-      grove_engine* e; const std::vector<grove_gang_t>* g; const std::vector<grove_clique_t>* c; const std::vector<grove_scope_t>* s; bool armed = true;
-      ~Restore() {
-        if (!armed) return;
-        const std::string keep = e->err;
-        cudaMemcpyAsync(e->d_nres.p, e->d_rc_base.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToDevice, e->stream);
-        cudaStreamSynchronize(e->stream);
-        grove_submit_gangs(e, g->data(), uint32_t(g->size()), c->data(), uint32_t(c->size()), s->data(), uint32_t(s->size()));
-        e->err = keep;
-      }
-    };
-    Restore restore{e, &gangs, &cliques, &scopes};
-    // running gangs by node (caller order), for the victim choice
-    size_t n_held = 0;   // (ranges of running gangs may overlap: size by what the fill below writes)
-    for (uint32_t r = 0; r < n_running; ++r) n_held += running[r].n_holdings;
-    std::vector<uint32_t> at_off(size_t(N) + 1, 0), at_run(n_held);
-    for (uint32_t r = 0; r < n_running; ++r) for (uint32_t h = 0; h < running[r].n_holdings; ++h) ++at_off[holdings[running[r].holding_off + h].node + 1];
-    for (uint32_t n = 0; n < N; ++n) at_off[n + 1] += at_off[n];
-    { std::vector<uint32_t> cur(at_off.begin(), at_off.end() - 1);
-      for (uint32_t r = 0; r < n_running; ++r) for (uint32_t h = 0; h < running[r].n_holdings; ++h) at_run[cur[holdings[running[r].holding_off + h].node]++] = r; }
-    std::vector<int32_t> slot(N, -1);   // node (caller order) -> its row in `rows` while a class chooses its victims
-    for (int32_t p : classes) {
-      if (!below(p)) break;   // E(p) only shrinks from one class to the next
-      // 2. the class's rejected gangs as a submission of their own: anchors pinned to what the ordinary pass used, no gating.
-      // A member holds its predecessor's holdings when that one still stands at or above p; below p it is evictable instead.
-      std::vector<uint32_t> ids, sub_rep;
-      std::vector<grove_gang_t> sg; std::vector<grove_clique_t> sq; std::vector<grove_scope_t> ss;
-      for (uint32_t g = 0; g < G; ++g) {
-        if (status[g].state != GROVE_GANG_REJECTED || gangs[g].priority != p) continue;
-        grove_gang_t x = gangs[g];
-        if (x.anchor_node == GROVE_NONE_U32) x.anchor_node = e->perm[fmix32(g) % N];
-        x.base_gang = GROVE_NONE_U32;
-        x.clique_off = uint32_t(sq.size()); x.scope_off = uint32_t(ss.size());
-        sq.insert(sq.end(), cliques.begin() + gangs[g].clique_off, cliques.begin() + gangs[g].clique_off + gangs[g].n_cliques);
-        ss.insert(ss.end(), scopes.begin() + gangs[g].scope_off, scopes.begin() + gangs[g].scope_off + gangs[g].n_scopes);
-        const uint32_t r = replaces[g];
-        ids.push_back(g); sg.push_back(x);
-        sub_rep.push_back(r != GROVE_NONE_U32 && !gone[r] && prio[r] >= p ? r : GROVE_NONE_U32);
-      }
-      // the class view, on the device: free + the standing holdings of E(p); the free table itself is kept for the victim choice
-      CU_TRY(e, cudaMemcpyAsync(e->d_rc_gone.p, gone.data(), gone.size(), cudaMemcpyHostToDevice, e->stream));
-      k_reclaim_view<<<nblk, 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_real.p, csr, N, p, 1u);
-      CU_TRY(e, cudaGetLastError());
-      rc = grove_submit_gangs(e, sg.data(), uint32_t(sg.size()), sq.data(), uint32_t(sq.size()), ss.data(), uint32_t(ss.size())); if (rc) return rc;
-      grove_cycle_stats_t stp{};
-      rc = run_cycle_holds(e, sub_rep.data(), running, holdings, false, &stp); if (rc) return rc;
-      st0.rounds += stp.rounds; st0.evaluations += stp.evaluations; st0.kernel_launches += stp.kernel_launches + 2;   // (+ the two k_reclaim_view)
-      st0.ms_fit += stp.ms_fit; st0.ms_admit += stp.ms_admit; st0.ms_commit += stp.ms_commit; st0.ms_total += stp.ms_total;
-      std::vector<grove_scope_status_t> ssp(std::max<size_t>(ss.size(), 1));
-      if (!ss.empty()) { rc = grove_get_scope_domains(e, ssp.data(), uint32_t(ss.size())); if (rc) return rc; }
-      // the free-table rows of the nodes the class's preemptors use
-      std::vector<uint32_t> used;
-      for (uint32_t k = 0; k < ids.size(); ++k) {
-        const grove_gang_status_t& sp = e->h_status.p[k];
-        if (sp.state != GROVE_GANG_ADMITTED) continue;
-        for (uint32_t i = 0; i < sp.n_pods; ++i) used.push_back(e->h_out.p[sp.placement_off + i].node);
-      }
-      std::sort(used.begin(), used.end());
-      used.erase(std::unique(used.begin(), used.end()), used.end());
-      std::vector<Res> rows(used.size());
-      if (!used.empty()) {
-        std::vector<uint32_t> idx(used.size());
-        for (size_t i = 0; i < used.size(); ++i) { idx[i] = e->inv[used[i]]; slot[used[i]] = int32_t(i); }
-        std::vector<uint4> got(used.size());
-        CU_TRY(e, e->d_rc_idx.ensure(idx.size())); CU_TRY(e, e->d_rc_rows.ensure(idx.size()));
-        CU_TRY(e, cudaMemcpyAsync(e->d_rc_idx.p, idx.data(), sizeof(uint32_t) * idx.size(), cudaMemcpyHostToDevice, e->stream));
-        k_reclaim_rows<<<uint32_t((idx.size() + 255) / 256), 256, 0, e->stream>>>(e->d_rc_real.p, e->d_rc_idx.p, e->d_rc_rows.p, uint32_t(idx.size()));
-        CU_TRY(e, cudaGetLastError());
-        CU_TRY(e, cudaMemcpyAsync(got.data(), e->d_rc_rows.p, sizeof(uint4) * got.size(), cudaMemcpyDeviceToHost, e->stream));
-        CU_TRY(e, cudaStreamSynchronize(e->stream));
-        for (size_t i = 0; i < got.size(); ++i) rows[i] = Res{got[i].x, got[i].y, got[i].z & 0xFFFFu, got[i].z >> 16};
-        st0.kernel_launches += 1;
-      }
-      auto release = [&](uint32_t v) {   // everything v held returns to the free table (only the tracked rows matter here)
-        gone[v] = 1;
-        for (uint32_t h = 0; h < running[v].n_holdings; ++h) {
-          const grove_holding_t& x = holdings[running[v].holding_off + h];
-          if (slot[x.node] < 0) continue;
-          Res& q = rows[slot[x.node]];
-          q.cpu += x.cpu_milli; q.mem += x.mem_mib; q.gpu += x.gpu; q.pods += x.pods;
-        }
-      };
-      // 3. victims, gang by gang in rank order (sub-submission order == order rank: one priority)
-      std::vector<uint32_t> skipped;   // admitted by the class cycle after E(p) ran out: they stay REJECTED
-      for (uint32_t k = 0; k < ids.size(); ++k) {
-        const grove_gang_status_t& sp = e->h_status.p[k];
-        if (sp.state != GROVE_GANG_ADMITTED) continue;
-        if (!below(p)) { skipped.push_back(k); continue; }
-        const uint32_t g = ids[k], r = replaces[g];
-        const bool holds = sub_rep[k] != GROVE_NONE_U32;
-        if (r != GROVE_NONE_U32 && !holds && !gone[r]) release(r);   // its predecessor is in E(p): released first, not a victim
-        std::vector<uint32_t> order; std::vector<Res> use, own;
-        for (uint32_t i = 0; i < sp.n_pods; ++i) {
-          const grove_placement_t pl = e->h_out.p[sp.placement_off + i];
-          const grove_clique_t& q = sq[pl.clique];
-          size_t j = 0;
-          for (; j < order.size(); ++j) if (order[j] == pl.node) break;
-          if (j == order.size()) { order.push_back(pl.node); use.emplace_back(); own.emplace_back(); }
-          use[j].cpu += q.req_cpu_milli; use[j].mem += q.req_mem_mib; use[j].gpu += q.req_gpu; use[j].pods += 1;
-          extra[g].push_back(grove_placement_t{gangs[g].clique_off + (pl.clique - sg[k].clique_off), pl.node});
-        }
-        if (holds)   // what its predecessor holds on each of those nodes: used first
-          for (uint32_t h = 0; h < running[r].n_holdings; ++h) {
-            const grove_holding_t& x = holdings[running[r].holding_off + h];
-            for (size_t j = 0; j < order.size(); ++j)
-              if (order[j] == x.node) { own[j].cpu += x.cpu_milli; own[j].mem += x.mem_mib; own[j].gpu += x.gpu; own[j].pods += x.pods; }
-          }
-        for (size_t j = 0; j < order.size(); ++j) {
-          const uint32_t n = order[j];
-          const Res need{std::max<int64_t>(use[j].cpu - own[j].cpu, 0), std::max<int64_t>(use[j].mem - own[j].mem, 0),
-                         std::max<int64_t>(use[j].gpu - own[j].gpu, 0), std::max<int64_t>(use[j].pods - own[j].pods, 0)};
-          Res& have = rows[slot[n]];
-          while (!(have.cpu >= need.cpu && have.mem >= need.mem && have.gpu >= need.gpu && have.pods >= need.pods)) {
-            uint32_t v = GROVE_NONE_U32;   // lowest priority first, then the highest running index
-            for (uint32_t a = at_off[n]; a < at_off[n + 1]; ++a) {
-              const uint32_t x = at_run[a];
-              if (gone[x] || prio[x] >= p) continue;
-              if (v == GROVE_NONE_U32 || prio[x] < prio[v] || (prio[x] == prio[v] && x > v)) v = x;
-            }
-            if (v == GROVE_NONE_U32) return fail(e, GROVE_ERR_STATE, "reclaim pass: a preemptor's node cannot be freed");
-            release(v);
-            victims.push_back(grove_victim_t{v, g});
-          }
-          have.cpu -= need.cpu; have.mem -= need.mem; have.gpu -= need.gpu; have.pods -= need.pods;
-        }
-        if (holds) gone[r] = 1;   // released; its leftover came back when the class cycle ended (k_hold_release)
-        grove_gang_status_t o = sp;
-        o.reserved0 = GROVE_STATUS_PREEMPTOR;
-        status[g] = o;   // placement_off is assigned when the outputs are merged
-        for (uint32_t si = 0; si < gangs[g].n_scopes; ++si) sstat[gangs[g].scope_off + si] = ssp[sg[k].scope_off + si];
-        st0.gangs_admitted += 1; st0.gangs_rejected -= 1;
-      }
-      for (uint32_t n : used) slot[n] = -1;
-      if (!skipped.empty()) {   // give back what the class cycle committed for them: +U, and -H for a member with a hold
-        std::vector<std::pair<uint32_t, std::array<int64_t, 4>>> d;   // (sorted node, change)
-        for (uint32_t k : skipped) {
-          const grove_gang_status_t& sp = e->h_status.p[k];
-          for (uint32_t i = 0; i < sp.n_pods; ++i) {
-            const grove_placement_t pl = e->h_out.p[sp.placement_off + i];
-            const grove_clique_t& q = sq[pl.clique];
-            d.push_back({e->inv[pl.node], {int64_t(q.req_cpu_milli), int64_t(q.req_mem_mib), int64_t(q.req_gpu), 1}});
-          }
-          if (sub_rep[k] != GROVE_NONE_U32)
-            for (uint32_t h = 0; h < running[sub_rep[k]].n_holdings; ++h) {
-              const grove_holding_t& x = holdings[running[sub_rep[k]].holding_off + h];
-              d.push_back({e->inv[x.node], {-int64_t(x.cpu_milli), -int64_t(x.mem_mib), -int64_t(x.gpu), -int64_t(x.pods)}});
-            }
-        }
-        rc = patch_nodes(e, d); if (rc) return rc;
-        st0.kernel_launches += 1;
-      }
-      // back to the free table: take off what the running gangs of E(p) that still stand hold
-      CU_TRY(e, cudaMemcpyAsync(e->d_rc_gone.p, gone.data(), gone.size(), cudaMemcpyHostToDevice, e->stream));
-      k_reclaim_view<<<nblk, 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_real.p, csr, N, p, 0u);
-      CU_TRY(e, cudaGetLastError());
-    }
-    // the handle goes back to the caller's submission; the device table is the free table
-    restore.armed = false;
-    rc = grove_submit_gangs(e, gangs.data(), G, cliques.data(), Q, scopes.data(), S); if (rc) return rc;
-  }
-  st0.kernel_launches += 1;   // k_reclaim_check
-  return publish_reclaim(e, status, place, extra, sstat, st0, std::move(victims), stats);
-}
-
-// ---------------------------------------------------------------------------------------------
-// Reclaim within queue limits (include/grove_place.h "reclaim within queue limits"; DESIGN.md section 1).  The ordinary pass is the
-// queue cycle.  Every priority class of the gangs it rejected is then ONE queue cycle over the class view of
-// grove_run_cycle_reuse_preempt (free + what the standing running gangs of E(p) hold, built by reclaim.cuh) with a queue set of
-// its own, whose `used` leave out what the gangs of E(p) hold: its loads are load'.  Queue loads are followed here, between
-// classes; victims are chosen here, node step then queue step, gang by gang in rank order.
-// ---------------------------------------------------------------------------------------------
-int32_t grove_run_cycle_preempt_queues(grove_engine_t* e, const grove_running_gang_t* running, uint32_t n_running,
-                                       const grove_holding_t* holdings, uint32_t n_holdings, const uint32_t* running_queue,
-                                       grove_cycle_stats_t* stats) {
-  static const char* kEntry = "grove_run_cycle_preempt_queues";
-  if (!e || (n_running && (!running || !running_queue)) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
-  if (e->sp_members) return refuse_spread(e, kEntry);
-  if (!e->fc_gangs.empty()) return refuse_fences(e, kEntry);
-  if (!e->qu_given) return fail(e, GROVE_ERR_STATE, "grove_run_cycle_preempt_queues: no queue set given for the current submission (grove_set_queues)");
-  NoDiagnosis no_diag{e};
-  if (e->wide) return refuse_wide(e, kEntry);
-  if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
-  for (uint32_t r = 0; r < n_running; ++r)
-    if (uint64_t(running[r].holding_off) + running[r].n_holdings > n_holdings) return fail(e, GROVE_ERR_INVALID_ARG, "running gang holdings out of range");
-  for (uint32_t h = 0; h < n_holdings; ++h)
-    if (holdings[h].node >= e->N) return fail(e, GROVE_ERR_INVALID_ARG, "holding on a node out of range");
-  // the set of the current submission (the class cycles re-use the handle) and what each running gang holds
-  const std::vector<grove_queue_t> queues = e->qu_queues;
-  const std::vector<uint32_t> gang_queue = e->qu_gang_queue;
-  const uint32_t NQ = uint32_t(queues.size());
-  std::vector<std::array<int64_t, 3>> usage(n_running, {0, 0, 0});
-  std::vector<std::array<int64_t, 3>> own(NQ, {0, 0, 0});   // own used, then followed through the cycle
-  for (uint32_t q = 0; q < NQ; ++q) for (int k = 0; k < 3; ++k) own[q][k] = int64_t(std::min<uint64_t>(queues[q].used[k], uint64_t(1) << 62));
-  {
-    std::vector<std::array<int64_t, 3>> run_use(NQ, {0, 0, 0});
-    for (uint32_t r = 0; r < n_running; ++r) {
-      for (uint32_t h = 0; h < running[r].n_holdings; ++h) {
-        const grove_holding_t& x = holdings[running[r].holding_off + h];
-        usage[r][0] += x.cpu_milli; usage[r][1] += x.mem_mib; usage[r][2] += x.gpu;
-      }
-      const uint32_t q = running_queue[r];
-      if (q == GROVE_NONE_U32) continue;
-      if (q >= NQ) return fail(e, GROVE_ERR_INVALID_ARG, "grove_run_cycle_preempt_queues: running_queue names a queue out of range");
-      for (int k = 0; k < 3; ++k) run_use[q][k] += usage[r][k];
-    }
-    for (uint32_t q = 0; q < NQ; ++q)
-      for (int k = 0; k < 3; ++k)
-        if (uint64_t(run_use[q][k]) > queues[q].used[k])
-          return fail(e, GROVE_ERR_INVALID_ARG, "grove_run_cycle_preempt_queues: the running gangs of a queue hold more than its used");
-  }
-  CU_TRY(e, cudaSetDevice(e->cfg.device));
-  const uint32_t N = e->N, nblk = (N + 255) / 256;
+  const uint32_t G = e->G, N = e->N, nblk = (N + 255) / 256;
   ReclaimCsr csr{};
   int32_t rc = upload_running(e, running, n_running, holdings, &csr);
   if (rc) return rc;
-  std::vector<int32_t> prio(std::max<uint32_t>(n_running, 1), 0);
-  for (uint32_t r = 0; r < n_running; ++r) prio[r] = running[r].priority;
-  std::vector<uint8_t> gone(std::max<uint32_t>(n_running, 1), 0);   // evicted
+  // without replacements nothing holds; without a queue set no gang and no running gang is in a queue, and the queue step never runs
+  std::vector<uint32_t> rep(G, GROVE_NONE_U32), run_queue(n_running, GROVE_NONE_U32);
+  if (replaces) std::copy(replaces, replaces + G, rep.begin());
+  if (running_queue) std::copy(running_queue, running_queue + n_running, run_queue.begin());
+  // the queue set of the current submission (the class cycles re-use the handle) and what each running gang holds
+  const std::vector<grove_queue_t> queues = running_queue ? e->qu_queues : std::vector<grove_queue_t>{};
+  const std::vector<uint32_t> gang_queue = running_queue ? e->qu_gang_queue : std::vector<uint32_t>(G, GROVE_NONE_U32);
+  const uint32_t NQ = uint32_t(queues.size());
+  std::vector<std::array<int64_t, 3>> usage(n_running);
+  for (uint32_t r = 0; r < n_running; ++r) usage[r] = usage_of(running[r], holdings);
+  std::vector<std::array<int64_t, 3>> own(NQ, {0, 0, 0});   // own used, then followed through the cycle
+  for (uint32_t q = 0; q < NQ; ++q) for (int k = 0; k < 3; ++k) own[q][k] = int64_t(std::min<uint64_t>(queues[q].used[k], uint64_t(1) << 62));
+  std::vector<uint8_t> gone(std::max<uint32_t>(n_running, 1), 0);   // released or evicted
 
-  // 1. the ordinary pass: the queue cycle
+  // 1. the ordinary pass: the cycle with holds (the reuse cycle; without replacements the ordinary cycle, under a queue set the
+  // queue cycle).  An admitted new version's predecessor is released.
   grove_cycle_stats_t st0{};
-  rc = run_cycle(e, &st0);
+  rc = run_cycle_holds(e, rep.data(), running, holdings, false, &st0);
   if (rc) return rc;
-  const uint32_t G = e->G, Q = e->Q, S = e->S;
-  std::vector<grove_gang_t> gangs(e->gangs.data(), e->gangs.data() + G);
-  std::vector<grove_clique_t> cliques(e->cliques.data(), e->cliques.data() + Q);
-  std::vector<grove_scope_t> scopes(e->scopes.data(), e->scopes.data() + S);
-  std::vector<grove_gang_status_t> status(e->h_status.p, e->h_status.p + G);
-  std::vector<grove_placement_t> place(e->h_out.p, e->h_out.p + e->n_out);
-  std::vector<grove_scope_status_t> sstat(std::max<uint32_t>(S, 1));
-  if (S) { rc = grove_get_scope_domains(e, sstat.data(), S); if (rc) return rc; }
+  Snapshot snap;
+  rc = snapshot(e, &snap);
+  if (rc) return rc;
+  for (uint32_t g = 0; g < G; ++g)
+    if (snap.status[g].state == GROVE_GANG_ADMITTED && rep[g] != GROVE_NONE_U32) gone[rep[g]] = 1;
   // the loads: own used + the admitted members' usage, then every queue's own plus its descendants'
   for (uint32_t g = 0; g < G; ++g) {
-    if (status[g].state != GROVE_GANG_ADMITTED || gang_queue[g] == GROVE_NONE_U32) continue;
-    int64_t u[3] = {0, 0, 0};
-    for (uint32_t i = 0; i < status[g].n_pods; ++i) {
-      const grove_clique_t& q = cliques[place[status[g].placement_off + i].clique];
-      u[0] += q.req_cpu_milli; u[1] += q.req_mem_mib; u[2] += q.req_gpu;
+    if (snap.status[g].state != GROVE_GANG_ADMITTED || gang_queue[g] == GROVE_NONE_U32) continue;
+    for (uint32_t i = 0; i < snap.status[g].n_pods; ++i) {
+      const grove_clique_t& q = snap.cliques[snap.place[snap.status[g].placement_off + i].clique];
+      own[gang_queue[g]][0] += q.req_cpu_milli; own[gang_queue[g]][1] += q.req_mem_mib; own[gang_queue[g]][2] += q.req_gpu;
     }
-    for (int k = 0; k < 3; ++k) own[gang_queue[g]][k] += u[k];
   }
   std::vector<std::array<int64_t, 3>> load(own);
   for (uint32_t q = NQ; q-- > 0;)
@@ -2455,167 +2248,135 @@ int32_t grove_run_cycle_preempt_queues(grove_engine_t* e, const grove_running_ga
     for (; q != GROVE_NONE_U32; q = queues[q].parent) if (q == Qx) return true;
     return false;
   };
-  std::vector<int32_t> classes;
-  for (uint32_t g = 0; g < G; ++g) if (status[g].state == GROVE_GANG_REJECTED) classes.push_back(gangs[g].priority);
+  std::vector<int32_t> classes;   // the rejected priority classes, descending
+  for (uint32_t g = 0; g < G; ++g) if (snap.status[g].state == GROVE_GANG_REJECTED) classes.push_back(snap.gangs[g].priority);
   std::sort(classes.begin(), classes.end(), std::greater<int32_t>());
   classes.erase(std::unique(classes.begin(), classes.end()), classes.end());
   auto below = [&](int32_t p) {   // is E(p) -- the standing running gangs of a priority below p -- non-empty?
-    for (uint32_t r = 0; r < n_running; ++r) if (!gone[r] && prio[r] < p) return true;
+    for (uint32_t r = 0; r < n_running; ++r) if (!gone[r] && running[r].priority < p) return true;
     return false;
   };
   std::vector<grove_victim_t> victims;
   std::vector<std::vector<grove_placement_t>> extra(G);   // placements of the preemptors, by gang
   if (!classes.empty() && below(classes.front())) {
-    // whatever goes wrong from here on, the handle goes back to the caller's submission and queue set on the free table the
-    // ordinary pass left
     CU_TRY(e, cudaMemcpyAsync(e->d_rc_base.p, e->d_nres.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToDevice, e->stream));
-    struct Restore {
-      grove_engine* e; const std::vector<grove_gang_t>* g; const std::vector<grove_clique_t>* c; const std::vector<grove_scope_t>* s;
-      const std::vector<grove_queue_t>* q; const std::vector<uint32_t>* gq; bool armed = true;
-      ~Restore() {
-        if (!armed) return;
-        const std::string keep = e->err;
-        cudaMemcpyAsync(e->d_nres.p, e->d_rc_base.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToDevice, e->stream);
-        cudaStreamSynchronize(e->stream);
-        if (grove_submit_gangs(e, g->data(), uint32_t(g->size()), c->data(), uint32_t(c->size()), s->data(), uint32_t(s->size())) == GROVE_OK &&
-            install_queues(e, q->data(), uint32_t(q->size()), gq->data()) == GROVE_OK) {
-          e->qu_queues = *q; e->qu_gang_queue = *gq; e->qu_given = true;
-        }
-        e->err = keep;
-      }
-    };
-    Restore restore{e, &gangs, &cliques, &scopes, &queues, &gang_queue};
-    // running gangs by node (caller order), for the victim choice
-    size_t n_held = 0;   // (ranges of running gangs may overlap: size by what the fill below writes)
-    for (uint32_t r = 0; r < n_running; ++r) n_held += running[r].n_holdings;
-    std::vector<uint32_t> at_off(size_t(N) + 1, 0), at_run(n_held);
-    for (uint32_t r = 0; r < n_running; ++r) for (uint32_t h = 0; h < running[r].n_holdings; ++h) ++at_off[holdings[running[r].holding_off + h].node + 1];
-    for (uint32_t n = 0; n < N; ++n) at_off[n + 1] += at_off[n];
-    { std::vector<uint32_t> cur(at_off.begin(), at_off.end() - 1);
-      for (uint32_t r = 0; r < n_running; ++r) for (uint32_t h = 0; h < running[r].n_holdings; ++h) at_run[cur[holdings[running[r].holding_off + h].node]++] = r; }
+    Restore restore{e, &snap, running_queue ? &queues : nullptr, &gang_queue};
+    const RunningByNode at = running_by_node(N, running, n_running, holdings);
     std::vector<int32_t> slot(N, -1);   // node (caller order) -> its row in `rows` while a class chooses its victims
     for (int32_t p : classes) {
       if (!below(p)) break;   // E(p) only shrinks from one class to the next
-      // 2. the class's rejected gangs as a submission of their own: anchors pinned to what the ordinary pass used, no gating
-      std::vector<uint32_t> ids, sub_queue;
-      std::vector<grove_gang_t> sg; std::vector<grove_clique_t> sq; std::vector<grove_scope_t> ss;
+      // 2. the class's rejected gangs as a submission of their own.  A member holds its predecessor's holdings when that one still
+      // stands at or above p; below p it is evictable instead.
+      Sub sub;
+      std::vector<uint32_t> sub_rep, sub_queue;
       for (uint32_t g = 0; g < G; ++g) {
-        if (status[g].state != GROVE_GANG_REJECTED || gangs[g].priority != p) continue;
-        grove_gang_t x = gangs[g];
-        if (x.anchor_node == GROVE_NONE_U32) x.anchor_node = e->perm[fmix32(g) % N];
-        x.base_gang = GROVE_NONE_U32;
-        x.clique_off = uint32_t(sq.size()); x.scope_off = uint32_t(ss.size());
-        sq.insert(sq.end(), cliques.begin() + gangs[g].clique_off, cliques.begin() + gangs[g].clique_off + gangs[g].n_cliques);
-        ss.insert(ss.end(), scopes.begin() + gangs[g].scope_off, scopes.begin() + gangs[g].scope_off + gangs[g].n_scopes);
-        ids.push_back(g); sg.push_back(x); sub_queue.push_back(gang_queue[g]);
+        if (snap.status[g].state != GROVE_GANG_REJECTED || snap.gangs[g].priority != p) continue;
+        add_gang(e, snap, g, sub);
+        const uint32_t r = rep[g];
+        sub_rep.push_back(r != GROVE_NONE_U32 && !gone[r] && running[r].priority >= p ? r : GROVE_NONE_U32);
+        sub_queue.push_back(gang_queue[g]);
       }
       // the class view, on the device: free + the standing holdings of E(p); the free table itself is kept for the victim choice
       CU_TRY(e, cudaMemcpyAsync(e->d_rc_gone.p, gone.data(), gone.size(), cudaMemcpyHostToDevice, e->stream));
       k_reclaim_view<<<nblk, 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_real.p, csr, N, p, 1u);
       CU_TRY(e, cudaGetLastError());
-      rc = grove_submit_gangs(e, sg.data(), uint32_t(sg.size()), sq.data(), uint32_t(sq.size()), ss.data(), uint32_t(ss.size())); if (rc) return rc;
-      // the class's queue set: own used without what the gangs of E(p) hold, so that its loads are load'
-      std::vector<grove_queue_t> cq(queues);
-      {
+      rc = submit_sub(e, sub); if (rc) return rc;
+      if (running_queue) {   // the class's queue set: own used without what the gangs of E(p) hold, so that its loads are load'
+        std::vector<grove_queue_t> cq(queues);
         std::vector<std::array<int64_t, 3>> o(own);
         for (uint32_t r = 0; r < n_running; ++r)
-          if (!gone[r] && prio[r] < p && running_queue[r] != GROVE_NONE_U32) for (int k = 0; k < 3; ++k) o[running_queue[r]][k] -= usage[r][k];
+          if (!gone[r] && running[r].priority < p && run_queue[r] != GROVE_NONE_U32) for (int k = 0; k < 3; ++k) o[run_queue[r]][k] -= usage[r][k];
         for (uint32_t q = 0; q < NQ; ++q) for (int k = 0; k < 3; ++k) cq[q].used[k] = uint64_t(o[q][k]);
+        rc = install_queues(e, cq.data(), NQ, sub_queue.data()); if (rc) return rc;
       }
-      rc = install_queues(e, cq.data(), NQ, sub_queue.data()); if (rc) return rc;
       grove_cycle_stats_t stp{};
-      rc = run_cycle(e, &stp); if (rc) return rc;
-      st0.rounds += stp.rounds; st0.evaluations += stp.evaluations; st0.kernel_launches += stp.kernel_launches + 2;   // (+ the two k_reclaim_view)
-      st0.ms_fit += stp.ms_fit; st0.ms_admit += stp.ms_admit; st0.ms_commit += stp.ms_commit; st0.ms_total += stp.ms_total;
-      std::vector<grove_scope_status_t> ssp(std::max<size_t>(ss.size(), 1));
-      if (!ss.empty()) { rc = grove_get_scope_domains(e, ssp.data(), uint32_t(ss.size())); if (rc) return rc; }
+      rc = run_cycle_holds(e, sub_rep.data(), running, holdings, false, &stp); if (rc) return rc;
+      accumulate(st0, stp); st0.kernel_launches += 2;   // (+ the two k_reclaim_view)
+      std::vector<grove_scope_status_t> ssp;
+      rc = sub_scope_domains(e, sub, ssp); if (rc) return rc;
       // the free-table rows of the nodes the class's preemptors use
       std::vector<uint32_t> used;
-      for (uint32_t k = 0; k < ids.size(); ++k) {
+      for (uint32_t k = 0; k < sub.ids.size(); ++k) {
         const grove_gang_status_t& sp = e->h_status.p[k];
         if (sp.state != GROVE_GANG_ADMITTED) continue;
         for (uint32_t i = 0; i < sp.n_pods; ++i) used.push_back(e->h_out.p[sp.placement_off + i].node);
       }
       std::sort(used.begin(), used.end());
       used.erase(std::unique(used.begin(), used.end()), used.end());
-      std::vector<Res> rows(used.size());
-      if (!used.empty()) {
-        std::vector<uint32_t> idx(used.size());
-        for (size_t i = 0; i < used.size(); ++i) { idx[i] = e->inv[used[i]]; slot[used[i]] = int32_t(i); }
-        std::vector<uint4> got(used.size());
-        CU_TRY(e, e->d_rc_idx.ensure(idx.size())); CU_TRY(e, e->d_rc_rows.ensure(idx.size()));
-        CU_TRY(e, cudaMemcpyAsync(e->d_rc_idx.p, idx.data(), sizeof(uint32_t) * idx.size(), cudaMemcpyHostToDevice, e->stream));
-        k_reclaim_rows<<<uint32_t((idx.size() + 255) / 256), 256, 0, e->stream>>>(e->d_rc_real.p, e->d_rc_idx.p, e->d_rc_rows.p, uint32_t(idx.size()));
-        CU_TRY(e, cudaGetLastError());
-        CU_TRY(e, cudaMemcpyAsync(got.data(), e->d_rc_rows.p, sizeof(uint4) * got.size(), cudaMemcpyDeviceToHost, e->stream));
-        CU_TRY(e, cudaStreamSynchronize(e->stream));
-        for (size_t i = 0; i < got.size(); ++i) rows[i] = Res{got[i].x, got[i].y, got[i].z & 0xFFFFu, got[i].z >> 16};
-        st0.kernel_launches += 1;
-      }
-      auto evict = [&](uint32_t v, uint32_t g) {   // everything v held returns to the free table, its usage leaves its queues
+      std::vector<Res> rows;
+      rc = read_rows(e, used, rows, st0); if (rc) return rc;
+      for (size_t i = 0; i < used.size(); ++i) slot[used[i]] = int32_t(i);
+      auto release = [&](uint32_t v) {   // everything v held returns to the free table (only the tracked rows matter here)
         gone[v] = 1;
         for (uint32_t h = 0; h < running[v].n_holdings; ++h) {
           const grove_holding_t& x = holdings[running[v].holding_off + h];
-          if (slot[x.node] < 0) continue;
-          Res& q = rows[slot[x.node]];
-          q.cpu += x.cpu_milli; q.mem += x.mem_mib; q.gpu += x.gpu; q.pods += x.pods;
+          if (slot[x.node] >= 0) rows[slot[x.node]].add(held(x));
         }
-        if (running_queue[v] != GROVE_NONE_U32) account(running_queue[v], usage[v].data(), -1);
+      };
+      auto evict = [&](uint32_t v, uint32_t g) {   // released, and its usage leaves its queues
+        release(v);
+        if (run_queue[v] != GROVE_NONE_U32) account(run_queue[v], usage[v].data(), -1);
         victims.push_back(grove_victim_t{v, g});
       };
       // 3. victims, gang by gang in rank order (sub-submission order == order rank: one priority)
-      std::vector<uint32_t> skipped;   // admitted by the class cycle after E(p) ran out: they stay as the ordinary pass left them
-      for (uint32_t k = 0; k < ids.size(); ++k) {
+      std::vector<std::pair<uint32_t, Res>> back;   // (sorted node, change)
+      for (uint32_t k = 0; k < sub.ids.size(); ++k) {
         const grove_gang_status_t& sp = e->h_status.p[k];
         if (sp.state != GROVE_GANG_ADMITTED) continue;
-        if (!below(p)) { skipped.push_back(k); continue; }
-        const uint32_t g = ids[k];
-        std::vector<uint32_t> order; std::vector<Res> use;
-        int64_t U[3] = {0, 0, 0};
-        for (uint32_t i = 0; i < sp.n_pods; ++i) {
-          const grove_placement_t pl = e->h_out.p[sp.placement_off + i];
-          const grove_clique_t& q = sq[pl.clique];
-          size_t j = 0;
-          for (; j < order.size(); ++j) if (order[j] == pl.node) break;
-          if (j == order.size()) { order.push_back(pl.node); use.emplace_back(); }
-          use[j].cpu += q.req_cpu_milli; use[j].mem += q.req_mem_mib; use[j].gpu += q.req_gpu; use[j].pods += 1;
-          U[0] += q.req_cpu_milli; U[1] += q.req_mem_mib; U[2] += q.req_gpu;
-          extra[g].push_back(grove_placement_t{gangs[g].clique_off + (pl.clique - sg[k].clique_off), pl.node});
-        }
-        // (a) the node step: the reclaim pass's rule
-        for (size_t j = 0; j < order.size(); ++j) {
-          const uint32_t n = order[j];
-          Res& have = rows[slot[n]];
-          const Res& need = use[j];
-          while (!(have.cpu >= need.cpu && have.mem >= need.mem && have.gpu >= need.gpu && have.pods >= need.pods)) {
-            uint32_t v = GROVE_NONE_U32;   // lowest priority first, then the highest running index
-            for (uint32_t a = at_off[n]; a < at_off[n + 1]; ++a) {
-              const uint32_t x = at_run[a];
-              if (gone[x] || prio[x] >= p) continue;
-              if (v == GROVE_NONE_U32 || prio[x] < prio[v] || (prio[x] == prio[v] && x > v)) v = x;
+        std::vector<uint32_t> nodes; std::vector<Res> use; std::vector<grove_placement_t> pl;
+        placed(e, snap, sub, k, nodes, use, pl);
+        if (!below(p)) {   // admitted by the class cycle after E(p) ran out: it stays as the ordinary pass left it.  What the class
+                           // cycle committed for it goes back: +U, and -H for a member with a hold (a queue charge was never taken here)
+          for (size_t j = 0; j < nodes.size(); ++j) back.push_back({e->inv[nodes[j]], use[j]});
+          if (sub_rep[k] != GROVE_NONE_U32)
+            for (uint32_t h = 0; h < running[sub_rep[k]].n_holdings; ++h) {
+              const grove_holding_t& x = holdings[running[sub_rep[k]].holding_off + h];
+              Res c; c.add(held(x), -1);
+              back.push_back({e->inv[x.node], c});
             }
+          continue;
+        }
+        const uint32_t g = sub.ids[k], r = rep[g];
+        const bool holds = sub_rep[k] != GROVE_NONE_U32;
+        if (r != GROVE_NONE_U32 && !holds && !gone[r]) release(r);   // its predecessor is in E(p): released first, not a victim
+        std::vector<Res> mine(nodes.size());
+        if (holds)   // what its predecessor holds on each of those nodes: used first
+          for (uint32_t h = 0; h < running[r].n_holdings; ++h) {
+            const grove_holding_t& x = holdings[running[r].holding_off + h];
+            for (size_t j = 0; j < nodes.size(); ++j) if (nodes[j] == x.node) mine[j].add(held(x));
+          }
+        // (a) the node step: the reclaim pass's rule
+        for (size_t j = 0; j < nodes.size(); ++j) {
+          const uint32_t n = nodes[j];
+          const Res need{std::max<int64_t>(use[j].cpu - mine[j].cpu, 0), std::max<int64_t>(use[j].mem - mine[j].mem, 0),
+                         std::max<int64_t>(use[j].gpu - mine[j].gpu, 0), std::max<int64_t>(use[j].pods - mine[j].pods, 0)};
+          Res& have = rows[slot[n]];
+          while (!have.covers(need)) {
+            const uint32_t v = choose_victim(at, n, running, [&](uint32_t x) { return !gone[x] && running[x].priority < p; });
             if (v == GROVE_NONE_U32) return fail(e, GROVE_ERR_STATE, "reclaim pass: a preemptor's node cannot be freed");
             evict(v, g);
           }
-          have.cpu -= need.cpu; have.mem -= need.mem; have.gpu -= need.gpu; have.pods -= need.pods;
+          have.add(need, -1);
         }
+        if (holds) gone[r] = 1;   // released; its leftover came back when the class cycle ended (k_hold_release)
         // (b) the queue step: g's chain, leaf first, back within its limits on the resources g uses
         const uint32_t gq = gang_queue[g];
         if (gq != GROVE_NONE_U32) {
+          int64_t U[3] = {0, 0, 0};
+          for (const Res& u : use) { U[0] += u.cpu; U[1] += u.mem; U[2] += u.gpu; }
           account(gq, U, 1);
           for (uint32_t Qx = gq; Qx != GROVE_NONE_U32; Qx = queues[Qx].parent) {
             for (;;) {
               uint32_t over = 0;   // the resources g uses on which Qx is over its finite limit
-              for (int r = 0; r < 3; ++r)
-                if (U[r] > 0 && queues[Qx].limit[r] != GROVE_QUEUE_UNLIMITED && load[Qx][r] > 0 && uint64_t(load[Qx][r]) > queues[Qx].limit[r]) over |= 1u << r;
+              for (int t = 0; t < 3; ++t)
+                if (U[t] > 0 && queues[Qx].limit[t] != GROVE_QUEUE_UNLIMITED && load[Qx][t] > 0 && uint64_t(load[Qx][t]) > queues[Qx].limit[t]) over |= 1u << t;
               if (!over) break;
-              uint32_t v = GROVE_NONE_U32;   // a gang of E(p) in Qx's subtree holding some of it: lowest priority, then highest index
+              uint32_t v = GROVE_NONE_U32;   // by the victim rule, among the gangs of E(p) in Qx's subtree that hold some of it
               for (uint32_t x = 0; x < n_running; ++x) {
-                if (gone[x] || prio[x] >= p || running_queue[x] == GROVE_NONE_U32 || !in_subtree(running_queue[x], Qx)) continue;
-                bool holds = false;
-                for (int r = 0; r < 3; ++r) holds |= ((over >> r) & 1u) && usage[x][r] > 0;
-                if (!holds) continue;
-                if (v == GROVE_NONE_U32 || prio[x] < prio[v] || (prio[x] == prio[v] && x > v)) v = x;
+                if (gone[x] || running[x].priority >= p || run_queue[x] == GROVE_NONE_U32 || !in_subtree(run_queue[x], Qx)) continue;
+                bool holds_some = false;
+                for (int t = 0; t < 3; ++t) holds_some |= ((over >> t) & 1u) && usage[x][t] > 0;
+                if (holds_some && evicted_before(running, x, v)) v = x;
               }
               if (v == GROVE_NONE_U32) return fail(e, GROVE_ERR_STATE, "reclaim pass: a preemptor's queue cannot be brought within its limit");
               evict(v, g);
@@ -2624,37 +2385,82 @@ int32_t grove_run_cycle_preempt_queues(grove_engine_t* e, const grove_running_ga
         }
         grove_gang_status_t o = sp;
         o.reserved0 = uint16_t(GROVE_STATUS_PREEMPTOR | (sp.reserved0 & GROVE_STATUS_SURPLUS_CAPPED));
-        status[g] = o;   // placement_off is assigned when the outputs are merged
-        for (uint32_t si = 0; si < gangs[g].n_scopes; ++si) sstat[gangs[g].scope_off + si] = ssp[sg[k].scope_off + si];
+        merge_gang(snap, sub, k, o, ssp);
+        extra[g] = std::move(pl);
         st0.gangs_admitted += 1; st0.gangs_rejected -= 1;
       }
       for (uint32_t n : used) slot[n] = -1;
-      if (!skipped.empty()) {   // give back what the class cycle committed for them (their queue charge was never taken here)
-        std::vector<std::pair<uint32_t, std::array<int64_t, 4>>> d;   // (sorted node, change)
-        for (uint32_t k : skipped) {
-          const grove_gang_status_t& sp = e->h_status.p[k];
-          for (uint32_t i = 0; i < sp.n_pods; ++i) {
-            const grove_placement_t pl = e->h_out.p[sp.placement_off + i];
-            const grove_clique_t& q = sq[pl.clique];
-            d.push_back({e->inv[pl.node], {int64_t(q.req_cpu_milli), int64_t(q.req_mem_mib), int64_t(q.req_gpu), 1}});
-          }
-        }
-        rc = patch_nodes(e, d); if (rc) return rc;
-        st0.kernel_launches += 1;
-      }
+      rc = patch_nodes(e, back, st0); if (rc) return rc;
       // back to the free table: take off what the running gangs of E(p) that still stand hold
       CU_TRY(e, cudaMemcpyAsync(e->d_rc_gone.p, gone.data(), gone.size(), cudaMemcpyHostToDevice, e->stream));
       k_reclaim_view<<<nblk, 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_real.p, csr, N, p, 0u);
       CU_TRY(e, cudaGetLastError());
     }
-    // the handle goes back to the caller's submission and queue set; the device table is the free table
+    // the handle goes back to the caller's submission (and queue set); the device table is the free table
     restore.armed = false;
-    rc = grove_submit_gangs(e, gangs.data(), G, cliques.data(), Q, scopes.data(), S); if (rc) return rc;
-    rc = install_queues(e, queues.data(), NQ, gang_queue.data()); if (rc) return rc;
-    e->qu_queues = queues; e->qu_gang_queue = gang_queue; e->qu_given = true;
+    rc = restore.put_back(); if (rc) return rc;
   }
   st0.kernel_launches += 1;   // k_reclaim_check
-  return publish_reclaim(e, status, place, extra, sstat, st0, std::move(victims), stats);
+  return publish_reclaim(e, snap.status, snap.place, extra, snap.sstat, st0, std::move(victims), stats);
+}
+
+int32_t grove_run_cycle_preempt(grove_engine_t* e, const grove_running_gang_t* running, uint32_t n_running,
+                                const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
+  if (!e || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
+  if (e->sp_members) return refuse_spread(e, "grove_run_cycle_preempt");
+  if (e->qu_members) return refuse_queues(e, "grove_run_cycle_preempt");
+  if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_preempt");
+  NoDiagnosis no_diag{e};
+  if (e->wide) return refuse_wide(e, "grove_run_cycle_preempt");
+  int32_t rc = check_ready(e);
+  if (rc) return rc;
+  rc = check_running(e, running, n_running, holdings, n_holdings);
+  if (rc) return rc;
+  return reclaim_cycle(e, nullptr, running, n_running, holdings, nullptr, stats);
+}
+
+int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs, const grove_running_gang_t* running,
+                                      uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
+  if (!e || (n_gangs && !replaces) || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
+  if (e->sp_members) return refuse_spread(e, "grove_run_cycle_reuse_preempt");
+  if (e->qu_members) return refuse_queues(e, "grove_run_cycle_reuse_preempt");
+  if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_reuse_preempt");
+  NoDiagnosis no_diag{e};
+  if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse_preempt");
+  const int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);
+  if (rc) return rc;
+  return reclaim_cycle(e, replaces, running, n_running, holdings, nullptr, stats);
+}
+
+int32_t grove_run_cycle_preempt_queues(grove_engine_t* e, const grove_running_gang_t* running, uint32_t n_running,
+                                       const grove_holding_t* holdings, uint32_t n_holdings, const uint32_t* running_queue,
+                                       grove_cycle_stats_t* stats) {
+  static const char* kEntry = "grove_run_cycle_preempt_queues";
+  if (!e || (n_running && (!running || !running_queue)) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
+  if (e->sp_members) return refuse_spread(e, kEntry);
+  if (!e->fc_gangs.empty()) return refuse_fences(e, kEntry);
+  if (!e->qu_given) return fail(e, GROVE_ERR_STATE, "grove_run_cycle_preempt_queues: no queue set given for the current submission (grove_set_queues)");
+  NoDiagnosis no_diag{e};
+  if (e->wide) return refuse_wide(e, kEntry);
+  if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
+  const int32_t rc = check_running(e, running, n_running, holdings, n_holdings);
+  if (rc) return rc;
+  // what the running gangs of each queue hold: within its used
+  const std::vector<grove_queue_t>& queues = e->qu_queues;
+  const uint32_t NQ = uint32_t(queues.size());
+  std::vector<std::array<int64_t, 3>> run_use(NQ, {0, 0, 0});
+  for (uint32_t r = 0; r < n_running; ++r) {
+    const uint32_t q = running_queue[r];
+    if (q == GROVE_NONE_U32) continue;
+    if (q >= NQ) return fail(e, GROVE_ERR_INVALID_ARG, "grove_run_cycle_preempt_queues: running_queue names a queue out of range");
+    const std::array<int64_t, 3> u = usage_of(running[r], holdings);
+    for (int k = 0; k < 3; ++k) run_use[q][k] += u[k];
+  }
+  for (uint32_t q = 0; q < NQ; ++q)
+    for (int k = 0; k < 3; ++k)
+      if (uint64_t(run_use[q][k]) > queues[q].used[k])
+        return fail(e, GROVE_ERR_INVALID_ARG, "grove_run_cycle_preempt_queues: the running gangs of a queue hold more than its used");
+  return reclaim_cycle(e, nullptr, running, n_running, holdings, running_queue, stats);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -2674,10 +2480,9 @@ int32_t grove_run_cycle_consolidate(grove_engine_t* e, const uint32_t* targets, 
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_consolidate");
   if (n_targets > GROVE_MAX_CONSOLIDATE_TARGETS) return fail(e, GROVE_ERR_LIMIT, "grove_run_cycle_consolidate: more than GROVE_MAX_CONSOLIDATE_TARGETS targets");
-  if (!e->nodes_loaded) return fail(e, GROVE_ERR_STATE, "no node snapshot loaded");
-  if (!e->gangs_loaded) return fail(e, GROVE_ERR_STATE, "no gangs submitted");
-  if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
-  const uint32_t G = e->G, Q = e->Q, S = e->S, N = e->N, nblk = (N + 255) / 256;
+  int32_t rc = check_ready(e);
+  if (rc) return rc;
+  const uint32_t G = e->G, N = e->N, nblk = (N + 255) / 256;
   std::vector<uint8_t> role(G, 0);   // 1: a target, 2: a spec row
   for (uint32_t k = 0; k < n_targets; ++k) {
     if (targets[k] >= G) return fail(e, GROVE_ERR_INVALID_ARG, "grove_run_cycle_consolidate: target out of range");
@@ -2693,26 +2498,21 @@ int32_t grove_run_cycle_consolidate(grove_engine_t* e, const uint32_t* targets, 
     if (!(e->gangs[s].flags & GROVE_GANG_GATED)) return fail(e, GROVE_ERR_INVALID_ARG, "grove_run_cycle_consolidate: a spec row must carry GROVE_GANG_GATED");
     role[s] = 2;
   }
-  for (uint32_t r = 0; r < n_running; ++r)
-    if (uint64_t(running[r].holding_off) + running[r].n_holdings > n_holdings) return fail(e, GROVE_ERR_INVALID_ARG, "running gang holdings out of range");
-  for (uint32_t h = 0; h < n_holdings; ++h)
-    if (holdings[h].node >= N) return fail(e, GROVE_ERR_INVALID_ARG, "holding on a node out of range");
+  rc = check_running(e, running, n_running, holdings, n_holdings);
+  if (rc) return rc;
   CU_TRY(e, cudaSetDevice(e->cfg.device));
   ReclaimCsr csr{};
-  int32_t rc = upload_running(e, running, n_running, holdings, &csr);
+  rc = upload_running(e, running, n_running, holdings, &csr);
   if (rc) return rc;
 
   // 1. the ordinary pass
   grove_cycle_stats_t st0{};
   rc = grove_run_cycle(e, &st0);
   if (rc) return rc;
-  std::vector<grove_gang_t> gangs(e->gangs.data(), e->gangs.data() + G);
-  std::vector<grove_clique_t> cliques(e->cliques.data(), e->cliques.data() + Q);
-  std::vector<grove_scope_t> scopes(e->scopes.data(), e->scopes.data() + S);
-  std::vector<grove_gang_status_t> status(e->h_status.p, e->h_status.p + G);
-  std::vector<grove_placement_t> place(e->h_out.p, e->h_out.p + e->n_out);
-  std::vector<grove_scope_status_t> sstat(std::max<uint32_t>(S, 1));
-  if (S) { rc = grove_get_scope_domains(e, sstat.data(), S); if (rc) return rc; }
+  Snapshot snap;
+  rc = snapshot(e, &snap);
+  if (rc) return rc;
+  const std::vector<grove_gang_t>& gangs = snap.gangs;
   std::vector<uint32_t> order(targets, targets + n_targets);
   std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) {   // rank order: priority desc, index asc
     return gangs[a].priority != gangs[b].priority ? gangs[a].priority > gangs[b].priority : a < b;
@@ -2726,48 +2526,22 @@ int32_t grove_run_cycle_consolidate(grove_engine_t* e, const uint32_t* targets, 
   std::vector<grove_move_t> moves;
   std::vector<std::vector<grove_placement_t>> extra(G);   // placements of the consolidated targets and the moved spec rows
   bool any = false;
-  for (uint32_t b : order) any |= status[b].state == GROVE_GANG_REJECTED && movable(gangs[b].priority);
+  for (uint32_t b : order) any |= snap.status[b].state == GROVE_GANG_REJECTED && movable(gangs[b].priority);
   if (any) {
-    // whatever goes wrong from here on, the handle goes back to the caller's submission on the free table the ordinary pass left
     CU_TRY(e, cudaMemcpyAsync(e->d_rc_base.p, e->d_nres.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToDevice, e->stream));
-    struct Restore {
-      grove_engine* e; const std::vector<grove_gang_t>* g; const std::vector<grove_clique_t>* c; const std::vector<grove_scope_t>* s; bool armed = true;
-      ~Restore() {
-        if (!armed) return;
-        const std::string keep = e->err;
-        cudaMemcpyAsync(e->d_nres.p, e->d_rc_base.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToDevice, e->stream);
-        cudaStreamSynchronize(e->stream);
-        grove_submit_gangs(e, g->data(), uint32_t(g->size()), c->data(), uint32_t(c->size()), s->data(), uint32_t(s->size()));
-        e->err = keep;
-      }
-    };
-    Restore restore{e, &gangs, &cliques, &scopes};
+    Restore restore{e, &snap, nullptr, nullptr};
     CU_TRY(e, e->d_cs_view.ensure(e->Npad)); CU_TRY(e, e->d_cs_rank.ensure(1 + 2 * kConsolTries)); CU_TRY(e, e->d_cs_zero.ensure(1));
     CU_TRY(e, cudaMemsetAsync(e->d_cs_zero.p, 0, sizeof(uint32_t), e->stream));   // k_fence_have's gang index and offset: 0
     // running gangs by node (caller order), for the choice of the displaced set
-    size_t n_held = 0;   // (ranges of running gangs may overlap: size by what the fill below writes)
-    for (uint32_t r = 0; r < n_running; ++r) n_held += running[r].n_holdings;
-    std::vector<uint32_t> at_off(size_t(N) + 1, 0), at_run(n_held);
-    for (uint32_t r = 0; r < n_running; ++r) for (uint32_t h = 0; h < running[r].n_holdings; ++h) ++at_off[holdings[running[r].holding_off + h].node + 1];
-    for (uint32_t n = 0; n < N; ++n) at_off[n + 1] += at_off[n];
-    { std::vector<uint32_t> cur(at_off.begin(), at_off.end() - 1);
-      for (uint32_t r = 0; r < n_running; ++r) for (uint32_t h = 0; h < running[r].n_holdings; ++h) at_run[cur[holdings[running[r].holding_off + h].node]++] = r; }
+    const RunningByNode at = running_by_node(N, running, n_running, holdings);
     std::vector<int32_t> slot(N, -1);   // node (caller order) -> its row in `rows` during a try
-    auto accumulate = [&](grove_cycle_stats_t& s) {
-      st0.rounds += s.rounds; st0.evaluations += s.evaluations; st0.kernel_launches += s.kernel_launches;
-      st0.ms_fit += s.ms_fit; st0.ms_admit += s.ms_admit; st0.ms_commit += s.ms_commit; st0.ms_total += s.ms_total;
-    };
     for (uint32_t b : order) {
       const int32_t p = gangs[b].priority;
-      if (status[b].state != GROVE_GANG_REJECTED || !movable(p)) continue;
+      if (snap.status[b].state != GROVE_GANG_REJECTED || !movable(p)) continue;
       // 2. b as a submission of its own (anchor pinned to the ordinary pass's, no gating); F aside, W = F + what M holds
-      grove_gang_t x = gangs[b];
-      if (x.anchor_node == GROVE_NONE_U32) x.anchor_node = e->perm[fmix32(b) % N];
-      x.base_gang = GROVE_NONE_U32; x.clique_off = 0; x.scope_off = 0;
-      const grove_clique_t* bq = cliques.data() + gangs[b].clique_off;
-      const grove_scope_t* bs = scopes.data() + gangs[b].scope_off;
-      auto submit_b = [&]() { return grove_submit_gangs(e, &x, 1, bq, x.n_cliques, bs, x.n_scopes); };
-      rc = submit_b(); if (rc) return rc;
+      Sub bsub;
+      const grove_gang_t& x = add_gang(e, snap, b, bsub);
+      rc = submit_sub(e, bsub); if (rc) return rc;
       CU_TRY(e, cudaMemcpyAsync(e->d_rc_gone.p, gone.data(), gone.size(), cudaMemcpyHostToDevice, e->stream));
       k_consol_view<<<nblk, 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_real.p, e->d_cs_view.p, csr, N, p);
       CU_TRY(e, cudaGetLastError());
@@ -2797,133 +2571,80 @@ int32_t grove_run_cycle_consolidate(grove_engine_t* e, const uint32_t* targets, 
       bool committed = false, b_loaded = true;
       for (const auto& [lo, hi] : tries) {
         // 4. evaluate b against W with every node outside D unschedulable
-        if (!b_loaded) { rc = submit_b(); if (rc) return rc; b_loaded = true; }
+        if (!b_loaded) { rc = submit_sub(e, bsub); if (rc) return rc; b_loaded = true; }
         k_consol_mask<<<nblk, 256, 0, e->stream>>>(e->d_cs_view.p, e->d_nres.p, N, lo, hi);
         CU_TRY(e, cudaGetLastError());
         grove_cycle_stats_t stb{};
         rc = grove_run_cycle(e, &stb); if (rc) return rc;
-        accumulate(stb); st0.kernel_launches += 1;
+        accumulate(st0, stb); st0.kernel_launches += 1;
         const grove_gang_status_t sb = e->h_status.p[0];
         if (sb.state != GROVE_GANG_ADMITTED) continue;
-        std::vector<grove_scope_status_t> ssb(std::max<uint32_t>(x.n_scopes, 1));
-        if (x.n_scopes) { rc = grove_get_scope_domains(e, ssb.data(), x.n_scopes); if (rc) return rc; }
-        // b's usage, nodes in the order its placement first names them
-        std::vector<uint32_t> nodes_b; std::vector<Res> use;
+        std::vector<grove_scope_status_t> ssb;
+        rc = sub_scope_domains(e, bsub, ssb); if (rc) return rc;
+        // b's usage, and the rows of F at its nodes
+        std::vector<uint32_t> nodes_b; std::vector<Res> use, rows;
         std::vector<grove_placement_t> plb;
-        for (uint32_t i = 0; i < sb.n_pods; ++i) {
-          const grove_placement_t pl = e->h_out.p[sb.placement_off + i];
-          const grove_clique_t& q = bq[pl.clique];
-          if (slot[pl.node] < 0) { slot[pl.node] = int32_t(nodes_b.size()); nodes_b.push_back(pl.node); use.emplace_back(); }
-          Res& u = use[slot[pl.node]];
-          u.cpu += q.req_cpu_milli; u.mem += q.req_mem_mib; u.gpu += q.req_gpu; u.pods += 1;
-          plb.push_back(grove_placement_t{gangs[b].clique_off + pl.clique, pl.node});
-        }
-        // the rows of F at those nodes
-        std::vector<Res> rows(nodes_b.size());
-        if (!nodes_b.empty()) {
-          std::vector<uint32_t> idx(nodes_b.size());
-          for (size_t i = 0; i < nodes_b.size(); ++i) idx[i] = e->inv[nodes_b[i]];
-          std::vector<uint4> got(idx.size());
-          CU_TRY(e, e->d_rc_idx.ensure(idx.size())); CU_TRY(e, e->d_rc_rows.ensure(idx.size()));
-          CU_TRY(e, cudaMemcpyAsync(e->d_rc_idx.p, idx.data(), sizeof(uint32_t) * idx.size(), cudaMemcpyHostToDevice, e->stream));
-          k_reclaim_rows<<<uint32_t((idx.size() + 255) / 256), 256, 0, e->stream>>>(e->d_rc_real.p, e->d_rc_idx.p, e->d_rc_rows.p, uint32_t(idx.size()));
-          CU_TRY(e, cudaGetLastError());
-          CU_TRY(e, cudaMemcpyAsync(got.data(), e->d_rc_rows.p, sizeof(uint4) * got.size(), cudaMemcpyDeviceToHost, e->stream));
-          CU_TRY(e, cudaStreamSynchronize(e->stream));
-          for (size_t i = 0; i < got.size(); ++i) rows[i] = Res{got[i].x, got[i].y, got[i].z & 0xFFFFu, got[i].z >> 16};
-          st0.kernel_launches += 1;
-        }
+        placed(e, snap, bsub, 0, nodes_b, use, plb);
+        rc = read_rows(e, nodes_b, rows, st0); if (rc) return rc;
+        for (size_t j = 0; j < nodes_b.size(); ++j) slot[nodes_b[j]] = int32_t(j);
         // the displaced set: node by node, while F plus what X holds does not cover U, the victim rule of the reclaim pass over M
         std::vector<uint32_t> X;
         std::vector<uint8_t> in_x(std::max<uint32_t>(n_running, 1), 0);
         for (size_t j = 0; j < nodes_b.size(); ++j) {
-          const uint32_t n = nodes_b[j];
-          const Res& u = use[j];
-          while (!(rows[j].cpu >= u.cpu && rows[j].mem >= u.mem && rows[j].gpu >= u.gpu && rows[j].pods >= u.pods)) {
-            uint32_t v = GROVE_NONE_U32;   // lowest priority first, then the highest running index
-            for (uint32_t a = at_off[n]; a < at_off[n + 1]; ++a) {
-              const uint32_t r = at_run[a];
-              if (gone[r] || in_x[r] || running[r].priority > p) continue;
-              if (v == GROVE_NONE_U32 || running[r].priority < running[v].priority || (running[r].priority == running[v].priority && r > v)) v = r;
-            }
+          while (!rows[j].covers(use[j])) {
+            const uint32_t v = choose_victim(at, nodes_b[j], running, [&](uint32_t r) { return !gone[r] && !in_x[r] && running[r].priority <= p; });
             if (v == GROVE_NONE_U32) return fail(e, GROVE_ERR_STATE, "consolidation: a target's node cannot be covered");
             in_x[v] = 1; X.push_back(v);
             for (uint32_t h = 0; h < running[v].n_holdings; ++h) {
               const grove_holding_t& y = holdings[running[v].holding_off + h];
-              if (slot[y.node] < 0) continue;
-              Res& q = rows[slot[y.node]];
-              q.cpu += y.cpu_milli; q.mem += y.mem_mib; q.gpu += y.gpu; q.pods += y.pods;
+              if (slot[y.node] >= 0) rows[slot[y.node]].add(held(y));
             }
           }
         }
         for (uint32_t n : nodes_b) slot[n] = -1;
         // F' = F + what X holds - U, patched into a copy of F
         {
-          std::vector<std::pair<uint32_t, std::array<int64_t, 4>>> d;   // (sorted node, change)
-          for (size_t j = 0; j < nodes_b.size(); ++j) d.push_back({e->inv[nodes_b[j]], {-use[j].cpu, -use[j].mem, -use[j].gpu, -use[j].pods}});
+          std::vector<std::pair<uint32_t, Res>> d;   // (sorted node, change)
+          for (size_t j = 0; j < nodes_b.size(); ++j) { Res c; c.add(use[j], -1); d.push_back({e->inv[nodes_b[j]], c}); }
           for (uint32_t r : X)
             for (uint32_t h = 0; h < running[r].n_holdings; ++h) {
               const grove_holding_t& y = holdings[running[r].holding_off + h];
-              d.push_back({e->inv[y.node], {int64_t(y.cpu_milli), int64_t(y.mem_mib), int64_t(y.gpu), int64_t(y.pods)}});
+              d.push_back({e->inv[y.node], held(y)});
             }
-          std::sort(d.begin(), d.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
-          std::vector<uint4> patch;
-          for (size_t i = 0; i < d.size();) {
-            const uint32_t n = d[i].first;
-            int64_t v[4] = {0, 0, 0, 0};
-            for (; i < d.size() && d[i].first == n; ++i) for (int k = 0; k < 4; ++k) v[k] += d[i].second[k];
-            patch.push_back(make_uint4(n, uint32_t(v[0]), uint32_t(v[1]), uint32_t(v[2] + v[3] * 65536)));
-          }
           CU_TRY(e, cudaMemcpyAsync(e->d_nres.p, e->d_rc_real.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToDevice, e->stream));
-          if (!patch.empty()) {
-            CU_TRY(e, e->d_rc_patch.ensure(patch.size()));
-            CU_TRY(e, cudaMemcpyAsync(e->d_rc_patch.p, patch.data(), sizeof(uint4) * patch.size(), cudaMemcpyHostToDevice, e->stream));
-            k_reclaim_patch<<<uint32_t((patch.size() + 255) / 256), 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_patch.p, uint32_t(patch.size()));
-            CU_TRY(e, cudaGetLastError());
-            st0.kernel_launches += 1;
-          }
+          rc = patch_nodes(e, d, st0); if (rc) return rc;
         }
         // relocate X: its spec rows as one sequential pass (running priority desc, running index asc), each with its own anchor
         std::vector<uint32_t> xs(X);
         std::sort(xs.begin(), xs.end(), [&](uint32_t a, uint32_t c) { return running[a].priority != running[c].priority ? running[a].priority > running[c].priority : a < c; });
-        std::vector<grove_gang_t> sg; std::vector<grove_clique_t> sq; std::vector<grove_scope_t> ss;
+        Sub xsub;
         for (uint32_t r : xs) {
-          const uint32_t s = spec_of[r];
-          grove_gang_t y = gangs[s];
-          if (y.anchor_node == GROVE_NONE_U32) y.anchor_node = e->perm[fmix32(s) % N];
-          y.priority = running[r].priority; y.base_gang = GROVE_NONE_U32; y.flags &= uint16_t(~GROVE_GANG_GATED);
-          y.clique_off = uint32_t(sq.size()); y.scope_off = uint32_t(ss.size());
-          sq.insert(sq.end(), cliques.begin() + gangs[s].clique_off, cliques.begin() + gangs[s].clique_off + gangs[s].n_cliques);
-          ss.insert(ss.end(), scopes.begin() + gangs[s].scope_off, scopes.begin() + gangs[s].scope_off + gangs[s].n_scopes);
-          sg.push_back(y);
+          grove_gang_t& y = add_gang(e, snap, spec_of[r], xsub);
+          y.priority = running[r].priority; y.flags &= uint16_t(~GROVE_GANG_GATED);
         }
-        std::vector<grove_scope_status_t> ssx(std::max<size_t>(ss.size(), 1));
+        std::vector<grove_scope_status_t> ssx;
         if (!xs.empty()) {
-          rc = grove_submit_gangs(e, sg.data(), uint32_t(sg.size()), sq.data(), uint32_t(sq.size()), ss.data(), uint32_t(ss.size())); if (rc) return rc;
+          rc = submit_sub(e, xsub); if (rc) return rc;
           b_loaded = false;
           grove_cycle_stats_t stx{};
           rc = grove_run_cycle(e, &stx); if (rc) return rc;
-          accumulate(stx);
+          accumulate(st0, stx);
           bool all = true;
           for (uint32_t k = 0; k < xs.size(); ++k) all &= e->h_status.p[k].state == GROVE_GANG_ADMITTED;
           if (!all) continue;   // rolled back: the next try starts from the view again, and F is still aside
-          if (!ss.empty()) { rc = grove_get_scope_domains(e, ssx.data(), uint32_t(ss.size())); if (rc) return rc; }
+          rc = sub_scope_domains(e, xsub, ssx); if (rc) return rc;
         }
         // commit: the device table is F' minus the relocated gangs' usage
         grove_gang_status_t ob = sb;
         ob.reserved0 = GROVE_STATUS_CONSOLIDATED;
-        status[b] = ob; extra[b] = std::move(plb);
-        for (uint32_t si = 0; si < x.n_scopes; ++si) sstat[gangs[b].scope_off + si] = ssb[si];
+        merge_gang(snap, bsub, 0, ob, ssb);
+        extra[b] = std::move(plb);
         for (uint32_t k = 0; k < xs.size(); ++k) {
-          const uint32_t s = spec_of[xs[k]];
+          std::vector<uint32_t> nodes_x; std::vector<Res> use_x;
+          placed(e, snap, xsub, k, nodes_x, use_x, extra[xsub.ids[k]]);
           grove_gang_status_t o = e->h_status.p[k];
-          for (uint32_t i = 0; i < o.n_pods; ++i) {
-            const grove_placement_t pl = e->h_out.p[o.placement_off + i];
-            extra[s].push_back(grove_placement_t{gangs[s].clique_off + (pl.clique - sg[k].clique_off), pl.node});
-          }
           o.reserved0 = GROVE_STATUS_MOVED;
-          status[s] = o;
-          for (uint32_t si = 0; si < gangs[s].n_scopes; ++si) sstat[gangs[s].scope_off + si] = ssx[sg[k].scope_off + si];
+          merge_gang(snap, xsub, k, o, ssx);
         }
         for (uint32_t r : X) { gone[r] = 1; moves.push_back(grove_move_t{r, b}); }
         st0.gangs_admitted += 1 + uint32_t(X.size()); st0.gangs_rejected -= 1;
@@ -2936,10 +2657,10 @@ int32_t grove_run_cycle_consolidate(grove_engine_t* e, const uint32_t* targets, 
     }
     // the handle goes back to the caller's submission; the device table is F after every commit
     restore.armed = false;
-    rc = grove_submit_gangs(e, gangs.data(), G, cliques.data(), Q, scopes.data(), S); if (rc) return rc;
+    rc = restore.put_back(); if (rc) return rc;
   }
   st0.kernel_launches += 1;   // k_reclaim_check
-  rc = publish_reclaim(e, status, place, extra, sstat, st0, {}, stats);
+  rc = publish_reclaim(e, snap.status, snap.place, extra, snap.sstat, st0, {}, stats);
   if (rc) return rc;
   e->moves = std::move(moves);
   return GROVE_OK;

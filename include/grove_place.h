@@ -245,7 +245,8 @@ int32_t grove_get_scope_domains(grove_engine_t* e, grove_scope_status_t* out, ui
  * PodGang"; PriorityClassName podgang.go:62-64); the arithmetic is ours (DESIGN.md section 1, "Reclaim pass").  RUNNING gangs
  * (admitted by earlier cycles) are handed in with what they hold per node.  After the ordinary pass every REJECTED gang, in
  * order rank, is evaluated once more against the RECLAIM VIEW of its priority p -- free resources plus everything held by
- * running gangs of priority < p that are still standing.  If it fits, it is admitted (GROVE_STATUS_PREEMPTOR) and, node by
+ * running gangs of priority < p that are still standing (E(p)) -- and skipped while E(p) is empty.  If it fits, it is admitted
+ * (GROVE_STATUS_PREEMPTOR) and, node by
  * node in the order of its placement, running gangs are evicted WHOLE (lowest priority first, then highest running index)
  * until the node's free resources cover what it puts there; everything an evicted gang held anywhere returns to the free
  * pool.  grove_get_victims lists (running gang, preemptor) pairs: the caller sets DisruptionTarget on them. */
@@ -266,7 +267,9 @@ typedef struct grove_victim {
 } grove_victim_t;
 #define GROVE_STATUS_PREEMPTOR 0x1u /* grove_gang_status_t.reserved0: admitted by the reclaim pass */
 /* ordinary pass + reclaim pass; outputs through the usual getters (statuses, placements, scope domains, node table = free
- * resources after evictions and admissions) */
+ * resources after evictions and admissions).  GROVE_ERR_INVALID_ARG when a running gang's holdings lie outside the holdings
+ * array, a holding lies on a node out of range, or free + the holdings of every running gang overflows a field of a node
+ * record. */
 int32_t grove_run_cycle_preempt(grove_engine_t* e, const grove_running_gang_t* running, uint32_t n_running,
                                 const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats);
 int32_t grove_get_victims(grove_engine_t* e, grove_victim_t* out, uint32_t cap, uint32_t* n_out);

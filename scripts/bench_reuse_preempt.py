@@ -7,8 +7,7 @@ the top class: they outrank part of what runs, and the reclaim pass evicts to pl
 Alternately, from the same node table:
   reuse_preempt  grove_run_cycle_reuse_preempt: the new versions reuse their predecessors' reservations, then the reclaim pass
                  with class views built on the device;
-  preempt        grove_run_cycle_preempt on the same submission with no replacements: the reclaim pass with a host round
-                 trip of the node table per class;
+  preempt        grove_run_cycle_preempt on the same submission with no replacements: the same reclaim loop with no holds;
   reuse, cycle   their ordinary passes alone (grove_run_cycle_reuse, grove_run_cycle), so that what the reclaim pass adds can
                  be told apart: (entry - its ordinary pass) / classes is the reclaim cost per class.
 Prints one JSON line: ms per cycle (device events summed over the cycles of the call, and the host clock around the blocking
