@@ -17,6 +17,8 @@
 #include <string>
 #include <vector>
 
+#include <cub/device/device_radix_sort.cuh>
+
 #include "kernels.cuh"
 
 using namespace grove;
@@ -272,6 +274,21 @@ struct grove_engine {
   DevBuf<long long> d_qu_rmin, d_qu_q_base, d_qu_head;
   DevBuf<unsigned long long> d_qu_use;
   DevBuf<uint8_t> d_qu_gate, d_qu_cap;
+  // bin-packing (grove_set_binpack; binpack.cuh): the pack level of every gang of the current submission (GROVE_LEVEL_NONE = not a
+  // member); the pick kernels run only while there are members (bp_members > 0)
+  std::vector<uint8_t> bp_level;
+  uint32_t bp_members = 0;
+  bool bp_given = false;                   // a set was given for the current submission, members or not
+  bool bp_anchors = false;                 // d_ginfo holds picked anchors (the host's ginfo keeps the defaults)
+  std::vector<uint32_t> bp_picks;          // caller index of each gang's pick in the last cycle that ran with a set
+  bool bp_have_picks = false;
+  PinBuf<uint4> h_bp_mem;
+  PinBuf<uint32_t> h_bp_pick;
+  DevBuf<uint4> d_bp_mem;
+  DevBuf<BpSum> d_bp_sum;
+  DevBuf<BpKey> d_bp_key;
+  DevBuf<uint32_t> d_bp_idx, d_bp_rank, d_bp_pick;
+  DevBuf<uint8_t> d_bp_tmp;
 };
 
 
@@ -295,6 +312,10 @@ static int32_t refuse_fences(grove_engine* e, const char* entry) {
 }
 static int32_t refuse_queues(grove_engine* e, const char* entry) {
   e->err = std::string(entry) + ": not supported while a queue set with members is in place (grove_set_queues)";
+  return GROVE_ERR_STATE;
+}
+static int32_t refuse_binpack(grove_engine* e, const char* entry) {
+  e->err = std::string(entry) + ": not supported while a bin-packing set with members is in place (grove_set_binpack)";
   return GROVE_ERR_STATE;
 }
 static int32_t refuse_wide(grove_engine* e, const char* entry) {
@@ -413,6 +434,15 @@ static int32_t build_topology(grove_engine* e, const grove_node_t* nodes, uint32
   return GROVE_OK;
 }
 
+// Gangs that relax concurrently: the knob, else all of them -- except in a cycle with bin-packing members, whose picks send many
+// gangs to the same fullest domains: every gang of the window then claims the same first nodes, and each such node's overflow
+// chain grows as long as the window (DESIGN.md section 1 "Bin-packing").  kBinpackWindow bounds it; cycle_begin sizes the pool.
+static constexpr uint32_t kBinpackWindow = 128;
+static uint32_t window_of(const grove_engine* e) {
+  if (e->tune_window) return e->tune_window;
+  return e->bp_members ? std::max(std::min(e->G, kBinpackWindow), 1u) : std::max(e->G, 1u);
+}
+
 static Topo make_topo(grove_engine* e) {
   Topo t{};
   t.nres = e->d_nres.p; t.ndom = e->d_ndom.p;
@@ -450,7 +480,7 @@ static Relax make_relax(grove_engine* e) {
   r.F = e->d_F.p; r.cap8 = e->d_cap8.p; r.capsum = e->d_capsum.p; r.capmax = e->d_capmax.p; r.T = e->d_T.p;
   r.shape_bits = e->shape_tables ? e->d_shape_bits.p : nullptr; r.pl_words = e->pl_words;
   for (uint32_t l = 0; l < GROVE_MAX_LEVELS; ++l) r.pl_off[l] = e->pl_off[l];
-  r.P = e->P; r.window = e->tune_window ? e->tune_window : (e->G ? e->G : 1u); r.entry = e->tune_entry ? e->tune_entry : r.window; r.heavy_att = e->tune_heavy_att;
+  r.P = e->P; r.window = window_of(e); r.entry = e->tune_entry ? e->tune_entry : r.window; r.heavy_att = e->tune_heavy_att;
   r.hold_off = e->holds_on ? e->d_hold_off.p : nullptr; r.hold = e->d_hold.p;
   r.dbg = e->dbg_on ? e->d_dbg.p : nullptr;
   r.live = e->d_live;
@@ -550,6 +580,7 @@ static int32_t load_nodes_common(grove_engine* e, const grove_node_t* host_nodes
   e->sp_groups = e->sp_members = 0;   // a spread set belongs to the nodes and gangs it was validated against
   e->fc_gangs.clear();                // (a fence set too)
   e->qu_members = 0; e->qu_given = false;   // (and a queue set)
+  e->bp_members = 0; e->bp_given = false;   // (and a bin-packing set)
   CU_TRY(e, cudaSetDevice(e->cfg.device));
   if (host_nodes) {
     CU_TRY(e, cudaEventSynchronize(e->ev_nodes_up));  // an earlier upload may still be reading the staging buffer
@@ -709,6 +740,7 @@ static int32_t submit(grove_engine* e, const grove_gang_t* gangs, uint32_t n_gan
   e->sp_groups = e->sp_members = 0;
   e->fc_gangs.clear();
   e->qu_members = 0; e->qu_given = false;
+  e->bp_members = 0; e->bp_given = false;
   int32_t rc = validate(e, gangs, n_gangs, cliques, ccount.data(), n_cliques, scopes, n_scopes, max_pods);
   if (rc) return rc;
   CU_TRY(e, cudaSetDevice(e->cfg.device));
@@ -1012,7 +1044,7 @@ static int32_t build_ginfo(grove_engine* e) {
     std::memcpy(e->shape_rep_pin.p, e->shape_rep.data(), sizeof(uint32_t) * e->n_shapes);   //  rewritten only after the cycle that reads it)
     CU_TRY(e, cudaMemcpyAsync(e->d_shape_rep.p, e->shape_rep_pin.p, sizeof(uint32_t) * e->n_shapes, cudaMemcpyHostToDevice, e->stream));
   }
-  e->ginfo_dirty = false;
+  e->ginfo_dirty = false; e->bp_anchors = false;
   if (std::getenv("GROVE_DEBUG_HOST")) {
     const auto t_b2 = std::chrono::steady_clock::now();
     auto us = [](auto a, auto b) { return (long)std::chrono::duration_cast<std::chrono::microseconds>(b - a).count(); };
@@ -1051,7 +1083,7 @@ static int32_t build_cap_tables(grove_engine* e, const Topo& tp, const Tables& t
 
 // K3 CTAs: they take work items from a queue; by default as many as are resident at once (heavy gangs take whole CTAs)
 static uint32_t eval_ctas(const grove_engine* e) {
-  const uint32_t W = e->tune_window ? e->tune_window : std::max(e->G, 1u);
+  const uint32_t W = window_of(e);
   return std::max(1u, e->tune_eval_ctas ? e->tune_eval_ctas : std::min(W, e->n_sm * e->tune_heavy_ctas));
 }
 
@@ -1079,7 +1111,10 @@ static int32_t cycle_begin(grove_engine* e) {
   CU_TRY(e, e->d_nxt_sc_lvl.ensure(s1)); CU_TRY(e, e->d_nxt_sc_lo.ensure(s1));
   CU_TRY(e, e->d_claims.ensure(size_t(N) * kClaimSlots)); CU_TRY(e, e->d_nlive.ensure(N / 4)); CU_TRY(e, e->d_ovf_head.ensure(N));
   // (the overflow pool takes the holds as well as the claims: a node's line may be full of both)
-  const size_t ovf = 4 * p1 + 1024 + (e->holds_on ? e->n_hold : 0u);
+  // (and in a cycle with bin-packing members, room on every node for a chain as long as the window -- the tentative claims of a
+  // pile-up -- plus 110, the Kubernetes default pod limit, for the settled ones; at most 2^26 entries)
+  size_t ovf = 4 * p1 + 1024 + (e->holds_on ? e->n_hold : 0u);
+  if (e->bp_members) ovf += std::min<size_t>(size_t(N) * (window_of(e) + 110u), size_t(1) << 26);
   CU_TRY(e, e->d_ovf_next.ensure(ovf)); CU_TRY(e, e->d_ovf_claim.ensure(ovf));
   CU_TRY(e, e->d_ctot.ensure(N)); CU_TRY(e, e->d_cmaxr.ensure(N));
   CU_TRY(e, e->d_add_stamp.ensure(N)); CU_TRY(e, e->d_rem_stamp.ensure(e->words)); CU_TRY(e, e->d_rem_round.ensure(e->words));
@@ -1111,7 +1146,7 @@ static int32_t cycle_begin(grove_engine* e) {
   }
   if (e->dbg_on) { CU_TRY(e, e->d_dbg.ensure(g1 * 8 + 8)); CU_TRY(e, cudaMemsetAsync(e->d_dbg.p, 0, g1 * 32 + 32, e->stream)); }
   {
-    const uint32_t W = e->tune_window ? e->tune_window : std::max(G, 1u);
+    const uint32_t W = window_of(e);
     const uint32_t E = e->tune_entry ? e->tune_entry : W;
     if (e->h_live) { std::memset(e->h_live, 0, sizeof(uint32_t) * kLiveWords); e->h_live[kLiveRound] = 1; }
     k_reset<<<e->n_sm * 4, 256, 0, e->stream>>>(make_relax(e), G, S, N, e->words, std::min(G, std::min(W, E)));
@@ -1167,6 +1202,56 @@ static int32_t finish_cycle(grove_engine* e) {
   return GROVE_OK;
 }
 
+// Bin-packing picks (binpack.cuh), after the first capacity-table build of a cycle with members: the per-domain sums of the levels
+// the members pack at, each level's domains ranked by (free GPUs, CPU, memory, first node), then a warp per member rewrites its
+// anchor.  The picks come back with the cycle's outputs (finish_cycle waits for the copy).
+static int32_t binpack_picks(grove_engine* e, const Topo& tp, const Tables& tb, const Relax& rx) {
+  const uint32_t G = e->G, M = e->bp_members;
+  CU_TRY(e, e->h_bp_mem.ensure(M)); CU_TRY(e, e->d_bp_mem.ensure(M));
+  uint32_t levels = 0;
+  for (uint32_t g = 0, k = 0; g < G; ++g) {
+    const uint8_t b = e->bp_level[g];
+    if (b == GROVE_LEVEL_NONE) continue;
+    e->h_bp_mem.p[k++] = make_uint4(g, b, e->ginfo[g].anchor, 0u);   // (the default anchor: the host's ginfo is never rewritten)
+    levels |= 1u << b;
+  }
+  BpOff off{};
+  uint32_t total = 0;
+  for (uint32_t l = 0; l < e->L; ++l) if ((levels >> l) & 1u) { off.o[l] = total; total += e->n_dom[l]; }
+  size_t tmp = 0;
+  for (uint32_t l = 0; l < e->L; ++l) {
+    if (!((levels >> l) & 1u)) continue;
+    size_t t = 0;
+    CU_TRY(e, cub::DeviceRadixSort::SortPairs(nullptr, t, e->d_bp_key.p, e->d_bp_key.p, e->d_bp_idx.p, e->d_bp_rank.p, e->n_dom[l], BpKeyDecomposer{}, e->stream));
+    tmp = std::max(tmp, t);
+  }
+  CU_TRY(e, e->d_bp_sum.ensure(std::max(total, 1u))); CU_TRY(e, e->d_bp_key.ensure(2 * size_t(std::max(total, 1u))));
+  CU_TRY(e, e->d_bp_idx.ensure(std::max(total, 1u))); CU_TRY(e, e->d_bp_rank.ensure(std::max(total, 1u)));
+  CU_TRY(e, e->d_bp_tmp.ensure(std::max<size_t>(tmp, 1))); CU_TRY(e, e->d_bp_pick.ensure(G)); CU_TRY(e, e->h_bp_pick.ensure(G));
+  CU_TRY(e, cudaMemcpyAsync(e->d_bp_mem.p, e->h_bp_mem.p, sizeof(uint4) * M, cudaMemcpyHostToDevice, e->stream));
+  CU_TRY(e, cudaMemsetAsync(e->d_bp_sum.p, 0, sizeof(BpSum) * total, e->stream));
+  CU_TRY(e, cudaMemsetAsync(e->d_bp_pick.p, 0xFF, sizeof(uint32_t) * G, e->stream));
+  k_binpack_sum<<<e->Npad / 256, 256, 0, e->stream>>>(tp, levels, off, e->d_bp_sum.p);
+  e->launches += 1;
+  BpKey* keys_out = e->d_bp_key.p + total;
+  for (uint32_t l = 0; l < e->L; ++l) {
+    if (!((levels >> l) & 1u)) continue;
+    const uint32_t o = off.o[l], nd = e->n_dom[l];
+    if (!nd) continue;   // (no node carries the level's label: no domain to rank)
+    k_binpack_keys<<<(nd + 255) / 256, 256, 0, e->stream>>>(e->d_bp_sum.p + o, nd, e->d_bp_key.p + o, e->d_bp_idx.p + o);
+    size_t t = e->d_bp_tmp.cap;
+    CU_TRY(e, cub::DeviceRadixSort::SortPairs(e->d_bp_tmp.p, t, e->d_bp_key.p + o, keys_out + o, e->d_bp_idx.p + o, e->d_bp_rank.p + o, nd,
+                                              BpKeyDecomposer{}, e->stream));
+    e->launches += 2;
+  }
+  k_binpack_pick<<<(M * 32 + 255) / 256, 256, 0, e->stream>>>(tp, tb, rx, e->d_bp_mem.p, M, e->d_bp_sum.p, e->d_bp_rank.p, off, e->d_ginfo.p, e->d_bp_pick.p);
+  CU_TRY(e, cudaGetLastError());
+  CU_TRY(e, cudaMemcpyAsync(e->h_bp_pick.p, e->d_bp_pick.p, sizeof(uint32_t) * G, cudaMemcpyDeviceToHost, e->stream));
+  e->launches += 1;
+  e->bp_anchors = true;
+  return GROVE_OK;
+}
+
 struct CycleGuard {   // every error exit of a cycle leaves the handle usable (ADVICE round 1: in_cycle stayed set)
   grove_engine* e; bool armed = true;
   ~CycleGuard() { if (armed) { e->in_cycle = false; cudaStreamSynchronize(e->stream); cudaStreamSynchronize(e->stream_score); } }
@@ -1180,6 +1265,13 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
   const uint32_t G = e->G;
   CU_TRY(e, cudaEventRecord(e->ev[8], e->stream));
   uint32_t rounds = 0;
+  if (G && e->bp_anchors) {   // an earlier cycle's picks: back to the default anchors (this cycle's members are picked again)
+    CU_TRY(e, cudaMemcpyAsync(e->d_ginfo.p, e->ginfo, sizeof(GangInfo) * G, cudaMemcpyHostToDevice, e->stream));
+    k_anchor<<<(G + 255) / 256, 256, 0, e->stream>>>(tp, e->d_ginfo.p, G);
+    CU_TRY(e, cudaGetLastError());
+    e->launches += 1;
+    e->bp_anchors = false;
+  }
   if (G && e->holds_on) {   // the holds join the committed state (so every table built from it bounds every gang's view) as claims
     k_hold_publish<<<(G * 32 + 255) / 256, 256, 0, e->stream>>>(tb, rx, e->d_nres.p);
     CU_TRY(e, cudaGetLastError());
@@ -1219,6 +1311,7 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
     rc = build_cap_tables(e, tp, tb, rx);
     if (rc) return rc;
     CU_TRY(e, cudaEventRecord(e->ev[1], e->stream));
+    if (e->bp_members) { rc = binpack_picks(e, tp, tb, rx); if (rc) return rc; }   // (before K2: it scores against the picks)
     CU_TRY(e, e->d_F0.ensure(std::max<size_t>(size_t(e->n_sigs) * e->words, 1)));
     CU_TRY(e, cudaMemcpyAsync(e->d_F0.p, e->d_F.p, sizeof(uint32_t) * size_t(e->n_sigs) * e->words, cudaMemcpyDeviceToDevice, e->stream));
     e->score_valid = false;
@@ -1386,6 +1479,12 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
   if (rc) return rc;
   if (spread)   // (finish_cycle waited for the copy)
     for (uint32_t g = 0; g < G; ++g) if (e->h_sp_skewed.p[g]) e->h_status.p[g].reserved0 |= GROVE_STATUS_SPREAD_SKEWED;
+  if (e->bp_given) {   // (so did it for the picks')
+    e->bp_picks.assign(G, GROVE_NONE_U32);
+    if (e->bp_members)
+      for (uint32_t g = 0; g < G; ++g) if (e->h_bp_pick.p[g] != kFull) e->bp_picks[g] = e->perm[e->h_bp_pick.p[g]];
+    e->bp_have_picks = true;
+  }
   CU_TRY(e, cudaEventRecord(e->ev[9], e->stream));
   CU_TRY(e, cudaEventSynchronize(e->ev[9]));
   guard.armed = false;
@@ -1421,6 +1520,8 @@ int32_t grove_run_cycle(grove_engine_t* e, grove_cycle_stats_t* stats) {
   if (spread && fences) return fail(e, GROVE_ERR_STATE, "grove_run_cycle: a spread set with members and a fence set together are not supported");
   if (e->qu_members && (spread || fences))
     return fail(e, GROVE_ERR_STATE, "grove_run_cycle: a queue set with members together with a spread set with members or a fence set is not supported");
+  if (e->bp_members && (spread || fences))
+    return fail(e, GROVE_ERR_STATE, "grove_run_cycle: a bin-packing set with members together with a spread set with members or a fence set is not supported");
   const int32_t rc = run_cycle(e, stats);
   if (rc == GROVE_OK) e->diag = spread ? grove_engine::kDiagSpread : fences ? grove_engine::kDiagFence : grove_engine::kDiagReady;
   return rc;
@@ -1580,6 +1681,39 @@ int32_t grove_set_fences(grove_engine_t* e, const uint32_t* gangs, uint32_t n) {
   if (words > (size_t(1) << 28))
     return fail(e, GROVE_ERR_LIMIT, "grove_set_fences: the per-domain sums (fencing gangs x cliques x domains of their level) exceed 1 GB");
   e->fc_gangs = std::move(v); e->fc_off = std::move(off); e->fc_words = words;
+  return GROVE_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Bin-packing (include/grove_place.h "bin-packing"; DESIGN.md section 1; kernels in binpack.cuh).  Validated against the
+// submission; the cycle makes the picks over its own F0.
+// ---------------------------------------------------------------------------------------------
+int32_t grove_set_binpack(grove_engine_t* e, const uint8_t* level_of, uint32_t n_gangs) {
+  if (!e) return GROVE_ERR_INVALID_ARG;
+  if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
+  if (!e->nodes_loaded || !e->gangs_loaded) return fail(e, GROVE_ERR_STATE, "grove_set_binpack: load nodes and submit gangs first");
+  if (n_gangs != e->G) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_binpack: n_gangs is not the number of gangs submitted");
+  if (n_gangs && !level_of) return GROVE_ERR_INVALID_ARG;
+  if (e->wide) return refuse_wide(e, "grove_set_binpack");
+  uint32_t members = 0;
+  for (uint32_t g = 0; g < n_gangs; ++g) {
+    const uint8_t b = level_of[g];
+    if (b == GROVE_LEVEL_NONE) continue;
+    if (b >= e->L) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_binpack: pack level out of range");
+    if (e->gangs[g].level != GROVE_LEVEL_NONE && b < e->gangs[g].level)
+      return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_binpack: a pack level above the gang's Required level");
+    ++members;
+  }
+  e->bp_level.assign(level_of, level_of + n_gangs);
+  e->bp_members = members; e->bp_given = true;
+  return GROVE_OK;
+}
+
+int32_t grove_get_binpack_picks(grove_engine_t* e, uint32_t* out, uint32_t cap) {
+  if (!e || !out) return GROVE_ERR_INVALID_ARG;
+  if (!e->bp_have_picks) return fail(e, GROVE_ERR_STATE, "grove_get_binpack_picks: no cycle has run with a bin-packing set");
+  if (cap < e->bp_picks.size()) return fail(e, GROVE_ERR_LIMIT, "output buffer too small");
+  std::copy(e->bp_picks.begin(), e->bp_picks.end(), out);
   return GROVE_OK;
 }
 
@@ -2139,6 +2273,7 @@ int32_t grove_run_cycle_reuse(grove_engine_t* e, const uint32_t* replaces, uint3
   if (e->sp_members) return refuse_spread(e, "grove_run_cycle_reuse");
   if (e->qu_members) return refuse_queues(e, "grove_run_cycle_reuse");
   if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_reuse");
+  if (e->bp_members) return refuse_binpack(e, "grove_run_cycle_reuse");
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse");
   const int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);
@@ -2410,6 +2545,7 @@ int32_t grove_run_cycle_preempt(grove_engine_t* e, const grove_running_gang_t* r
   if (e->sp_members) return refuse_spread(e, "grove_run_cycle_preempt");
   if (e->qu_members) return refuse_queues(e, "grove_run_cycle_preempt");
   if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_preempt");
+  if (e->bp_members) return refuse_binpack(e, "grove_run_cycle_preempt");
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_preempt");
   int32_t rc = check_ready(e);
@@ -2425,6 +2561,7 @@ int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replace
   if (e->sp_members) return refuse_spread(e, "grove_run_cycle_reuse_preempt");
   if (e->qu_members) return refuse_queues(e, "grove_run_cycle_reuse_preempt");
   if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_reuse_preempt");
+  if (e->bp_members) return refuse_binpack(e, "grove_run_cycle_reuse_preempt");
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse_preempt");
   const int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);
@@ -2439,6 +2576,7 @@ int32_t grove_run_cycle_preempt_queues(grove_engine_t* e, const grove_running_ga
   if (!e || (n_running && (!running || !running_queue)) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
   if (e->sp_members) return refuse_spread(e, kEntry);
   if (!e->fc_gangs.empty()) return refuse_fences(e, kEntry);
+  if (e->bp_members) return refuse_binpack(e, kEntry);
   if (!e->qu_given) return fail(e, GROVE_ERR_STATE, "grove_run_cycle_preempt_queues: no queue set given for the current submission (grove_set_queues)");
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, kEntry);
@@ -2477,6 +2615,7 @@ int32_t grove_run_cycle_consolidate(grove_engine_t* e, const uint32_t* targets, 
   if (e->sp_members) return refuse_spread(e, "grove_run_cycle_consolidate");
   if (e->qu_members) return refuse_queues(e, "grove_run_cycle_consolidate");
   if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_consolidate");
+  if (e->bp_members) return refuse_binpack(e, "grove_run_cycle_consolidate");
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_consolidate");
   if (n_targets > GROVE_MAX_CONSOLIDATE_TARGETS) return fail(e, GROVE_ERR_LIMIT, "grove_run_cycle_consolidate: more than GROVE_MAX_CONSOLIDATE_TARGETS targets");

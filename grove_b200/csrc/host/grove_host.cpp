@@ -765,19 +765,19 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
       reuse = std::any_of(replaces.begin(), replaces.end(), [](uint32_t r) { return r != GROVE_NONE_U32; });
     }
   }
+  bool wide = false;   // a row beyond the ordinary limits makes the submission wide, which takes no fence or bin-packing set
+  for (const grove_gang_t& g : t.gangs) {
+    uint32_t pods = 0;
+    for (uint32_t c = g.clique_off; c < g.clique_off + g.n_cliques; ++c) {
+      const uint32_t rep = large ? t.counts[c].replicas : t.cliques[c].replicas;
+      pods += rep; wide |= rep > 255u;
+    }
+    wide |= pods > GROVE_MAX_GANG_PODS;
+  }
   // the starvation guard: the highest-ranked rows (priority desc, row asc = the engine's rank) of the PodGangs rejected often
   // enough, in an ordinary pass only
   std::vector<uint32_t> fences;
   if (guardMax && !both && !reuse && !preempt && !spread) {
-    bool wide = false;   // a row beyond the ordinary limits makes the submission wide, which takes no fence set
-    for (const grove_gang_t& g : t.gangs) {
-      uint32_t pods = 0;
-      for (uint32_t c = g.clique_off; c < g.clique_off + g.n_cliques; ++c) {
-        const uint32_t rep = large ? t.counts[c].replicas : t.cliques[c].replicas;
-        pods += rep; wide |= rep > 255u;
-      }
-      wide |= pods > GROVE_MAX_GANG_PODS;
-    }
     std::vector<uint32_t> rows;
     for (uint32_t g = 0; g < t.gangs.size() && !wide; ++g) {
       auto it = rejectedFor.find(t.gangNames[g]);
@@ -788,6 +788,19 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
     fences = rows;
     if (!fences.empty())
       if (auto e = chk(grove_set_fences(engine_, fences.data(), uint32_t(fences.size())), "grove_set_fences")) return e;
+  }
+  // bin-packing: every row a member, at the level of the key or its own Required level when deeper, in an ordinary or queue pass
+  if (!both && !reuse && !preempt && !consolidate && !spread && fences.empty() && !wide) {
+    uint8_t lv = GROVE_LEVEL_NONE;
+    {
+      std::lock_guard<std::mutex> l(mu_);
+      for (size_t i = 0; i < levels_.size() && !binpackKey_.empty(); ++i) if (levels_[i].Key == binpackKey_) lv = uint8_t(i);
+    }
+    if (lv != GROVE_LEVEL_NONE) {
+      std::vector<uint8_t> packAt(t.gangs.size());
+      for (size_t g = 0; g < t.gangs.size(); ++g) packAt[g] = t.gangs[g].level == GROVE_LEVEL_NONE ? lv : std::max(lv, t.gangs[g].level);
+      if (auto e = chk(grove_set_binpack(engine_, packAt.data(), uint32_t(packAt.size())), "grove_set_binpack")) return e;
+    }
   }
   if (both) { if (auto e = chk(grove_run_cycle_reuse_preempt(engine_, replaces.data(), uint32_t(replaces.size()), run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_reuse_preempt")) return e; }
   else if (reuse) { if (auto e = chk(grove_run_cycle_reuse(engine_, replaces.data(), uint32_t(replaces.size()), run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_reuse")) return e; }

@@ -320,6 +320,13 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   // PodGang beyond the ordinary limits (SetLargePodGangs), nothing is fenced (the counts go on).  maxGangs = 0 turns it off (the
   // default); afterCycles >= 1, maxGangs <= GROVE_MAX_FENCES.
   Err SetStarvationGuard(uint32_t afterCycles, uint32_t maxGangs);
+  // Bin-packing (grove_set_binpack; DESIGN.md section 1 "Bin-packing"): with the key of a topology level, every PodGang of an
+  // ordinary or queue pass starts its search at the fullest domain of that level -- or of its own Required level when that is
+  // deeper -- that can hold it on the cycle's node table, so that empty domains stay empty for large PodGangs.  A preference, not a
+  // constraint: in a pass with preemption, reservation reuse, consolidation, topology spread members, fences or a PodGang beyond the
+  // ordinary limits (SetLargePodGangs) the pass runs without it, and so does every pass while the key names no level of the
+  // topology.  An empty key (the default) turns it off.
+  void SetBinPacking(const std::string& levelKey) { std::lock_guard<std::mutex> l(mu_); binpackKey_ = levelKey; }
   // Consolidation (grove_run_cycle_consolidate; DESIGN.md section 1 "Consolidation"): the spec of every PodGang this backend
   // scheduled is remembered, and each running PodGang it scheduled whole (nothing left pending) is restated as a gated row, which
   // makes it movable.  Each cycle the <= maxTargets highest-ranked pending PodGangs rejected at least afterCycles times in a row
@@ -380,6 +387,7 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   bool preemptQueues_ = false;
   bool large_ = false;
   bool explain_ = false;
+  std::string binpackKey_;                             // bin-packing level (off: empty)
   uint32_t guardAfter_ = 1, guardMax_ = 0;             // starvation guard (off: guardMax_ == 0)
   std::map<std::string, uint32_t> rejectedFor_;        // pending PodGang -> consecutive Unschedulable cycles
   uint32_t consAfter_ = 1, consMax_ = 0;               // consolidation (off: consMax_ == 0)

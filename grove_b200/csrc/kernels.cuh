@@ -13,6 +13,8 @@
 //   fence.cuh    k_fence_have / k_fence_pick / k_fence_status  the domain each fencing gang fences (grove_set_fences)
 //   consolidate.cuh k_consol_view / k_consol_rank / k_consol_mask  the views of a consolidation try (grove_run_cycle_consolidate)
 //   queue.cuh    k_queue_scan / k_queue_gate  the headroom, gate and surplus caps of the queue members (grove_set_queues)
+//   binpack.cuh  k_binpack_sum / k_binpack_keys / k_binpack_pick  the fullest domain each bin-packing member is anchored at
+//                (grove_set_binpack)
 //
 // Semantics are DESIGN.md "Placement semantics"; the reference contract they restate is cited in
 // include/grove_place.h.  Integer / compare work only: no tensor cores, no floating point.
@@ -29,3 +31,4 @@
 #include "fence.cuh"
 #include "consolidate.cuh"
 #include "queue.cuh"
+#include "binpack.cuh"

@@ -27,6 +27,7 @@ SYMBOLS = [
     "grove_build_score_matrix", "grove_run_cycle_preempt", "grove_get_victims", "grove_run_cycle_reuse",
     "grove_run_cycle_reuse_preempt", "grove_diagnose", "grove_set_spread", "grove_set_fences", "grove_set_queues",
     "grove_run_cycle_consolidate", "grove_get_moves", "grove_run_cycle_preempt_queues",
+    "grove_set_binpack", "grove_get_binpack_picks",
     "grove_shard_range", "grove_run_score_pass", "grove_shard_summary_device",
     "grove_debug_get_perm", "grove_debug_get_fit_row", "grove_debug_get_score_row",
 ]
@@ -166,6 +167,21 @@ class PlacementEngine:
         queues = np.ascontiguousarray(queues, dtype=T.queue_dt)
         gang_queue = np.ascontiguousarray(gang_queue, dtype=np.uint32)
         self._check(self.lib.grove_set_queues(self.h, _p(queues), C.c_uint32(len(queues)), _p(gang_queue), C.c_uint32(len(gang_queue))))
+
+    def set_binpack(self, levels):
+        """grove_set_binpack: the pack level of every submitted gang (tables.LEVEL_NONE = not a member; at or below the gang's
+        Required level).  A member's anchor becomes the first node of the fullest level-b domain that holds it on the table the
+        cycle starts from, so its search starts there; binpack_picks() reports the picks.  Call after submit_gangs; the next
+        submit / load_nodes clears it (include/grove_place.h "bin-packing")."""
+        levels = np.ascontiguousarray(levels, dtype=np.uint8)
+        self._check(self.lib.grove_set_binpack(self.h, _p(levels), C.c_uint32(len(levels))))
+
+    def binpack_picks(self) -> np.ndarray:
+        """caller index of the first node of each gang's pick in the last cycle that ran with a set_binpack set (tables.NONE_U32:
+        not a member, or no domain qualified)"""
+        out = np.zeros(max(self.G, 1), dtype=np.uint32)
+        self._check(self.lib.grove_get_binpack_picks(self.h, _p(out), C.c_uint32(len(out))))
+        return out[: self.G]
 
     # ---- the cycle ----
     def run_cycle(self) -> dict:

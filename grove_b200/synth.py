@@ -216,6 +216,15 @@ def c4_spread_groups(gangs, cliques, size=8, level=0, mode=T.SPREAD_HARD, max_sk
     return groups, gang_group
 
 
+def binpack_levels(gangs, level=None):
+    """Pack levels for grove_set_binpack over a C4-style submission: every gang is a member, at its Required level, or at `level`
+    when that is deeper (a gang without a Required level packs at `level`, and is no member when `level` is None)."""
+    req = gangs["level"].astype(np.int64)
+    if level is None:
+        return np.where(req == T.LEVEL_NONE, T.LEVEL_NONE, req).astype(np.uint8)
+    return np.where(req == T.LEVEL_NONE, level, np.maximum(req, level)).astype(np.uint8)
+
+
 def config_c4_large(n=50000, g=10000, n_large=24, seed=SEED_BASE + 44, max_used_pct=90):
     """C4 (config_c4) plus `n_large` PodGangs of 256-2048 pods, for grove_submit_gangs_wide: a leader (Required host) and a
     worker PodGroup of 255-2047 one-GPU pods under a Required zone with a Preferred block, priorities drawn from C4's three

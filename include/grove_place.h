@@ -407,6 +407,30 @@ int32_t grove_set_spread(grove_engine_t* e, const grove_spread_t* groups, uint32
 #define GROVE_STATUS_FENCING 0x4u       /* grove_gang_status_t.reserved0: a REJECTED gang whose fence held at the end of the cycle */
 int32_t grove_set_fences(grove_engine_t* e, const uint32_t* gangs, uint32_t n);
 
+/* ---- bin-packing ---------------------------------------------------------------------------------------
+ * A member starts its search at the fullest domain that can hold it, so that empty domains stay empty for large gangs (DESIGN.md
+ * section 1, "Bin-packing"; KAI-Scheduler's default bin-pack placement).  level_of[g] is the pack level b of submitted gang g, or
+ * GROVE_LEVEL_NONE when g is not a member; b < n_levels, and b is the gang's Required level or deeper when it has one.
+ *   Picks, on F0 (the table the cycle starts from), for every member on its own: the candidates are the level-b domains (nodes
+ *   lacking the label are in none); S_D = the 64-bit sums of free cpu, mem, gpu and pods over the SCHEDULABLE nodes of D.  D qualifies
+ *   when every clique q with MinReplicas m_q > 0 has sum over n in D of cap(q, n) >= m_q (grove_diagnose's exact capacity, 0 where
+ *   K1 fit fails), and sum over q of m_q * request_q <= S_D for cpu, mem and gpu, and sum of m_q <= S_D.pods.  The pick is the
+ *   qualifying D of least (S_D.gpu, S_D.cpu, S_D.mem, first node in topology order); none: the member keeps its default anchor.
+ *   The cycle: the cycle that would run otherwise (grove_run_cycle, or the queue cycle with a queue set), with each picked member's
+ *   anchor_node replaced by the caller index of its pick's first node.  Nothing else changes.
+ * grove_get_binpack_picks: per gang of the last cycle that ran with a set, the caller index of the first node of its pick, or
+ * GROVE_NONE_U32 (not a member, or no qualifying domain); GROVE_ERR_STATE before such a cycle.
+ * Call after grove_submit_gangs and before the cycle; the next grove_submit_gangs* or grove_load_nodes* clears the set,
+ * grove_update_nodes keeps it (the picks are made again each cycle).  A set without members changes nothing.  GROVE_ERR_INVALID_ARG
+ * for a wrong n_gangs, b >= n_levels, or b above the gang's Required level; GROVE_ERR_LIMIT for a wide submission; GROVE_ERR_STATE
+ * before nodes are loaded and gangs submitted.  While a set with members is in place grove_run_cycle_preempt / _reuse /
+ * _reuse_preempt / _preempt_queues / _consolidate return GROVE_ERR_STATE, and so does grove_run_cycle with a spread set with
+ * members or a fence set.  grove_diagnose accepts a bin-packing cycle; grove_build_score_matrix scores against the anchors the
+ * last cycle used.  Members that share a pick depend on one another, so a cycle with members relaxes at most 128 gangs at a time
+ * unless grove_config_t.window says otherwise (DESIGN.md section 1, "Bin-packing": the measured cost). */
+int32_t grove_set_binpack(grove_engine_t* e, const uint8_t* level_of, uint32_t n_gangs);
+int32_t grove_get_binpack_picks(grove_engine_t* e, uint32_t* out, uint32_t cap);
+
 /* ---- consolidation ------------------------------------------------------------------------------------
  * Running gangs are relocated so that a blocked gang fits, and only when every relocated gang finds a new place (DESIGN.md
  * section 1, "Consolidation"; after KAI-Scheduler's consolidation action).  Running gangs and holdings are as for

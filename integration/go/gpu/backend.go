@@ -66,6 +66,8 @@ type schedulerBackend struct {
 	setOf  map[string]string
 	// starvation guard (SetStarvationGuard): off while guardMax == 0; rejectedFor: pending PodGang -> consecutive Unschedulable cycles
 	guardAfter, guardMax int
+	// bin-packing (SetBinPacking): the level key every PodGang of an ordinary or queue pass packs at; off while empty
+	binpackKey string
 	rejectedFor          map[string]int
 	// consolidation (SetConsolidation): off while consMax == 0; specOf: scheduled PodGang -> its spec (restated as a gated row to
 	// make it movable); moveAnchor: moved PodGang -> the first node of the placement the cycle planned for it
@@ -505,6 +507,17 @@ func (b *schedulerBackend) SetStarvationGuard(afterCycles, maxGangs int) error {
 	return nil
 }
 
+// SetBinPacking makes every PodGang of an ordinary or queue pass start its search at the fullest domain of the level `levelKey`
+// (or of its own Required level when that is deeper) that can hold it on the cycle's node table, so that empty domains stay empty
+// for large PodGangs (grove_set_binpack; GpuBackend::SetBinPacking in the C++ mirror).  A preference, not a constraint: a pass with
+// preemption, consolidation, topology spread members, fences or a large PodGang runs without it, and so does every pass while the
+// key names no level of the topology.  An empty key (the default) turns it off.
+func (b *schedulerBackend) SetBinPacking(levelKey string) {
+	b.mu.Lock()
+	defer b.mu.Unlock()
+	b.binpackKey = levelKey
+}
+
 // SetConsolidation makes, each cycle, the <= maxTargets highest-ranked pending PodGangs that came back Unschedulable at least
 // afterCycles cycles in a row (counted as the starvation guard counts) targets of grove_run_cycle_consolidate: running PodGangs
 // this backend scheduled, restated as gated rows, are relocated out of the domain closest to fitting a target when every one of
@@ -794,6 +807,17 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 		}
 		if len(moved) == 0 {
 			t.targets = nil
+		}
+	}
+	// bin-packing: every row a member, at the key's level or its own Required level when deeper, in an ordinary or queue pass
+	if lv := levelIndex(levels, &b.binpackKey); b.binpackKey != "" && lv != C.GROVE_LEVEL_NONE && !preempt && !wideAny &&
+		len(t.spreadGroups) == 0 && len(t.fences) == 0 && len(t.targets) == 0 {
+		t.binpack = make([]C.uint8_t, len(t.gangs))
+		for gi := range t.gangs {
+			t.binpack[gi] = lv
+			if req := t.gangs[gi].level; req != C.GROVE_LEVEL_NONE && req > lv {
+				t.binpack[gi] = req
+			}
 		}
 	}
 	if queuesOn && queueWhy == "" {

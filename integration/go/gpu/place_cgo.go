@@ -62,6 +62,8 @@ type tables struct {
 	spreadSeeds  []C.grove_spread_seed_t
 	// fences (optional; ordinary passes only): the gang rows the starvation guard fences (grove_set_fences)
 	fences []C.uint32_t
+	// bin-packing (optional; ordinary and queue passes only): each gang row's pack level (grove_set_binpack)
+	binpack []C.uint8_t
 	// queue limits (optional; ordinary passes only): the queues, parents first, each gang row's queue (GROVE_NONE_U32 = none) and
 	// the queue names in table order (grove_set_queues)
 	queues     []C.grove_queue_t
@@ -119,6 +121,11 @@ func (e *engine) cycle(t *tables, preempt, large, explain bool) (*result, error)
 	}
 	if len(t.fences) > 0 {
 		if err := e.err(C.grove_set_fences(e.h, &t.fences[0], C.uint32_t(len(t.fences)))); err != nil {
+			return nil, err
+		}
+	}
+	if len(t.binpack) > 0 {
+		if err := e.err(C.grove_set_binpack(e.h, &t.binpack[0], C.uint32_t(len(t.binpack)))); err != nil {
 			return nil, err
 		}
 	}
