@@ -1,6 +1,7 @@
 // admit.cuh -- K3: evaluation of one gang against its view of the cluster (warp-cooperative packing).
 #pragma once
 #include "common.cuh"
+#include "imex.cuh"
 
 #ifdef GROVE_INLINE_ALL
 #define GROVE_NI __forceinline__
@@ -169,7 +170,8 @@ __device__ __forceinline__ uint32_t visit_pos(const GangRegs& g, uint32_t n) {
 
 // ---- the evaluator: the whole warp packs ONE candidate range ------------------------------------------
 // kFence: the nodes of the fences active for the gang (fm0 / fm1, common.cuh fenced) take no pod
-template <bool kPref_, bool kHolds, bool kWide_ = false, bool kFence = false>
+// kImex: the nodes another CD holds in the gang's view (imex.cuh imex_foreign) take no pod of its enrolled cliques (enr)
+template <bool kPref_, bool kHolds, bool kWide_ = false, bool kFence = false, bool kImex = false>
 struct Ev {
   static constexpr bool kPref = kPref_;
   static constexpr bool kWide = kWide_;
@@ -177,6 +179,7 @@ struct Ev {
   const Topo& tp; const Relax& rb; GangShared& sh; const GangRegs& g; uint32_t lane;
   uint32_t np;
   uint32_t fm0 = 0, fm1 = 0;   // (kFence) the active fences
+  uint32_t enr = 0, icd = GROVE_CD_NONE;   // (kImex) bit cr set for every enrolled clique; the gang's CD
   uint32_t tmask = 0;   // bit (n & 31) set for every node the gang has put a pod on: quick 'untouched' test
   uint32_t ext = 0;     // see the file comment
   uint32_t t_stage = 0, t_pre = 0, t_pack = 0, n_stage = 0;
@@ -211,6 +214,7 @@ struct Ev {
   // pods of clique cr that still fit on node n under the gang's view, after what the gang itself put there (kWide: o, from own_word)
   __device__ __forceinline__ uint32_t cap_view(uint32_t cr, uint32_t n, int4 o = int4{}) const {
     if constexpr (kFence) if (fenced(rb.fc, fm0, fm1, n)) return 0u;
+    if constexpr (kImex) if (((enr >> cr) & 1u) && imex_foreign(rb, icd, g.rank, n)) return 0u;
     const uint32_t live = (__ldg(rb.nlive + (n >> 2)) >> ((n & 3u) * 8u)) & 0xFFu;
     const bool own = (tmask >> (n & 31u)) & 1u;
     if (!live && !own) {
@@ -230,13 +234,13 @@ struct Ev {
 #pragma unroll
           for (uint32_t s = 0; s < kClaimSlots; ++s) {
             const uint4 c = __ldg(line + s);
-            if (gives_back<kHolds>(c.x, g.rank)) { cpu += int(c.y); mem += int(c.z); gpu += int(c.w & 0xFFFFu); pods += int(c.w >> 16); }
+            if (gives_back<kHolds, kImex>(c.x, g.rank)) { cpu += int(c.y); mem += int(c.z); gpu += int(c.w & 0xFFFFu); pods += int(c.w >> 16); }
           }
         }
         if (live & kHasOvf) {
           for (uint32_t i = __ldg(rb.ovf_head + n); i; i = __ldg(rb.ovf_next + i - 1)) {
             const uint4 c = __ldg(rb.ovf_claim + i - 1);
-            if (gives_back<kHolds>(c.x, g.rank)) { cpu += int(c.y); mem += int(c.z); gpu += int(c.w & 0xFFFFu); pods += int(c.w >> 16); }
+            if (gives_back<kHolds, kImex>(c.x, g.rank)) { cpu += int(c.y); mem += int(c.z); gpu += int(c.w & 0xFFFFu); pods += int(c.w >> 16); }
           }
         }
       }
@@ -354,7 +358,7 @@ struct Ev {
 // instead of a chain of dependent L2 look-ups per 32 nodes.
 constexpr uint32_t kStageMax = 128;
 
-template <bool kPref_, bool kHolds, bool kWide_ = false, bool kFence = false>
+template <bool kPref_, bool kHolds, bool kWide_ = false, bool kFence = false, bool kImex = false>
 struct EvS {
   static constexpr bool kPref = kPref_;
   static constexpr bool kWide = kWide_;
@@ -370,6 +374,7 @@ struct EvS {
   uint32_t vlo = 0, vhi = 0;
   uint32_t np;
   uint32_t fm0 = 0, fm1 = 0;   // (kFence) the active fences: their nodes are staged unschedulable
+  uint32_t enr = 0, icd = GROVE_CD_NONE;   // (kImex) the enrolled cliques and the gang's CD: foreign nodes are staged kForeignFlag
   uint32_t tmask = 0;
   uint32_t ext = 0;
   // the entry stack: shared memory, or (kWide) the warp's own stack in global memory
@@ -390,6 +395,7 @@ struct EvS {
     __syncwarp();
     constexpr uint32_t kPer = kStageMax / 32;
     uint4 r[kPer]; int4 t[kPer]; uint32_t live[kPer], mr[kPer];
+    uint32_t io[kPer], ine[kPer];   // (kImex) the node's committed owner and enrolled claims, asked for with its record
 #pragma unroll
     for (uint32_t k = 0; k < kPer; ++k) {
       const uint32_t n = dl + k * 32u + lane;
@@ -398,6 +404,7 @@ struct EvS {
       t[k] = in ? __ldg(rb.ctot + n) : make_int4(0, 0, 0, 0);
       mr[k] = in ? __ldg(rb.cmaxr + n) : 0u;
       live[k] = in ? (__ldg(rb.nlive + (n >> 2)) >> ((n & 3u) * 8u)) & 0x7Fu : 0u;
+      if constexpr (kImex) { io[k] = in && enr ? __ldg(rb.im.owner + n) : GROVE_CD_NONE; ine[k] = in && enr ? __ldg(rb.im.nenr + n) : 0u; }
     }
     const long long tc0 = rb.dbg ? clock64() : 0;
 #pragma unroll
@@ -412,18 +419,19 @@ struct EvS {
           for (uint32_t s = 0; s < kClaimSlots; ++s) c[s] = __ldg(line + s);
 #pragma unroll
           for (uint32_t s = 0; s < kClaimSlots; ++s)
-            if (gives_back<kHolds>(c[s].x, g.rank)) { cpu += int(c[s].y); mem += int(c[s].z); gpu += int(c[s].w & 0xFFFFu); pods += int(c[s].w >> 16); }
+            if (gives_back<kHolds, kImex>(c[s].x, g.rank)) { cpu += int(c[s].y); mem += int(c[s].z); gpu += int(c[s].w & 0xFFFFu); pods += int(c[s].w >> 16); }
         }
         if (live[k] & kHasOvf) {
           for (uint32_t i = __ldg(rb.ovf_head + n); i; i = __ldg(rb.ovf_next + i - 1)) {
             const uint4 c = __ldg(rb.ovf_claim + i - 1);
-            if (gives_back<kHolds>(c.x, g.rank)) { cpu += int(c.y); mem += int(c.z); gpu += int(c.w & 0xFFFFu); pods += int(c.w >> 16); }
+            if (gives_back<kHolds, kImex>(c.x, g.rank)) { cpu += int(c.y); mem += int(c.z); gpu += int(c.w & 0xFFFFu); pods += int(c.w >> 16); }
           }
         }
       }
       view[k * 32u + lane] = make_int4(cpu, mem, gpu, pods);
       uint32_t f = r[k].w;
       if constexpr (kFence) if (n < dh && fenced(rb.fc, fm0, fm1, n)) f &= ~uint32_t(GROVE_NODE_SCHEDULABLE);
+      if constexpr (kImex) if (enr && n < dh && imex_foreign(rb, icd, g.rank, n, io[k], ine[k])) f |= kForeignFlag;   // (the CD is the gang's: once per attempt)
       vflag[k * 32u + lane] = f;
     }
     __syncwarp();
@@ -436,7 +444,8 @@ struct EvS {
     const int4 v = view[n - vlo];
     const uint32_t f = vflag[n - vlo];
     const uint32_t sm = sh.smask[cr];
-    const bool usable = (f & GROVE_NODE_SCHEDULABLE) && ((sm >> ((f >> GROVE_NODE_CLASS_SHIFT) & 0xFu)) & 1u) && ((f >> 16) & 0xFu) >= (sm >> 16);
+    bool usable = (f & GROVE_NODE_SCHEDULABLE) && ((sm >> ((f >> GROVE_NODE_CLASS_SHIFT) & 0xFu)) & 1u) && ((f >> 16) & 0xFu) >= (sm >> 16);
+    if constexpr (kImex) usable = usable && !((f & kForeignFlag) && ((enr >> cr) & 1u));
     const uint32_t c = cap_from_rcp<kWide>(uint32_t(max(v.x, 0)), uint32_t(max(v.y, 0)), uint32_t(max(v.z, 0)), uint32_t(max(v.w, 0)), sh.clq[cr], sh.rcp[cr]);
     return usable ? c : 0u;
   }
@@ -853,7 +862,9 @@ constexpr int kEvalWarps = 8;
 // shape bits come from the committed table and stay upper bounds.
 // kQueue: the instantiation of a cycle with queue members (queue.cuh): a member whose gate is closed is REJECTED without evaluation,
 // and an admitted member packs each clique's surplus up to the replicas k_queue_gate allows.
-template <bool kPref, bool kHolds, bool kWide, bool kSpread = false, bool kFence = false, bool kQueue = false>
+// kImex: the instantiation of a cycle with enrolled cliques (imex.cuh): a node another CD holds in the gang's view fails K1 fit for
+// the gang's enrolled cliques wherever a view is formed, like a fenced node.  Tables and shape bits stay ownership-blind upper bounds.
+template <bool kPref, bool kHolds, bool kWide, bool kSpread = false, bool kFence = false, bool kQueue = false, bool kImex = false>
 __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb, Relax rx, uint32_t max_att) {
   __shared__ GangShared shs[kEvalWarps];
   __shared__ int4 s_view[kEvalWarps][kStageMax];
@@ -950,14 +961,18 @@ __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb,
     // shrink otherwise (claims are added, settled claims move into the committed state).  So a re-evaluation skips the
     // candidates in front of its last answer that no withdrawal touched -- gangs that meet a nearly full cluster would
     // otherwise re-run dozens of failing attempts every round.  (Single candidate level only.)
-    Ev<kPref, kHolds, kWide, kFence> ev(tp, rx, sh, g, lane);                         // candidates of any size, node state from L2
-    EvS<kPref, kHolds, kWide, kFence> evs(tp, rx, sh, g, lane, s_view[warp], s_vflag[warp], s_rk[warp]);         // candidates of <= kStageMax nodes, node state staged in shared memory
+    Ev<kPref, kHolds, kWide, kFence, kImex> ev(tp, rx, sh, g, lane);                  // candidates of any size, node state from L2
+    EvS<kPref, kHolds, kWide, kFence, kImex> evs(tp, rx, sh, g, lane, s_view[warp], s_vflag[warp], s_rk[warp]);         // candidates of <= kStageMax nodes, node state staged in shared memory
     if constexpr (kWide) { ev.wn = evs.wn = wide_node; ev.wm = evs.wm = wide_meta; }
     if constexpr (kFence) {   // the fences active for this gang: a lane per entry (at most 64), fixed for the round (k_apply writes tstate)
       bool a0 = false, a1 = false;
       if (lane < rx.fc.n) { const uint4 f = rx.fc.list[lane]; a0 = f.x != kFull && f.z < g.rank && rx.tstate[f.w] == GROVE_GANG_REJECTED; }
       if (lane + 32u < rx.fc.n) { const uint4 f = rx.fc.list[lane + 32u]; a1 = f.x != kFull && f.z < g.rank && rx.tstate[f.w] == GROVE_GANG_REJECTED; }
       ev.fm0 = evs.fm0 = __ballot_sync(kFull, a0); ev.fm1 = evs.fm1 = __ballot_sync(kFull, a1);
+    }
+    if constexpr (kImex) {   // the enrolled cliques (a lane each) and the gang's CD, fixed for the cycle
+      ev.enr = evs.enr = __ballot_sync(kFull, has_c && __ldg(rx.im.cd + gg.clique_off + lane) != GROVE_CD_NONE);
+      ev.icd = evs.icd = __ldg(rx.im.rank_cd + g.rank);
     }
     bool staged = false;  // the winning attempt ran on evs
     bool won = false;     // this warp holds the answer

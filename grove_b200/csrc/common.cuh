@@ -17,13 +17,18 @@ constexpr uint32_t kHasOvf = 0x40u;           // nlive8 bit: the node has (had) 
 constexpr uint32_t kTagRounds = 254u;         // rounds per stamp epoch (stamps carry a round tag in their top byte)
 constexpr uint32_t kHold = 1u << 24;          // claim tag bit above the 24 rank bits: the claim is the HOLD of the gang of that rank
                                               // (what the running gang it replaces holds on the node; grove_run_cycle_reuse)
+constexpr uint32_t kEnrolled = 1u << 25;     // claim tag bit (kImex cycles): the claim is a run of an enrolled clique's pods
+constexpr uint32_t kRankBits = 0xFFFFFFu;
 
 // Does the gang of rank `rank` give claim tag x back, i.e. not subtract it from its view?  The claims of the ranks after it, and
 // (kHolds: a cycle with holds) its own hold; every other hold is subtracted by everybody.  Without holds this is the plain rank
-// test: the kernels of an ordinary cycle are instantiated without the hold logic.
-template <bool kHolds>
+// test: the kernels of an ordinary cycle are instantiated without the hold logic.  (kImex: a cycle with ComputeDomains, whose
+// tags may carry kEnrolled; such a cycle has no holds.)
+template <bool kHolds, bool kImex = false>
 __device__ __forceinline__ bool gives_back(uint32_t x, uint32_t rank) {
-  if constexpr (kHolds) return (x >= rank && x < kHold) || x == (rank | kHold);   // (kClaimEmpty has the hold bit set)
+  static_assert(!(kHolds && kImex), "a ComputeDomain cycle has no holds");
+  if constexpr (kImex) return x != kClaimEmpty && (x & kRankBits) >= rank;
+  else if constexpr (kHolds) return (x >= rank && x < kHold) || x == (rank | kHold);   // (kClaimEmpty has the hold bit set)
   else return x >= rank && x != kClaimEmpty;
 }
 
@@ -144,6 +149,15 @@ struct Queue {
   uint32_t n_mem;
 };
 
+// ComputeDomain exclusivity (grove_set_compute_domains; imex.cuh), read only by the kImex instantiations.  The claims of an enrolled
+// clique's runs carry kEnrolled in their tag, and the rank in the tag names the claim's CD through rank_cd.
+struct Imex {
+  const uint32_t* cd;       // [Q] CD of the clique's pods, GROVE_CD_NONE = not enrolled
+  const uint32_t* rank_cd;  // [G] CD of the gang of each rank (GROVE_CD_NONE: it has no enrolled clique)
+  uint32_t* owner;          // [npad] committed holder of the node's IMEX channel: owner0, then the CDs k_fold moves in
+  uint32_t* nenr;           // [npad] live claims tagged kEnrolled on the node (k_apply / k_fold)
+};
+
 // Relaxation state.  A gang's tentative result ("cur") lives in its own slots of the entry arrays and becomes final
 // in place; "nxt" is the scratch an evaluation writes before k_apply compares and publishes it.
 struct Relax {
@@ -213,6 +227,7 @@ struct Relax {
   Spread sp;                // topology spread (the kSpread instantiations of k_eval / k_apply / k_detect)
   Fence fc;                 // fences (the kFence instantiations of k_eval / k_apply)
   Queue qu;                 // queue limits (the kQueue instantiations of k_eval / k_apply)
+  Imex im;                  // ComputeDomain exclusivity (the kImex instantiations of k_eval / k_apply / k_fold)
 };
 
 // Is sorted node n inside a fence that is active for the evaluating gang?  m0 / m1: bit j of the 64 entries of `fc.list` is set

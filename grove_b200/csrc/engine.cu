@@ -238,7 +238,7 @@ struct grove_engine {
   DevBuf<uint8_t> d_rc_gone;
   // grove_diagnose (diagnose.cuh): whether the outputs on the device describe an ordinary cycle over the current inputs, the
   // per-node usage lists, the batch descriptors, the per-domain capacity sums and the records
-  enum Diag : uint8_t { kDiagNoCycle, kDiagReady, kDiagRunning, kDiagChanged, kDiagSpread, kDiagFence } diag = kDiagNoCycle;
+  enum Diag : uint8_t { kDiagNoCycle, kDiagReady, kDiagRunning, kDiagChanged, kDiagSpread, kDiagFence, kDiagImex } diag = kDiagNoCycle;
   DevBuf<uint32_t> d_dg_cnt, d_dg_off, d_dg_cur, d_dg_minr;
   DevBuf<uint4> d_dg_rec;
   DevBuf<DiagGang> d_dg_gang;
@@ -289,6 +289,14 @@ struct grove_engine {
   DevBuf<BpKey> d_bp_key;
   DevBuf<uint32_t> d_bp_idx, d_bp_rank, d_bp_pick;
   DevBuf<uint8_t> d_bp_tmp;
+  // ComputeDomain exclusivity (grove_set_compute_domains; imex.cuh): the CD of every clique and gang of the current submission and
+  // owner0 in caller order; the kImex kernels run only while some clique is enrolled (im_enrolled > 0)
+  std::vector<uint32_t> im_cd, im_gang_cd, im_owner0, im_owners;
+  uint32_t im_enrolled = 0;
+  bool im_given = false;                   // a set was given for the current submission, enrolled cliques or not
+  bool im_have_owners = false;             // im_owners holds the owners after the last cycle that ran with a set
+  std::vector<uint32_t> h_im_rank_cd, h_im_owner;
+  DevBuf<uint32_t> d_im_cd, d_im_rank_cd, d_im_owner, d_im_nenr;
 };
 
 
@@ -316,6 +324,10 @@ static int32_t refuse_queues(grove_engine* e, const char* entry) {
 }
 static int32_t refuse_binpack(grove_engine* e, const char* entry) {
   e->err = std::string(entry) + ": not supported while a bin-packing set with members is in place (grove_set_binpack)";
+  return GROVE_ERR_STATE;
+}
+static int32_t refuse_imex(grove_engine* e, const char* entry) {
+  e->err = std::string(entry) + ": not supported while a ComputeDomain set with an enrolled clique is in place (grove_set_compute_domains)";
   return GROVE_ERR_STATE;
 }
 static int32_t refuse_wide(grove_engine* e, const char* entry) {
@@ -499,6 +511,7 @@ static Relax make_relax(grove_engine* e) {
     qu.q_off = e->d_qu_q_off.p; qu.q_base = e->d_qu_q_base.p; qu.pr = e->d_qu_pr.p; qu.head = e->d_qu_head.p; qu.use = e->d_qu_use.p;
     qu.gate = e->d_qu_gate.p; qu.cap = e->d_qu_cap.p; qu.n_mem = e->qu_members;
   }
+  if (e->im_enrolled) { r.im.cd = e->d_im_cd.p; r.im.rank_cd = e->d_im_rank_cd.p; r.im.owner = e->d_im_owner.p; r.im.nenr = e->d_im_nenr.p; }
   return r;
 }
 
@@ -576,11 +589,13 @@ void grove_engine_destroy(grove_engine_t* e) {
 static int32_t load_nodes_common(grove_engine* e, const grove_node_t* host_nodes, const void* dev_nodes, uint32_t n) {
   if (n == 0 || n > GROVE_MAX_NODES) return fail(e, GROVE_ERR_INVALID_ARG, "node count out of range");
   if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
-  if (e->diag == grove_engine::kDiagReady || e->diag == grove_engine::kDiagSpread || e->diag == grove_engine::kDiagFence) e->diag = grove_engine::kDiagChanged;
+  if (e->diag == grove_engine::kDiagReady || e->diag == grove_engine::kDiagSpread || e->diag == grove_engine::kDiagFence ||
+      e->diag == grove_engine::kDiagImex) e->diag = grove_engine::kDiagChanged;
   e->sp_groups = e->sp_members = 0;   // a spread set belongs to the nodes and gangs it was validated against
   e->fc_gangs.clear();                // (a fence set too)
   e->qu_members = 0; e->qu_given = false;   // (and a queue set)
   e->bp_members = 0; e->bp_given = false;   // (and a bin-packing set)
+  e->im_enrolled = 0; e->im_given = false;  // (and a ComputeDomain set)
   CU_TRY(e, cudaSetDevice(e->cfg.device));
   if (host_nodes) {
     CU_TRY(e, cudaEventSynchronize(e->ev_nodes_up));  // an earlier upload may still be reading the staging buffer
@@ -632,7 +647,8 @@ int32_t grove_update_nodes(grove_engine_t* e, const uint32_t* idx, const grove_n
   if (!e || (n && (!idx || !recs))) return GROVE_ERR_INVALID_ARG;
   if (!e->nodes_loaded) return fail(e, GROVE_ERR_STATE, "no node snapshot loaded");
   if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
-  if (e->diag == grove_engine::kDiagReady || e->diag == grove_engine::kDiagSpread || e->diag == grove_engine::kDiagFence) e->diag = grove_engine::kDiagChanged;
+  if (e->diag == grove_engine::kDiagReady || e->diag == grove_engine::kDiagSpread || e->diag == grove_engine::kDiagFence ||
+      e->diag == grove_engine::kDiagImex) e->diag = grove_engine::kDiagChanged;
   if (n == 0) return GROVE_OK;
   e->score_pass_valid = false;
   CU_TRY(e, cudaSetDevice(e->cfg.device));
@@ -735,12 +751,14 @@ static int32_t validate(grove_engine* e, const grove_gang_t* gangs, uint32_t G, 
 static int32_t submit(grove_engine* e, const grove_gang_t* gangs, uint32_t n_gangs, const grove_clique_t* cliques,
                       const std::vector<uint32_t>& ccount, uint32_t n_cliques, const grove_scope_t* scopes, uint32_t n_scopes, uint32_t max_pods) {
   if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
-  if (e->diag == grove_engine::kDiagReady || e->diag == grove_engine::kDiagSpread || e->diag == grove_engine::kDiagFence) e->diag = grove_engine::kDiagChanged;
+  if (e->diag == grove_engine::kDiagReady || e->diag == grove_engine::kDiagSpread || e->diag == grove_engine::kDiagFence ||
+      e->diag == grove_engine::kDiagImex) e->diag = grove_engine::kDiagChanged;
   if (n_gangs >= (1u << 24)) return fail(e, GROVE_ERR_LIMIT, "too many gangs");  // order rank + round tag share a stamp word
   e->sp_groups = e->sp_members = 0;
   e->fc_gangs.clear();
   e->qu_members = 0; e->qu_given = false;
   e->bp_members = 0; e->bp_given = false;
+  e->im_enrolled = 0; e->im_given = false;
   int32_t rc = validate(e, gangs, n_gangs, cliques, ccount.data(), n_cliques, scopes, n_scopes, max_pods);
   if (rc) return rc;
   CU_TRY(e, cudaSetDevice(e->cfg.device));
@@ -1144,6 +1162,10 @@ static int32_t cycle_begin(grove_engine* e) {
     const size_t nf = e->fc_gangs.size();
     CU_TRY(e, e->d_fc_gang.ensure(nf)); CU_TRY(e, e->d_fc_off.ensure(nf)); CU_TRY(e, e->d_fc_list.ensure(nf)); CU_TRY(e, e->d_fc_slot.ensure(g1));
   }
+  if (e->im_enrolled) {   // the ComputeDomain set's buffers (make_relax hands their pointers to every kernel of the cycle)
+    CU_TRY(e, e->d_im_cd.ensure(std::max<size_t>(Q, 1))); CU_TRY(e, e->d_im_rank_cd.ensure(g1));
+    CU_TRY(e, e->d_im_owner.ensure(N)); CU_TRY(e, e->d_im_nenr.ensure(N));
+  }
   if (e->dbg_on) { CU_TRY(e, e->d_dbg.ensure(g1 * 8 + 8)); CU_TRY(e, cudaMemsetAsync(e->d_dbg.p, 0, g1 * 32 + 32, e->stream)); }
   {
     const uint32_t W = window_of(e);
@@ -1287,6 +1309,16 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
   }
   const bool fences = !e->fc_gangs.empty();   // (the running-gang entries and spread cycles refuse a fence set)
   const bool queues = e->qu_members > 0;   // (the running-gang entries, spread and fenced cycles refuse a queue set)
+  const bool imex = e->im_enrolled > 0;    // (the running-gang entries and the other sets' cycles refuse an enrolled clique)
+  if (G && imex) {   // the CD of every clique and of every rank's gang, owner0 in sorted order (padding: no owner), no enrolled claim
+    e->h_im_rank_cd.resize(G); e->h_im_owner.resize(e->Npad);
+    for (uint32_t g = 0; g < G; ++g) e->h_im_rank_cd[e->ginfo[g].order] = e->im_gang_cd[g];
+    for (uint32_t i = 0; i < e->Npad; ++i) e->h_im_owner[i] = i < e->N ? e->im_owner0[e->perm[i]] : GROVE_CD_NONE;
+    CU_TRY(e, cudaMemcpyAsync(e->d_im_cd.p, e->im_cd.data(), sizeof(uint32_t) * e->Q, cudaMemcpyHostToDevice, e->stream));
+    CU_TRY(e, cudaMemcpyAsync(e->d_im_rank_cd.p, e->h_im_rank_cd.data(), sizeof(uint32_t) * G, cudaMemcpyHostToDevice, e->stream));
+    CU_TRY(e, cudaMemcpyAsync(e->d_im_owner.p, e->h_im_owner.data(), sizeof(uint32_t) * e->Npad, cudaMemcpyHostToDevice, e->stream));
+    CU_TRY(e, cudaMemsetAsync(e->d_im_nenr.p, 0, sizeof(uint32_t) * e->Npad, e->stream));
+  }
   if (G && queues) {   // the members' gates and caps before round 1: no member holds anything yet, H_Q = limit - load
     k_queue_scan<<<e->qu_scanned, 256, 0, e->stream>>>(tb, rx, 0u);
     k_queue_gate<<<(e->qu_members + 255) / 256, 256, 0, e->stream>>>(tb, rx, 0u, nullptr);
@@ -1360,6 +1392,15 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
         ++next_round;
         return GROVE_OK;
       }
+      if (imex) {   // a cycle with enrolled cliques: its own instantiations of K3 and k_apply
+        CU_TRY(e, launch_chained(e->any_preferred ? k_eval<true, false, false, false, false, false, true> : k_eval<false, false, false, false, false, false, true>,
+                                 n_eval_ctas, kEvalWarps * 32, e->stream, tp, tb, rx, e->tune_max_att));
+        CU_TRY(e, launch_chained(k_apply<false, false, false, false, true>, warp_ctas, 256, e->stream, tb, rx));
+        CU_TRY(e, launch_chained(k_detect<false>, warp_ctas, 256, e->stream, tp, tb, rx, e->tune_refresh));
+        e->launches += 3;
+        ++next_round;
+        return GROVE_OK;
+      }
       if (queues) {   // a queue cycle: its own instantiations of K3 and k_apply, then the headroom and the gates before k_detect
         CU_TRY(e, launch_chained(e->any_preferred ? k_eval<true, false, false, false, false, true> : k_eval<false, false, false, false, false, true>,
                                  n_eval_ctas, kEvalWarps * 32, e->stream, tp, tb, rx, e->tune_max_att));
@@ -1384,7 +1425,7 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
       return GROVE_OK;
     };
     auto fold = [&]() -> int32_t {   // the final gangs' claims -> committed state (relax.cuh k_fold)
-      CU_TRY(e, launch_chained(e->holds_on ? k_fold<true> : k_fold<false>, warp_ctas, 256, e->stream, tb, rx, e->d_nres.p));
+      CU_TRY(e, launch_chained(imex ? k_fold<false, true> : e->holds_on ? k_fold<true> : k_fold<false>, warp_ctas, 256, e->stream, tb, rx, e->d_nres.p));
       CU_TRY(e, launch_chained(k_fold_mark, 1, 1, e->stream, rx));
       e->launches += 2;
       CU_TRY(e, cudaGetLastError());
@@ -1458,6 +1499,8 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
       rounds = e->h_ctl.p[kRound] - 1;
     }
     rc = fold(); if (rc) return rc;   // everything is final now: the committed state and the final states of the outputs
+    if (imex)   // the owners after the last fold (read back with the statuses: finish_cycle waits for the copy)
+      CU_TRY(e, cudaMemcpyAsync(e->h_im_owner.data(), e->d_im_owner.p, sizeof(uint32_t) * e->N, cudaMemcpyDeviceToHost, e->stream));
     if (e->holds_on) {   // the admitted owners' leftovers: the running gangs they replace are gone
       k_hold_release<<<(G * 32 + 255) / 256, 256, 0, e->stream>>>(tb, rx, e->d_nres.p);
       CU_TRY(e, cudaGetLastError());
@@ -1484,6 +1527,11 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
     if (e->bp_members)
       for (uint32_t g = 0; g < G; ++g) if (e->h_bp_pick.p[g] != kFull) e->bp_picks[g] = e->perm[e->h_bp_pick.p[g]];
     e->bp_have_picks = true;
+  }
+  if (e->im_given) {   // owner0, plus the CD of every admitted gang's enrolled pods
+    e->im_owners = e->im_owner0;
+    if (imex && G) for (uint32_t i = 0; i < e->N; ++i) e->im_owners[e->perm[i]] = e->h_im_owner[i];
+    e->im_have_owners = true;
   }
   CU_TRY(e, cudaEventRecord(e->ev[9], e->stream));
   CU_TRY(e, cudaEventSynchronize(e->ev[9]));
@@ -1522,8 +1570,12 @@ int32_t grove_run_cycle(grove_engine_t* e, grove_cycle_stats_t* stats) {
     return fail(e, GROVE_ERR_STATE, "grove_run_cycle: a queue set with members together with a spread set with members or a fence set is not supported");
   if (e->bp_members && (spread || fences))
     return fail(e, GROVE_ERR_STATE, "grove_run_cycle: a bin-packing set with members together with a spread set with members or a fence set is not supported");
+  if (e->im_enrolled && (spread || fences || e->qu_members || e->bp_members))
+    return fail(e, GROVE_ERR_STATE, "grove_run_cycle: a ComputeDomain set with an enrolled clique together with a spread set with members, a fence set, "
+                                    "a queue set with members or a bin-packing set with members is not supported");
   const int32_t rc = run_cycle(e, stats);
-  if (rc == GROVE_OK) e->diag = spread ? grove_engine::kDiagSpread : fences ? grove_engine::kDiagFence : grove_engine::kDiagReady;
+  if (rc == GROVE_OK)
+    e->diag = spread ? grove_engine::kDiagSpread : fences ? grove_engine::kDiagFence : e->im_enrolled ? grove_engine::kDiagImex : grove_engine::kDiagReady;
   return rc;
 }
 
@@ -1718,6 +1770,46 @@ int32_t grove_get_binpack_picks(grove_engine_t* e, uint32_t* out, uint32_t cap) 
 }
 
 // ---------------------------------------------------------------------------------------------
+// ComputeDomain exclusivity (include/grove_place.h "ComputeDomain exclusivity"; DESIGN.md section 1; imex.cuh).  Validated against
+// the submission and the node table; the cycle uploads the set and runs the kImex instantiations.
+// ---------------------------------------------------------------------------------------------
+int32_t grove_set_compute_domains(grove_engine_t* e, const uint32_t* cd, uint32_t n_cliques, const uint32_t* owner0, uint32_t n_nodes) {
+  if (!e) return GROVE_ERR_INVALID_ARG;
+  if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
+  if (!e->nodes_loaded || !e->gangs_loaded) return fail(e, GROVE_ERR_STATE, "grove_set_compute_domains: load nodes and submit gangs first");
+  if (n_cliques != e->Q) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_compute_domains: n_cliques is not the number of cliques submitted");
+  if (n_nodes != e->N) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_compute_domains: n_nodes is not the number of nodes loaded");
+  if ((n_cliques && !cd) || !owner0) return GROVE_ERR_INVALID_ARG;
+  if (e->wide) return refuse_wide(e, "grove_set_compute_domains");
+  std::vector<uint32_t> gang_cd(e->G, GROVE_CD_NONE);
+  uint32_t enrolled = 0;
+  for (uint32_t g = 0; g < e->G; ++g) {
+    const grove_gang_t& gg = e->gangs[g];
+    for (uint32_t c = 0; c < gg.n_cliques; ++c) {
+      const uint32_t q = gg.clique_off + c, v = cd[q];
+      if (v == GROVE_CD_NONE) continue;
+      if (v == GROVE_CD_NO_IMEX) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_compute_domains: GROVE_CD_NO_IMEX is not a clique's CD");
+      if (e->cliques[q].req_gpu == 0) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_compute_domains: an enrolled clique requests no GPU");
+      if (gang_cd[g] != GROVE_CD_NONE && gang_cd[g] != v)
+        return fail(e, GROVE_ERR_LIMIT, "grove_set_compute_domains: the enrolled cliques of one gang name two CDs");
+      gang_cd[g] = v;
+      ++enrolled;
+    }
+  }
+  e->im_cd.assign(cd, cd + n_cliques); e->im_gang_cd = std::move(gang_cd); e->im_owner0.assign(owner0, owner0 + n_nodes);
+  e->im_enrolled = enrolled; e->im_given = true;
+  return GROVE_OK;
+}
+
+int32_t grove_get_compute_domain_owners(grove_engine_t* e, uint32_t* out, uint32_t cap) {
+  if (!e || !out) return GROVE_ERR_INVALID_ARG;
+  if (!e->im_have_owners) return fail(e, GROVE_ERR_STATE, "grove_get_compute_domain_owners: no cycle has run with a ComputeDomain set");
+  if (cap < e->im_owners.size()) return fail(e, GROVE_ERR_LIMIT, "output buffer too small");
+  std::copy(e->im_owners.begin(), e->im_owners.end(), out);
+  return GROVE_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
 // Queue limits (include/grove_place.h "queue limits"; DESIGN.md section 1; kernels in queue.cuh).  Validated against the submission;
 // the tables the kernels read are built here once: the members in rank order with their chains and R_min, the queues with a
 // finite limit with limit - load, and the (queue, member) pairs sorted by (queue, rank).
@@ -1856,6 +1948,8 @@ int32_t grove_diagnose(grove_engine_t* e, grove_gang_diag_t* gangs, uint32_t cap
       return fail(e, GROVE_ERR_STATE, "grove_diagnose: the last cycle had topology spread members, which the diagnosis does not model");
     case grove_engine::kDiagFence:
       return fail(e, GROVE_ERR_STATE, "grove_diagnose: the last cycle had fences, which the diagnosis does not model");
+    case grove_engine::kDiagImex:
+      return fail(e, GROVE_ERR_STATE, "grove_diagnose: the last cycle had enrolled cliques (ComputeDomains), which the diagnosis does not model");
     default: return fail(e, GROVE_ERR_STATE, "grove_diagnose: nodes or gangs were loaded, updated or submitted since the last cycle");
   }
   const uint32_t G = e->G, Q = e->Q;
@@ -2274,6 +2368,7 @@ int32_t grove_run_cycle_reuse(grove_engine_t* e, const uint32_t* replaces, uint3
   if (e->qu_members) return refuse_queues(e, "grove_run_cycle_reuse");
   if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_reuse");
   if (e->bp_members) return refuse_binpack(e, "grove_run_cycle_reuse");
+  if (e->im_enrolled) return refuse_imex(e, "grove_run_cycle_reuse");
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse");
   const int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);
@@ -2546,6 +2641,7 @@ int32_t grove_run_cycle_preempt(grove_engine_t* e, const grove_running_gang_t* r
   if (e->qu_members) return refuse_queues(e, "grove_run_cycle_preempt");
   if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_preempt");
   if (e->bp_members) return refuse_binpack(e, "grove_run_cycle_preempt");
+  if (e->im_enrolled) return refuse_imex(e, "grove_run_cycle_preempt");
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_preempt");
   int32_t rc = check_ready(e);
@@ -2562,6 +2658,7 @@ int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replace
   if (e->qu_members) return refuse_queues(e, "grove_run_cycle_reuse_preempt");
   if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_reuse_preempt");
   if (e->bp_members) return refuse_binpack(e, "grove_run_cycle_reuse_preempt");
+  if (e->im_enrolled) return refuse_imex(e, "grove_run_cycle_reuse_preempt");
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse_preempt");
   const int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);
@@ -2577,6 +2674,7 @@ int32_t grove_run_cycle_preempt_queues(grove_engine_t* e, const grove_running_ga
   if (e->sp_members) return refuse_spread(e, kEntry);
   if (!e->fc_gangs.empty()) return refuse_fences(e, kEntry);
   if (e->bp_members) return refuse_binpack(e, kEntry);
+  if (e->im_enrolled) return refuse_imex(e, kEntry);
   if (!e->qu_given) return fail(e, GROVE_ERR_STATE, "grove_run_cycle_preempt_queues: no queue set given for the current submission (grove_set_queues)");
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, kEntry);
@@ -2616,6 +2714,7 @@ int32_t grove_run_cycle_consolidate(grove_engine_t* e, const uint32_t* targets, 
   if (e->qu_members) return refuse_queues(e, "grove_run_cycle_consolidate");
   if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_consolidate");
   if (e->bp_members) return refuse_binpack(e, "grove_run_cycle_consolidate");
+  if (e->im_enrolled) return refuse_imex(e, "grove_run_cycle_consolidate");
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_consolidate");
   if (n_targets > GROVE_MAX_CONSOLIDATE_TARGETS) return fail(e, GROVE_ERR_LIMIT, "grove_run_cycle_consolidate: more than GROVE_MAX_CONSOLIDATE_TARGETS targets");

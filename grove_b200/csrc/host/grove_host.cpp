@@ -466,6 +466,41 @@ Err GpuBackend::EncodeLocked(const std::vector<Node>& nodes, Tables* out, const 
       for (const auto& kv : pending_)
         if (!out->skipped.count(kv.first) && !queueOfPg(kv.second).empty()) out->skipped[kv.first] = why;
   }
+  // ComputeDomain exclusivity: one ComputeDomain per PodGang, and only in a pass that can take the set (grove_set_compute_domains
+  // is refused with the running-gang entries, the other sets' members and wide submissions): otherwise the enrolled PodGangs stay out
+  if (imex_) {
+    auto cdOf = [](const PodGang& pg, bool* two) {   // the ComputeDomain of its enrolled PodGroups ("" = none)
+      std::string cd; *two = false;
+      for (const auto& grp : pg.Spec.PodGroups) {
+        auto it = pg.PodGroupRequests.find(grp.Name);
+        if (it == pg.PodGroupRequests.end() || it->second.ComputeDomain.empty() || !it->second.gpu) continue;
+        if (!cd.empty() && cd != it->second.ComputeDomain) *two = true;
+        cd = it->second.ComputeDomain;
+      }
+      return cd;
+    };
+    bool wideAny = false, spreadAny = false, queueAny = false;
+    for (const auto& kv : pending_) {
+      if (out->skipped.count(kv.first)) continue;
+      wideAny |= large_ && !WhyNotEncodable(kv.second, false).empty();
+      spreadAny |= spreadSetOf(kv.second) != nullptr;
+      queueAny |= !queueOfPg(kv.second).empty();
+    }
+    const char* why = runningCycles ? "ComputeDomain exclusivity is not applied while preemption or reservation reuse is on"
+                      : consMax_ ? "ComputeDomain exclusivity is not applied while consolidation is on"
+                      : guardMax_ ? "ComputeDomain exclusivity is not applied while the starvation guard is on"
+                      : !binpackKey_.empty() ? "ComputeDomain exclusivity is not applied while bin-packing is on"
+                      : spreadAny ? "ComputeDomain exclusivity is not applied in a pass with topology spread members"
+                      : queueAny ? "ComputeDomain exclusivity is not applied in a pass with queue members"
+                      : wideAny ? "ComputeDomain exclusivity is not applied in a pass with PodGangs beyond the ordinary limits" : nullptr;
+    for (const auto& kv : pending_) {
+      if (out->skipped.count(kv.first)) continue;
+      bool two = false;
+      const std::string cd = cdOf(kv.second, &two);
+      if (two) out->skipped[kv.first] = "the PodGroups of this PodGang name two ComputeDomains (MNNVL groups); one per PodGang is supported";
+      else if (!cd.empty() && why) out->skipped[kv.first] = why;
+    }
+  }
   for (const auto& kv : pending_)
     if (!out->skipped.count(kv.first) && !kv.second.BasePodGangName.empty() && out->skipped.count(kv.second.Namespace + "/" + kv.second.BasePodGangName))
       out->skipped[kv.first] = "base PodGang " + kv.second.BasePodGangName + " cannot be scheduled: " + out->skipped[kv.second.Namespace + "/" + kv.second.BasePodGangName];
@@ -802,6 +837,43 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
       if (auto e = chk(grove_set_binpack(engine_, packAt.data(), uint32_t(packAt.size())), "grove_set_binpack")) return e;
     }
   }
+  // ComputeDomain exclusivity (Encode left enrolled rows only in a pass that takes the set): the ComputeDomain of every enrolled
+  // clique row, and every node's holder -- the one observed, else the one of the enrolled pods this backend bound there for a
+  // PodGang that still runs
+  std::vector<std::string> cdName;   // clique row -> its ComputeDomain ("" = not enrolled)
+  bool imexOn = false;
+  { std::lock_guard<std::mutex> l(mu_); imexOn = imex_; }
+  if (imexOn && !both && !reuse && !preempt && !consolidate) {
+    cdName.assign(t.cliques.size(), std::string());
+    bool any = false;
+    for (uint32_t q = 0; q < t.cliques.size(); ++q) {
+      const auto [grow, pgi] = t.cliqueOf[q];
+      if (grow >= t.specRow || !t.cliques[q].req_gpu) continue;
+      const PodGang& pg = snap.at(t.gangNames[grow]);
+      auto it = pg.PodGroupRequests.find(pg.Spec.PodGroups[pgi].Name);
+      if (it != pg.PodGroupRequests.end() && !it->second.ComputeDomain.empty()) { cdName[q] = it->second.ComputeDomain; any = true; }
+    }
+    if (any) {
+      std::map<std::string, uint32_t> ids;
+      auto id = [&ids](const std::string& name) { return ids.emplace(name, uint32_t(ids.size())).first->second; };
+      std::vector<uint32_t> cd(t.cliques.size(), GROVE_CD_NONE), owner0(nodes.size(), GROVE_CD_NONE);
+      for (uint32_t q = 0; q < t.cliques.size(); ++q) if (!cdName[q].empty()) cd[q] = id(cdName[q]);
+      std::map<std::string, std::string> boundBy;   // node -> ComputeDomain of the enrolled pods this backend bound there
+      {
+        std::lock_guard<std::mutex> l(mu_);
+        for (const auto& kv : running_) for (const auto& [node, c] : kv.second.cdOn) boundBy.emplace(node, c);
+      }
+      for (uint32_t n = 0; n < nodes.size(); ++n) {
+        if (!nodes[n].ImexCapable) owner0[n] = GROVE_CD_NO_IMEX;
+        else if (!nodes[n].ComputeDomain.empty()) owner0[n] = id(nodes[n].ComputeDomain);
+        else if (auto it = boundBy.find(nodes[n].Name); it != boundBy.end()) owner0[n] = id(it->second);
+      }
+      if (auto e = chk(grove_set_compute_domains(engine_, cd.data(), uint32_t(cd.size()), owner0.data(), uint32_t(owner0.size())),
+                       "grove_set_compute_domains")) return e;
+    } else {
+      cdName.clear();
+    }
+  }
   if (both) { if (auto e = chk(grove_run_cycle_reuse_preempt(engine_, replaces.data(), uint32_t(replaces.size()), run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_reuse_preempt")) return e; }
   else if (reuse) { if (auto e = chk(grove_run_cycle_reuse(engine_, replaces.data(), uint32_t(replaces.size()), run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_reuse")) return e; }
   else if (preempt && !t.queues.empty()) {   // (Encode keeps queue members in a pass with preemption only with SetPreemptionWithinQueues)
@@ -964,6 +1036,7 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
         auto it = std::find_if(rg.held.begin(), rg.held.end(), [&](const Held& h) { return h.node == nn; });
         if (it == rg.held.end()) { rg.held.push_back(Held{nn}); it = rg.held.end() - 1; }
         it->cpu_milli += q.req_cpu_milli; it->mem_mib += q.req_mem_mib; it->gpu = uint16_t(it->gpu + q.req_gpu); it->pods = uint16_t(it->pods + 1);
+        if (!cdName.empty() && !cdName[e.clique].empty()) rg.cdOn[nn] = cdName[e.clique];   // its IMEX channel, while the PodGang runs
       }
     }
     if (gs[i].n_pods && !lastNode_.count(key)) lastNode_[key] = nodes[pl[gs[i].placement_off].node].Name;

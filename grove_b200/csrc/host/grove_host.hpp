@@ -76,7 +76,12 @@ struct PodGang {
   PodGangSpec Spec;
   PodGangStatus Status;
   // not part of the CRD: what the pod template of each PodGroup requests (a scheduler reads it from the Pods)
-  struct Requests { uint32_t cpu_milli = 0, mem_mib = 0; uint16_t gpu = 0; std::map<std::string, std::string> nodeSelector; std::vector<std::string> tolerationKeys; };
+  struct Requests {
+    uint32_t cpu_milli = 0, mem_mib = 0; uint16_t gpu = 0; std::map<std::string, std::string> nodeSelector; std::vector<std::string> tolerationKeys;
+    // auto-MNNVL: the resourceClaimTemplateName of the pod template's `mnnvl-claim` entry, i.e. the ComputeDomain its pods join;
+    // empty = not enrolled (the operator injects the claim only into GPU containers: a PodGroup without GPUs is never enrolled)
+    std::string ComputeDomain;
+  };
   std::map<std::string, Requests> PodGroupRequests;  // by PodGroup name
   std::string BasePodGangName;                        // scaled PodGang: gated behind this one (syncflow.go:319-358)
   bool Gated = false;                                 // pods still carry grove.io/podgang-pending-creation
@@ -170,6 +175,8 @@ struct Node {   // the slice of corev1.Node + bound Pods a scheduler snapshots; 
   uint32_t used_cpu_milli = 0, used_mem_mib = 0; uint16_t used_gpu = 0, used_pods = 0;
   bool Unschedulable = false;                 // cordon
   std::vector<std::string> TaintKeys;         // NoSchedule taints
+  std::string ComputeDomain;                  // the ComputeDomain whose pods hold the node's IMEX channel, as observed ("" = none seen)
+  bool ImexCapable = true;                    // false: the node runs no IMEX driver (no enrolled pod may land on it)
 };
 
 struct Binding { std::string PodNamespace, PodName, NodeName; };   // Pod.spec.nodeName
@@ -327,6 +334,14 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   // ordinary limits (SetLargePodGangs) the pass runs without it, and so does every pass while the key names no level of the
   // topology.  An empty key (the default) turns it off.
   void SetBinPacking(const std::string& levelKey) { std::lock_guard<std::mutex> l(mu_); binpackKey_ = levelKey; }
+  // ComputeDomain exclusivity (grove_set_compute_domains; DESIGN.md section 1 "ComputeDomain exclusivity"): a node's GPUs take part
+  // in one IMEX channel at a time, so the pods of an enrolled PodGroup (Requests::ComputeDomain) land only on nodes no other
+  // ComputeDomain holds.  A node's holder when the pass starts is Node::ComputeDomain, else the ComputeDomain of the enrolled pods
+  // this backend bound there for a PodGang that still runs; a node that is not ImexCapable takes no enrolled pod.  A PodGang whose
+  // PodGroups name two ComputeDomains stays out of the pass (Unschedulable, with the reason), and so does every enrolled PodGang
+  // while preemption, reservation reuse, consolidation, the starvation guard, bin-packing, topology spread members, queue members
+  // or a PodGang beyond the ordinary limits could be in the pass.  Off (the default): the pass is as before.
+  void SetComputeDomainExclusivity(bool on) { std::lock_guard<std::mutex> l(mu_); imex_ = on; }
   // Consolidation (grove_run_cycle_consolidate; DESIGN.md section 1 "Consolidation"): the spec of every PodGang this backend
   // scheduled is remembered, and each running PodGang it scheduled whole (nothing left pending) is restated as a gated row, which
   // makes it movable.  Each cycle the <= maxTargets highest-ranked pending PodGangs rejected at least afterCycles times in a row
@@ -379,7 +394,8 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   std::map<std::string, std::string> lastNode_;  // scheduled PodGang -> a node it landed on (ReuseReservationRef hint)
   std::map<std::string, std::vector<uint32_t>> bound_;  // scheduled PodGang still pending with unbound pods -> pods bound per PodGroup
   struct Held { std::string node; uint32_t cpu_milli = 0, mem_mib = 0; uint16_t gpu = 0, pods = 0; };
-  struct RunningGang { int32_t priority = 0; std::vector<Held> held; };
+  struct RunningGang { int32_t priority = 0; std::vector<Held> held; std::map<std::string, std::string> cdOn; };   // cdOn: node -> the
+                                                                                                                  // ComputeDomain of its enrolled pods there
   std::map<std::string, RunningGang> running_;   // PodGangs scheduled by this backend and not deleted since
   bool preemption_ = false;
   bool reuse_ = false;
@@ -388,6 +404,7 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   bool large_ = false;
   bool explain_ = false;
   std::string binpackKey_;                             // bin-packing level (off: empty)
+  bool imex_ = false;                                  // ComputeDomain exclusivity
   uint32_t guardAfter_ = 1, guardMax_ = 0;             // starvation guard (off: guardMax_ == 0)
   std::map<std::string, uint32_t> rejectedFor_;        // pending PodGang -> consecutive Unschedulable cycles
   uint32_t consAfter_ = 1, consMax_ = 0;               // consolidation (off: consMax_ == 0)

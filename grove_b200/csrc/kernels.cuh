@@ -15,6 +15,8 @@
 //   queue.cuh    k_queue_scan / k_queue_gate  the headroom, gate and surplus caps of the queue members (grove_set_queues)
 //   binpack.cuh  k_binpack_sum / k_binpack_keys / k_binpack_pick  the fullest domain each bin-packing member is anchored at
 //                (grove_set_binpack)
+//   imex.cuh     imex_foreign  which nodes another ComputeDomain holds in a gang's view (grove_set_compute_domains; the kImex
+//                instantiations of k_eval / k_apply / k_fold)
 //
 // Semantics are DESIGN.md "Placement semantics"; the reference contract they restate is cited in
 // include/grove_place.h.  Integer / compare work only: no tensor cores, no floating point.

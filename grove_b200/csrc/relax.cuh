@@ -207,8 +207,9 @@ __global__ void __launch_bounds__(256) k_hold_release(Tables tb, Relax rx, uint4
 
 // one warp per evaluated gang: publish a changed result (kHolds: a cycle with holds; kSpread: a cycle with spread members, whose
 // changed results leave a stamp per group; kFence: a cycle with fences, whose gangs' flips to or from REJECTED stamp their fence;
-// kQueue: a cycle with queue members, whose changed results record their usage U for k_queue_scan)
-template <bool kHolds, bool kSpread = false, bool kFence = false, bool kQueue = false>
+// kQueue: a cycle with queue members, whose changed results record their usage U for k_queue_scan; kImex: a cycle with enrolled
+// cliques, whose runs' claims carry kEnrolled and are counted per node)
+template <bool kHolds, bool kSpread = false, bool kFence = false, bool kQueue = false, bool kImex = false>
 __global__ void __launch_bounds__(256) k_apply(Tables tb, Relax rx) {
   cudaGridDependencySynchronize();   // (launched chained: engine.cu launch_chained)
   const uint32_t lane = threadIdx.x & 31;
@@ -267,7 +268,9 @@ __global__ void __launch_bounds__(256) k_apply(Tables tb, Relax rx) {
     for (uint32_t i = lane; i < on; i += 32) {
       if (!run_length(rx.ent_node + po, rx.ent_meta + po, i, on)) continue;
       const uint32_t n = rx.ent_node[po + i];
-      claim_remove(rx, n, rank);
+      uint32_t tag = rank;
+      if constexpr (kImex) { tag = imex_tag(rx, gg.clique_off + rx.ent_meta[po + i], rank); if (tag & kEnrolled) atomicSub(rx.im.nenr + n, 1u); }
+      claim_remove(rx, n, tag);
       atomicMin(rx.rem_stamp + (n >> 5), stamp);
       atomicMax(rx.rem_round + (n >> 5), round);
     }
@@ -281,8 +284,10 @@ __global__ void __launch_bounds__(256) k_apply(Tables tb, Relax rx) {
       if (t) {
         const grove_clique_t q = tb.cliques[gg.clique_off + m];
         if constexpr (kQueue) { u0 += uint64_t(t) * q.req_cpu_milli; u1 += uint64_t(t) * q.req_mem_mib; u2 += uint64_t(t) * q.req_gpu; }
+        uint32_t tag = rank;
+        if constexpr (kImex) { tag = imex_tag(rx, gg.clique_off + m, rank); if (tag & kEnrolled) atomicAdd(rx.im.nenr + n, 1u); }
         if (owner) { const uint3 c = owner_claim(tb, rx, g, rx.nxt_node + po, rx.nxt_meta + po, i, t); claim_add(rx, n, rank, c.x, c.y, c.z, rank); }
-        else claim_add(rx, n, rank, t * q.req_cpu_milli, t * q.req_mem_mib, t * uint32_t(q.req_gpu) | (t << 16), rank);
+        else claim_add(rx, n, tag, t * q.req_cpu_milli, t * q.req_mem_mib, t * uint32_t(q.req_gpu) | (t << 16), rank);
         atomicMin(rx.add_stamp + n, stamp);
       }
     }
@@ -394,7 +399,8 @@ __global__ void __launch_bounds__(256) k_detect(Topo tp, Tables tb, Relax rx, ui
 // one warp per gang that became final since the last fold: its claims move into the committed state.  Not every round: the
 // claims of final gangs are as good as committed for everybody who ranks after them, so the fold runs before a capacity-table
 // rebuild (the tables are built from the committed state) and when the cycle ends; k_fold_mark then moves the marker.
-template <bool kHolds>
+// (kImex: an enrolled run's CD becomes the node's committed owner)
+template <bool kHolds, bool kImex = false>
 __global__ void __launch_bounds__(256) k_fold(Tables tb, Relax rx, uint4* nres) {
   cudaGridDependencySynchronize();
   const uint32_t lane = threadIdx.x & 31;
@@ -421,7 +427,12 @@ __global__ void __launch_bounds__(256) k_fold(Tables tb, Relax rx, uint4* nres) 
       if (!len) continue;
       const uint32_t n = rx.ent_node[po + i];
       const grove_clique_t q = tb.cliques[coff + rx.ent_meta[po + i]];
-      claim_remove(rx, n, p);
+      uint32_t tag = p;
+      if constexpr (kImex) {
+        tag = imex_tag(rx, coff + rx.ent_meta[po + i], p);
+        if (tag & kEnrolled) { atomicSub(rx.im.nenr + n, 1u); rx.im.owner[n] = rx.im.cd[coff + rx.ent_meta[po + i]]; }
+      }
+      claim_remove(rx, n, tag);
       uint32_t* r = reinterpret_cast<uint32_t*>(nres + n);
       if (owner) {   // the claim it published (k_apply)
         const uint3 c = owner_claim(tb, rx, g, rx.ent_node + po, rx.ent_meta + po, i, len);

@@ -27,7 +27,7 @@ SYMBOLS = [
     "grove_build_score_matrix", "grove_run_cycle_preempt", "grove_get_victims", "grove_run_cycle_reuse",
     "grove_run_cycle_reuse_preempt", "grove_diagnose", "grove_set_spread", "grove_set_fences", "grove_set_queues",
     "grove_run_cycle_consolidate", "grove_get_moves", "grove_run_cycle_preempt_queues",
-    "grove_set_binpack", "grove_get_binpack_picks",
+    "grove_set_binpack", "grove_get_binpack_picks", "grove_set_compute_domains", "grove_get_compute_domain_owners",
     "grove_shard_range", "grove_run_score_pass", "grove_shard_summary_device",
     "grove_debug_get_perm", "grove_debug_get_fit_row", "grove_debug_get_score_row",
 ]
@@ -182,6 +182,23 @@ class PlacementEngine:
         out = np.zeros(max(self.G, 1), dtype=np.uint32)
         self._check(self.lib.grove_get_binpack_picks(self.h, _p(out), C.c_uint32(len(out))))
         return out[: self.G]
+
+    def set_compute_domains(self, cd, owner0):
+        """grove_set_compute_domains: the ComputeDomain of every submitted clique's pods (tables.CD_NONE = not enrolled) and the
+        CD holding every loaded node's IMEX channel when the cycle starts (tables.CD_NONE, or tables.CD_NO_IMEX for a node
+        without an IMEX driver).  An enrolled clique's pods land only on nodes that no other CD holds at its gang's turn;
+        compute_domain_owners() reports the owners after the cycle.  Call after submit_gangs; the next submit / load_nodes
+        clears it (include/grove_place.h "ComputeDomain exclusivity")."""
+        cd = np.ascontiguousarray(cd, dtype=np.uint32)
+        owner0 = np.ascontiguousarray(owner0, dtype=np.uint32)
+        self._check(self.lib.grove_set_compute_domains(self.h, _p(cd), C.c_uint32(len(cd)), _p(owner0), C.c_uint32(len(owner0))))
+
+    def compute_domain_owners(self) -> np.ndarray:
+        """per loaded node (caller order), the CD holding its IMEX channel after the last cycle that ran with a
+        set_compute_domains set: owner0 plus the CD of every admitted gang's enrolled pods -- the next cycle's owner0"""
+        out = np.zeros(max(self.n, 1), dtype=np.uint32)
+        self._check(self.lib.grove_get_compute_domain_owners(self.h, _p(out), C.c_uint32(len(out))))
+        return out[: self.n]
 
     # ---- the cycle ----
     def run_cycle(self) -> dict:

@@ -242,6 +242,30 @@ def podgroup_queues(podgangs, template_queue):
     return out
 
 
+MNNVL_CLAIM = "mnnvl-claim"   # the resource claim auto-MNNVL injects into an enrolled pod (operator/internal/mnnvl)
+
+
+def compute_domains(podgangs, template_pod_spec, intern=None):
+    """PodGroup name -> ComputeDomain id for grove_set_compute_domains (tables.CD_NONE when not enrolled): the
+    resourceClaimTemplateName of the `mnnvl-claim` entry of the pod spec's resourceClaims, in the PodClique template each PodGroup
+    was stamped from (matched as podgroup_queues does).  template_pod_spec: template name -> pod spec dict.  Names are interned in
+    `intern` (name -> id, extended in place, new ids from len(intern)), so that a caller keeps ids stable across cycles."""
+    intern = {} if intern is None else intern
+    names = sorted(template_pod_spec, key=len, reverse=True)
+    out = {}
+    for pg in podgangs:
+        for grp in pg["spec"]["podgroups"]:
+            t = next((n for n in names if grp["name"].endswith("-" + n)), None)
+            spec = template_pod_spec[t] if t is not None else None
+            claims = (spec or {}).get("resourceClaims") or []
+            tmpl = next((c.get("resourceClaimTemplateName") for c in claims if c.get("name") == MNNVL_CLAIM), None)
+            if tmpl is None:
+                out[grp["name"]] = T.CD_NONE
+                continue
+            out[grp["name"]] = intern.setdefault(tmpl, len(intern))
+    return out
+
+
 def _queue_limit(res, key, scale):
     lim = ((res or {}).get(key) or {}).get("limit", -1)
     if lim is None or float(lim) < 0:

@@ -225,6 +225,25 @@ def binpack_levels(gangs, level=None):
     return np.where(req == T.LEVEL_NONE, level, np.maximum(req, level)).astype(np.uint8)
 
 
+def c4_compute_domains(nodes, gangs, cliques, owned=0.5, seed=SEED_BASE + 417):
+    """ComputeDomains for grove_set_compute_domains over a C4-style submission, as Grove's auto-MNNVL makes them: one CD per PCS
+    replica, i.e. per base gang and the gangs scaled from it, with every GPU clique enrolled; the CD id is the base gang's index.
+    A share `owned` of the pre-used nodes (fewer free GPUs than the fullest node) is held by CDs of replicas that already run,
+    ids from len(gangs) up.  -> (cd [Q], owner0 [N])"""
+    cd = np.full(len(cliques), T.CD_NONE, dtype=np.uint32)
+    for g in range(len(gangs)):
+        b = int(gangs["base_gang"][g])
+        co, nq = int(gangs["clique_off"][g]), int(gangs["n_cliques"][g])
+        q = np.arange(co, co + nq)
+        cd[q[cliques["req_gpu"][q] > 0]] = g if b == T.NONE_U32 else b
+    rng = np.random.default_rng(seed)
+    used = nodes["free_gpu"] < nodes["free_gpu"].max()
+    owner0 = np.full(len(nodes), T.CD_NONE, dtype=np.uint32)
+    pick = used & (rng.random(len(nodes)) < owned)
+    owner0[pick] = len(gangs) + rng.integers(0, max(1, len(gangs) // 4), int(pick.sum()))
+    return cd, owner0
+
+
 def config_c4_large(n=50000, g=10000, n_large=24, seed=SEED_BASE + 44, max_used_pct=90):
     """C4 (config_c4) plus `n_large` PodGangs of 256-2048 pods, for grove_submit_gangs_wide: a leader (Required host) and a
     worker PodGroup of 255-2047 one-GPU pods under a Required zone with a Preferred block, priorities drawn from C4's three

@@ -82,6 +82,10 @@ spread_seed_dt = np.dtype([("group", "<u4"), ("node", "<u4")])
 MAX_FENCES = 64
 STATUS_FENCING = 0x4              # status reserved0: a REJECTED gang whose fence held (level, domain_node name the fenced domain)
 
+# ComputeDomain exclusivity (grove_set_compute_domains, include/grove_place.h "ComputeDomain exclusivity")
+CD_NONE = NONE_U32                # a clique that is not enrolled / a node no CD holds
+CD_NO_IMEX = 0xFFFFFFFE           # owner0: a node without an IMEX driver
+
 # consolidation (grove_run_cycle_consolidate, include/grove_place.h "consolidation")
 MAX_CONSOLIDATE_TARGETS = 16
 CONSOLIDATE_TRIES = 4

@@ -431,6 +431,32 @@ int32_t grove_set_fences(grove_engine_t* e, const uint32_t* gangs, uint32_t n);
 int32_t grove_set_binpack(grove_engine_t* e, const uint8_t* level_of, uint32_t n_gangs);
 int32_t grove_get_binpack_picks(grove_engine_t* e, uint32_t* out, uint32_t cap);
 
+/* ---- ComputeDomain exclusivity -------------------------------------------------------------------------
+ * A node's GPUs take part in at most one IMEX channel, hence one NVIDIA ComputeDomain (CD), at a time: pods of MNNVL-enrolled
+ * PodGroups of different CDs never share a node (DESIGN.md section 1, "ComputeDomain exclusivity"; Grove's auto-MNNVL).
+ * cd[q] (one per submitted clique) is the CD of clique q's pods, a caller-interned id, or GROVE_CD_NONE when q is not enrolled.
+ * owner0[n] (one per loaded node, caller order) is the CD that holds node n's IMEX channel when the cycle starts, GROVE_CD_NONE,
+ * or GROVE_CD_NO_IMEX (the node has no IMEX driver).
+ * The sequential pass is unchanged except at gang g's turn: owner(n) = owner0[n] if that is not GROVE_CD_NONE, else the CD of the
+ * enrolled pods that gangs ranked before g put on n in this cycle (at most one), else GROVE_CD_NONE.  An enrolled clique q of g
+ * fails K1 fit on n unless owner(n) is GROVE_CD_NONE or cd[q] (MinReplicas and surplus alike); cliques that are not enrolled are
+ * unaffected.  Candidate order, anchors, gating, the base-gang rule and PlacementScore do not change.  All enrolled cliques of a
+ * gang share one CD; a scaled gang carries its base gang's CD, so it may join the nodes its base holds.
+ * grove_get_compute_domain_owners: per loaded node (caller order), its owner at the end of the last cycle that ran with a set:
+ * owner0, plus the CD of every admitted gang's enrolled pods -- the next cycle's owner0.  GROVE_ERR_STATE before such a cycle.
+ * Call after grove_submit_gangs and before the cycle; the next grove_submit_gangs* or grove_load_nodes* clears the set,
+ * grove_update_nodes keeps it.  A set without an enrolled clique runs the ordinary cycle; the owners are then owner0.
+ * GROVE_ERR_INVALID_ARG for n_cliques / n_nodes other than the counts submitted / loaded, GROVE_CD_NO_IMEX as a clique's CD, or an
+ * enrolled clique with req_gpu == 0; GROVE_ERR_LIMIT for two CDs in one gang or a wide submission; GROVE_ERR_STATE before nodes
+ * are loaded and gangs submitted.  While a set with an enrolled clique is in place grove_run_cycle_preempt / _reuse /
+ * _reuse_preempt / _preempt_queues / _consolidate return GROVE_ERR_STATE, and so does grove_run_cycle with a spread set with
+ * members, a fence set, a queue set with members or a bin-packing set with members; grove_diagnose returns GROVE_ERR_STATE after
+ * such a cycle. */
+#define GROVE_CD_NONE GROVE_NONE_U32    /* not enrolled / no CD holds the node */
+#define GROVE_CD_NO_IMEX 0xFFFFFFFEu    /* owner0: the node has no IMEX driver (no enrolled pod may land on it) */
+int32_t grove_set_compute_domains(grove_engine_t* e, const uint32_t* cd, uint32_t n_cliques, const uint32_t* owner0, uint32_t n_nodes);
+int32_t grove_get_compute_domain_owners(grove_engine_t* e, uint32_t* out, uint32_t cap);
+
 /* ---- consolidation ------------------------------------------------------------------------------------
  * Running gangs are relocated so that a blocked gang fits, and only when every relocated gang finds a new place (DESIGN.md
  * section 1, "Consolidation"; after KAI-Scheduler's consolidation action).  Running gangs and holdings are as for

@@ -68,6 +68,8 @@ type schedulerBackend struct {
 	guardAfter, guardMax int
 	// bin-packing (SetBinPacking): the level key every PodGang of an ordinary or queue pass packs at; off while empty
 	binpackKey string
+	// ComputeDomain exclusivity (SetComputeDomainExclusivity)
+	imex bool
 	rejectedFor          map[string]int
 	// consolidation (SetConsolidation): off while consMax == 0; specOf: scheduled PodGang -> its spec (restated as a gated row to
 	// make it movable); moveAnchor: moved PodGang -> the first node of the placement the cycle planned for it
@@ -518,6 +520,28 @@ func (b *schedulerBackend) SetBinPacking(levelKey string) {
 	b.binpackKey = levelKey
 }
 
+// SetComputeDomainExclusivity keeps the pods of MNNVL-enrolled PodGroups (a pod's `mnnvl-claim` resource claim names the
+// ComputeDomain through its resourceClaimTemplateName) off nodes that another ComputeDomain holds (grove_set_compute_domains;
+// GpuBackend::SetComputeDomainExclusivity in the C++ mirror).  A node's holder when the pass starts is the ComputeDomain of the
+// enrolled pods bound to it.  A PodGang whose PodGroups name two ComputeDomains stays out of the pass, and so does every enrolled
+// PodGang in a pass with preemption, consolidation, the starvation guard, bin-packing, topology spread, queue limits or large
+// PodGangs.  Off (the default): the pass is as before.
+func (b *schedulerBackend) SetComputeDomainExclusivity(on bool) {
+	b.mu.Lock()
+	defer b.mu.Unlock()
+	b.imex = on
+}
+
+// mnnvlClaim is the resourceClaimTemplateName of the pod's `mnnvl-claim` entry, or "" (not enrolled)
+func mnnvlClaim(pod *corev1.Pod) string {
+	for _, c := range pod.Spec.ResourceClaims {
+		if c.Name == "mnnvl-claim" && c.ResourceClaimTemplateName != nil {
+			return *c.ResourceClaimTemplateName
+		}
+	}
+	return ""
+}
+
 // SetConsolidation makes, each cycle, the <= maxTargets highest-ranked pending PodGangs that came back Unschedulable at least
 // afterCycles cycles in a row (counted as the starvation guard counts) targets of grove_run_cycle_consolidate: running PodGangs
 // this backend scheduled, restated as gated rows, are relocated out of the domain closest to fitting a target when every one of
@@ -672,6 +696,20 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 		snap = append(snap, pg)
 	}
 	levels, eng, preempt, large, explain := b.levels, b.eng, b.preempt, b.largePodGangs, b.explainUnschedulable
+	imexOn := b.imex
+	imexWhy := "" // a pass that takes no ComputeDomain set: the enrolled PodGangs stay out
+	switch {
+	case preempt:
+		imexWhy = "ComputeDomain exclusivity is not applied while preemption is on"
+	case b.consMax > 0:
+		imexWhy = "ComputeDomain exclusivity is not applied while consolidation is on"
+	case b.guardMax > 0:
+		imexWhy = "ComputeDomain exclusivity is not applied while the starvation guard is on"
+	case b.binpackKey != "":
+		imexWhy = "ComputeDomain exclusivity is not applied while bin-packing is on"
+	case len(b.queues) > 0:
+		imexWhy = "ComputeDomain exclusivity is not applied while queue limits are set"
+	}
 	spreadOn := len(b.spread) > 0
 	queuesOn := len(b.queues) > 0
 	queueWhy := "" // a pass that takes no queue set: its members stay out
@@ -712,6 +750,24 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 	if queueWhy == "" && wideAny {
 		queueWhy = "queue limits are not applied in a pass with large PodGangs"
 	}
+	if imexWhy == "" && spreadAny {
+		imexWhy = "ComputeDomain exclusivity is not applied in a pass with topology spread members"
+	}
+	if imexWhy == "" && wideAny {
+		imexWhy = "ComputeDomain exclusivity is not applied in a pass with large PodGangs"
+	}
+	podByKey := make(map[string]*corev1.Pod, len(podList.Items))
+	for i := range podList.Items {
+		podByKey[podList.Items[i].Namespace+"/"+podList.Items[i].Name] = &podList.Items[i]
+	}
+	groupCD := func(pg *groveschedulerv1alpha1.PodGang, pgi int) string { // the ComputeDomain of a PodGroup's pods ("" = none)
+		for _, ref := range pg.Spec.PodGroups[pgi].PodReferences {
+			if p, ok := podByKey[ref.Namespace+"/"+ref.Name]; ok {
+				return mnnvlClaim(p)
+			}
+		}
+		return ""
+	}
 	for _, pg := range snap {
 		if why := whyNotEncodable(pg, large, preempt); why != "" { // large && preempt: within the old limits only
 			b.setUnschedulable(ctx, pg, why)
@@ -727,6 +783,23 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 			b.mu.Unlock()
 			if member {
 				b.setUnschedulable(ctx, pg, queueWhy)
+				continue
+			}
+		}
+		if imexOn {
+			cd, two := "", false
+			for pgi := range pg.Spec.PodGroups {
+				if c := groupCD(pg, pgi); c != "" {
+					two = two || (cd != "" && cd != c)
+					cd = c
+				}
+			}
+			if two {
+				b.setUnschedulable(ctx, pg, "the PodGroups of this PodGang name two ComputeDomains (MNNVL groups); one per PodGang is supported")
+				continue
+			}
+			if cd != "" && imexWhy != "" {
+				b.setUnschedulable(ctx, pg, imexWhy)
 				continue
 			}
 		}
@@ -834,6 +907,43 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 					}
 				}
 			}
+		}
+	}
+	// ComputeDomain exclusivity, in an ordinary pass: every enrolled GPU clique row's ComputeDomain, every node's holder (the
+	// ComputeDomain of the enrolled pods bound to it)
+	if imexOn && imexWhy == "" && len(t.targets) == 0 && len(t.fences) == 0 {
+		ids := map[string]C.uint32_t{}
+		id := func(name string) C.uint32_t {
+			if v, ok := ids[name]; ok {
+				return v
+			}
+			ids[name] = C.uint32_t(len(ids))
+			return ids[name]
+		}
+		cd := make([]C.uint32_t, len(t.cliques))
+		enrolled := false
+		for c := range t.cliques {
+			cd[c] = C.GROVE_CD_NONE
+			if gi, pgi := cliqueOwner(t, c); gi < len(rows) && t.cliques[c].req_gpu > 0 {
+				if name := groupCD(rows[gi], pgi); name != "" {
+					cd[c], enrolled = id(name), true
+				}
+			}
+		}
+		if enrolled {
+			owner0 := make([]C.uint32_t, len(nodeNames))
+			for i := range owner0 {
+				owner0[i] = C.GROVE_CD_NONE
+			}
+			for i := range podList.Items {
+				p := &podList.Items[i]
+				if n, ok := nodeIdx[p.Spec.NodeName]; ok && p.Status.Phase != corev1.PodSucceeded && p.Status.Phase != corev1.PodFailed {
+					if name := mnnvlClaim(p); name != "" {
+						owner0[n] = id(name)
+					}
+				}
+			}
+			t.cd, t.owner0 = cd, owner0
 		}
 	}
 	rejectedFor := map[string]int{}

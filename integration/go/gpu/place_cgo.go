@@ -64,6 +64,9 @@ type tables struct {
 	fences []C.uint32_t
 	// bin-packing (optional; ordinary and queue passes only): each gang row's pack level (grove_set_binpack)
 	binpack []C.uint8_t
+	// ComputeDomain exclusivity (optional; ordinary passes only): each clique row's ComputeDomain (GROVE_CD_NONE: not enrolled)
+	// and each node's holder when the pass starts (grove_set_compute_domains)
+	cd, owner0 []C.uint32_t
 	// queue limits (optional; ordinary passes only): the queues, parents first, each gang row's queue (GROVE_NONE_U32 = none) and
 	// the queue names in table order (grove_set_queues)
 	queues     []C.grove_queue_t
@@ -126,6 +129,11 @@ func (e *engine) cycle(t *tables, preempt, large, explain bool) (*result, error)
 	}
 	if len(t.binpack) > 0 {
 		if err := e.err(C.grove_set_binpack(e.h, &t.binpack[0], C.uint32_t(len(t.binpack)))); err != nil {
+			return nil, err
+		}
+	}
+	if len(t.cd) > 0 {
+		if err := e.err(C.grove_set_compute_domains(e.h, &t.cd[0], C.uint32_t(len(t.cd)), &t.owner0[0], C.uint32_t(len(t.owner0)))); err != nil {
 			return nil, err
 		}
 	}
