@@ -235,7 +235,14 @@ struct grove_engine {
   DevBuf<uint32_t> d_rc_off, d_rc_idx, d_rc_bad;
   DevBuf<uint4> d_rc_ent, d_rc_real, d_rc_base, d_rc_rows, d_rc_patch;
   DevBuf<int32_t> d_rc_prio;
-  DevBuf<uint8_t> d_rc_gone;
+  DevBuf<uint8_t> d_rc_gone, d_rc_evict;
+  // the donor sets of grove_run_cycle_reclaim_queues (donor.cuh): per scanned queue its pairs in victim order, the quotas, the
+  // running gangs' usage, queues and chains, the per-class loads and the per-(running gang, depth) verdicts
+  DevBuf<uint32_t> d_dn_off, d_dn_qid, d_dn_parent, d_dn_rq;
+  DevBuf<uint2> d_dn_pr;
+  DevBuf<unsigned long long> d_dn_quota;
+  DevBuf<long long> d_dn_load, d_dn_use;
+  DevBuf<uint8_t> d_dn_fin, d_dn_bits;
   // grove_diagnose (diagnose.cuh): whether the outputs on the device describe an ordinary cycle over the current inputs, the
   // per-node usage lists, the batch descriptors, the per-domain capacity sums and the records
   enum Diag : uint8_t { kDiagNoCycle, kDiagReady, kDiagRunning, kDiagChanged, kDiagSpread, kDiagFence, kDiagImex } diag = kDiagNoCycle;
@@ -2241,7 +2248,7 @@ static int32_t patch_nodes(grove_engine* e, std::vector<std::pair<uint32_t, Res>
 }
 
 // the outputs of a cycle with a reclaim or consolidation pass, merged: placements grouped by gang in submission order (those of a
-// preemptor, a consolidated target or a moved spec row from `extra`)
+// preemptor, a reclaimer, a consolidated target or a moved spec row from `extra`)
 static int32_t publish_reclaim(grove_engine* e, std::vector<grove_gang_status_t>& status, const std::vector<grove_placement_t>& place,
                                const std::vector<std::vector<grove_placement_t>>& extra, const std::vector<grove_scope_status_t>& sstat,
                                grove_cycle_stats_t st0, std::vector<grove_victim_t> victims, grove_cycle_stats_t* stats) {
@@ -2254,7 +2261,8 @@ static int32_t publish_reclaim(grove_engine* e, std::vector<grove_gang_status_t>
   for (uint32_t g = 0; g < G; ++g) {
     if (status[g].state != GROVE_GANG_ADMITTED) continue;
     const uint32_t off = uint32_t(merged.size());
-    if (status[g].reserved0 & (GROVE_STATUS_PREEMPTOR | GROVE_STATUS_CONSOLIDATED | GROVE_STATUS_MOVED)) merged.insert(merged.end(), extra[g].begin(), extra[g].end());
+    if (status[g].reserved0 & (GROVE_STATUS_PREEMPTOR | GROVE_STATUS_RECLAIMER | GROVE_STATUS_CONSOLIDATED | GROVE_STATUS_MOVED))
+      merged.insert(merged.end(), extra[g].begin(), extra[g].end());
     else merged.insert(merged.end(), place.begin() + status[g].placement_off, place.begin() + status[g].placement_off + status[g].n_pods);
     status[g].placement_off = off;
   }
@@ -2426,15 +2434,90 @@ static int32_t upload_running(grove_engine* e, const grove_running_gang_t* runni
   return GROVE_OK;
 }
 
+// The donor sets of grove_run_cycle_reclaim_queues on the device (donor.cuh): the (scanned queue, running gang) pairs in victim
+// order with the depth of the queue in the running gang's chain, and what k_donor_scan / k_donor_mark read besides, uploaded
+// once per call.  -> the number of scanned queues (those with a finite quota on some resource); 0: every E(Q) is empty.
+static int32_t upload_donors(grove_engine* e, const grove_running_gang_t* running, uint32_t n_running, const uint32_t* run_queue,
+                             const std::vector<grove_queue_t>& queues, const grove_queue_quota_t* quotas,
+                             const std::vector<std::array<int64_t, 3>>& usage, uint32_t* scanned, DonorSet* d) {
+  const uint32_t NQ = uint32_t(queues.size());
+  std::vector<uint32_t> scan_id(NQ, GROVE_NONE_U32), q_id, parent(std::max<uint32_t>(NQ, 1), GROVE_NONE_U32);
+  std::vector<uint8_t> fin(std::max<uint32_t>(NQ, 1), 0);
+  std::vector<unsigned long long> quota(std::max<size_t>(size_t(NQ) * 3, 1), GROVE_QUEUE_UNLIMITED);
+  for (uint32_t q = 0; q < NQ; ++q) {
+    parent[q] = queues[q].parent;
+    for (int k = 0; k < 3; ++k) { quota[q * 3 + k] = quotas[q].deserved[k]; fin[q] |= quotas[q].deserved[k] != GROVE_QUEUE_UNLIMITED; }
+    if (fin[q]) { scan_id[q] = uint32_t(q_id.size()); q_id.push_back(q); }
+  }
+  *scanned = uint32_t(q_id.size());
+  if (!*scanned || !n_running) { *scanned = 0; return GROVE_OK; }
+  // the running gangs in victim order (evicted_before), each appended to the pairs of every scanned queue of its chain
+  std::vector<uint32_t> order(n_running);
+  std::iota(order.begin(), order.end(), 0u);
+  std::sort(order.begin(), order.end(), [running](uint32_t a, uint32_t b) { return a != b && evicted_before(running, a, b); });
+  std::vector<std::vector<uint2>> per(q_id.size());
+  for (uint32_t r : order) {
+    uint32_t k = 0;
+    for (uint32_t X = run_queue[r]; X != GROVE_NONE_U32; X = queues[X].parent, ++k)
+      if (scan_id[X] != GROVE_NONE_U32) per[scan_id[X]].push_back(make_uint2(r, k));
+  }
+  std::vector<uint32_t> off(q_id.size() + 1, 0);
+  std::vector<uint2> pr;
+  for (size_t i = 0; i < per.size(); ++i) { pr.insert(pr.end(), per[i].begin(), per[i].end()); off[i + 1] = uint32_t(pr.size()); }
+  if (pr.empty()) pr.push_back(make_uint2(0u, 0u));
+  std::vector<long long> use(size_t(n_running) * 3);
+  for (uint32_t r = 0; r < n_running; ++r) for (int k = 0; k < 3; ++k) use[r * 3 + k] = usage[r][k];
+  auto up = [e](auto& dv, const auto& h) -> cudaError_t {
+    cudaError_t c = dv.ensure(h.size());
+    if (c == cudaSuccess) c = cudaMemcpyAsync(dv.p, h.data(), sizeof(h[0]) * h.size(), cudaMemcpyHostToDevice, e->stream);
+    return c;
+  };
+  const std::vector<uint32_t> rq(run_queue, run_queue + n_running);
+  CU_TRY(e, up(e->d_dn_off, off)); CU_TRY(e, up(e->d_dn_qid, q_id)); CU_TRY(e, up(e->d_dn_pr, pr)); CU_TRY(e, up(e->d_dn_quota, quota));
+  CU_TRY(e, up(e->d_dn_use, use)); CU_TRY(e, up(e->d_dn_parent, parent)); CU_TRY(e, up(e->d_dn_rq, rq)); CU_TRY(e, up(e->d_dn_fin, fin));
+  CU_TRY(e, e->d_dn_load.ensure(std::max<size_t>(size_t(NQ) * 3, 1))); CU_TRY(e, e->d_dn_bits.ensure(size_t(n_running) * GROVE_MAX_QUEUE_DEPTH));
+  CU_TRY(e, e->d_rc_evict.ensure(n_running));
+  CU_TRY(e, cudaStreamSynchronize(e->stream));   // (pageable sources)
+  *d = DonorSet{e->d_dn_off.p, e->d_dn_qid.p, e->d_dn_pr.p, e->d_dn_quota.p, e->d_dn_load.p, e->d_dn_use.p, e->d_dn_parent.p,
+                e->d_dn_rq.p, e->d_dn_fin.p, e->d_rc_gone.p, e->d_dn_bits.p};
+  return GROVE_OK;
+}
+
+// share_Q = max over the resources x with a finite deserved_Q[x] of load_Q[x] / deserved_Q[x] as (num, den), den 0 = +inf; 0/0 and
+// no finite quota = 0.  less() compares two exactly (128-bit cross products).
+namespace {
+struct Share {
+  uint64_t num = 0, den = 1;
+  static bool less(const Share& a, const Share& b) {
+    if (b.den == 0) return a.den != 0;
+    if (a.den == 0) return false;
+    return (unsigned __int128)a.num * b.den < (unsigned __int128)b.num * a.den;
+  }
+};
+}  // namespace
+static Share share_of(const grove_queue_quota_t& q, const std::array<int64_t, 3>& load) {
+  Share s;
+  for (int k = 0; k < 3; ++k) {
+    if (q.deserved[k] == GROVE_QUEUE_UNLIMITED) continue;
+    const uint64_t l = uint64_t(std::max<int64_t>(load[k], 0));
+    const Share x = q.deserved[k] ? Share{l, q.deserved[k]} : (l ? Share{1, 0} : Share{0, 1});
+    if (Share::less(s, x)) s = x;
+  }
+  return s;
+}
+
 // replaces (null: no gang replaces a running gang) as for grove_run_cycle_reuse; running_queue (null: no queue set) the queue of each
-// running gang in the queue set of the current submission.  Inputs checked by the entry.
+// running gang in the queue set of the current submission; quotas (null: priority classes) one row per queue of that set, and then
+// the classes are queues (grove_run_cycle_reclaim_queues).  Inputs checked by the entry.
 static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const grove_running_gang_t* running, uint32_t n_running,
-                             const grove_holding_t* holdings, const uint32_t* running_queue, grove_cycle_stats_t* stats) {
+                             const grove_holding_t* holdings, const uint32_t* running_queue, const grove_queue_quota_t* quotas,
+                             grove_cycle_stats_t* stats) {
   CU_TRY(e, cudaSetDevice(e->cfg.device));
   const uint32_t G = e->G, N = e->N, nblk = (N + 255) / 256;
   ReclaimCsr csr{};
   int32_t rc = upload_running(e, running, n_running, holdings, &csr);
   if (rc) return rc;
+  CU_TRY(e, e->d_rc_evict.ensure(std::max<uint32_t>(n_running, 1)));
   // without replacements nothing holds; without a queue set no gang and no running gang is in a queue, and the queue step never runs
   std::vector<uint32_t> rep(G, GROVE_NONE_U32), run_queue(n_running, GROVE_NONE_U32);
   if (replaces) std::copy(replaces, replaces + G, rep.begin());
@@ -2448,6 +2531,10 @@ static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const gr
   std::vector<std::array<int64_t, 3>> own(NQ, {0, 0, 0});   // own used, then followed through the cycle
   for (uint32_t q = 0; q < NQ; ++q) for (int k = 0; k < 3; ++k) own[q][k] = int64_t(std::min<uint64_t>(queues[q].used[k], uint64_t(1) << 62));
   std::vector<uint8_t> gone(std::max<uint32_t>(n_running, 1), 0);   // released or evicted
+  // the caps of the class pass: the limits, or with quotas min(limit, deserved)
+  std::vector<std::array<uint64_t, 3>> cap(NQ);
+  for (uint32_t q = 0; q < NQ; ++q)
+    for (int k = 0; k < 3; ++k) cap[q][k] = quotas ? std::min(queues[q].limit[k], quotas[q].deserved[k]) : queues[q].limit[k];
 
   // 1. the ordinary pass: the cycle with holds (the reuse cycle; without replacements the ordinary cycle, under a queue set the
   // queue cycle).  An admitted new version's predecessor is released.
@@ -2478,157 +2565,226 @@ static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const gr
     for (; q != GROVE_NONE_U32; q = queues[q].parent) if (q == Qx) return true;
     return false;
   };
-  std::vector<int32_t> classes;   // the rejected priority classes, descending
-  for (uint32_t g = 0; g < G; ++g) if (snap.status[g].state == GROVE_GANG_REJECTED) classes.push_back(snap.gangs[g].priority);
-  std::sort(classes.begin(), classes.end(), std::greater<int32_t>());
-  classes.erase(std::unique(classes.begin(), classes.end()), classes.end());
-  auto below = [&](int32_t p) {   // is E(p) -- the standing running gangs of a priority below p -- non-empty?
-    for (uint32_t r = 0; r < n_running; ++r) if (!gone[r] && running[r].priority < p) return true;
+  // evict[r]: running gang r may be evicted by the current class (fixed when the class starts: it stood then)
+  std::vector<uint8_t> evict(std::max<uint32_t>(n_running, 1), 0);
+  auto standing = [&]() {   // does a running gang the class may evict still stand?
+    for (uint32_t r = 0; r < n_running; ++r) if (evict[r] && !gone[r]) return true;
     return false;
   };
   std::vector<grove_victim_t> victims;
-  std::vector<std::vector<grove_placement_t>> extra(G);   // placements of the preemptors, by gang
-  if (!classes.empty() && below(classes.front())) {
-    CU_TRY(e, cudaMemcpyAsync(e->d_rc_base.p, e->d_nres.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToDevice, e->stream));
-    Restore restore{e, &snap, running_queue ? &queues : nullptr, &gang_queue};
-    const RunningByNode at = running_by_node(N, running, n_running, holdings);
-    std::vector<int32_t> slot(N, -1);   // node (caller order) -> its row in `rows` while a class chooses its victims
-    for (int32_t p : classes) {
-      if (!below(p)) break;   // E(p) only shrinks from one class to the next
-      // 2. the class's rejected gangs as a submission of their own.  A member holds its predecessor's holdings when that one still
-      // stands at or above p; below p it is evictable instead.
-      Sub sub;
-      std::vector<uint32_t> sub_rep, sub_queue;
-      for (uint32_t g = 0; g < G; ++g) {
-        if (snap.status[g].state != GROVE_GANG_REJECTED || snap.gangs[g].priority != p) continue;
-        add_gang(e, snap, g, sub);
-        const uint32_t r = rep[g];
-        sub_rep.push_back(r != GROVE_NONE_U32 && !gone[r] && running[r].priority >= p ? r : GROVE_NONE_U32);
-        sub_queue.push_back(gang_queue[g]);
-      }
-      // the class view, on the device: free + the standing holdings of E(p); the free table itself is kept for the victim choice
-      CU_TRY(e, cudaMemcpyAsync(e->d_rc_gone.p, gone.data(), gone.size(), cudaMemcpyHostToDevice, e->stream));
-      k_reclaim_view<<<nblk, 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_real.p, csr, N, p, 1u);
-      CU_TRY(e, cudaGetLastError());
-      rc = submit_sub(e, sub); if (rc) return rc;
-      if (running_queue) {   // the class's queue set: own used without what the gangs of E(p) hold, so that its loads are load'
-        std::vector<grove_queue_t> cq(queues);
-        std::vector<std::array<int64_t, 3>> o(own);
-        for (uint32_t r = 0; r < n_running; ++r)
-          if (!gone[r] && running[r].priority < p && run_queue[r] != GROVE_NONE_U32) for (int k = 0; k < 3; ++k) o[run_queue[r]][k] -= usage[r][k];
-        for (uint32_t q = 0; q < NQ; ++q) for (int k = 0; k < 3; ++k) cq[q].used[k] = uint64_t(o[q][k]);
-        rc = install_queues(e, cq.data(), NQ, sub_queue.data()); if (rc) return rc;
-      }
-      grove_cycle_stats_t stp{};
-      rc = run_cycle_holds(e, sub_rep.data(), running, holdings, false, &stp); if (rc) return rc;
-      accumulate(st0, stp); st0.kernel_launches += 2;   // (+ the two k_reclaim_view)
-      std::vector<grove_scope_status_t> ssp;
-      rc = sub_scope_domains(e, sub, ssp); if (rc) return rc;
-      // the free-table rows of the nodes the class's preemptors use
-      std::vector<uint32_t> used;
-      for (uint32_t k = 0; k < sub.ids.size(); ++k) {
-        const grove_gang_status_t& sp = e->h_status.p[k];
-        if (sp.state != GROVE_GANG_ADMITTED) continue;
-        for (uint32_t i = 0; i < sp.n_pods; ++i) used.push_back(e->h_out.p[sp.placement_off + i].node);
-      }
-      std::sort(used.begin(), used.end());
-      used.erase(std::unique(used.begin(), used.end()), used.end());
-      std::vector<Res> rows;
-      rc = read_rows(e, used, rows, st0); if (rc) return rc;
-      for (size_t i = 0; i < used.size(); ++i) slot[used[i]] = int32_t(i);
-      auto release = [&](uint32_t v) {   // everything v held returns to the free table (only the tracked rows matter here)
-        gone[v] = 1;
-        for (uint32_t h = 0; h < running[v].n_holdings; ++h) {
-          const grove_holding_t& x = holdings[running[v].holding_off + h];
-          if (slot[x.node] >= 0) rows[slot[x.node]].add(held(x));
-        }
-      };
-      auto evict = [&](uint32_t v, uint32_t g) {   // released, and its usage leaves its queues
-        release(v);
-        if (run_queue[v] != GROVE_NONE_U32) account(run_queue[v], usage[v].data(), -1);
-        victims.push_back(grove_victim_t{v, g});
-      };
-      // 3. victims, gang by gang in rank order (sub-submission order == order rank: one priority)
-      std::vector<std::pair<uint32_t, Res>> back;   // (sorted node, change)
-      for (uint32_t k = 0; k < sub.ids.size(); ++k) {
-        const grove_gang_status_t& sp = e->h_status.p[k];
-        if (sp.state != GROVE_GANG_ADMITTED) continue;
-        std::vector<uint32_t> nodes; std::vector<Res> use; std::vector<grove_placement_t> pl;
-        placed(e, snap, sub, k, nodes, use, pl);
-        if (!below(p)) {   // admitted by the class cycle after E(p) ran out: it stays as the ordinary pass left it.  What the class
-                           // cycle committed for it goes back: +U, and -H for a member with a hold (a queue charge was never taken here)
-          for (size_t j = 0; j < nodes.size(); ++j) back.push_back({e->inv[nodes[j]], use[j]});
-          if (sub_rep[k] != GROVE_NONE_U32)
-            for (uint32_t h = 0; h < running[sub_rep[k]].n_holdings; ++h) {
-              const grove_holding_t& x = holdings[running[sub_rep[k]].holding_off + h];
-              Res c; c.add(held(x), -1);
-              back.push_back({e->inv[x.node], c});
-            }
-          continue;
-        }
-        const uint32_t g = sub.ids[k], r = rep[g];
-        const bool holds = sub_rep[k] != GROVE_NONE_U32;
-        if (r != GROVE_NONE_U32 && !holds && !gone[r]) release(r);   // its predecessor is in E(p): released first, not a victim
-        std::vector<Res> mine(nodes.size());
-        if (holds)   // what its predecessor holds on each of those nodes: used first
-          for (uint32_t h = 0; h < running[r].n_holdings; ++h) {
-            const grove_holding_t& x = holdings[running[r].holding_off + h];
-            for (size_t j = 0; j < nodes.size(); ++j) if (nodes[j] == x.node) mine[j].add(held(x));
-          }
-        // (a) the node step: the reclaim pass's rule
-        for (size_t j = 0; j < nodes.size(); ++j) {
-          const uint32_t n = nodes[j];
-          const Res need{std::max<int64_t>(use[j].cpu - mine[j].cpu, 0), std::max<int64_t>(use[j].mem - mine[j].mem, 0),
-                         std::max<int64_t>(use[j].gpu - mine[j].gpu, 0), std::max<int64_t>(use[j].pods - mine[j].pods, 0)};
-          Res& have = rows[slot[n]];
-          while (!have.covers(need)) {
-            const uint32_t v = choose_victim(at, n, running, [&](uint32_t x) { return !gone[x] && running[x].priority < p; });
-            if (v == GROVE_NONE_U32) return fail(e, GROVE_ERR_STATE, "reclaim pass: a preemptor's node cannot be freed");
-            evict(v, g);
-          }
-          have.add(need, -1);
-        }
-        if (holds) gone[r] = 1;   // released; its leftover came back when the class cycle ended (k_hold_release)
-        // (b) the queue step: g's chain, leaf first, back within its limits on the resources g uses
-        const uint32_t gq = gang_queue[g];
-        if (gq != GROVE_NONE_U32) {
-          int64_t U[3] = {0, 0, 0};
-          for (const Res& u : use) { U[0] += u.cpu; U[1] += u.mem; U[2] += u.gpu; }
-          account(gq, U, 1);
-          for (uint32_t Qx = gq; Qx != GROVE_NONE_U32; Qx = queues[Qx].parent) {
-            for (;;) {
-              uint32_t over = 0;   // the resources g uses on which Qx is over its finite limit
-              for (int t = 0; t < 3; ++t)
-                if (U[t] > 0 && queues[Qx].limit[t] != GROVE_QUEUE_UNLIMITED && load[Qx][t] > 0 && uint64_t(load[Qx][t]) > queues[Qx].limit[t]) over |= 1u << t;
-              if (!over) break;
-              uint32_t v = GROVE_NONE_U32;   // by the victim rule, among the gangs of E(p) in Qx's subtree that hold some of it
-              for (uint32_t x = 0; x < n_running; ++x) {
-                if (gone[x] || running[x].priority >= p || run_queue[x] == GROVE_NONE_U32 || !in_subtree(run_queue[x], Qx)) continue;
-                bool holds_some = false;
-                for (int t = 0; t < 3; ++t) holds_some |= ((over >> t) & 1u) && usage[x][t] > 0;
-                if (holds_some && evicted_before(running, x, v)) v = x;
-              }
-              if (v == GROVE_NONE_U32) return fail(e, GROVE_ERR_STATE, "reclaim pass: a preemptor's queue cannot be brought within its limit");
-              evict(v, g);
-            }
-          }
-        }
-        grove_gang_status_t o = sp;
-        o.reserved0 = uint16_t(GROVE_STATUS_PREEMPTOR | (sp.reserved0 & GROVE_STATUS_SURPLUS_CAPPED));
-        merge_gang(snap, sub, k, o, ssp);
-        extra[g] = std::move(pl);
-        st0.gangs_admitted += 1; st0.gangs_rejected -= 1;
-      }
-      for (uint32_t n : used) slot[n] = -1;
-      rc = patch_nodes(e, back, st0); if (rc) return rc;
-      // back to the free table: take off what the running gangs of E(p) that still stand hold
-      CU_TRY(e, cudaMemcpyAsync(e->d_rc_gone.p, gone.data(), gone.size(), cudaMemcpyHostToDevice, e->stream));
-      k_reclaim_view<<<nblk, 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_real.p, csr, N, p, 0u);
-      CU_TRY(e, cudaGetLastError());
+  std::vector<std::vector<grove_placement_t>> extra(G);   // placements of the preemptors and reclaimers, by gang
+  RunningByNode at;
+  std::vector<int32_t> slot;   // node (caller order) -> its row in `rows` while a class chooses its victims
+
+  // One class: its members (the gangs the ordinary pass rejected, in rank order) against the running gangs `evict` marks.  Its
+  // admitted members carry `flag`; give_back: a member admitted by the class cycle once none of them stands any more gives its room
+  // back (the priority classes' rule).
+  auto run_class = [&](const std::vector<uint32_t>& members, uint16_t flag, bool give_back) -> int32_t {
+    // 2. the class's members as a submission of their own.  A member holds its predecessor's holdings when that one still stands
+    // and is not evictable; when it is, it is released instead.
+    Sub sub;
+    std::vector<uint32_t> sub_rep, sub_queue;
+    for (uint32_t g : members) {
+      add_gang(e, snap, g, sub);
+      const uint32_t r = rep[g];
+      sub_rep.push_back(r != GROVE_NONE_U32 && !gone[r] && !evict[r] ? r : GROVE_NONE_U32);
+      sub_queue.push_back(gang_queue[g]);
     }
-    // the handle goes back to the caller's submission (and queue set); the device table is the free table
-    restore.armed = false;
-    rc = restore.put_back(); if (rc) return rc;
+    // the class view, on the device: free + the standing holdings the class may evict; the free table itself is kept for the
+    // victim choice
+    CU_TRY(e, cudaMemcpyAsync(e->d_rc_evict.p, evict.data(), n_running, cudaMemcpyHostToDevice, e->stream));
+    k_reclaim_view<<<nblk, 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_real.p, csr.off, csr.ent, e->d_rc_evict.p, N, 1u);
+    CU_TRY(e, cudaGetLastError());
+    int32_t rc = submit_sub(e, sub); if (rc) return rc;
+    if (running_queue) {   // the class's queue set: own used without what the evictable gangs hold, so that its loads are load';
+                           // the caps in place of the limits
+      std::vector<grove_queue_t> cq(queues);
+      std::vector<std::array<int64_t, 3>> o(own);
+      for (uint32_t r = 0; r < n_running; ++r)
+        if (evict[r] && run_queue[r] != GROVE_NONE_U32) for (int k = 0; k < 3; ++k) o[run_queue[r]][k] -= usage[r][k];
+      for (uint32_t q = 0; q < NQ; ++q) for (int k = 0; k < 3; ++k) { cq[q].used[k] = uint64_t(o[q][k]); cq[q].limit[k] = cap[q][k]; }
+      rc = install_queues(e, cq.data(), NQ, sub_queue.data()); if (rc) return rc;
+    }
+    grove_cycle_stats_t stp{};
+    rc = run_cycle_holds(e, sub_rep.data(), running, holdings, false, &stp); if (rc) return rc;
+    accumulate(st0, stp); st0.kernel_launches += 2;   // (+ the two k_reclaim_view)
+    std::vector<grove_scope_status_t> ssp;
+    rc = sub_scope_domains(e, sub, ssp); if (rc) return rc;
+    // the free-table rows of the nodes the class's admitted members use
+    std::vector<uint32_t> used;
+    for (uint32_t k = 0; k < sub.ids.size(); ++k) {
+      const grove_gang_status_t& sp = e->h_status.p[k];
+      if (sp.state != GROVE_GANG_ADMITTED) continue;
+      for (uint32_t i = 0; i < sp.n_pods; ++i) used.push_back(e->h_out.p[sp.placement_off + i].node);
+    }
+    std::sort(used.begin(), used.end());
+    used.erase(std::unique(used.begin(), used.end()), used.end());
+    std::vector<Res> rows;
+    rc = read_rows(e, used, rows, st0); if (rc) return rc;
+    for (size_t i = 0; i < used.size(); ++i) slot[used[i]] = int32_t(i);
+    auto release = [&](uint32_t v) {   // everything v held returns to the free table (only the tracked rows matter here)
+      gone[v] = 1;
+      for (uint32_t h = 0; h < running[v].n_holdings; ++h) {
+        const grove_holding_t& x = holdings[running[v].holding_off + h];
+        if (slot[x.node] >= 0) rows[slot[x.node]].add(held(x));
+      }
+    };
+    auto evict_one = [&](uint32_t v, uint32_t g) {   // released, and its usage leaves its queues
+      release(v);
+      if (run_queue[v] != GROVE_NONE_U32) account(run_queue[v], usage[v].data(), -1);
+      victims.push_back(grove_victim_t{v, g});
+    };
+    // 3. victims, gang by gang in rank order (sub-submission order == order rank)
+    std::vector<std::pair<uint32_t, Res>> back;   // (sorted node, change)
+    for (uint32_t k = 0; k < sub.ids.size(); ++k) {
+      const grove_gang_status_t& sp = e->h_status.p[k];
+      if (sp.state != GROVE_GANG_ADMITTED) continue;
+      std::vector<uint32_t> nodes; std::vector<Res> use; std::vector<grove_placement_t> pl;
+      placed(e, snap, sub, k, nodes, use, pl);
+      if (give_back && !standing()) {   // admitted by the class cycle after E(p) ran out: it stays as the ordinary pass left it.
+                                        // What the class cycle committed for it goes back: +U, and -H for a member with a hold (a
+                                        // queue charge was never taken here)
+        for (size_t j = 0; j < nodes.size(); ++j) back.push_back({e->inv[nodes[j]], use[j]});
+        if (sub_rep[k] != GROVE_NONE_U32)
+          for (uint32_t h = 0; h < running[sub_rep[k]].n_holdings; ++h) {
+            const grove_holding_t& x = holdings[running[sub_rep[k]].holding_off + h];
+            Res c; c.add(held(x), -1);
+            back.push_back({e->inv[x.node], c});
+          }
+        continue;
+      }
+      const uint32_t g = sub.ids[k], r = rep[g];
+      const bool holds = sub_rep[k] != GROVE_NONE_U32;
+      if (r != GROVE_NONE_U32 && !holds && !gone[r]) release(r);   // its predecessor is evictable: released first, not a victim
+      std::vector<Res> mine(nodes.size());
+      if (holds)   // what its predecessor holds on each of those nodes: used first
+        for (uint32_t h = 0; h < running[r].n_holdings; ++h) {
+          const grove_holding_t& x = holdings[running[r].holding_off + h];
+          for (size_t j = 0; j < nodes.size(); ++j) if (nodes[j] == x.node) mine[j].add(held(x));
+        }
+      // (a) the node step: the reclaim pass's rule
+      for (size_t j = 0; j < nodes.size(); ++j) {
+        const uint32_t n = nodes[j];
+        const Res need{std::max<int64_t>(use[j].cpu - mine[j].cpu, 0), std::max<int64_t>(use[j].mem - mine[j].mem, 0),
+                       std::max<int64_t>(use[j].gpu - mine[j].gpu, 0), std::max<int64_t>(use[j].pods - mine[j].pods, 0)};
+        Res& have = rows[slot[n]];
+        while (!have.covers(need)) {
+          const uint32_t v = choose_victim(at, n, running, [&](uint32_t x) { return evict[x] && !gone[x]; });
+          if (v == GROVE_NONE_U32) return fail(e, GROVE_ERR_STATE, "reclaim pass: a preemptor's node cannot be freed");
+          evict_one(v, g);
+        }
+        have.add(need, -1);
+      }
+      if (holds) gone[r] = 1;   // released; its leftover came back when the class cycle ended (k_hold_release)
+      // (b) the queue step: g's chain, leaf first, back within its caps on the resources g uses
+      const uint32_t gq = gang_queue[g];
+      if (gq != GROVE_NONE_U32) {
+        int64_t U[3] = {0, 0, 0};
+        for (const Res& u : use) { U[0] += u.cpu; U[1] += u.mem; U[2] += u.gpu; }
+        account(gq, U, 1);
+        for (uint32_t Qx = gq; Qx != GROVE_NONE_U32; Qx = queues[Qx].parent) {
+          for (;;) {
+            uint32_t over = 0;   // the resources g uses on which Qx is over its finite cap
+            for (int t = 0; t < 3; ++t)
+              if (U[t] > 0 && cap[Qx][t] != GROVE_QUEUE_UNLIMITED && load[Qx][t] > 0 && uint64_t(load[Qx][t]) > cap[Qx][t]) over |= 1u << t;
+            if (!over) break;
+            uint32_t v = GROVE_NONE_U32;   // by the victim rule, among the evictable gangs in Qx's subtree that hold some of it
+            for (uint32_t x = 0; x < n_running; ++x) {
+              if (!evict[x] || gone[x] || run_queue[x] == GROVE_NONE_U32 || !in_subtree(run_queue[x], Qx)) continue;
+              bool holds_some = false;
+              for (int t = 0; t < 3; ++t) holds_some |= ((over >> t) & 1u) && usage[x][t] > 0;
+              if (holds_some && evicted_before(running, x, v)) v = x;
+            }
+            if (v == GROVE_NONE_U32) return fail(e, GROVE_ERR_STATE, "reclaim pass: a preemptor's queue cannot be brought within its limit");
+            evict_one(v, g);
+          }
+        }
+      }
+      grove_gang_status_t o = sp;
+      o.reserved0 = uint16_t(flag | (sp.reserved0 & GROVE_STATUS_SURPLUS_CAPPED));
+      merge_gang(snap, sub, k, o, ssp);
+      extra[g] = std::move(pl);
+      st0.gangs_admitted += 1; st0.gangs_rejected -= 1;
+    }
+    for (uint32_t n : used) slot[n] = -1;
+    rc = patch_nodes(e, back, st0); if (rc) return rc;
+    // back to the free table: take off what the evictable running gangs that still stand hold
+    for (uint32_t r = 0; r < n_running; ++r) evict[r] = evict[r] && !gone[r];
+    CU_TRY(e, cudaMemcpyAsync(e->d_rc_evict.p, evict.data(), n_running, cudaMemcpyHostToDevice, e->stream));
+    k_reclaim_view<<<nblk, 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_real.p, csr.off, csr.ent, e->d_rc_evict.p, N, 0u);
+    CU_TRY(e, cudaGetLastError());
+    return GROVE_OK;
+  };
+  auto arm = [&]() -> cudaError_t {   // before the first class: the free table after the ordinary pass is kept aside
+    at = running_by_node(N, running, n_running, holdings);
+    slot.assign(N, -1);
+    return cudaMemcpyAsync(e->d_rc_base.p, e->d_nres.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToDevice, e->stream);
+  };
+
+  if (!quotas) {
+    // priority classes: every priority of a rejected gang, descending, while E(p) -- the standing running gangs of a priority below
+    // p -- is non-empty (it only shrinks from one class to the next)
+    std::vector<int32_t> classes;
+    for (uint32_t g = 0; g < G; ++g) if (snap.status[g].state == GROVE_GANG_REJECTED) classes.push_back(snap.gangs[g].priority);
+    std::sort(classes.begin(), classes.end(), std::greater<int32_t>());
+    classes.erase(std::unique(classes.begin(), classes.end()), classes.end());
+    auto mark = [&](int32_t p) { for (uint32_t r = 0; r < n_running; ++r) evict[r] = !gone[r] && running[r].priority < p; };
+    if (!classes.empty()) mark(classes.front());
+    if (!classes.empty() && standing()) {
+      CU_TRY(e, arm());
+      Restore restore{e, &snap, running_queue ? &queues : nullptr, &gang_queue};
+      for (int32_t p : classes) {
+        mark(p);
+        if (!standing()) break;
+        std::vector<uint32_t> members;   // (one priority: submission order is rank order)
+        for (uint32_t g = 0; g < G; ++g)
+          if (snap.status[g].state == GROVE_GANG_REJECTED && snap.gangs[g].priority == p) members.push_back(g);
+        rc = run_class(members, GROVE_STATUS_PREEMPTOR, true); if (rc) return rc;
+      }
+      // the handle goes back to the caller's submission (and queue set); the device table is the free table
+      restore.armed = false;
+      rc = restore.put_back(); if (rc) return rc;
+    }
+  } else {
+    // queue classes: the queues of the rejected gangs, by ascending share at the start of the pass, ties by queue index; each
+    // against its donor set E(Q)
+    std::vector<uint32_t> classes;
+    for (uint32_t g = 0; g < G; ++g)
+      if (snap.status[g].state == GROVE_GANG_REJECTED && gang_queue[g] != GROVE_NONE_U32) classes.push_back(gang_queue[g]);
+    std::sort(classes.begin(), classes.end());
+    classes.erase(std::unique(classes.begin(), classes.end()), classes.end());
+    std::vector<Share> share(NQ);
+    for (uint32_t q : classes) share[q] = share_of(quotas[q], load[q]);
+    std::stable_sort(classes.begin(), classes.end(), [&](uint32_t a, uint32_t b) { return Share::less(share[a], share[b]); });
+    uint32_t scanned = 0;
+    DonorSet dn{};
+    if (!classes.empty()) { rc = upload_donors(e, running, n_running, run_queue.data(), queues, quotas, usage, &scanned, &dn); if (rc) return rc; }
+    if (scanned) {
+      CU_TRY(e, arm());
+      Restore restore{e, &snap, &queues, &gang_queue};
+      std::vector<long long> ld(size_t(NQ) * 3);
+      for (uint32_t Q : classes) {
+        // E(Q) on the device, from the current loads and the standing set
+        for (uint32_t q = 0; q < NQ; ++q) for (int k = 0; k < 3; ++k) ld[q * 3 + k] = load[q][k];
+        CU_TRY(e, cudaMemcpyAsync(e->d_dn_load.p, ld.data(), sizeof(long long) * ld.size(), cudaMemcpyHostToDevice, e->stream));
+        CU_TRY(e, cudaMemcpyAsync(e->d_rc_gone.p, gone.data(), n_running, cudaMemcpyHostToDevice, e->stream));
+        k_donor_scan<<<scanned, 256, 0, e->stream>>>(dn);
+        CU_TRY(e, cudaGetLastError());
+        k_donor_mark<<<(n_running + 255) / 256, 256, 0, e->stream>>>(dn, Q, n_running, e->d_rc_evict.p);
+        CU_TRY(e, cudaGetLastError());
+        CU_TRY(e, cudaMemcpyAsync(evict.data(), e->d_rc_evict.p, n_running, cudaMemcpyDeviceToHost, e->stream));
+        CU_TRY(e, cudaStreamSynchronize(e->stream));
+        st0.kernel_launches += 2;
+        if (!standing()) continue;   // an empty donor set: the members keep their ordinary-pass outcome
+        std::vector<uint32_t> members;
+        for (uint32_t g = 0; g < G; ++g)
+          if (snap.status[g].state == GROVE_GANG_REJECTED && gang_queue[g] == Q) members.push_back(g);
+        std::stable_sort(members.begin(), members.end(), [&](uint32_t a, uint32_t b) { return snap.gangs[a].priority > snap.gangs[b].priority; });
+        rc = run_class(members, GROVE_STATUS_RECLAIMER, false); if (rc) return rc;
+      }
+      restore.armed = false;
+      rc = restore.put_back(); if (rc) return rc;
+    }
   }
   st0.kernel_launches += 1;   // k_reclaim_check
   return publish_reclaim(e, snap.status, snap.place, extra, snap.sstat, st0, std::move(victims), stats);
@@ -2648,7 +2804,7 @@ int32_t grove_run_cycle_preempt(grove_engine_t* e, const grove_running_gang_t* r
   if (rc) return rc;
   rc = check_running(e, running, n_running, holdings, n_holdings);
   if (rc) return rc;
-  return reclaim_cycle(e, nullptr, running, n_running, holdings, nullptr, stats);
+  return reclaim_cycle(e, nullptr, running, n_running, holdings, nullptr, nullptr, stats);
 }
 
 int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs, const grove_running_gang_t* running,
@@ -2663,40 +2819,68 @@ int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replace
   if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse_preempt");
   const int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);
   if (rc) return rc;
-  return reclaim_cycle(e, replaces, running, n_running, holdings, nullptr, stats);
+  return reclaim_cycle(e, replaces, running, n_running, holdings, nullptr, nullptr, stats);
 }
 
-int32_t grove_run_cycle_preempt_queues(grove_engine_t* e, const grove_running_gang_t* running, uint32_t n_running,
-                                       const grove_holding_t* holdings, uint32_t n_holdings, const uint32_t* running_queue,
-                                       grove_cycle_stats_t* stats) {
-  static const char* kEntry = "grove_run_cycle_preempt_queues";
-  if (!e || (n_running && (!running || !running_queue)) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
-  if (e->sp_members) return refuse_spread(e, kEntry);
-  if (!e->fc_gangs.empty()) return refuse_fences(e, kEntry);
-  if (e->bp_members) return refuse_binpack(e, kEntry);
-  if (e->im_enrolled) return refuse_imex(e, kEntry);
-  if (!e->qu_given) return fail(e, GROVE_ERR_STATE, "grove_run_cycle_preempt_queues: no queue set given for the current submission (grove_set_queues)");
-  NoDiagnosis no_diag{e};
-  if (e->wide) return refuse_wide(e, kEntry);
+// The checks grove_run_cycle_preempt_queues and grove_run_cycle_reclaim_queues share.  First the sets the entries refuse (a refusal
+// here leaves grove_diagnose as it was) ...
+static int32_t check_queue_sets(grove_engine* e, const char* entry) {
+  if (e->sp_members) return refuse_spread(e, entry);
+  if (!e->fc_gangs.empty()) return refuse_fences(e, entry);
+  if (e->bp_members) return refuse_binpack(e, entry);
+  if (e->im_enrolled) return refuse_imex(e, entry);
+  if (!e->qu_given) { e->err = std::string(entry) + ": no queue set given for the current submission (grove_set_queues)"; return GROVE_ERR_STATE; }
+  return GROVE_OK;
+}
+
+// ... then the submission, the running gangs, and what the running gangs of each queue hold, within its used
+static int32_t check_queue_running(grove_engine* e, const char* entry, const grove_running_gang_t* running, uint32_t n_running,
+                                   const grove_holding_t* holdings, uint32_t n_holdings, const uint32_t* running_queue) {
+  const std::string kEntry(entry);
+  if (e->wide) return refuse_wide(e, entry);
   if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
   const int32_t rc = check_running(e, running, n_running, holdings, n_holdings);
   if (rc) return rc;
-  // what the running gangs of each queue hold: within its used
   const std::vector<grove_queue_t>& queues = e->qu_queues;
   const uint32_t NQ = uint32_t(queues.size());
   std::vector<std::array<int64_t, 3>> run_use(NQ, {0, 0, 0});
   for (uint32_t r = 0; r < n_running; ++r) {
     const uint32_t q = running_queue[r];
     if (q == GROVE_NONE_U32) continue;
-    if (q >= NQ) return fail(e, GROVE_ERR_INVALID_ARG, "grove_run_cycle_preempt_queues: running_queue names a queue out of range");
+    if (q >= NQ) { e->err = kEntry + ": running_queue names a queue out of range"; return GROVE_ERR_INVALID_ARG; }
     const std::array<int64_t, 3> u = usage_of(running[r], holdings);
     for (int k = 0; k < 3; ++k) run_use[q][k] += u[k];
   }
   for (uint32_t q = 0; q < NQ; ++q)
     for (int k = 0; k < 3; ++k)
-      if (uint64_t(run_use[q][k]) > queues[q].used[k])
-        return fail(e, GROVE_ERR_INVALID_ARG, "grove_run_cycle_preempt_queues: the running gangs of a queue hold more than its used");
-  return reclaim_cycle(e, nullptr, running, n_running, holdings, running_queue, stats);
+      if (uint64_t(run_use[q][k]) > queues[q].used[k]) { e->err = kEntry + ": the running gangs of a queue hold more than its used"; return GROVE_ERR_INVALID_ARG; }
+  return GROVE_OK;
+}
+
+int32_t grove_run_cycle_preempt_queues(grove_engine_t* e, const grove_running_gang_t* running, uint32_t n_running,
+                                       const grove_holding_t* holdings, uint32_t n_holdings, const uint32_t* running_queue,
+                                       grove_cycle_stats_t* stats) {
+  if (!e || (n_running && (!running || !running_queue)) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
+  int32_t rc = check_queue_sets(e, "grove_run_cycle_preempt_queues");
+  if (rc) return rc;
+  NoDiagnosis no_diag{e};
+  rc = check_queue_running(e, "grove_run_cycle_preempt_queues", running, n_running, holdings, n_holdings, running_queue);
+  if (rc) return rc;
+  return reclaim_cycle(e, nullptr, running, n_running, holdings, running_queue, nullptr, stats);
+}
+
+int32_t grove_run_cycle_reclaim_queues(grove_engine_t* e, const grove_queue_quota_t* quotas, uint32_t n_queues,
+                                       const grove_running_gang_t* running, uint32_t n_running, const grove_holding_t* holdings,
+                                       uint32_t n_holdings, const uint32_t* running_queue, grove_cycle_stats_t* stats) {
+  if (!e || (n_queues && !quotas) || (n_running && (!running || !running_queue)) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
+  int32_t rc = check_queue_sets(e, "grove_run_cycle_reclaim_queues");
+  if (rc) return rc;
+  NoDiagnosis no_diag{e};
+  rc = check_queue_running(e, "grove_run_cycle_reclaim_queues", running, n_running, holdings, n_holdings, running_queue);
+  if (rc) return rc;
+  if (n_queues != e->qu_queues.size())
+    return fail(e, GROVE_ERR_INVALID_ARG, "grove_run_cycle_reclaim_queues: n_queues is not the number of queues of the set");
+  return reclaim_cycle(e, nullptr, running, n_running, holdings, running_queue, quotas, stats);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -416,7 +416,7 @@ Err GpuBackend::EncodeLocked(const std::vector<Node>& nodes, Tables* out, const 
   // PodGangs the packed tables cannot hold are left out of the pass (and so is a scaled PodGang behind one); everybody else
   // is scheduled as usual
   // (a large PodGang -- SetLargePodGangs -- only when no running-gang cycle may run: those take no wide submission)
-  const bool runningCycles = preemption_ || reuse_ || reclaimReuse_;
+  const bool runningCycles = preemption_ || reuse_ || reclaimReuse_ || reclaimQueues_;
   for (const auto& kv : pending_) {
     std::string why = WhyNotEncodable(kv.second, large_);
     if (why.empty() && large_ && runningCycles) {
@@ -456,7 +456,8 @@ Err GpuBackend::EncodeLocked(const std::vector<Node>& nodes, Tables* out, const 
       wideAny |= large_ && !WhyNotEncodable(kv.second, false).empty();
       spreadAny |= spreadSetOf(kv.second) != nullptr;
     }
-    const bool withinQueues = preemptQueues_ && preemption_ && !reuse_ && !reclaimReuse_;   // grove_run_cycle_preempt_queues
+    // grove_run_cycle_preempt_queues / grove_run_cycle_reclaim_queues
+    const bool withinQueues = (reclaimQueues_ || (preemptQueues_ && preemption_)) && !reuse_ && !reclaimReuse_;
     const char* why = runningCycles && !withinQueues ? "queue limits are not applied while preemption or reservation reuse is on"
                       : consMax_ ? "queue limits are not applied while consolidation is on"
                       : guardMax_ ? "queue limits are not applied while the starvation guard is on"
@@ -664,6 +665,8 @@ Err GpuBackend::EncodeLocked(const std::vector<Node>& nodes, Tables* out, const 
       r.parent = q.Parent.empty() ? GROVE_NONE_U32 : idx.at(q.Parent);
       r.limit[0] = q.CpuMilli.value_or(GROVE_QUEUE_UNLIMITED); r.limit[1] = q.MemMiB.value_or(GROVE_QUEUE_UNLIMITED); r.limit[2] = q.Gpu.value_or(GROVE_QUEUE_UNLIMITED);
       out->queues.push_back(r);
+      out->quotas.push_back(grove_queue_quota_t{{q.DeservedCpuMilli.value_or(GROVE_QUEUE_UNLIMITED), q.DeservedMemMiB.value_or(GROVE_QUEUE_UNLIMITED),
+                                                 q.DeservedGpu.value_or(GROVE_QUEUE_UNLIMITED)}});
     }
     for (const auto& [key, qn] : queueOf_) {
       auto it = idx.find(qn); auto rg = running_.find(key);
@@ -764,12 +767,17 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
   // running PodGangs -> the reclaim pass's / reservation reuse's tables (holdings on nodes that left the snapshot are dropped)
   std::vector<grove_running_gang_t> run; std::vector<grove_holding_t> held; std::vector<std::string> runNames;
   bool preempt = false, reuse = false, both = false;   // both: SetReclaimWithReuse, one grove_run_cycle_reuse_preempt
+  bool acrossQueues = false;                           // SetReclaimAcrossQueues with queue members: grove_run_cycle_reclaim_queues
   std::vector<uint32_t> replaces;   // reservation reuse: per gang row, the running gang it is the new version of
   {
     std::lock_guard<std::mutex> l(mu_);
     if (preemption_ && reuse_ && !reclaimReuse_) return mkerr("ERR_SYNC_PODGANG", "RunCycle", "preemption and reservation reuse cannot both be on");
+    if (reclaimQueues_ && preemptQueues_)
+      return mkerr("ERR_SYNC_PODGANG", "RunCycle", "reclaim across queues and preemption within queues cannot both be on");
     both = reclaimReuse_ && !running_.empty();
-    preempt = (preemption_ || reclaimReuse_) && !running_.empty();
+    // (Encode keeps queue members in the pass only when reuse and reuse with reclaim are off)
+    acrossQueues = reclaimQueues_ && !t.queues.empty() && !running_.empty();
+    preempt = ((preemption_ || reclaimReuse_) && !running_.empty()) || acrossQueues;
     reuse = (reuse_ || reclaimReuse_) && !running_.empty();
     if (preempt || reuse) {
       std::map<std::string, uint32_t> nodeIdx;
@@ -876,7 +884,8 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
   }
   if (both) { if (auto e = chk(grove_run_cycle_reuse_preempt(engine_, replaces.data(), uint32_t(replaces.size()), run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_reuse_preempt")) return e; }
   else if (reuse) { if (auto e = chk(grove_run_cycle_reuse(engine_, replaces.data(), uint32_t(replaces.size()), run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_reuse")) return e; }
-  else if (preempt && !t.queues.empty()) {   // (Encode keeps queue members in a pass with preemption only with SetPreemptionWithinQueues)
+  else if (preempt && !t.queues.empty()) {   // (Encode keeps queue members in a pass with preemption only with SetPreemptionWithinQueues
+                                             // or SetReclaimAcrossQueues)
     std::vector<uint32_t> runQueue(run.size(), GROVE_NONE_U32);   // the queue each running PodGang was scheduled in
     {
       std::lock_guard<std::mutex> l(mu_);
@@ -884,8 +893,11 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
         if (auto it = queueOf_.find(runNames[r]); it != queueOf_.end())
           if (auto n = std::find(t.queueNames.begin(), t.queueNames.end(), it->second); n != t.queueNames.end()) runQueue[r] = uint32_t(n - t.queueNames.begin());
     }
-    if (auto e = chk(grove_run_cycle_preempt_queues(engine_, run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), runQueue.data(), &st),
-                     "grove_run_cycle_preempt_queues")) return e;
+    if (acrossQueues) {
+      if (auto e = chk(grove_run_cycle_reclaim_queues(engine_, t.quotas.data(), uint32_t(t.quotas.size()), run.data(), uint32_t(run.size()), held.data(),
+                                                      uint32_t(held.size()), runQueue.data(), &st), "grove_run_cycle_reclaim_queues")) return e;
+    } else if (auto e = chk(grove_run_cycle_preempt_queues(engine_, run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), runQueue.data(), &st),
+                            "grove_run_cycle_preempt_queues")) return e;
   }
   else if (preempt) { if (auto e = chk(grove_run_cycle_preempt(engine_, run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_preempt")) return e; }
   else if (consolidate) {
@@ -1002,7 +1014,10 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
     if (auto e = chk(grove_get_victims(engine_, vs.data(), uint32_t(vs.size()), &nv), "grove_get_victims")) return e;
     for (uint32_t i = 0; i < nv; ++i) {
       PodGangStatus s; s.Phase = PodGangPhase::Running; s.Scheduled = true;
-      s.DisruptionTarget = true; s.DisruptionMessage = "preempted by higher priority PodGang " + t.gangNames[vs[i].preemptor];
+      s.DisruptionTarget = true;
+      const uint32_t g = vs[i].preemptor;
+      s.DisruptionMessage = acrossQueues ? "reclaimed by PodGang " + t.gangNames[g] + " of queue " + t.queueNames[t.queueOf[g]]
+                                         : "preempted by higher priority PodGang " + t.gangNames[g];
       (*statuses)[runNames[vs[i].running]] = s;
       running_.erase(runNames[vs[i].running]);
     }

@@ -212,10 +212,13 @@ struct TopologySpread {
 };
 
 // a KAI queue's hard limits (scheduling.run.ai/v2 Queue: spec.parentQueue, spec.resources.{cpu,memory,gpu}.limit; DESIGN.md
-// section 1 "Queue limits"), in the engine's units: millicores, MiB, GPUs.  nullopt = no limit (KAI's -1).
+// section 1 "Queue limits"), in the engine's units: millicores, MiB, GPUs.  nullopt = no limit (KAI's -1).  The deserved quota
+// (spec.resources.{cpu,memory,gpu}.quota; DESIGN.md section 1 "Reclaim across queues") in the same units; nullopt = KAI's -1, the
+// queue deserves whatever it holds.  Only SetReclaimAcrossQueues reads it.
 struct Queue {
   std::string Parent;                            // "" = a root queue; otherwise a queue set earlier
   std::optional<uint64_t> CpuMilli, MemMiB, Gpu;
+  std::optional<uint64_t> DeservedCpuMilli, DeservedMemMiB, DeservedGpu;
 };
 
 // packed tables of one cycle, as handed to libgrove_place.so
@@ -238,6 +241,7 @@ struct Tables {
   // queue limits (SetQueue): the queues (parents first) with what the running PodGangs of each hold, each gang row's queue
   // (GROVE_NONE_U32: none)
   std::vector<grove_queue_t> queues;
+  std::vector<grove_queue_quota_t> quotas;              // per queue of `queues`, its deserved quota
   std::vector<std::string> queueNames;
   std::vector<uint32_t> queueOf;
   // consolidation (SetConsolidation): rows [specRow, gangs.size()) are gated rows restating running PodGangs, which makes them
@@ -295,6 +299,13 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   // queues are the ones their PodGangs were scheduled in.  A member its queue chain turns away may then evict lower-priority
   // PodGangs of its own queues; victims get DisruptionTarget naming their preemptor, as with preemption.  Off by default.
   void SetPreemptionWithinQueues(bool on) { std::lock_guard<std::mutex> l(mu_); preemptQueues_ = on; }
+  // Reclaim across queues (KAI's reclaim action; DESIGN.md section 1 "Reclaim across queues"): with it on (reservation reuse and
+  // reuse with reclaim off), queue members stay in the pass and a pass with members and running PodGangs is
+  // grove_run_cycle_reclaim_queues, with each Queue's deserved quota and each running PodGang's queue the one it was scheduled in.
+  // A queue below its quota may then evict running PodGangs of queues above theirs, whatever the priorities; victims get
+  // DisruptionTarget naming the reclaimer and its queue.  Off by default; a cycle with both this and SetPreemptionWithinQueues on
+  // fails.
+  void SetReclaimAcrossQueues(bool on) { std::lock_guard<std::mutex> l(mu_); reclaimQueues_ = on; }
   // Large PodGangs: with it on, PodGangs of up to GROVE_MAX_WIDE_GANG_PODS pods (PodGroups of up to as many) are encoded and a
   // cycle submits through grove_submit_gangs_wide; ValidatePodCliqueSet accepts base PodGangs of that size.  The running-gang
   // cycles (preemption, reservation reuse, reuse with reclaim) do not take such PodGangs: while one of those switches is on too,
@@ -401,6 +412,7 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   bool reuse_ = false;
   bool reclaimReuse_ = false;
   bool preemptQueues_ = false;
+  bool reclaimQueues_ = false;
   bool large_ = false;
   bool explain_ = false;
   std::string binpackKey_;                             // bin-packing level (off: empty)

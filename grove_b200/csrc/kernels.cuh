@@ -8,6 +8,7 @@
 //   relax.cuh    k_select / k_apply / k_detect / k_fold    the relaxation that makes the evaluations of all gangs
 //                agree with the sequential, priority-ordered pass; k_fin_* / k_emit  outputs
 //   reclaim.cuh  k_reclaim_*  reclaim-class views over the running gangs' holdings (grove_run_cycle_reuse_preempt)
+//   donor.cuh    k_donor_scan / k_donor_mark  the donor set of a reclaim-across-queues class (grove_run_cycle_reclaim_queues)
 //   diagnose.cuh k_diag_*  why each rejected gang did not fit, after the cycle (grove_diagnose)
 //   spread.cuh   k_spread_classes / k_spread  allowed level-l_s domains of the topology spread members (grove_set_spread)
 //   fence.cuh    k_fence_have / k_fence_pick / k_fence_status  the domain each fencing gang fences (grove_set_fences)
@@ -28,6 +29,7 @@
 #include "admit.cuh"
 #include "relax.cuh"
 #include "reclaim.cuh"
+#include "donor.cuh"
 #include "diagnose.cuh"
 #include "spread.cuh"
 #include "fence.cuh"

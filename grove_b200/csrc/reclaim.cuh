@@ -1,9 +1,10 @@
-// Device-resident reclaim views of grove_run_cycle_reuse_preempt (DESIGN.md section 1, "Reuse with reclaim").
+// Device-resident reclaim views of the reclaim loop (DESIGN.md section 1, "Reuse with reclaim", "Reclaim across queues").
 //
 // The running gangs' holdings are uploaded once per call as a per-node CSR over the sorted node order: row n lists every
 // (running gang, what it holds on n), running gangs ascending.  A mask marks the running gangs that are gone (released or
-// evicted).  A class view is the committed table plus the standing holdings of the running gangs below the class's priority;
-// one thread per node sums its own row, so no atomics and the table does not depend on thread order.
+// evicted); an evict mask marks the standing running gangs a class may evict (below the class's priority, or the donor set of
+// donor.cuh).  A class view is the committed table plus what they hold; one thread per node sums its own row, so no atomics and the
+// table does not depend on thread order.
 #pragma once
 #include "common.cuh"
 
@@ -27,15 +28,17 @@ __global__ void __launch_bounds__(256) k_reclaim_check(const uint4* nres, Reclai
   if (v[0] > 0xFFFFFFFFull || v[1] > 0xFFFFFFFFull || v[2] > 0xFFFFu || v[3] > 0xFFFFu) *bad = 1u;
 }
 
-// add > 0: real = the committed table as it is (the class's free table), then table += standing holdings of priority < p (the
-// class view).  add == 0: table -= the same sum (back to the free table once the class's victims are marked gone).
-__global__ void __launch_bounds__(256) k_reclaim_view(uint4* nres, uint4* real, ReclaimCsr c, uint32_t N, int32_t p, uint32_t add) {
+// add > 0: real = the committed table as it is (the class's free table), then table += the holdings of the running gangs the
+// evict mask marks (the class view: the standing gangs the class may evict).  add == 0: table -= the same sum, with the mask then
+// marking those of them still standing (back to the free table once the class's victims are gone).
+__global__ void __launch_bounds__(256) k_reclaim_view(uint4* nres, uint4* real, const uint32_t* off, const uint4* ent, const uint8_t* evict,
+                                                      uint32_t N, uint32_t add) {
   const uint32_t n = blockIdx.x * blockDim.x + threadIdx.x;
   if (n >= N) return;
   uint32_t s0 = 0, s1 = 0, s2 = 0;   // (gpu | pods << 16 sums field by field: the check above rules out a carry)
-  for (uint32_t i = c.off[n]; i < c.off[n + 1]; ++i) {
-    const uint4 h = c.ent[i];
-    if (!c.gone[h.x] && c.prio[h.x] < p) { s0 += h.y; s1 += h.z; s2 += h.w; }
+  for (uint32_t i = off[n]; i < off[n + 1]; ++i) {
+    const uint4 h = ent[i];
+    if (evict[h.x]) { s0 += h.y; s1 += h.z; s2 += h.w; }
   }
   uint4 r = nres[n];
   if (add) real[n] = r;

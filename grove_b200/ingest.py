@@ -266,8 +266,8 @@ def compute_domains(podgangs, template_pod_spec, intern=None):
     return out
 
 
-def _queue_limit(res, key, scale):
-    lim = ((res or {}).get(key) or {}).get("limit", -1)
+def _queue_limit(res, key, scale, field="limit"):
+    lim = ((res or {}).get(key) or {}).get(field, -1)
     if lim is None or float(lim) < 0:
         return T.QUEUE_UNLIMITED
     return int(_quantity(lim) * scale)
@@ -309,6 +309,19 @@ def queues_from_manifests(queue_docs, podgangs, podgroup_queue, used=None):
         if named and next(iter(named)) in idx:
             gq[g] = idx[next(iter(named))]
     return q, gq, names
+
+
+def queue_quotas_from_manifests(queue_docs, names):
+    """Queue manifests + the queue names in table order (as queues_from_manifests returns them) -> tables.queue_quota_dt[n] for
+    grove_run_cycle_reclaim_queues.  spec.resources.{cpu,memory,gpu}.quota is the queue's deserved quota, -1 (or absent) none; the
+    units are those of the limits (cpu in cores x 1000, memory in MiB, gpu in whole GPUs)."""
+    docs = {d["metadata"]["name"]: d for d in queue_docs if d and d.get("kind", "Queue") == "Queue"}
+    out = np.zeros(len(names), dtype=T.queue_quota_dt)
+    for i, n in enumerate(names):
+        res = (docs[n].get("spec") or {}).get("resources")
+        out["deserved"][i] = [_queue_limit(res, "cpu", 1000, "quota"), _queue_limit(res, "memory", 1, "quota"),
+                              _queue_limit(res, "gpu", 1, "quota")]
+    return out
 
 
 def tables_from_pcs(pcs: dict, topology_levels, tas_enabled: bool = True, class_mask=0xFFFF):

@@ -363,6 +363,24 @@ def c4_queues(gangs, cliques, share=0.3):
 
 
 
+def c4_queue_quotas(queues, running, holdings, running_queue, spread=0.6):
+    """Deserved GPU quotas for the synth.c4_queues layout with synth.queue_running's running gangs: leaf i deserves (1 - spread/2 +
+    spread * i / 7) times the GPUs its running gangs hold, so the first leaves are above their quota (donors) and the last below it
+    (reclaimers); each parent deserves the sum of its leaves' quotas.  cpu and memory stay unlimited -> tables.queue_quota_dt[10]"""
+    gpu = np.zeros(len(queues), dtype=np.int64)
+    for r in range(len(running)):
+        if running_queue[r] != T.NONE_U32:
+            o, n = int(running["holding_off"][r]), int(running["n_holdings"][r])
+            gpu[int(running_queue[r])] += int(holdings["gpu"][o: o + n].astype(np.int64).sum())
+    q = np.zeros(len(queues), dtype=T.queue_quota_dt)
+    q["deserved"] = T.QUEUE_UNLIMITED
+    for i in range(8):
+        q["deserved"][2 + i, 2] = int(gpu[2 + i] * (1 - spread / 2 + spread * i / 7))
+    q["deserved"][0, 2] = int(q["deserved"][2:6, 2].sum())
+    q["deserved"][1, 2] = int(q["deserved"][6:10, 2].sum())
+    return q
+
+
 def queue_running(tables, queues, gang_queue, placements, status, seed=0, boost=2, share=0.5):
     """A running-gang layout for a queue set (synth.c4_queues): the gangs a queue cycle over `tables` admitted (its placements and
     statuses) run in their queues at priorities 0-2, and the submission is the same gangs again at priorities 0-2, about `share` of

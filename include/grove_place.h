@@ -152,7 +152,8 @@ typedef struct grove_gang_status {
                               GROVE_STATUS_SPREAD_SKEWED = a SOFT spread member placed outside its allowed domains,
                               GROVE_STATUS_FENCING = a REJECTED fencing gang whose fence held (grove_set_fences),
                               GROVE_STATUS_OVER_LIMIT / GROVE_STATUS_SURPLUS_CAPPED = a queue member held back by its queue
-                              chain's limits (grove_set_queues); else 0 */
+                              chain's limits (grove_set_queues), GROVE_STATUS_RECLAIMER = admitted by the class pass of
+                              grove_run_cycle_reclaim_queues; else 0 */
   uint16_t score_num;      /* PlacementScore = score_num / score_den (podgang.go:187-189): over the gang, its scopes and
                               its cliques that carry a pack constraint, (levels honoured) / (levels asked for), where
                               asked = Preferred if set else Required; 1/1 when nothing was asked or everything held;
@@ -554,6 +555,42 @@ int32_t grove_set_queues(grove_engine_t* e, const grove_queue_t* queues, uint32_
  * for the inputs grove_run_cycle_preempt rejects, a running_queue entry out of range, or running usage of a queue above its used.
  * grove_diagnose refuses the cycle that follows. */
 int32_t grove_run_cycle_preempt_queues(grove_engine_t* e, const grove_running_gang_t* running, uint32_t n_running,
+                                       const grove_holding_t* holdings, uint32_t n_holdings,
+                                       const uint32_t* running_queue, grove_cycle_stats_t* stats);
+
+/* ---- reclaim across queues -----------------------------------------------------------------------------
+ * A queue below its deserved quota takes room back from queues above theirs, whatever the priorities (DESIGN.md section 1,
+ * "Reclaim across queues"; after KAI-Scheduler's reclaim action and Queue `spec.resources.*.quota`).  Inputs are those of
+ * grove_run_cycle_preempt_queues plus one quota row per queue of the set: deserved[r] per resource (cpu milli, mem MiB, gpu;
+ * GROVE_QUEUE_UNLIMITED = KAI's quota -1, the queue deserves whatever it holds).  cap_X = min(limit_X, deserved_X) per resource.
+ * load_X is as in "reclaim within queue limits", kept up to date as gangs are evicted and admitted; the victim order is lowest
+ * priority first, then the highest running index; a running gang stands until it is evicted.
+ *   1. The ordinary pass: grove_run_cycle with the queue set.
+ *   2. Classes: every queue Q that is the queue of a gang the ordinary pass left REJECTED (OVER_LIMIT ones included), in ascending
+ *      order of share_Q at the start of the pass = the max over resources x with a finite deserved_Q[x] of load_Q[x] / deserved_Q[x]
+ *      (0/0 = 0, l/0 = +inf for l > 0, no finite quota = 0; compared exactly), ties by queue index.  Members M(Q): those gangs, in
+ *      rank order.
+ *   3. The donor set E(Q), fixed when class Q starts.  For a queue X and a standing running gang r of X's subtree, P_X(r) = what
+ *      the standing running gangs r' of X's subtree with r' no later than r in victim order hold; ok_X(r): load_X[x] - P_X(r)[x] >=
+ *      deserved_X[x] on every resource x that r holds with a finite deserved_X[x]; over_X(r): there is such an x.
+ *      D(r, Q) = chain(queue(r)) \ chain(Q).  r is in E(Q) when it has a queue, neither queue(r) nor Q lies in the other's chain,
+ *      ok_X(r) holds for every X of D(r, Q) and over_X(r) for some.  An empty E(Q) skips the class.
+ *   4. The members, one at a time in rank order, against the node view free + what E(Q) holds and the queue rules of
+ *      "queue limits" with load'_X = load_X - what the gangs of E(Q) in X's subtree hold and cap in place of limit.  Admitted:
+ *      GROVE_STATUS_RECLAIMER, ORed with GROVE_STATUS_SURPLUS_CAPPED; rejected again: its ordinary-pass status, flags included.
+ *   5. Victims of an admitted g, from the standing gangs of E(Q) only: (a) node by node, as grove_run_cycle_preempt evicts; (b) for
+ *      each X of chain(Q), leaf first, while load_X[r] > cap_X[r] for a resource r with U(g)[r] > 0 and a finite cap, the first gang
+ *      in victim order of E(Q) in X's subtree that holds some of such a resource.  An eviction returns the victim's holdings to the
+ *      free table and takes its usage off every queue of its chain.  grove_get_victims lists (victim, reclaimer) in eviction order.
+ * A victim never lies in its reclaimer's queue, an ancestor or its subtree, and may outrank its reclaimer.  Outputs through the
+ * usual getters; the queue set stays in place.  Refusals are those of grove_run_cycle_preempt_queues, plus GROVE_ERR_INVALID_ARG
+ * when n_queues is not the set's number of queues.  grove_diagnose refuses the cycle that follows. */
+#define GROVE_STATUS_RECLAIMER 0x80u /* grove_gang_status_t.reserved0: admitted by grove_run_cycle_reclaim_queues's class pass */
+typedef struct grove_queue_quota {
+  uint64_t deserved[3];             /* cpu milli, mem MiB, gpu; GROVE_QUEUE_UNLIMITED = whatever the queue holds */
+} grove_queue_quota_t;
+int32_t grove_run_cycle_reclaim_queues(grove_engine_t* e, const grove_queue_quota_t* quotas, uint32_t n_queues,
+                                       const grove_running_gang_t* running, uint32_t n_running,
                                        const grove_holding_t* holdings, uint32_t n_holdings,
                                        const uint32_t* running_queue, grove_cycle_stats_t* stats);
 

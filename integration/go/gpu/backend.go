@@ -54,6 +54,9 @@ type schedulerBackend struct {
 	// preemptQueues: with preempt also on, queue members stay in the pass and a pass with members is
 	// grove_run_cycle_preempt_queues (GpuBackend::SetPreemptionWithinQueues in the C++ mirror)
 	preemptQueues bool
+	// reclaimQueues: queue members stay in the pass and a pass with members and running gangs is grove_run_cycle_reclaim_queues
+	// with each queue's deserved quota (GpuBackend::SetReclaimAcrossQueues in the C++ mirror)
+	reclaimQueues bool
 	// largePodGangs: PodGangs of up to maxWideGangPods pods are encoded (a counts row per clique) and submitted through
 	// grove_submit_gangs_wide.  The reclaim pass takes no such PodGang: with preempt also on, one beyond maxGangPods pods or 255
 	// replicas is reported Unschedulable (GpuBackend::SetLargePodGangs in the C++ mirror).
@@ -106,6 +109,16 @@ func (b *schedulerBackend) SetPreemptionWithinQueues(on bool) {
 	b.mu.Lock()
 	defer b.mu.Unlock()
 	b.preemptQueues = on
+}
+
+// SetReclaimAcrossQueues: with it on, queue members stay in the pass, and a pass with members and running PodGangs runs
+// grove_run_cycle_reclaim_queues with each Queue's deserved quota: a queue below its quota may evict running PodGangs of queues
+// above theirs, whatever the priorities (DESIGN.md section 1 "Reclaim across queues").  Victims get DisruptionTarget naming the
+// reclaimer.  Off by default; a cycle with both this and SetPreemptionWithinQueues on fails.
+func (b *schedulerBackend) SetReclaimAcrossQueues(on bool) {
+	b.mu.Lock()
+	defer b.mu.Unlock()
+	b.reclaimQueues = on
 }
 
 // SetTopologySpread sets (nil: removes) the topology spread of PodCliqueSet pcs.  Its pending base PodGangs with a Required level
@@ -193,11 +206,13 @@ func (b *schedulerBackend) encodeSpread(t *tables, rows []*groveschedulerv1alpha
 	}
 }
 
-// Queue is a KAI queue's hard limits in the engine's units (millicores, MiB, GPUs; nil = no limit, KAI's -1), and its parent
-// ("" = a root queue).  GpuBackend::SetQueue in the C++ mirror; DESIGN.md section 1 "Queue limits".
+// Queue is a KAI queue's hard limits in the engine's units (millicores, MiB, GPUs; nil = no limit, KAI's -1), its deserved quota
+// in the same units (spec.resources.*.quota; nil = KAI's -1, read only by SetReclaimAcrossQueues), and its parent ("" = a root
+// queue).  GpuBackend::SetQueue in the C++ mirror; DESIGN.md section 1 "Queue limits" and "Reclaim across queues".
 type Queue struct {
-	Parent                string
-	CpuMilli, MemMiB, Gpu *uint64
+	Parent                                        string
+	CpuMilli, MemMiB, Gpu                         *uint64
+	DeservedCpuMilli, DeservedMemMiB, DeservedGpu *uint64
 }
 
 const labelQueue = "kai.scheduler/queue"
@@ -303,6 +318,9 @@ func (b *schedulerBackend) encodeQueues(t *tables, rows []*groveschedulerv1alpha
 		}
 		r.limit = [3]C.uint64_t{lim(q.CpuMilli), lim(q.MemMiB), lim(q.Gpu)}
 		t.queues = append(t.queues, r)
+		if b.reclaimQueues {
+			t.quotas = append(t.quotas, C.grove_queue_quota_t{deserved: [3]C.uint64_t{lim(q.DeservedCpuMilli), lim(q.DeservedMemMiB), lim(q.DeservedGpu)}})
+		}
 	}
 	for key, qn := range b.queueOf {
 		i, ok := idx[qn]
@@ -696,6 +714,10 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 		snap = append(snap, pg)
 	}
 	levels, eng, preempt, large, explain := b.levels, b.eng, b.preempt, b.largePodGangs, b.explainUnschedulable
+	if b.reclaimQueues && b.preemptQueues {
+		b.mu.Unlock()
+		return fmt.Errorf("reclaim across queues and preemption within queues cannot both be on")
+	}
 	imexOn := b.imex
 	imexWhy := "" // a pass that takes no ComputeDomain set: the enrolled PodGangs stay out
 	switch {
@@ -714,7 +736,7 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 	queuesOn := len(b.queues) > 0
 	queueWhy := "" // a pass that takes no queue set: its members stay out
 	switch {
-	case preempt && !b.preemptQueues:
+	case preempt && !b.preemptQueues && !b.reclaimQueues:
 		queueWhy = "queue limits are not applied while preemption is on"
 	case b.consMax > 0:
 		queueWhy = "queue limits are not applied while consolidation is on"
@@ -895,7 +917,7 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 	}
 	if queuesOn && queueWhy == "" {
 		b.encodeQueues(t, rows)
-		if preempt && len(t.queues) > 0 { // the queue of every running gang of t.running (runningKeys: its PodGang), or none
+		if (preempt || b.reclaimQueues) && len(t.queues) > 0 { // the queue of every running gang of t.running (runningKeys: its PodGang), or none
 			t.runningQueue = make([]C.uint32_t, len(t.running))
 			for r := range t.running {
 				t.runningQueue[r] = C.GROVE_NONE_U32
@@ -951,7 +973,7 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 		rejectedFor[k] = v
 	}
 	b.mu.Unlock()
-	res, err := eng.cycle(t, preempt, large, explain)
+	res, err := eng.cycle(t, preempt || len(t.quotas) > 0, large, explain)
 	if err != nil {
 		return err
 	}

@@ -74,6 +74,8 @@ type tables struct {
 	// reclaim within queue limits: the queue of each running gang of `running` (GROVE_NONE_U32: none); set only in a pass with
 	// preemption and queue members
 	runningQueue []C.uint32_t
+	// reclaim across queues: each queue's deserved quota, in `queues` order; set only with SetReclaimAcrossQueues
+	quotas []C.grove_queue_quota_t
 	queueNames []string
 	// consolidation (optional; ordinary passes only, never with fences): the target rows, and for each running gang of `running`
 	// the gated row that restates it (grove_run_cycle_consolidate)
@@ -148,7 +150,12 @@ func (e *engine) cycle(t *tables, preempt, large, explain bool) (*result, error)
 		if len(t.holdings) > 0 {
 			hp = &t.holdings[0]
 		}
-		if len(t.runningQueue) > 0 {
+		if len(t.runningQueue) > 0 && len(t.quotas) > 0 {
+			if err := e.err(C.grove_run_cycle_reclaim_queues(e.h, &t.quotas[0], C.uint32_t(len(t.quotas)), &t.running[0],
+				C.uint32_t(len(t.running)), hp, C.uint32_t(len(t.holdings)), &t.runningQueue[0], &r.stats)); err != nil {
+				return nil, err
+			}
+		} else if len(t.runningQueue) > 0 {
 			if err := e.err(C.grove_run_cycle_preempt_queues(e.h, &t.running[0], C.uint32_t(len(t.running)), hp,
 				C.uint32_t(len(t.holdings)), &t.runningQueue[0], &r.stats)); err != nil {
 				return nil, err
