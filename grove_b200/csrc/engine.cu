@@ -2507,11 +2507,12 @@ static Share share_of(const grove_queue_quota_t& q, const std::array<int64_t, 3>
 }
 
 // replaces (null: no gang replaces a running gang) as for grove_run_cycle_reuse; running_queue (null: no queue set) the queue of each
-// running gang in the queue set of the current submission; quotas (null: priority classes) one row per queue of that set, and then
-// the classes are queues (grove_run_cycle_reclaim_queues).  Inputs checked by the entry.
+// running gang in the queue set of the current submission; quotas (null: no queue classes) one row per queue of that set, and then
+// the queue classes run first (grove_run_cycle_reclaim_queues); priority: the priority classes run (after the queue classes, from
+// the state they leave: grove_run_cycle_reclaim_preempt_queues).  Inputs checked by the entry.
 static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const grove_running_gang_t* running, uint32_t n_running,
                              const grove_holding_t* holdings, const uint32_t* running_queue, const grove_queue_quota_t* quotas,
-                             grove_cycle_stats_t* stats) {
+                             bool priority, grove_cycle_stats_t* stats) {
   CU_TRY(e, cudaSetDevice(e->cfg.device));
   const uint32_t G = e->G, N = e->N, nblk = (N + 255) / 256;
   ReclaimCsr csr{};
@@ -2531,10 +2532,13 @@ static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const gr
   std::vector<std::array<int64_t, 3>> own(NQ, {0, 0, 0});   // own used, then followed through the cycle
   for (uint32_t q = 0; q < NQ; ++q) for (int k = 0; k < 3; ++k) own[q][k] = int64_t(std::min<uint64_t>(queues[q].used[k], uint64_t(1) << 62));
   std::vector<uint8_t> gone(std::max<uint32_t>(n_running, 1), 0);   // released or evicted
-  // the caps of the class pass: the limits, or with quotas min(limit, deserved)
-  std::vector<std::array<uint64_t, 3>> cap(NQ);
+  // the caps of a class: the limits for a priority class, min(limit, deserved) for a queue class
+  std::vector<std::array<uint64_t, 3>> limit(NQ), cap(NQ);
   for (uint32_t q = 0; q < NQ; ++q)
-    for (int k = 0; k < 3; ++k) cap[q][k] = quotas ? std::min(queues[q].limit[k], quotas[q].deserved[k]) : queues[q].limit[k];
+    for (int k = 0; k < 3; ++k) {
+      limit[q][k] = queues[q].limit[k];
+      cap[q][k] = quotas ? std::min(queues[q].limit[k], quotas[q].deserved[k]) : queues[q].limit[k];
+    }
 
   // 1. the ordinary pass: the cycle with holds (the reuse cycle; without replacements the ordinary cycle, under a queue set the
   // queue cycle).  An admitted new version's predecessor is released.
@@ -2576,10 +2580,11 @@ static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const gr
   RunningByNode at;
   std::vector<int32_t> slot;   // node (caller order) -> its row in `rows` while a class chooses its victims
 
-  // One class: its members (the gangs the ordinary pass rejected, in rank order) against the running gangs `evict` marks.  Its
-  // admitted members carry `flag`; give_back: a member admitted by the class cycle once none of them stands any more gives its room
-  // back (the priority classes' rule).
-  auto run_class = [&](const std::vector<uint32_t>& members, uint16_t flag, bool give_back) -> int32_t {
+  // One class: its members (gangs still rejected, in rank order) against the running gangs `evict` marks, under the queue caps
+  // `caps`.  Its admitted members carry `flag`; give_back: a member admitted by the class cycle once none of them stands any more
+  // gives its room back (the priority classes' rule).
+  auto run_class = [&](const std::vector<uint32_t>& members, const std::vector<std::array<uint64_t, 3>>& caps, uint16_t flag,
+                       bool give_back) -> int32_t {
     // 2. the class's members as a submission of their own.  A member holds its predecessor's holdings when that one still stands
     // and is not evictable; when it is, it is released instead.
     Sub sub;
@@ -2602,7 +2607,7 @@ static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const gr
       std::vector<std::array<int64_t, 3>> o(own);
       for (uint32_t r = 0; r < n_running; ++r)
         if (evict[r] && run_queue[r] != GROVE_NONE_U32) for (int k = 0; k < 3; ++k) o[run_queue[r]][k] -= usage[r][k];
-      for (uint32_t q = 0; q < NQ; ++q) for (int k = 0; k < 3; ++k) { cq[q].used[k] = uint64_t(o[q][k]); cq[q].limit[k] = cap[q][k]; }
+      for (uint32_t q = 0; q < NQ; ++q) for (int k = 0; k < 3; ++k) { cq[q].used[k] = uint64_t(o[q][k]); cq[q].limit[k] = caps[q][k]; }
       rc = install_queues(e, cq.data(), NQ, sub_queue.data()); if (rc) return rc;
     }
     grove_cycle_stats_t stp{};
@@ -2686,7 +2691,7 @@ static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const gr
           for (;;) {
             uint32_t over = 0;   // the resources g uses on which Qx is over its finite cap
             for (int t = 0; t < 3; ++t)
-              if (U[t] > 0 && cap[Qx][t] != GROVE_QUEUE_UNLIMITED && load[Qx][t] > 0 && uint64_t(load[Qx][t]) > cap[Qx][t]) over |= 1u << t;
+              if (U[t] > 0 && caps[Qx][t] != GROVE_QUEUE_UNLIMITED && load[Qx][t] > 0 && uint64_t(load[Qx][t]) > caps[Qx][t]) over |= 1u << t;
             if (!over) break;
             uint32_t v = GROVE_NONE_U32;   // by the victim rule, among the evictable gangs in Qx's subtree that hold some of it
             for (uint32_t x = 0; x < n_running; ++x) {
@@ -2720,34 +2725,19 @@ static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const gr
     slot.assign(N, -1);
     return cudaMemcpyAsync(e->d_rc_base.p, e->d_nres.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToDevice, e->stream);
   };
+  // armed once, before the first class of either loop; the handle goes back to the caller's submission (and queue set) after the
+  // last, and the device table is then the free table
+  Restore restore{e, &snap, running_queue ? &queues : nullptr, &gang_queue, false};
+  auto ensure_armed = [&]() -> int32_t {
+    if (restore.armed) return GROVE_OK;
+    CU_TRY(e, arm());
+    restore.armed = true;
+    return GROVE_OK;
+  };
 
-  if (!quotas) {
-    // priority classes: every priority of a rejected gang, descending, while E(p) -- the standing running gangs of a priority below
-    // p -- is non-empty (it only shrinks from one class to the next)
-    std::vector<int32_t> classes;
-    for (uint32_t g = 0; g < G; ++g) if (snap.status[g].state == GROVE_GANG_REJECTED) classes.push_back(snap.gangs[g].priority);
-    std::sort(classes.begin(), classes.end(), std::greater<int32_t>());
-    classes.erase(std::unique(classes.begin(), classes.end()), classes.end());
-    auto mark = [&](int32_t p) { for (uint32_t r = 0; r < n_running; ++r) evict[r] = !gone[r] && running[r].priority < p; };
-    if (!classes.empty()) mark(classes.front());
-    if (!classes.empty() && standing()) {
-      CU_TRY(e, arm());
-      Restore restore{e, &snap, running_queue ? &queues : nullptr, &gang_queue};
-      for (int32_t p : classes) {
-        mark(p);
-        if (!standing()) break;
-        std::vector<uint32_t> members;   // (one priority: submission order is rank order)
-        for (uint32_t g = 0; g < G; ++g)
-          if (snap.status[g].state == GROVE_GANG_REJECTED && snap.gangs[g].priority == p) members.push_back(g);
-        rc = run_class(members, GROVE_STATUS_PREEMPTOR, true); if (rc) return rc;
-      }
-      // the handle goes back to the caller's submission (and queue set); the device table is the free table
-      restore.armed = false;
-      rc = restore.put_back(); if (rc) return rc;
-    }
-  } else {
+  if (quotas) {
     // queue classes: the queues of the rejected gangs, by ascending share at the start of the pass, ties by queue index; each
-    // against its donor set E(Q)
+    // against its donor set E(Q) under the caps
     std::vector<uint32_t> classes;
     for (uint32_t g = 0; g < G; ++g)
       if (snap.status[g].state == GROVE_GANG_REJECTED && gang_queue[g] != GROVE_NONE_U32) classes.push_back(gang_queue[g]);
@@ -2760,8 +2750,7 @@ static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const gr
     DonorSet dn{};
     if (!classes.empty()) { rc = upload_donors(e, running, n_running, run_queue.data(), queues, quotas, usage, &scanned, &dn); if (rc) return rc; }
     if (scanned) {
-      CU_TRY(e, arm());
-      Restore restore{e, &snap, &queues, &gang_queue};
+      rc = ensure_armed(); if (rc) return rc;
       std::vector<long long> ld(size_t(NQ) * 3);
       for (uint32_t Q : classes) {
         // E(Q) on the device, from the current loads and the standing set
@@ -2780,11 +2769,34 @@ static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const gr
         for (uint32_t g = 0; g < G; ++g)
           if (snap.status[g].state == GROVE_GANG_REJECTED && gang_queue[g] == Q) members.push_back(g);
         std::stable_sort(members.begin(), members.end(), [&](uint32_t a, uint32_t b) { return snap.gangs[a].priority > snap.gangs[b].priority; });
-        rc = run_class(members, GROVE_STATUS_RECLAIMER, false); if (rc) return rc;
+        rc = run_class(members, cap, GROVE_STATUS_RECLAIMER, false); if (rc) return rc;
       }
-      restore.armed = false;
-      rc = restore.put_back(); if (rc) return rc;
     }
+  }
+  if (priority) {
+    // priority classes: every priority of a gang still rejected, descending, while E(p) -- the standing running gangs of a priority
+    // below p -- is non-empty (it only shrinks from one class to the next); each under the limits
+    std::vector<int32_t> classes;
+    for (uint32_t g = 0; g < G; ++g) if (snap.status[g].state == GROVE_GANG_REJECTED) classes.push_back(snap.gangs[g].priority);
+    std::sort(classes.begin(), classes.end(), std::greater<int32_t>());
+    classes.erase(std::unique(classes.begin(), classes.end()), classes.end());
+    auto mark = [&](int32_t p) { for (uint32_t r = 0; r < n_running; ++r) evict[r] = !gone[r] && running[r].priority < p; };
+    if (!classes.empty()) mark(classes.front());
+    if (!classes.empty() && standing()) {
+      rc = ensure_armed(); if (rc) return rc;
+      for (int32_t p : classes) {
+        mark(p);
+        if (!standing()) break;
+        std::vector<uint32_t> members;   // (one priority: submission order is rank order)
+        for (uint32_t g = 0; g < G; ++g)
+          if (snap.status[g].state == GROVE_GANG_REJECTED && snap.gangs[g].priority == p) members.push_back(g);
+        rc = run_class(members, limit, GROVE_STATUS_PREEMPTOR, true); if (rc) return rc;
+      }
+    }
+  }
+  if (restore.armed) {
+    restore.armed = false;
+    rc = restore.put_back(); if (rc) return rc;
   }
   st0.kernel_launches += 1;   // k_reclaim_check
   return publish_reclaim(e, snap.status, snap.place, extra, snap.sstat, st0, std::move(victims), stats);
@@ -2804,7 +2816,7 @@ int32_t grove_run_cycle_preempt(grove_engine_t* e, const grove_running_gang_t* r
   if (rc) return rc;
   rc = check_running(e, running, n_running, holdings, n_holdings);
   if (rc) return rc;
-  return reclaim_cycle(e, nullptr, running, n_running, holdings, nullptr, nullptr, stats);
+  return reclaim_cycle(e, nullptr, running, n_running, holdings, nullptr, nullptr, true, stats);
 }
 
 int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs, const grove_running_gang_t* running,
@@ -2819,7 +2831,7 @@ int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replace
   if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse_preempt");
   const int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);
   if (rc) return rc;
-  return reclaim_cycle(e, replaces, running, n_running, holdings, nullptr, nullptr, stats);
+  return reclaim_cycle(e, replaces, running, n_running, holdings, nullptr, nullptr, true, stats);
 }
 
 // The checks grove_run_cycle_preempt_queues and grove_run_cycle_reclaim_queues share.  First the sets the entries refuse (a refusal
@@ -2866,21 +2878,35 @@ int32_t grove_run_cycle_preempt_queues(grove_engine_t* e, const grove_running_ga
   NoDiagnosis no_diag{e};
   rc = check_queue_running(e, "grove_run_cycle_preempt_queues", running, n_running, holdings, n_holdings, running_queue);
   if (rc) return rc;
-  return reclaim_cycle(e, nullptr, running, n_running, holdings, running_queue, nullptr, stats);
+  return reclaim_cycle(e, nullptr, running, n_running, holdings, running_queue, nullptr, true, stats);
+}
+
+// grove_run_cycle_reclaim_queues, and with priority grove_run_cycle_reclaim_preempt_queues: the same inputs, the same refusals
+static int32_t reclaim_queues_entry(grove_engine* e, const char* entry, const grove_queue_quota_t* quotas, uint32_t n_queues,
+                                    const grove_running_gang_t* running, uint32_t n_running, const grove_holding_t* holdings,
+                                    uint32_t n_holdings, const uint32_t* running_queue, bool priority, grove_cycle_stats_t* stats) {
+  if (!e || (n_queues && !quotas) || (n_running && (!running || !running_queue)) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
+  int32_t rc = check_queue_sets(e, entry);
+  if (rc) return rc;
+  NoDiagnosis no_diag{e};
+  rc = check_queue_running(e, entry, running, n_running, holdings, n_holdings, running_queue);
+  if (rc) return rc;
+  if (n_queues != e->qu_queues.size()) { e->err = std::string(entry) + ": n_queues is not the number of queues of the set"; return GROVE_ERR_INVALID_ARG; }
+  return reclaim_cycle(e, nullptr, running, n_running, holdings, running_queue, quotas, priority, stats);
 }
 
 int32_t grove_run_cycle_reclaim_queues(grove_engine_t* e, const grove_queue_quota_t* quotas, uint32_t n_queues,
                                        const grove_running_gang_t* running, uint32_t n_running, const grove_holding_t* holdings,
                                        uint32_t n_holdings, const uint32_t* running_queue, grove_cycle_stats_t* stats) {
-  if (!e || (n_queues && !quotas) || (n_running && (!running || !running_queue)) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
-  int32_t rc = check_queue_sets(e, "grove_run_cycle_reclaim_queues");
-  if (rc) return rc;
-  NoDiagnosis no_diag{e};
-  rc = check_queue_running(e, "grove_run_cycle_reclaim_queues", running, n_running, holdings, n_holdings, running_queue);
-  if (rc) return rc;
-  if (n_queues != e->qu_queues.size())
-    return fail(e, GROVE_ERR_INVALID_ARG, "grove_run_cycle_reclaim_queues: n_queues is not the number of queues of the set");
-  return reclaim_cycle(e, nullptr, running, n_running, holdings, running_queue, quotas, stats);
+  return reclaim_queues_entry(e, "grove_run_cycle_reclaim_queues", quotas, n_queues, running, n_running, holdings, n_holdings,
+                              running_queue, false, stats);
+}
+
+int32_t grove_run_cycle_reclaim_preempt_queues(grove_engine_t* e, const grove_queue_quota_t* quotas, uint32_t n_queues,
+                                               const grove_running_gang_t* running, uint32_t n_running, const grove_holding_t* holdings,
+                                               uint32_t n_holdings, const uint32_t* running_queue, grove_cycle_stats_t* stats) {
+  return reclaim_queues_entry(e, "grove_run_cycle_reclaim_preempt_queues", quotas, n_queues, running, n_running, holdings, n_holdings,
+                              running_queue, true, stats);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -456,8 +456,8 @@ Err GpuBackend::EncodeLocked(const std::vector<Node>& nodes, Tables* out, const 
       wideAny |= large_ && !WhyNotEncodable(kv.second, false).empty();
       spreadAny |= spreadSetOf(kv.second) != nullptr;
     }
-    // grove_run_cycle_preempt_queues / grove_run_cycle_reclaim_queues
-    const bool withinQueues = (reclaimQueues_ || (preemptQueues_ && preemption_)) && !reuse_ && !reclaimReuse_;
+    // grove_run_cycle_preempt_queues / grove_run_cycle_reclaim_queues / grove_run_cycle_reclaim_preempt_queues
+    const bool withinQueues = (reclaimQueues_ || ((preemptQueues_ || reclaimThenPreempt_) && preemption_)) && !reuse_ && !reclaimReuse_;
     const char* why = runningCycles && !withinQueues ? "queue limits are not applied while preemption or reservation reuse is on"
                       : consMax_ ? "queue limits are not applied while consolidation is on"
                       : guardMax_ ? "queue limits are not applied while the starvation guard is on"
@@ -768,15 +768,18 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
   std::vector<grove_running_gang_t> run; std::vector<grove_holding_t> held; std::vector<std::string> runNames;
   bool preempt = false, reuse = false, both = false;   // both: SetReclaimWithReuse, one grove_run_cycle_reuse_preempt
   bool acrossQueues = false;                           // SetReclaimAcrossQueues with queue members: grove_run_cycle_reclaim_queues
+  bool thenPreempt = false;                            // SetReclaimThenPreempt with queue members: grove_run_cycle_reclaim_preempt_queues
   std::vector<uint32_t> replaces;   // reservation reuse: per gang row, the running gang it is the new version of
   {
     std::lock_guard<std::mutex> l(mu_);
     if (preemption_ && reuse_ && !reclaimReuse_) return mkerr("ERR_SYNC_PODGANG", "RunCycle", "preemption and reservation reuse cannot both be on");
-    if (reclaimQueues_ && preemptQueues_)
+    const bool reclaimThenPreempt = reclaimThenPreempt_ && preemption_;   // (whatever the two switches below say)
+    if (reclaimQueues_ && preemptQueues_ && !reclaimThenPreempt)
       return mkerr("ERR_SYNC_PODGANG", "RunCycle", "reclaim across queues and preemption within queues cannot both be on");
     both = reclaimReuse_ && !running_.empty();
     // (Encode keeps queue members in the pass only when reuse and reuse with reclaim are off)
-    acrossQueues = reclaimQueues_ && !t.queues.empty() && !running_.empty();
+    thenPreempt = reclaimThenPreempt && !t.queues.empty() && !running_.empty();
+    acrossQueues = !thenPreempt && reclaimQueues_ && !t.queues.empty() && !running_.empty();
     preempt = ((preemption_ || reclaimReuse_) && !running_.empty()) || acrossQueues;
     reuse = (reuse_ || reclaimReuse_) && !running_.empty();
     if (preempt || reuse) {
@@ -884,8 +887,8 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
   }
   if (both) { if (auto e = chk(grove_run_cycle_reuse_preempt(engine_, replaces.data(), uint32_t(replaces.size()), run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_reuse_preempt")) return e; }
   else if (reuse) { if (auto e = chk(grove_run_cycle_reuse(engine_, replaces.data(), uint32_t(replaces.size()), run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_reuse")) return e; }
-  else if (preempt && !t.queues.empty()) {   // (Encode keeps queue members in a pass with preemption only with SetPreemptionWithinQueues
-                                             // or SetReclaimAcrossQueues)
+  else if (preempt && !t.queues.empty()) {   // (Encode keeps queue members in a pass with preemption only with SetPreemptionWithinQueues,
+                                             // SetReclaimAcrossQueues or SetReclaimThenPreempt)
     std::vector<uint32_t> runQueue(run.size(), GROVE_NONE_U32);   // the queue each running PodGang was scheduled in
     {
       std::lock_guard<std::mutex> l(mu_);
@@ -893,7 +896,10 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
         if (auto it = queueOf_.find(runNames[r]); it != queueOf_.end())
           if (auto n = std::find(t.queueNames.begin(), t.queueNames.end(), it->second); n != t.queueNames.end()) runQueue[r] = uint32_t(n - t.queueNames.begin());
     }
-    if (acrossQueues) {
+    if (thenPreempt) {
+      if (auto e = chk(grove_run_cycle_reclaim_preempt_queues(engine_, t.quotas.data(), uint32_t(t.quotas.size()), run.data(), uint32_t(run.size()),
+                                                              held.data(), uint32_t(held.size()), runQueue.data(), &st), "grove_run_cycle_reclaim_preempt_queues")) return e;
+    } else if (acrossQueues) {
       if (auto e = chk(grove_run_cycle_reclaim_queues(engine_, t.quotas.data(), uint32_t(t.quotas.size()), run.data(), uint32_t(run.size()), held.data(),
                                                       uint32_t(held.size()), runQueue.data(), &st), "grove_run_cycle_reclaim_queues")) return e;
     } else if (auto e = chk(grove_run_cycle_preempt_queues(engine_, run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), runQueue.data(), &st),
@@ -1016,7 +1022,9 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
       PodGangStatus s; s.Phase = PodGangPhase::Running; s.Scheduled = true;
       s.DisruptionTarget = true;
       const uint32_t g = vs[i].preemptor;
-      s.DisruptionMessage = acrossQueues ? "reclaimed by PodGang " + t.gangNames[g] + " of queue " + t.queueNames[t.queueOf[g]]
+      // (after both passes, the evictor's flag says which pass chose the victim)
+      const bool reclaimed = acrossQueues || (thenPreempt && (gs[g].reserved0 & GROVE_STATUS_RECLAIMER));
+      s.DisruptionMessage = reclaimed ? "reclaimed by PodGang " + t.gangNames[g] + " of queue " + t.queueNames[t.queueOf[g]]
                                          : "preempted by higher priority PodGang " + t.gangNames[g];
       (*statuses)[runNames[vs[i].running]] = s;
       running_.erase(runNames[vs[i].running]);

@@ -306,6 +306,12 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   // DisruptionTarget naming the reclaimer and its queue.  Off by default; a cycle with both this and SetPreemptionWithinQueues on
   // fails.
   void SetReclaimAcrossQueues(bool on) { std::lock_guard<std::mutex> l(mu_); reclaimQueues_ = on; }
+  // Reclaim, then preempt (KAI's reclaim action, then its preempt action; DESIGN.md section 1 "Reclaim, then preempt"): with it
+  // and SetPreemption on (reservation reuse and reuse with reclaim off), queue members stay in the pass and a pass with members
+  // and running PodGangs is grove_run_cycle_reclaim_preempt_queues, whatever SetReclaimAcrossQueues and
+  // SetPreemptionWithinQueues say.  Victims of the reclaim pass get DisruptionTarget naming the reclaimer and its queue, those of
+  // the preempt pass naming their preemptor.  Off by default.
+  void SetReclaimThenPreempt(bool on) { std::lock_guard<std::mutex> l(mu_); reclaimThenPreempt_ = on; }
   // Large PodGangs: with it on, PodGangs of up to GROVE_MAX_WIDE_GANG_PODS pods (PodGroups of up to as many) are encoded and a
   // cycle submits through grove_submit_gangs_wide; ValidatePodCliqueSet accepts base PodGangs of that size.  The running-gang
   // cycles (preemption, reservation reuse, reuse with reclaim) do not take such PodGangs: while one of those switches is on too,
@@ -413,6 +419,7 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   bool reclaimReuse_ = false;
   bool preemptQueues_ = false;
   bool reclaimQueues_ = false;
+  bool reclaimThenPreempt_ = false;
   bool large_ = false;
   bool explain_ = false;
   std::string binpackKey_;                             // bin-packing level (off: empty)

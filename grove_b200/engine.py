@@ -27,7 +27,7 @@ SYMBOLS = [
     "grove_build_score_matrix", "grove_run_cycle_preempt", "grove_get_victims", "grove_run_cycle_reuse",
     "grove_run_cycle_reuse_preempt", "grove_diagnose", "grove_set_spread", "grove_set_fences", "grove_set_queues",
     "grove_run_cycle_consolidate", "grove_get_moves", "grove_run_cycle_preempt_queues",
-    "grove_run_cycle_reclaim_queues",
+    "grove_run_cycle_reclaim_queues", "grove_run_cycle_reclaim_preempt_queues",
     "grove_set_binpack", "grove_get_binpack_picks", "grove_set_compute_domains", "grove_get_compute_domain_owners",
     "grove_shard_range", "grove_run_score_pass", "grove_shard_summary_device",
     "grove_debug_get_perm", "grove_debug_get_fit_row", "grove_debug_get_score_row",
@@ -275,9 +275,27 @@ class PlacementEngine:
                                                             _p(running_queue), _p(st)))
         return {k: st[k][0].item() for k in T.stats_dt.names}
 
+    def run_cycle_reclaim_preempt_queues(self, quotas: np.ndarray, running: np.ndarray, holdings: np.ndarray,
+                                         running_queue: np.ndarray) -> dict:
+        """the queue cycle of the set_queues set, then both queue eviction passes in KAI-Scheduler's order: reclaim across queues
+        (its admitted gangs carry tables.STATUS_RECLAIMER), then reclaim within queue limits for every gang still rejected, from
+        the state the first pass left (tables.STATUS_PREEMPTOR).  Inputs as for run_cycle_reclaim_queues (include/grove_place.h
+        "reclaim, then preempt"); victims() lists the evictions of both passes, the reclaim pass's first"""
+        quotas = np.ascontiguousarray(quotas, dtype=T.queue_quota_dt)
+        running = np.ascontiguousarray(running, dtype=T.running_dt)
+        holdings = np.ascontiguousarray(holdings, dtype=T.holding_dt)
+        running_queue = np.ascontiguousarray(running_queue, dtype=np.uint32)
+        if len(running_queue) != len(running):
+            raise ValueError("one running_queue entry per running gang")
+        st = np.zeros(1, dtype=T.stats_dt)
+        self._check(self.lib.grove_run_cycle_reclaim_preempt_queues(self.h, _p(quotas), C.c_uint32(len(quotas)), _p(running),
+                                                                    C.c_uint32(len(running)), _p(holdings), C.c_uint32(len(holdings)),
+                                                                    _p(running_queue), _p(st)))
+        return {k: st[k][0].item() for k in T.stats_dt.names}
+
     def victims(self) -> np.ndarray:
         """(running gang, preemptor gang) pairs of the last run_cycle_preempt / run_cycle_reuse_preempt /
-        run_cycle_preempt_queues / run_cycle_reclaim_queues: the caller sets
+        run_cycle_preempt_queues / run_cycle_reclaim_queues / run_cycle_reclaim_preempt_queues: the caller sets
         DisruptionTarget on them"""
         n = C.c_uint32(0)
         self._check(self.lib.grove_get_victims(self.h, None, C.c_uint32(0), C.byref(n)))

@@ -98,7 +98,8 @@ QUEUE_UNLIMITED = 0xFFFFFFFFFFFFFFFF   # a queue limit that is not set (KAI's -1
 STATUS_OVER_LIMIT = 0x20          # status reserved0: REJECTED by its queue chain's headroom, not evaluated
 STATUS_SURPLUS_CAPPED = 0x40      # status reserved0: ADMITTED with fewer best-effort pods allowed than it asked for
 queue_dt = np.dtype([("parent", np.uint32), ("reserved", np.uint32), ("limit", "<u8", (3,)), ("used", "<u8", (3,))])
-STATUS_RECLAIMER = 0x80           # status reserved0: admitted by the class pass of grove_run_cycle_reclaim_queues
+STATUS_RECLAIMER = 0x80           # status reserved0: admitted by the class pass of grove_run_cycle_reclaim_queues (or
+                                  # the reclaim pass of grove_run_cycle_reclaim_preempt_queues)
 queue_quota_dt = np.dtype([("deserved", "<u8", (3,))])   # per resource, QUEUE_UNLIMITED = whatever the queue holds (KAI's -1)
 
 assert node_dt.itemsize == 32 and clique_dt.itemsize == 16 and scope_dt.itemsize == 8

@@ -153,7 +153,8 @@ typedef struct grove_gang_status {
                               GROVE_STATUS_FENCING = a REJECTED fencing gang whose fence held (grove_set_fences),
                               GROVE_STATUS_OVER_LIMIT / GROVE_STATUS_SURPLUS_CAPPED = a queue member held back by its queue
                               chain's limits (grove_set_queues), GROVE_STATUS_RECLAIMER = admitted by the class pass of
-                              grove_run_cycle_reclaim_queues; else 0 */
+                              grove_run_cycle_reclaim_queues (or the reclaim pass of
+                              grove_run_cycle_reclaim_preempt_queues, whose preempt pass sets GROVE_STATUS_PREEMPTOR); else 0 */
   uint16_t score_num;      /* PlacementScore = score_num / score_den (podgang.go:187-189): over the gang, its scopes and
                               its cliques that carry a pack constraint, (levels honoured) / (levels asked for), where
                               asked = Preferred if set else Required; 1/1 when nothing was asked or everything held;
@@ -593,6 +594,27 @@ int32_t grove_run_cycle_reclaim_queues(grove_engine_t* e, const grove_queue_quot
                                        const grove_running_gang_t* running, uint32_t n_running,
                                        const grove_holding_t* holdings, uint32_t n_holdings,
                                        const uint32_t* running_queue, grove_cycle_stats_t* stats);
+
+/* ---- reclaim, then preempt, across and within queues ---------------------------------------------------
+ * Both queue eviction passes in one cycle, in KAI-Scheduler's order: its reclaim action, then its preempt action (DESIGN.md
+ * section 1, "Reclaim, then preempt").  Inputs, the queue set it runs on and the victim order are those of
+ * grove_run_cycle_reclaim_queues.
+ *   1. The ordinary pass: grove_run_cycle with the queue set.
+ *   2. The reclaim pass: steps 2-5 of "reclaim across queues" (queue classes in ascending share at the start of the pass, donor
+ *      sets E(Q), cap = min(limit, deserved), the node step and then the queue step).  Admitted: GROVE_STATUS_RECLAIMER, ORed
+ *      with GROVE_STATUS_SURPLUS_CAPPED.
+ *   3. The preempt pass: steps 2-3 of "reclaim within queue limits" from the state step 2 leaves (its free table, its queue
+ *      loads, its standing set).  Every gang still REJECTED -- OVER_LIMIT ones, members of skipped or unsuccessful queue classes
+ *      and gangs without a queue included; a reclaimer never -- is reconsidered once, in rank order, while E(p) (the standing
+ *      running gangs of a priority below p) is non-empty, under the queue LIMITS.  Admitted: GROVE_STATUS_PREEMPTOR, ORed with
+ *      GROVE_STATUS_SURPLUS_CAPPED; rejected again: its ordinary-pass status, flags included.
+ * grove_get_victims lists every eviction in order, those of step 2 first; the flag of the gang named in a pair says which pass
+ * chose it.  Outputs through the usual getters; the queue set stays in place.  Refusals are those of
+ * grove_run_cycle_reclaim_queues, with the same codes; grove_diagnose refuses the cycle that follows. */
+int32_t grove_run_cycle_reclaim_preempt_queues(grove_engine_t* e, const grove_queue_quota_t* quotas, uint32_t n_queues,
+                                               const grove_running_gang_t* running, uint32_t n_running,
+                                               const grove_holding_t* holdings, uint32_t n_holdings,
+                                               const uint32_t* running_queue, grove_cycle_stats_t* stats);
 
 /* K2: the topology-distance score matrix T[clique][node] = fit ? 1 + levels shared with the gang's anchor : 0 (u8) over the
  * snapshot the last cycle started from -- what a scheduler's Score extension point would hand out.  The admission does

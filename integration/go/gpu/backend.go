@@ -57,6 +57,10 @@ type schedulerBackend struct {
 	// reclaimQueues: queue members stay in the pass and a pass with members and running gangs is grove_run_cycle_reclaim_queues
 	// with each queue's deserved quota (GpuBackend::SetReclaimAcrossQueues in the C++ mirror)
 	reclaimQueues bool
+	// reclaimThenPreempt: with preempt also on, queue members stay in the pass and a pass with members and running gangs is
+	// grove_run_cycle_reclaim_preempt_queues, whatever preemptQueues and reclaimQueues say (GpuBackend::SetReclaimThenPreempt in
+	// the C++ mirror)
+	reclaimThenPreempt bool
 	// largePodGangs: PodGangs of up to maxWideGangPods pods are encoded (a counts row per clique) and submitted through
 	// grove_submit_gangs_wide.  The reclaim pass takes no such PodGang: with preempt also on, one beyond maxGangPods pods or 255
 	// replicas is reported Unschedulable (GpuBackend::SetLargePodGangs in the C++ mirror).
@@ -119,6 +123,17 @@ func (b *schedulerBackend) SetReclaimAcrossQueues(on bool) {
 	b.mu.Lock()
 	defer b.mu.Unlock()
 	b.reclaimQueues = on
+}
+
+// SetReclaimThenPreempt: with it and preemption on, queue members stay in the pass, and a pass with members and running PodGangs
+// runs grove_run_cycle_reclaim_preempt_queues: reclaim across queues, then preemption within queue limits for every PodGang still
+// pending, in one cycle as KAI-Scheduler runs its reclaim and preempt actions (DESIGN.md section 1 "Reclaim, then preempt").  It
+// overrides SetReclaimAcrossQueues and SetPreemptionWithinQueues, whose combination then no longer fails.  Victims get
+// DisruptionTarget naming the PodGang that evicted them.  Off by default.
+func (b *schedulerBackend) SetReclaimThenPreempt(on bool) {
+	b.mu.Lock()
+	defer b.mu.Unlock()
+	b.reclaimThenPreempt = on
 }
 
 // SetTopologySpread sets (nil: removes) the topology spread of PodCliqueSet pcs.  Its pending base PodGangs with a Required level
@@ -318,7 +333,7 @@ func (b *schedulerBackend) encodeQueues(t *tables, rows []*groveschedulerv1alpha
 		}
 		r.limit = [3]C.uint64_t{lim(q.CpuMilli), lim(q.MemMiB), lim(q.Gpu)}
 		t.queues = append(t.queues, r)
-		if b.reclaimQueues {
+		if b.reclaimQueues || (b.reclaimThenPreempt && b.preempt) {
 			t.quotas = append(t.quotas, C.grove_queue_quota_t{deserved: [3]C.uint64_t{lim(q.DeservedCpuMilli), lim(q.DeservedMemMiB), lim(q.DeservedGpu)}})
 		}
 	}
@@ -714,7 +729,8 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 		snap = append(snap, pg)
 	}
 	levels, eng, preempt, large, explain := b.levels, b.eng, b.preempt, b.largePodGangs, b.explainUnschedulable
-	if b.reclaimQueues && b.preemptQueues {
+	thenPreempt := b.reclaimThenPreempt && preempt
+	if b.reclaimQueues && b.preemptQueues && !thenPreempt {
 		b.mu.Unlock()
 		return fmt.Errorf("reclaim across queues and preemption within queues cannot both be on")
 	}
@@ -736,7 +752,7 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 	queuesOn := len(b.queues) > 0
 	queueWhy := "" // a pass that takes no queue set: its members stay out
 	switch {
-	case preempt && !b.preemptQueues && !b.reclaimQueues:
+	case preempt && !b.preemptQueues && !b.reclaimQueues && !thenPreempt:
 		queueWhy = "queue limits are not applied while preemption is on"
 	case b.consMax > 0:
 		queueWhy = "queue limits are not applied while consolidation is on"
@@ -917,6 +933,7 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 	}
 	if queuesOn && queueWhy == "" {
 		b.encodeQueues(t, rows)
+		t.thenPreempt = thenPreempt
 		if (preempt || b.reclaimQueues) && len(t.queues) > 0 { // the queue of every running gang of t.running (runningKeys: its PodGang), or none
 			t.runningQueue = make([]C.uint32_t, len(t.running))
 			for r := range t.running {

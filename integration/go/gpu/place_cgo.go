@@ -76,6 +76,9 @@ type tables struct {
 	runningQueue []C.uint32_t
 	// reclaim across queues: each queue's deserved quota, in `queues` order; set only with SetReclaimAcrossQueues
 	quotas []C.grove_queue_quota_t
+	// reclaim, then preempt: with quotas and runningQueue, both passes in one grove_run_cycle_reclaim_preempt_queues; set only
+	// with SetReclaimThenPreempt and preemption
+	thenPreempt bool
 	queueNames []string
 	// consolidation (optional; ordinary passes only, never with fences): the target rows, and for each running gang of `running`
 	// the gated row that restates it (grove_run_cycle_consolidate)
@@ -150,7 +153,12 @@ func (e *engine) cycle(t *tables, preempt, large, explain bool) (*result, error)
 		if len(t.holdings) > 0 {
 			hp = &t.holdings[0]
 		}
-		if len(t.runningQueue) > 0 && len(t.quotas) > 0 {
+		if len(t.runningQueue) > 0 && len(t.quotas) > 0 && t.thenPreempt {
+			if err := e.err(C.grove_run_cycle_reclaim_preempt_queues(e.h, &t.quotas[0], C.uint32_t(len(t.quotas)), &t.running[0],
+				C.uint32_t(len(t.running)), hp, C.uint32_t(len(t.holdings)), &t.runningQueue[0], &r.stats)); err != nil {
+				return nil, err
+			}
+		} else if len(t.runningQueue) > 0 && len(t.quotas) > 0 {
 			if err := e.err(C.grove_run_cycle_reclaim_queues(e.h, &t.quotas[0], C.uint32_t(len(t.quotas)), &t.running[0],
 				C.uint32_t(len(t.running)), hp, C.uint32_t(len(t.holdings)), &t.runningQueue[0], &r.stats)); err != nil {
 				return nil, err
