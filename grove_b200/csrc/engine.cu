@@ -17,7 +17,9 @@
 #include <string>
 #include <vector>
 
+#include <cub/device/device_merge_sort.cuh>
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 
 #include "kernels.cuh"
 
@@ -245,7 +247,7 @@ struct grove_engine {
   DevBuf<uint8_t> d_dn_fin, d_dn_bits;
   // grove_diagnose (diagnose.cuh): whether the outputs on the device describe an ordinary cycle over the current inputs, the
   // per-node usage lists, the batch descriptors, the per-domain capacity sums and the records
-  enum Diag : uint8_t { kDiagNoCycle, kDiagReady, kDiagRunning, kDiagChanged, kDiagSpread, kDiagFence, kDiagImex } diag = kDiagNoCycle;
+  enum Diag : uint8_t { kDiagNoCycle, kDiagReady, kDiagRunning, kDiagChanged, kDiagSpread, kDiagFence, kDiagImex, kDiagFairShare } diag = kDiagNoCycle;
   DevBuf<uint32_t> d_dg_cnt, d_dg_off, d_dg_cur, d_dg_minr;
   DevBuf<uint4> d_dg_rec;
   DevBuf<DiagGang> d_dg_gang;
@@ -304,6 +306,19 @@ struct grove_engine {
   bool im_have_owners = false;             // im_owners holds the owners after the last cycle that ran with a set
   std::vector<uint32_t> h_im_rank_cd, h_im_owner;
   DevBuf<uint32_t> d_im_cd, d_im_rank_cd, d_im_owner, d_im_nenr;
+  // fair-share order (grove_set_fair_share; fairshare.cuh): the quotas of the queue set, kept with it; the turn order and the
+  // fixed-point counts of the last fair-share cycle; the tree and per-gang tables of O(R) and its sort / scan buffers
+  bool fs_given = false, fs_have_order = false;
+  std::vector<grove_queue_quota_t> fs_quotas;
+  std::vector<uint32_t> fs_order;
+  grove_fair_share_stats_t fs_stats{};
+  DevBuf<uint32_t> d_fs_parent, d_fs_leaf, d_fs_rank, d_fs_owner, d_fs_vals, d_fs_prev, d_fs_first;
+  DevBuf<uint8_t> d_fs_depth, d_fs_tmp;
+  DevBuf<long long> d_fs_load0;
+  DevBuf<unsigned long long> d_fs_quota;
+  DevBuf<FsKey> d_fs_keys, d_fs_keys2;
+  DevBuf<FsUse> d_fs_use, d_fs_useq, d_fs_before;
+  PinBuf<uint32_t> h_fs_order;
 };
 
 
@@ -600,7 +615,8 @@ static int32_t load_nodes_common(grove_engine* e, const grove_node_t* host_nodes
       e->diag == grove_engine::kDiagImex) e->diag = grove_engine::kDiagChanged;
   e->sp_groups = e->sp_members = 0;   // a spread set belongs to the nodes and gangs it was validated against
   e->fc_gangs.clear();                // (a fence set too)
-  e->qu_members = 0; e->qu_given = false;   // (and a queue set)
+  e->qu_members = 0; e->qu_given = false;   // (and a queue set, with its fair-share set)
+  e->fs_given = false; e->fs_have_order = false;
   e->bp_members = 0; e->bp_given = false;   // (and a bin-packing set)
   e->im_enrolled = 0; e->im_given = false;  // (and a ComputeDomain set)
   CU_TRY(e, cudaSetDevice(e->cfg.device));
@@ -764,6 +780,7 @@ static int32_t submit(grove_engine* e, const grove_gang_t* gangs, uint32_t n_gan
   e->sp_groups = e->sp_members = 0;
   e->fc_gangs.clear();
   e->qu_members = 0; e->qu_given = false;
+  e->fs_given = false; e->fs_have_order = false;
   e->bp_members = 0; e->bp_given = false;
   e->im_enrolled = 0; e->im_given = false;
   int32_t rc = validate(e, gangs, n_gangs, cliques, ccount.data(), n_cliques, scopes, n_scopes, max_pods);
@@ -1569,8 +1586,11 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
   return GROVE_OK;
 }
 
+static int32_t fair_share_cycle(grove_engine* e, grove_cycle_stats_t* stats);
+
 int32_t grove_run_cycle(grove_engine_t* e, grove_cycle_stats_t* stats) {
   if (!e) return GROVE_ERR_INVALID_ARG;
+  if (e->fs_given) return fair_share_cycle(e, stats);
   const bool spread = e->sp_members > 0, fences = !e->fc_gangs.empty();
   if (spread && fences) return fail(e, GROVE_ERR_STATE, "grove_run_cycle: a spread set with members and a fence set together are not supported");
   if (e->qu_members && (spread || fences))
@@ -1841,7 +1861,7 @@ int32_t grove_set_queues(grove_engine_t* e, const grove_queue_t* queues, uint32_
   }
   for (uint32_t g = 0; g < n_gangs; ++g)
     if (gang_queue[g] != GROVE_NONE_U32 && gang_queue[g] >= n_queues) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_queues: queue index out of range");
-  e->qu_given = false;
+  e->qu_given = false; e->fs_given = false; e->fs_have_order = false;
   const int32_t rc = install_queues(e, queues, n_queues, gang_queue);
   if (rc) return rc;
   e->qu_queues.assign(queues, queues + n_queues);
@@ -1957,6 +1977,8 @@ int32_t grove_diagnose(grove_engine_t* e, grove_gang_diag_t* gangs, uint32_t cap
       return fail(e, GROVE_ERR_STATE, "grove_diagnose: the last cycle had fences, which the diagnosis does not model");
     case grove_engine::kDiagImex:
       return fail(e, GROVE_ERR_STATE, "grove_diagnose: the last cycle had enrolled cliques (ComputeDomains), which the diagnosis does not model");
+    case grove_engine::kDiagFairShare:
+      return fail(e, GROVE_ERR_STATE, "grove_diagnose: the last cycle ran in fair-share order, which the diagnosis does not model");
     default: return fail(e, GROVE_ERR_STATE, "grove_diagnose: nodes or gangs were loaded, updated or submitted since the last cycle");
   }
   const uint32_t G = e->G, Q = e->Q;
@@ -2842,6 +2864,7 @@ static int32_t check_queue_sets(grove_engine* e, const char* entry) {
   if (e->bp_members) return refuse_binpack(e, entry);
   if (e->im_enrolled) return refuse_imex(e, entry);
   if (!e->qu_given) { e->err = std::string(entry) + ": no queue set given for the current submission (grove_set_queues)"; return GROVE_ERR_STATE; }
+  if (e->fs_given) { e->err = std::string(entry) + ": not supported while a fair-share set is in place (grove_set_fair_share)"; return GROVE_ERR_STATE; }
   return GROVE_OK;
 }
 
@@ -2907,6 +2930,310 @@ int32_t grove_run_cycle_reclaim_preempt_queues(grove_engine_t* e, const grove_qu
                                                uint32_t n_holdings, const uint32_t* running_queue, grove_cycle_stats_t* stats) {
   return reclaim_queues_entry(e, "grove_run_cycle_reclaim_preempt_queues", quotas, n_queues, running, n_running, holdings, n_holdings,
                               running_queue, true, stats);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Fair-share order (include/grove_place.h "fair-share order"; DESIGN.md section 1; kernels in fairshare.cuh).  The turn order
+// depends on which gangs are admitted, so the cycle is a fixed point: run the queue cycle in order O_i, compute O_{i+1} = O(R_i)
+// from its outcomes on the device, and start the next queue cycle at the first turn d where the two differ -- every turn before d
+// is final.  Each later cycle is a sub-submission of the turns from d on, in that order (one priority, so that its rank is its
+// order), over the node table at d (the last cycle's table with what the turns from d on took given back) and a queue set whose
+// `used` are the loads at d.  Per iteration the host reads d and then the order from d on.
+// ---------------------------------------------------------------------------------------------
+int32_t grove_set_fair_share(grove_engine_t* e, const grove_queue_quota_t* quotas, uint32_t n_queues) {
+  if (!e || (n_queues && !quotas)) return GROVE_ERR_INVALID_ARG;
+  if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
+  if (!e->qu_given) return fail(e, GROVE_ERR_STATE, "grove_set_fair_share: no queue set given for the current submission (grove_set_queues)");
+  if (n_queues != e->qu_queues.size()) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_fair_share: n_queues is not the number of queues of the set");
+  std::vector<uint8_t> inner(n_queues, 0);
+  for (uint32_t q = 0; q < n_queues; ++q) if (e->qu_queues[q].parent != GROVE_NONE_U32) inner[e->qu_queues[q].parent] = 1;
+  for (uint32_t g = 0; g < e->G; ++g)
+    if (e->qu_gang_queue[g] != GROVE_NONE_U32 && inner[e->qu_gang_queue[g]])
+      return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_fair_share: a gang sits in a queue that has children (members must be in leaf queues)");
+  e->fs_quotas.assign(quotas, quotas + n_queues);
+  e->fs_given = true; e->fs_have_order = false;
+  return GROVE_OK;
+}
+
+int32_t grove_get_turn_order(grove_engine_t* e, uint32_t* out, uint32_t cap) {
+  if (!e || (e->G && !out)) return GROVE_ERR_INVALID_ARG;
+  if (!e->fs_have_order) return fail(e, GROVE_ERR_STATE, "grove_get_turn_order: no fair-share cycle since the last submission");
+  if (cap < e->G) return fail(e, GROVE_ERR_LIMIT, "output buffer too small");
+  if (e->G) std::memcpy(out, e->fs_order.data(), sizeof(uint32_t) * e->G);
+  return GROVE_OK;
+}
+
+int32_t grove_get_fair_share_stats(grove_engine_t* e, grove_fair_share_stats_t* out) {
+  if (!e || !out) return GROVE_ERR_INVALID_ARG;
+  if (!e->fs_have_order) return fail(e, GROVE_ERR_STATE, "grove_get_fair_share_stats: no fair-share cycle since the last submission");
+  *out = e->fs_stats;
+  return GROVE_OK;
+}
+
+static FsTree fs_tree(const grove_engine* e) {
+  return FsTree{e->d_fs_parent.p, e->d_fs_depth.p, e->d_fs_load0.p, e->d_fs_quota.p, e->d_fs_leaf.p, e->d_fs_rank.p};
+}
+
+// The tables of O(R) for the current submission and queue set, uploaded once per cycle, and the scratch of its scans and sorts.
+// -> the depth of the deepest tree node (the pseudo-queue has depth 1)
+static int32_t fs_tables(grove_engine* e, const std::vector<uint32_t>& rank, uint32_t* max_depth) {
+  const std::vector<grove_queue_t>& queues = e->qu_queues;
+  const uint32_t G = e->G, NQ = uint32_t(queues.size()), NT = NQ + 2;
+  std::vector<uint32_t> parent(NT, NQ + 1), leaf(G);
+  std::vector<uint8_t> depth(NT, 1);
+  std::vector<long long> load(size_t(NT) * 3, 0);
+  std::vector<unsigned long long> quota(size_t(NT) * 3, GROVE_QUEUE_UNLIMITED);
+  depth[NQ + 1] = 0;
+  *max_depth = 1;
+  for (uint32_t q = 0; q < NQ; ++q) {
+    if (queues[q].parent != GROVE_NONE_U32) { parent[q] = queues[q].parent; depth[q] = uint8_t(depth[parent[q]] + 1); }
+    *max_depth = std::max<uint32_t>(*max_depth, depth[q]);
+    for (int k = 0; k < 3; ++k) { load[q * 3 + k] = (long long)std::min<uint64_t>(queues[q].used[k], uint64_t(1) << 62); quota[q * 3 + k] = e->fs_quotas[q].deserved[k]; }
+  }
+  for (uint32_t q = NQ; q-- > 0;)
+    if (queues[q].parent != GROVE_NONE_U32) for (int k = 0; k < 3; ++k) load[queues[q].parent * 3 + k] += load[q * 3 + k];
+  for (uint32_t g = 0; g < G; ++g) leaf[g] = e->qu_gang_queue[g] == GROVE_NONE_U32 ? NQ : e->qu_gang_queue[g];
+  auto up = [e](auto& d, const auto& h) -> cudaError_t {
+    cudaError_t c = d.ensure(std::max<size_t>(h.size(), 1));
+    if (c == cudaSuccess && !h.empty()) c = cudaMemcpyAsync(d.p, h.data(), sizeof(h[0]) * h.size(), cudaMemcpyHostToDevice, e->stream);
+    return c;
+  };
+  CU_TRY(e, up(e->d_fs_parent, parent)); CU_TRY(e, up(e->d_fs_depth, depth)); CU_TRY(e, up(e->d_fs_load0, load));
+  CU_TRY(e, up(e->d_fs_quota, quota)); CU_TRY(e, up(e->d_fs_leaf, leaf)); CU_TRY(e, up(e->d_fs_rank, rank));
+  CU_TRY(e, e->d_fs_owner.ensure(G)); CU_TRY(e, e->d_fs_vals.ensure(G)); CU_TRY(e, e->d_fs_prev.ensure(G)); CU_TRY(e, e->d_fs_first.ensure(1));
+  CU_TRY(e, e->d_fs_keys.ensure(G)); CU_TRY(e, e->d_fs_keys2.ensure(G));
+  CU_TRY(e, e->d_fs_use.ensure(G)); CU_TRY(e, e->d_fs_useq.ensure(G)); CU_TRY(e, e->d_fs_before.ensure(G));
+  CU_TRY(e, e->h_fs_order.ensure(G));
+  size_t t0 = 0, t1 = 0, t2 = 0;
+  CU_TRY(e, cub::DeviceScan::ExclusiveScanByKey(nullptr, t0, e->d_fs_owner.p, e->d_fs_useq.p, e->d_fs_before.p, FsSum{}, FsUse{}, G,
+                                                ::cuda::std::equal_to<>{}, e->stream));
+  CU_TRY(e, cub::DeviceScan::InclusiveScanByKey(nullptr, t1, e->d_fs_owner.p, e->d_fs_keys.p, e->d_fs_keys2.p, FsMax{}, G,
+                                                ::cuda::std::equal_to<>{}, e->stream));
+  CU_TRY(e, cub::DeviceMergeSort::StableSortPairs(nullptr, t2, e->d_fs_keys.p, e->d_fs_vals.p, G, FsSortLess{}, e->stream));
+  CU_TRY(e, e->d_fs_tmp.ensure(std::max<size_t>(std::max(t0, std::max(t1, t2)), 1)));
+  CU_TRY(e, cudaStreamSynchronize(e->stream));   // (pageable sources)
+  return GROVE_OK;
+}
+
+// O(use) into d_fs_vals: every leaf's sequence in rank order, then per tree level, deepest first, the load of each element's node
+// at its turn (segmented exclusive scan), its key, the key's prefix max along the node's sequence (segmented inclusive scan), and
+// the parents' sequences (stable sort by (parent, key)).  Then, unless first is null (the cycle's first order, with nothing to
+// compare against), *first = the first position where the order differs from the one in d_fs_prev (G: none), which is all the
+// host reads.  *ms: the device time of it all, in events.
+static int32_t fs_order(grove_engine* e, uint32_t max_depth, const std::vector<FsUse>& use, uint32_t* first, float* ms) {
+  const uint32_t G = uint32_t(use.size()), nb = (G + 255) / 256;   // (the whole submission: e->G is that of the last sub-cycle)
+  const cudaStream_t s = e->stream;
+  const FsTree t = fs_tree(e);
+  FsKey* a = e->d_fs_keys.p;
+  FsKey* b = e->d_fs_keys2.p;
+  uint32_t* vals = e->d_fs_vals.p;
+  size_t tmp = e->d_fs_tmp.cap;
+  CU_TRY(e, cudaMemcpyAsync(e->d_fs_use.p, use.data(), sizeof(FsUse) * G, cudaMemcpyHostToDevice, s));
+  CU_TRY(e, cudaEventRecord(e->ev[0], s));
+  k_fs_init<<<nb, 256, 0, s>>>(t, G, a, vals);
+  CU_TRY(e, cudaGetLastError());
+  CU_TRY(e, cub::DeviceMergeSort::StableSortPairs(e->d_fs_tmp.p, tmp, a, vals, G, FsSortLess{}, s));
+  for (uint32_t d = max_depth; d >= 1; --d) {
+    k_fs_gather<<<nb, 256, 0, s>>>(G, a, vals, e->d_fs_use.p, e->d_fs_owner.p, e->d_fs_useq.p);
+    CU_TRY(e, cudaGetLastError());
+    tmp = e->d_fs_tmp.cap;
+    CU_TRY(e, cub::DeviceScan::ExclusiveScanByKey(e->d_fs_tmp.p, tmp, e->d_fs_owner.p, e->d_fs_useq.p, e->d_fs_before.p, FsSum{}, FsUse{}, G,
+                                                  ::cuda::std::equal_to<>{}, s));
+    k_fs_key<<<nb, 256, 0, s>>>(t, G, d, e->d_fs_owner.p, vals, e->d_fs_before.p, a);
+    CU_TRY(e, cudaGetLastError());
+    tmp = e->d_fs_tmp.cap;
+    CU_TRY(e, cub::DeviceScan::InclusiveScanByKey(e->d_fs_tmp.p, tmp, e->d_fs_owner.p, a, b, FsMax{}, G, ::cuda::std::equal_to<>{}, s));
+    tmp = e->d_fs_tmp.cap;
+    CU_TRY(e, cub::DeviceMergeSort::StableSortPairs(e->d_fs_tmp.p, tmp, b, vals, G, FsSortLess{}, s));
+    std::swap(a, b);
+  }
+  if (first) {
+    const uint32_t none = G;
+    CU_TRY(e, cudaMemcpyAsync(e->d_fs_first.p, &none, sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+    k_fs_diff<<<nb, 256, 0, s>>>(G, vals, e->d_fs_prev.p, e->d_fs_first.p);
+    CU_TRY(e, cudaGetLastError());
+    CU_TRY(e, cudaMemcpyAsync(first, e->d_fs_first.p, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    e->launches += 1;
+  }
+  CU_TRY(e, cudaEventRecord(e->ev[1], s));
+  CU_TRY(e, cudaStreamSynchronize(s));
+  CU_TRY(e, cudaEventElapsedTime(ms, e->ev[0], e->ev[1]));
+  e->launches += 2 + 5 * max_depth;
+  return GROVE_OK;
+}
+
+// the order O(use) from position d on, into order[d..G), and kept in d_fs_prev for the next comparison
+static int32_t fs_take_order(grove_engine* e, uint32_t d, std::vector<uint32_t>& order) {
+  const uint32_t G = uint32_t(order.size());
+  CU_TRY(e, cudaMemcpyAsync(e->h_fs_order.p, e->d_fs_vals.p + d, sizeof(uint32_t) * (G - d), cudaMemcpyDeviceToHost, e->stream));
+  CU_TRY(e, cudaMemcpyAsync(e->d_fs_prev.p, e->d_fs_vals.p, sizeof(uint32_t) * G, cudaMemcpyDeviceToDevice, e->stream));
+  CU_TRY(e, cudaStreamSynchronize(e->stream));
+  std::copy(e->h_fs_order.p, e->h_fs_order.p + (G - d), order.begin() + d);
+  return GROVE_OK;
+}
+
+static int32_t fair_share_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
+  int32_t rc = check_ready(e);
+  if (rc) return rc;
+  if (e->bp_members) return refuse_binpack(e, "grove_run_cycle with a fair-share set");
+  if (e->im_enrolled) return refuse_imex(e, "grove_run_cycle with a fair-share set");
+  if (e->sp_members) return refuse_spread(e, "grove_run_cycle with a fair-share set");
+  if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle with a fair-share set");
+  if (!e->qu_given) return fail(e, GROVE_ERR_STATE, "grove_run_cycle: the fair-share set has no queue set (grove_set_queues)");
+  struct Diag { grove_engine* e; ~Diag() { e->diag = grove_engine::kDiagFairShare; } } diag_guard{e};
+  CU_TRY(e, cudaSetDevice(e->cfg.device));
+  const uint32_t G = e->G;
+  const std::vector<grove_queue_t> queues = e->qu_queues;
+  const std::vector<uint32_t> gang_queue = e->qu_gang_queue;
+  const std::vector<grove_queue_quota_t> quotas = e->fs_quotas;
+  const uint32_t NQ = uint32_t(queues.size());
+  std::vector<uint32_t> by_rank(G), rank(G);
+  std::iota(by_rank.begin(), by_rank.end(), 0u);
+  std::stable_sort(by_rank.begin(), by_rank.end(), [e](uint32_t a, uint32_t b) { return e->gangs[a].priority > e->gangs[b].priority; });
+  for (uint32_t k = 0; k < G; ++k) rank[by_rank[k]] = k;
+  if (std::all_of(gang_queue.begin(), gang_queue.end(), [](uint32_t q) { return q == GROVE_NONE_U32; })) {
+    rc = run_cycle(e, stats);   // no member: every share is 0 and the order is rank order
+    if (rc) return rc;
+    e->fs_order = by_rank; e->fs_stats = grove_fair_share_stats_t{1, 0}; e->fs_have_order = true;
+    return GROVE_OK;
+  }
+  Snapshot snap;
+  snap.gangs.assign(e->gangs.data(), e->gangs.data() + G);
+  snap.cliques.assign(e->cliques.data(), e->cliques.data() + e->Q);
+  snap.scopes.assign(e->scopes.data(), e->scopes.data() + e->S);
+  snap.status.assign(G, grove_gang_status_t{});
+  snap.sstat.assign(std::max<uint32_t>(e->S, 1), grove_scope_status_t{});
+  // U of the first order: R_min of every member
+  std::vector<FsUse> use(G, FsUse{});
+  for (uint32_t g = 0; g < G; ++g) {
+    if (gang_queue[g] == GROVE_NONE_U32) continue;
+    for (uint32_t c = 0; c < snap.gangs[g].n_cliques; ++c) {
+      const grove_clique_t& q = snap.cliques[snap.gangs[g].clique_off + c];
+      use[g].v[0] += (long long)q.min_replicas * q.req_cpu_milli; use[g].v[1] += (long long)q.min_replicas * q.req_mem_mib;
+      use[g].v[2] += (long long)q.min_replicas * q.req_gpu;
+    }
+  }
+  uint32_t max_depth = 1;
+  rc = fs_tables(e, rank, &max_depth);
+  if (rc) return rc;
+  // whatever goes wrong from here, the handle goes back to the caller's submission, queue set and fair-share set on the starting
+  // node table (the fair-share set only when the queue set could be put back)
+  struct Keep {
+    grove_engine* e; const std::vector<grove_queue_quota_t>* q;
+    ~Keep() { if (e->qu_given) { e->fs_quotas = *q; e->fs_given = true; } }
+  } keep{e, &quotas};
+  CU_TRY(e, e->d_rc_base.ensure(e->Npad));
+  CU_TRY(e, cudaMemcpyAsync(e->d_rc_base.p, e->d_nres.p, sizeof(uint4) * e->Npad, cudaMemcpyDeviceToDevice, e->stream));
+  Restore restore{e, &snap, &queues, &gang_queue, true};
+  const uint64_t launches0 = e->launches;
+  uint32_t d = 0, iterations = 0, first = 0;
+  uint64_t rerun = 0;
+  std::vector<uint32_t> order(G), pos(G);
+  std::vector<std::vector<grove_placement_t>> pl(G);
+  grove_cycle_stats_t st0{};
+  float ms_order = 0.f;
+  rc = fs_order(e, max_depth, use, nullptr, &ms_order); if (rc) return rc;
+  rc = fs_take_order(e, 0, order); if (rc) return rc;
+  st0.kernel_launches += e->launches - launches0;
+  st0.ms_total += ms_order;
+  for (;;) {
+    ++iterations;
+    if (iterations > 1) rerun += G - d;
+    for (uint32_t p = 0; p < G; ++p) pos[order[p]] = p;
+    // the queue loads at turn d: own used plus what the members admitted before d charged (members sit in leaves)
+    std::vector<grove_queue_t> cq(queues);
+    for (uint32_t p = 0; p < d; ++p) {
+      const uint32_t g = order[p];
+      if (snap.status[g].state == GROVE_GANG_ADMITTED && gang_queue[g] != GROVE_NONE_U32)
+        for (int k = 0; k < 3; ++k) cq[gang_queue[g]].used[k] += uint64_t(use[g].v[k]);
+    }
+    // a gang from d on whose base had its turn before d and was not admitted -- or is itself such a gang -- comes back
+    // BASE_REJECTED without a turn of the engine; a gated one is skipped first, as always
+    std::vector<uint8_t> dropped(G, 0);
+    for (bool more = true; more;) {
+      more = false;
+      for (uint32_t p = d; p < G; ++p) {
+        const uint32_t g = order[p], b = snap.gangs[g].base_gang;
+        if (dropped[g] || (snap.gangs[g].flags & GROVE_GANG_GATED) || b == GROVE_NONE_U32) continue;
+        if ((pos[b] < d && snap.status[b].state != GROVE_GANG_ADMITTED) || dropped[b]) { dropped[g] = 1; more = true; }
+      }
+    }
+    std::vector<uint32_t> sub_of(G, GROVE_NONE_U32), sub_queue;
+    for (uint32_t p = d, k = 0; p < G; ++p) if (!dropped[order[p]]) sub_of[order[p]] = k++;
+    Sub sub;
+    for (uint32_t p = d; p < G; ++p) {
+      const uint32_t g = order[p];
+      pl[g].clear(); use[g] = FsUse{};
+      if (dropped[g]) {
+        grove_gang_status_t o{};
+        o.state = GROVE_GANG_BASE_REJECTED; o.level = GROVE_LEVEL_NONE; o.domain_node = GROVE_NONE_U32;
+        snap.status[g] = o;
+        for (uint32_t si = 0; si < snap.gangs[g].n_scopes; ++si)
+          snap.sstat[snap.gangs[g].scope_off + si] = grove_scope_status_t{GROVE_LEVEL_NONE, {0, 0, 0}, GROVE_NONE_U32};
+        continue;
+      }
+      grove_gang_t& x = add_gang(e, snap, g, sub);
+      x.priority = 0;   // one priority: the sub-submission's rank is its order, the turn order from d on
+      const uint32_t b = snap.gangs[g].base_gang;
+      if (b != GROVE_NONE_U32 && pos[b] >= d) x.base_gang = sub_of[b];   // (before d: admitted, so no base to wait for)
+      sub_queue.push_back(gang_queue[g]);
+    }
+    if (!sub.ids.empty()) {
+      rc = submit_sub(e, sub); if (rc) return rc;
+      rc = install_queues(e, cq.data(), NQ, sub_queue.data()); if (rc) return rc;
+      grove_cycle_stats_t stp{};
+      rc = run_cycle(e, &stp); if (rc) return rc;
+      accumulate(st0, stp);
+      std::vector<grove_scope_status_t> ssp;
+      rc = sub_scope_domains(e, sub, ssp); if (rc) return rc;
+      for (uint32_t k = 0; k < sub.ids.size(); ++k) {
+        const uint32_t g = sub.ids[k];
+        const grove_gang_status_t sp = e->h_status.p[k];
+        merge_gang(snap, sub, k, sp, ssp);
+        if (sp.state != GROVE_GANG_ADMITTED) continue;
+        std::vector<uint32_t> nodes; std::vector<Res> u;
+        placed(e, snap, sub, k, nodes, u, pl[g]);
+        for (const Res& r : u) { use[g].v[0] += r.cpu; use[g].v[1] += r.mem; use[g].v[2] += r.gpu; }
+      }
+    }
+    // the order these outcomes give; the turns before `first` are final
+    const uint64_t l0 = e->launches;
+    rc = fs_order(e, max_depth, use, &first, &ms_order); if (rc) return rc;
+    st0.kernel_launches += e->launches - l0;
+    st0.ms_total += ms_order;
+    if (first >= G) break;
+    if (first <= d) return fail(e, GROVE_ERR_STATE, "fair-share order: the fixed point did not advance");
+    // the node table at `first`: what the turns from there on took goes back (the same gangs in either order)
+    std::vector<std::pair<uint32_t, Res>> back;
+    for (uint32_t p = first; p < G; ++p) {
+      const uint32_t g = order[p];
+      if (snap.status[g].state != GROVE_GANG_ADMITTED) continue;
+      for (const grove_placement_t& x : pl[g]) {
+        const grove_clique_t& q = snap.cliques[x.clique];
+        back.push_back({e->inv[x.node], Res{q.req_cpu_milli, q.req_mem_mib, q.req_gpu, 1}});
+      }
+    }
+    rc = patch_nodes(e, back, st0); if (rc) return rc;
+    rc = fs_take_order(e, first, order); if (rc) return rc;
+    d = first;
+  }
+  restore.armed = false;
+  rc = restore.put_back(); if (rc) return rc;
+  // the outputs: placements grouped by gang in submission order
+  std::vector<grove_placement_t> place;
+  uint32_t admitted = 0, rejected = 0;
+  for (uint32_t g = 0; g < G; ++g) {
+    snap.status[g].placement_off = uint32_t(place.size());
+    if (snap.status[g].state == GROVE_GANG_ADMITTED) { place.insert(place.end(), pl[g].begin(), pl[g].end()); ++admitted; }
+    else if (snap.status[g].state == GROVE_GANG_REJECTED || snap.status[g].state == GROVE_GANG_BASE_REJECTED) ++rejected;
+  }
+  st0.gangs_admitted = admitted; st0.gangs_rejected = rejected;
+  rc = publish_reclaim(e, snap.status, place, std::vector<std::vector<grove_placement_t>>(G), snap.sstat, st0, {}, stats);
+  if (rc) return rc;
+  e->fs_order = std::move(order);
+  e->fs_stats = grove_fair_share_stats_t{iterations, uint32_t(std::min<uint64_t>(rerun, UINT32_MAX))};
+  e->fs_have_order = true;
+  return GROVE_OK;
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -769,6 +769,7 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
   bool preempt = false, reuse = false, both = false;   // both: SetReclaimWithReuse, one grove_run_cycle_reuse_preempt
   bool acrossQueues = false;                           // SetReclaimAcrossQueues with queue members: grove_run_cycle_reclaim_queues
   bool thenPreempt = false;                            // SetReclaimThenPreempt with queue members: grove_run_cycle_reclaim_preempt_queues
+  bool fairShare = false;                              // SetFairShareOrder with queue members: the queue cycle in fair-share order
   std::vector<uint32_t> replaces;   // reservation reuse: per gang row, the running gang it is the new version of
   {
     std::lock_guard<std::mutex> l(mu_);
@@ -782,6 +783,7 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
     acrossQueues = !thenPreempt && reclaimQueues_ && !t.queues.empty() && !running_.empty();
     preempt = ((preemption_ || reclaimReuse_) && !running_.empty()) || acrossQueues;
     reuse = (reuse_ || reclaimReuse_) && !running_.empty();
+    fairShare = fairShare_ && !t.queues.empty() && !both && !preempt && !reuse && !consolidate;
     if (preempt || reuse) {
       std::map<std::string, uint32_t> nodeIdx;
       for (uint32_t i = 0; i < nodes.size(); ++i) nodeIdx[nodes[i].Name] = i;
@@ -836,7 +838,7 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
       if (auto e = chk(grove_set_fences(engine_, fences.data(), uint32_t(fences.size())), "grove_set_fences")) return e;
   }
   // bin-packing: every row a member, at the level of the key or its own Required level when deeper, in an ordinary or queue pass
-  if (!both && !reuse && !preempt && !consolidate && !spread && fences.empty() && !wide) {
+  if (!both && !reuse && !preempt && !consolidate && !spread && fences.empty() && !wide && !fairShare) {
     uint8_t lv = GROVE_LEVEL_NONE;
     {
       std::lock_guard<std::mutex> l(mu_);
@@ -910,7 +912,11 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
     if (auto e = chk(grove_run_cycle_consolidate(engine_, targets.data(), uint32_t(targets.size()), specOf.data(), crun.data(), uint32_t(crun.size()),
                                                  cheld.data(), uint32_t(cheld.size()), &st), "grove_run_cycle_consolidate")) return e;
   }
-  else if (auto e = chk(grove_run_cycle(engine_, &st), "grove_run_cycle")) return e;
+  else {
+    if (fairShare)
+      if (auto e = chk(grove_set_fair_share(engine_, t.quotas.data(), uint32_t(t.quotas.size())), "grove_set_fair_share")) return e;
+    if (auto e = chk(grove_run_cycle(engine_, &st), "grove_run_cycle")) return e;
+  }
   if (stats) *stats = st;
   std::vector<grove_placement_t> pl(st.pods_bound + 1);
   uint32_t n = 0;

@@ -312,6 +312,11 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   // SetPreemptionWithinQueues say.  Victims of the reclaim pass get DisruptionTarget naming the reclaimer and its queue, those of
   // the preempt pass naming their preemptor.  Off by default.
   void SetReclaimThenPreempt(bool on) { std::lock_guard<std::mutex> l(mu_); reclaimThenPreempt_ = on; }
+  // Fair-share order (KAI's allocate order; DESIGN.md section 1 "Fair-share order"): with it on, a pass with queue members and no
+  // preemption, reservation reuse or consolidation runs the queue cycle with grove_set_fair_share and each Queue's deserved quota:
+  // the next turn goes to the queue furthest below its quota, priority orders PodGangs only inside a queue.  Members must sit in
+  // leaf queues (a cycle with a member in a parent queue fails).  Bin-packing is not applied in such a pass.  Off by default.
+  void SetFairShareOrder(bool on) { std::lock_guard<std::mutex> l(mu_); fairShare_ = on; }
   // Large PodGangs: with it on, PodGangs of up to GROVE_MAX_WIDE_GANG_PODS pods (PodGroups of up to as many) are encoded and a
   // cycle submits through grove_submit_gangs_wide; ValidatePodCliqueSet accepts base PodGangs of that size.  The running-gang
   // cycles (preemption, reservation reuse, reuse with reclaim) do not take such PodGangs: while one of those switches is on too,
@@ -420,6 +425,7 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   bool preemptQueues_ = false;
   bool reclaimQueues_ = false;
   bool reclaimThenPreempt_ = false;
+  bool fairShare_ = false;
   bool large_ = false;
   bool explain_ = false;
   std::string binpackKey_;                             // bin-packing level (off: empty)

@@ -14,6 +14,8 @@
 //   fence.cuh    k_fence_have / k_fence_pick / k_fence_status  the domain each fencing gang fences (grove_set_fences)
 //   consolidate.cuh k_consol_view / k_consol_rank / k_consol_mask  the views of a consolidation try (grove_run_cycle_consolidate)
 //   queue.cuh    k_queue_scan / k_queue_gate  the headroom, gate and surplus caps of the queue members (grove_set_queues)
+//   fairshare.cuh k_fs_init / k_fs_gather / k_fs_key / k_fs_diff  the turn order of a fair-share cycle (grove_set_fair_share), with
+//                cub's segmented scans and stable merge sort
 //   binpack.cuh  k_binpack_sum / k_binpack_keys / k_binpack_pick  the fullest domain each bin-packing member is anchored at
 //                (grove_set_binpack)
 //   imex.cuh     imex_foreign  which nodes another ComputeDomain holds in a gang's view (grove_set_compute_domains; the kImex
@@ -30,6 +32,7 @@
 #include "relax.cuh"
 #include "reclaim.cuh"
 #include "donor.cuh"
+#include "fairshare.cuh"
 #include "diagnose.cuh"
 #include "spread.cuh"
 #include "fence.cuh"

@@ -28,6 +28,7 @@ SYMBOLS = [
     "grove_run_cycle_reuse_preempt", "grove_diagnose", "grove_set_spread", "grove_set_fences", "grove_set_queues",
     "grove_run_cycle_consolidate", "grove_get_moves", "grove_run_cycle_preempt_queues",
     "grove_run_cycle_reclaim_queues", "grove_run_cycle_reclaim_preempt_queues",
+    "grove_set_fair_share", "grove_get_turn_order", "grove_get_fair_share_stats",
     "grove_set_binpack", "grove_get_binpack_picks", "grove_set_compute_domains", "grove_get_compute_domain_owners",
     "grove_shard_range", "grove_run_score_pass", "grove_shard_summary_device",
     "grove_debug_get_perm", "grove_debug_get_fit_row", "grove_debug_get_score_row",
@@ -176,6 +177,27 @@ class PlacementEngine:
         submit / load_nodes clears it (include/grove_place.h "bin-packing")."""
         levels = np.ascontiguousarray(levels, dtype=np.uint8)
         self._check(self.lib.grove_set_binpack(self.h, _p(levels), C.c_uint32(len(levels))))
+
+    def set_fair_share(self, quotas: np.ndarray):
+        """grove_set_fair_share: one quota row per queue of the set_queues set (tables.queue_quota_dt; QUEUE_UNLIMITED = KAI's
+        quota -1).  run_cycle then gives the next turn to the gang at the head of the queue furthest below its deserved quota --
+        priority orders gangs only inside a queue -- and turn_order() reports the order.  Every member must sit in a leaf queue.
+        Cleared with the queue set (include/grove_place.h "fair-share order")."""
+        quotas = np.ascontiguousarray(quotas, dtype=T.queue_quota_dt)
+        self._check(self.lib.grove_set_fair_share(self.h, _p(quotas), C.c_uint32(len(quotas))))
+
+    def turn_order(self) -> np.ndarray:
+        """the gangs in the order they had their turn in the last fair-share cycle"""
+        out = np.zeros(max(self.G, 1), dtype=np.uint32)
+        self._check(self.lib.grove_get_turn_order(self.h, _p(out), C.c_uint32(len(out))))
+        return out[: self.G]
+
+    def fair_share_stats(self) -> dict:
+        """{iterations, turns_rerun} of the last fair-share cycle: the queue cycles run to reach its order, and the turns the
+        cycles after the first ran again"""
+        st = np.zeros(1, dtype=T.fair_share_stats_dt)
+        self._check(self.lib.grove_get_fair_share_stats(self.h, _p(st)))
+        return {k: st[k][0].item() for k in T.fair_share_stats_dt.names}
 
     def binpack_picks(self) -> np.ndarray:
         """caller index of the first node of each gang's pick in the last cycle that ran with a set_binpack set (tables.NONE_U32:

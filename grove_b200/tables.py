@@ -101,6 +101,7 @@ queue_dt = np.dtype([("parent", np.uint32), ("reserved", np.uint32), ("limit", "
 STATUS_RECLAIMER = 0x80           # status reserved0: admitted by the class pass of grove_run_cycle_reclaim_queues (or
                                   # the reclaim pass of grove_run_cycle_reclaim_preempt_queues)
 queue_quota_dt = np.dtype([("deserved", "<u8", (3,))])   # per resource, QUEUE_UNLIMITED = whatever the queue holds (KAI's -1)
+fair_share_stats_dt = np.dtype([("iterations", "<u4"), ("turns_rerun", "<u4")])   # grove_get_fair_share_stats
 
 assert node_dt.itemsize == 32 and clique_dt.itemsize == 16 and scope_dt.itemsize == 8
 assert gang_dt.itemsize == 32 and placement_dt.itemsize == 8 and status_dt.itemsize == 32 and scope_status_dt.itemsize == 8

@@ -616,6 +616,33 @@ int32_t grove_run_cycle_reclaim_preempt_queues(grove_engine_t* e, const grove_qu
                                                const grove_holding_t* holdings, uint32_t n_holdings,
                                                const uint32_t* running_queue, grove_cycle_stats_t* stats);
 
+/* ---- fair-share order ----------------------------------------------------------------------------------
+ * The queue cycle's turns go by fair share: the queue furthest below its deserved quota takes the next turn (DESIGN.md section 1,
+ * "Fair-share order"; after KAI-Scheduler's allocate action, which takes the next job from the queue with the lowest share).
+ * grove_set_fair_share gives one quota row per queue of the set grove_set_queues gave the current submission.  With it in place,
+ * grove_run_cycle runs the queue cycle ("queue limits", rules 1-4) with one change, the turn order:
+ *   share_X = max over resources x with a finite deserved_X[x] of load_X[x] / deserved_X[x] (0/0 = 0, l/0 = +inf for l > 0, no
+ *   finite quota = 0; compared exactly), load_X taken at the turn: its starting load plus U of every member of X's subtree
+ *   admitted earlier in the cycle.  The gangs with no queue form one more top-level pseudo-queue of share 0.  The next gang is
+ *   next(root): for a leaf, its first waiting gang in rank order; for an inner node, next(C) of the child C that still has a
+ *   waiting gang with the smallest (share_C, rank(next(C))).
+ * Each turn is then the queue cycle's: gated gangs are skipped, a scaled gang needs its base admitted at an earlier turn, the gate
+ * and the surplus caps read "ranked before g" as "took its turn before g", and K3 runs with the gang's ordinary anchor.  Every
+ * member must sit in a leaf queue (GROVE_ERR_INVALID_ARG otherwise).  The set is cleared with the queue set (next
+ * grove_submit_gangs* / grove_load_nodes* / grove_set_queues) and kept by grove_update_nodes.  Refused: n_queues other than the
+ * set's queue count (GROVE_ERR_INVALID_ARG); no queue set (GROVE_ERR_STATE).  While it is in place, grove_run_cycle with a
+ * bin-packing set with members, an enrolled ComputeDomain, a spread set with members or a fence set, and
+ * grove_run_cycle_{preempt,reclaim,reclaim_preempt}_queues, return GROVE_ERR_STATE; so does grove_diagnose after the cycle.
+ * grove_get_turn_order: the gangs in the order they had their turn (GROVE_ERR_STATE before a fair-share cycle);
+ * grove_get_fair_share_stats: the queue cycles the engine ran to find that order and how many turns they ran again. */
+typedef struct grove_fair_share_stats {
+  uint32_t iterations;    /* relaxation cycles run (the first over every gang, each later one over the turns from the first changed one) */
+  uint32_t turns_rerun;   /* turns the cycles after the first ran again */
+} grove_fair_share_stats_t;
+int32_t grove_set_fair_share(grove_engine_t* e, const grove_queue_quota_t* quotas, uint32_t n_queues);
+int32_t grove_get_turn_order(grove_engine_t* e, uint32_t* out, uint32_t cap);
+int32_t grove_get_fair_share_stats(grove_engine_t* e, grove_fair_share_stats_t* out);
+
 /* K2: the topology-distance score matrix T[clique][node] = fit ? 1 + levels shared with the gang's anchor : 0 (u8) over the
  * snapshot the last cycle started from -- what a scheduler's Score extension point would hand out.  The admission does
  * not read it (its visiting order comes from the anchor's domain ranges), so it is built on request; GROVE_TUNE_SCORE=1

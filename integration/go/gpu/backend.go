@@ -61,6 +61,9 @@ type schedulerBackend struct {
 	// grove_run_cycle_reclaim_preempt_queues, whatever preemptQueues and reclaimQueues say (GpuBackend::SetReclaimThenPreempt in
 	// the C++ mirror)
 	reclaimThenPreempt bool
+	// fairShare: a pass with queue members and no preemption runs the queue cycle in fair-share order (grove_set_fair_share with
+	// each queue's deserved quota; GpuBackend::SetFairShareOrder in the C++ mirror)
+	fairShare bool
 	// largePodGangs: PodGangs of up to maxWideGangPods pods are encoded (a counts row per clique) and submitted through
 	// grove_submit_gangs_wide.  The reclaim pass takes no such PodGang: with preempt also on, one beyond maxGangPods pods or 255
 	// replicas is reported Unschedulable (GpuBackend::SetLargePodGangs in the C++ mirror).
@@ -134,6 +137,16 @@ func (b *schedulerBackend) SetReclaimThenPreempt(on bool) {
 	b.mu.Lock()
 	defer b.mu.Unlock()
 	b.reclaimThenPreempt = on
+}
+
+// SetFairShareOrder: with it on, a pass with queue members and no preemption runs the queue cycle in fair-share order, as
+// KAI-Scheduler's allocate action orders its jobs: the next turn goes to the queue furthest below its deserved quota, priority
+// orders PodGangs only inside a queue (DESIGN.md section 1 "Fair-share order").  Members must sit in leaf queues.  Bin-packing is
+// not applied in such a pass.  Off by default.
+func (b *schedulerBackend) SetFairShareOrder(on bool) {
+	b.mu.Lock()
+	defer b.mu.Unlock()
+	b.fairShare = on
 }
 
 // SetTopologySpread sets (nil: removes) the topology spread of PodCliqueSet pcs.  Its pending base PodGangs with a Required level
@@ -333,8 +346,11 @@ func (b *schedulerBackend) encodeQueues(t *tables, rows []*groveschedulerv1alpha
 		}
 		r.limit = [3]C.uint64_t{lim(q.CpuMilli), lim(q.MemMiB), lim(q.Gpu)}
 		t.queues = append(t.queues, r)
+		quota := C.grove_queue_quota_t{deserved: [3]C.uint64_t{lim(q.DeservedCpuMilli), lim(q.DeservedMemMiB), lim(q.DeservedGpu)}}
 		if b.reclaimQueues || (b.reclaimThenPreempt && b.preempt) {
-			t.quotas = append(t.quotas, C.grove_queue_quota_t{deserved: [3]C.uint64_t{lim(q.DeservedCpuMilli), lim(q.DeservedMemMiB), lim(q.DeservedGpu)}})
+			t.quotas = append(t.quotas, quota)
+		} else if b.fairShare && !b.preempt {
+			t.fairShare = append(t.fairShare, quota)
 		}
 	}
 	for key, qn := range b.queueOf {
@@ -921,8 +937,9 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 		}
 	}
 	// bin-packing: every row a member, at the key's level or its own Required level when deeper, in an ordinary or queue pass
+	fairShare := b.fairShare && !preempt && !b.reclaimQueues && queuesOn && queueWhy == ""
 	if lv := levelIndex(levels, &b.binpackKey); b.binpackKey != "" && lv != C.GROVE_LEVEL_NONE && !preempt && !wideAny &&
-		len(t.spreadGroups) == 0 && len(t.fences) == 0 && len(t.targets) == 0 {
+		len(t.spreadGroups) == 0 && len(t.fences) == 0 && len(t.targets) == 0 && !fairShare {
 		t.binpack = make([]C.uint8_t, len(t.gangs))
 		for gi := range t.gangs {
 			t.binpack[gi] = lv

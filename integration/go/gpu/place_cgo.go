@@ -79,6 +79,9 @@ type tables struct {
 	// reclaim, then preempt: with quotas and runningQueue, both passes in one grove_run_cycle_reclaim_preempt_queues; set only
 	// with SetReclaimThenPreempt and preemption
 	thenPreempt bool
+	// fair-share order: each queue's deserved quota, in `queues` order (grove_set_fair_share); set only with SetFairShareOrder in a
+	// pass with queue members and no preemption
+	fairShare []C.grove_queue_quota_t
 	queueNames []string
 	// consolidation (optional; ordinary passes only, never with fences): the target rows, and for each running gang of `running`
 	// the gated row that restates it (grove_run_cycle_consolidate)
@@ -200,6 +203,13 @@ func (e *engine) cycle(t *tables, preempt, large, explain bool) (*result, error)
 			if err := e.err(C.grove_get_moves(e.h, &r.moves[0], n, &n)); err != nil {
 				return nil, err
 			}
+		}
+	} else if len(t.fairShare) > 0 && len(t.queues) > 0 {
+		if err := e.err(C.grove_set_fair_share(e.h, &t.fairShare[0], C.uint32_t(len(t.fairShare)))); err != nil {
+			return nil, err
+		}
+		if err := e.err(C.grove_run_cycle(e.h, &r.stats)); err != nil {
+			return nil, err
 		}
 	} else if err := e.err(C.grove_run_cycle(e.h, &r.stats)); err != nil {
 		return nil, err
