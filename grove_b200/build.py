@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libgrove_place.so")
 SOURCES = ["engine.cu"]
 DEPS = ["engine.cu", "kernels.cuh", "common.cuh", "tables.cuh", "fit.cuh", "score.cuh", "admit.cuh", "relax.cuh",
-        "reclaim.cuh", "donor.cuh", "fairshare.cuh", "diagnose.cuh", "spread.cuh", "fence.cuh", "consolidate.cuh", "queue.cuh", "binpack.cuh", "imex.cuh", os.path.join("..", "..", "include", "grove_place.h")]
+        "reclaim.cuh", "donor.cuh", "fairshare.cuh", "overquota.cuh", "diagnose.cuh", "spread.cuh", "fence.cuh", "consolidate.cuh", "queue.cuh", "binpack.cuh", "imex.cuh", os.path.join("..", "..", "include", "grove_place.h")]
 NVCC_FLAGS = [
     "-DGROVE_INLINE_ALL",
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

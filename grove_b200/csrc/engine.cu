@@ -319,6 +319,13 @@ struct grove_engine {
   DevBuf<FsKey> d_fs_keys, d_fs_keys2;
   DevBuf<FsUse> d_fs_use, d_fs_useq, d_fs_before;
   PinBuf<uint32_t> h_fs_order;
+  // over-quota weights (grove_set_over_quota; overquota.cuh): one row per queue of the queue set, kept with it; the fair shares
+  // (queue * 3 + resource) the last call that ran with them computed; the tree tables of the division
+  bool oq_given = false, oq_have_fair = false;
+  std::vector<grove_queue_weight_t> oq_weights;
+  std::vector<unsigned long long> oq_fair;
+  DevBuf<uint32_t> d_oq_parent, d_oq_off, d_oq_child, d_oq_plist, d_oq_weight, d_oq_gq;
+  DevBuf<unsigned long long> d_oq_des, d_oq_lim, d_oq_dem, d_oq_pool, d_oq_need, d_oq_fair;
 };
 
 
@@ -615,8 +622,9 @@ static int32_t load_nodes_common(grove_engine* e, const grove_node_t* host_nodes
       e->diag == grove_engine::kDiagImex) e->diag = grove_engine::kDiagChanged;
   e->sp_groups = e->sp_members = 0;   // a spread set belongs to the nodes and gangs it was validated against
   e->fc_gangs.clear();                // (a fence set too)
-  e->qu_members = 0; e->qu_given = false;   // (and a queue set, with its fair-share set)
+  e->qu_members = 0; e->qu_given = false;   // (and a queue set, with its fair-share set and over-quota weights)
   e->fs_given = false; e->fs_have_order = false;
+  e->oq_given = false; e->oq_have_fair = false;
   e->bp_members = 0; e->bp_given = false;   // (and a bin-packing set)
   e->im_enrolled = 0; e->im_given = false;  // (and a ComputeDomain set)
   CU_TRY(e, cudaSetDevice(e->cfg.device));
@@ -781,6 +789,7 @@ static int32_t submit(grove_engine* e, const grove_gang_t* gangs, uint32_t n_gan
   e->fc_gangs.clear();
   e->qu_members = 0; e->qu_given = false;
   e->fs_given = false; e->fs_have_order = false;
+  e->oq_given = false; e->oq_have_fair = false;
   e->bp_members = 0; e->bp_given = false;
   e->im_enrolled = 0; e->im_given = false;
   int32_t rc = validate(e, gangs, n_gangs, cliques, ccount.data(), n_cliques, scopes, n_scopes, max_pods);
@@ -1861,7 +1870,7 @@ int32_t grove_set_queues(grove_engine_t* e, const grove_queue_t* queues, uint32_
   }
   for (uint32_t g = 0; g < n_gangs; ++g)
     if (gang_queue[g] != GROVE_NONE_U32 && gang_queue[g] >= n_queues) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_queues: queue index out of range");
-  e->qu_given = false; e->fs_given = false; e->fs_have_order = false;
+  e->qu_given = false; e->fs_given = false; e->fs_have_order = false; e->oq_given = false; e->oq_have_fair = false;
   const int32_t rc = install_queues(e, queues, n_queues, gang_queue);
   if (rc) return rc;
   e->qu_queues.assign(queues, queues + n_queues);
@@ -2084,11 +2093,15 @@ struct Snapshot {
 };
 
 // Whatever goes wrong while armed, the handle goes back to the caller's submission, and queue set when one was given (queues
-// non-null), on the free table the ordinary pass left, kept in d_rc_base; the error of the failing call is what the caller sees.
+// non-null) with the over-quota weights and fair shares it had when the Restore was made (the sub-submissions clear them with the
+// queue set), on the free table the ordinary pass left, kept in d_rc_base; the error of the failing call is what the caller sees.
 // put_back() alone is the normal end: the device table is then the free table as it is.
 struct Restore {
   grove_engine* e; const Snapshot* s; const std::vector<grove_queue_t>* queues; const std::vector<uint32_t>* gang_queue;
   bool armed = true;
+  bool oq_given = e->oq_given, oq_have_fair = e->oq_have_fair;
+  std::vector<grove_queue_weight_t> oq_weights = e->oq_weights;
+  std::vector<unsigned long long> oq_fair = e->oq_fair;
   int32_t put_back() const {
     int32_t rc = grove_submit_gangs(e, s->gangs.data(), uint32_t(s->gangs.size()), s->cliques.data(), uint32_t(s->cliques.size()),
                                     s->scopes.data(), uint32_t(s->scopes.size()));
@@ -2097,6 +2110,7 @@ struct Restore {
     rc = install_queues(e, queues->data(), uint32_t(queues->size()), gang_queue->data());
     if (rc) return rc;
     e->qu_queues = *queues; e->qu_gang_queue = *gang_queue; e->qu_given = true;
+    e->oq_given = oq_given; e->oq_have_fair = oq_have_fair; e->oq_weights = oq_weights; e->oq_fair = oq_fair;
     return GROVE_OK;
   }
   ~Restore() {
@@ -2856,6 +2870,98 @@ int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replace
   return reclaim_cycle(e, replaces, running, n_running, holdings, nullptr, nullptr, true, stats);
 }
 
+// ---------------------------------------------------------------------------------------------
+// Over-quota weight (include/grove_place.h "over-quota weight"; DESIGN.md section 1; kernels in overquota.cuh).  The fair shares of
+// the queue set under a call's deserved quotas, once at the start of a call that runs with weights: the tree tables and the
+// starting loads go up, k_oq_demand and k_oq_capacity fill in the demands and the root's pool, k_oq_fill divides one depth per
+// launch, and the host reads back NQ x 3 words, which the call then takes as its quotas.
+// ---------------------------------------------------------------------------------------------
+int32_t grove_set_over_quota(grove_engine_t* e, const grove_queue_weight_t* w, uint32_t n_queues) {
+  if (!e || (n_queues && !w)) return GROVE_ERR_INVALID_ARG;
+  if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
+  if (!e->qu_given) return fail(e, GROVE_ERR_STATE, "grove_set_over_quota: no queue set given for the current submission (grove_set_queues)");
+  if (n_queues != e->qu_queues.size()) return fail(e, GROVE_ERR_INVALID_ARG, "grove_set_over_quota: n_queues is not the number of queues of the set");
+  e->oq_weights.assign(w, w + n_queues);
+  e->oq_given = true; e->oq_have_fair = false;
+  return GROVE_OK;
+}
+
+int32_t grove_get_fair_shares(grove_engine_t* e, uint64_t* out, uint32_t cap_queues) {
+  if (!e) return GROVE_ERR_INVALID_ARG;
+  if (!e->oq_have_fair) return fail(e, GROVE_ERR_STATE, "grove_get_fair_shares: no call has run with the over-quota weights since they were given");
+  const size_t NQ = e->oq_fair.size() / 3;
+  if (cap_queues < NQ) return fail(e, GROVE_ERR_LIMIT, "output buffer too small");
+  if (NQ && !out) return GROVE_ERR_INVALID_ARG;
+  if (NQ) std::memcpy(out, e->oq_fair.data(), sizeof(uint64_t) * e->oq_fair.size());
+  return GROVE_OK;
+}
+
+// the fair shares of the current queue set and submission under `quotas` (one row per queue) and the set's weights, into out (as
+// quota rows) and e->oq_fair
+static int32_t over_quota_shares(grove_engine* e, const grove_queue_quota_t* quotas, std::vector<grove_queue_quota_t>& out) {
+  const std::vector<grove_queue_t>& queues = e->qu_queues;
+  const uint32_t NQ = uint32_t(queues.size()), G = e->G;
+  const size_t n3 = std::max<size_t>(size_t(NQ) * 3, 1);
+  constexpr uint64_t kClamp = uint64_t(1) << 62;
+  std::vector<uint32_t> parent(std::max<uint32_t>(NQ, 1), GROVE_NONE_U32), off(size_t(NQ) + 2, 0), child(std::max<uint32_t>(NQ, 1), 0);
+  std::vector<uint32_t> weight(n3, 0), depth(size_t(NQ) + 1, 0);
+  std::vector<unsigned long long> des(n3, GROVE_QUEUE_UNLIMITED), lim(n3, GROVE_QUEUE_UNLIMITED), load(n3, 0), pool((size_t(NQ) + 1) * 3, 0);
+  for (uint32_t q = 0; q < NQ; ++q) {
+    parent[q] = queues[q].parent;
+    depth[q] = parent[q] == GROVE_NONE_U32 ? 1 : depth[parent[q]] + 1;
+    for (int r = 0; r < 3; ++r) {
+      des[q * 3 + r] = quotas[q].deserved[r]; lim[q * 3 + r] = queues[q].limit[r];
+      weight[q * 3 + r] = e->oq_weights[q].over_quota[r]; load[q * 3 + r] = std::min(queues[q].used[r], kClamp);
+    }
+  }
+  for (uint32_t q = NQ; q-- > 0;)   // (parents come first: one pass from the back)
+    for (int r = 0; r < 3; ++r) {
+      unsigned long long& to = parent[q] == GROVE_NONE_U32 ? pool[size_t(NQ) * 3 + r] : load[parent[q] * 3 + r];
+      to = std::min<unsigned long long>(to + load[q * 3 + r], kClamp);
+    }
+  // the children of every node (NQ = the root) in queue order, and the nodes with children by depth, the root first
+  for (uint32_t q = 0; q < NQ; ++q) ++off[(parent[q] == GROVE_NONE_U32 ? NQ : parent[q]) + 1];
+  for (uint32_t n = 0; n <= NQ; ++n) off[n + 1] += off[n];
+  std::vector<uint32_t> cur(off.begin(), off.end() - 1), plist, per_depth(GROVE_MAX_QUEUE_DEPTH + 1, 0);
+  for (uint32_t q = 0; q < NQ; ++q) child[cur[parent[q] == GROVE_NONE_U32 ? NQ : parent[q]]++] = q;
+  for (uint32_t d = 0; d <= GROVE_MAX_QUEUE_DEPTH; ++d)
+    for (uint32_t n = 0; n <= NQ; ++n)
+      if (off[n + 1] > off[n] && (n == NQ ? 0u : depth[n]) == d) { plist.push_back(n); ++per_depth[d]; }
+  if (plist.empty()) plist.push_back(NQ);
+  auto up = [e](auto& dv, const auto& h) -> cudaError_t {
+    cudaError_t c = dv.ensure(h.size());
+    if (c == cudaSuccess) c = cudaMemcpyAsync(dv.p, h.data(), sizeof(h[0]) * h.size(), cudaMemcpyHostToDevice, e->stream);
+    return c;
+  };
+  const std::vector<uint32_t> gq = e->qu_gang_queue.empty() ? std::vector<uint32_t>(1, GROVE_NONE_U32) : e->qu_gang_queue;
+  CU_TRY(e, up(e->d_oq_parent, parent)); CU_TRY(e, up(e->d_oq_off, off)); CU_TRY(e, up(e->d_oq_child, child));
+  CU_TRY(e, up(e->d_oq_plist, plist)); CU_TRY(e, up(e->d_oq_weight, weight)); CU_TRY(e, up(e->d_oq_gq, gq));
+  CU_TRY(e, up(e->d_oq_des, des)); CU_TRY(e, up(e->d_oq_lim, lim)); CU_TRY(e, up(e->d_oq_dem, load)); CU_TRY(e, up(e->d_oq_pool, pool));
+  CU_TRY(e, e->d_oq_need.ensure(n3)); CU_TRY(e, e->d_oq_fair.ensure(n3));
+  const OqTree t{e->d_oq_parent.p, e->d_oq_off.p, e->d_oq_child.p, e->d_oq_plist.p, e->d_oq_des.p, e->d_oq_lim.p, e->d_oq_weight.p,
+                 e->d_oq_dem.p, e->d_oq_pool.p, e->d_oq_need.p, e->d_oq_fair.p};
+  k_oq_capacity<<<1, 1024, 0, e->stream>>>(t, e->d_nres.p, e->N, NQ);
+  CU_TRY(e, cudaGetLastError());
+  if (G) {
+    k_oq_demand<<<(G + 255) / 256, 256, 0, e->stream>>>(t, e->d_gangs.p, e->d_cliques.p, e->d_oq_gq.p, G);
+    CU_TRY(e, cudaGetLastError());
+  }
+  e->launches += 2;
+  for (uint32_t d = 0, first = 0; d <= GROVE_MAX_QUEUE_DEPTH; first += per_depth[d++]) {
+    if (!per_depth[d]) continue;
+    k_oq_fill<<<per_depth[d], 256, 0, e->stream>>>(t, first);
+    CU_TRY(e, cudaGetLastError());
+    e->launches += 1;
+  }
+  e->oq_fair.assign(size_t(NQ) * 3, 0);
+  if (NQ) CU_TRY(e, cudaMemcpyAsync(e->oq_fair.data(), e->d_oq_fair.p, sizeof(unsigned long long) * NQ * 3, cudaMemcpyDeviceToHost, e->stream));
+  CU_TRY(e, cudaStreamSynchronize(e->stream));   // (pageable sources and destination)
+  out.assign(NQ, grove_queue_quota_t{});
+  for (uint32_t q = 0; q < NQ; ++q) for (int r = 0; r < 3; ++r) out[q].deserved[r] = e->oq_fair[q * 3 + r];
+  e->oq_have_fair = true;
+  return GROVE_OK;
+}
+
 // The checks grove_run_cycle_preempt_queues and grove_run_cycle_reclaim_queues share.  First the sets the entries refuse (a refusal
 // here leaves grove_diagnose as it was) ...
 static int32_t check_queue_sets(grove_engine* e, const char* entry) {
@@ -2915,6 +3021,13 @@ static int32_t reclaim_queues_entry(grove_engine* e, const char* entry, const gr
   rc = check_queue_running(e, entry, running, n_running, holdings, n_holdings, running_queue);
   if (rc) return rc;
   if (n_queues != e->qu_queues.size()) { e->err = std::string(entry) + ": n_queues is not the number of queues of the set"; return GROVE_ERR_INVALID_ARG; }
+  std::vector<grove_queue_quota_t> fair;   // with over-quota weights, the fair shares stand in for the quotas (reclaim_cycle's
+                                           // Restore puts the weights and these shares back with the queue set)
+  if (e->oq_given) {
+    CU_TRY(e, cudaSetDevice(e->cfg.device));
+    rc = over_quota_shares(e, quotas, fair); if (rc) return rc;
+    quotas = fair.data();
+  }
   return reclaim_cycle(e, nullptr, running, n_running, holdings, running_queue, quotas, priority, stats);
 }
 
@@ -2976,7 +3089,8 @@ static FsTree fs_tree(const grove_engine* e) {
 
 // The tables of O(R) for the current submission and queue set, uploaded once per cycle, and the scratch of its scans and sorts.
 // -> the depth of the deepest tree node (the pseudo-queue has depth 1)
-static int32_t fs_tables(grove_engine* e, const std::vector<uint32_t>& rank, uint32_t* max_depth) {
+static int32_t fs_tables(grove_engine* e, const std::vector<uint32_t>& rank, const std::vector<grove_queue_quota_t>& quotas,
+                         uint32_t* max_depth) {
   const std::vector<grove_queue_t>& queues = e->qu_queues;
   const uint32_t G = e->G, NQ = uint32_t(queues.size()), NT = NQ + 2;
   std::vector<uint32_t> parent(NT, NQ + 1), leaf(G);
@@ -2988,7 +3102,7 @@ static int32_t fs_tables(grove_engine* e, const std::vector<uint32_t>& rank, uin
   for (uint32_t q = 0; q < NQ; ++q) {
     if (queues[q].parent != GROVE_NONE_U32) { parent[q] = queues[q].parent; depth[q] = uint8_t(depth[parent[q]] + 1); }
     *max_depth = std::max<uint32_t>(*max_depth, depth[q]);
-    for (int k = 0; k < 3; ++k) { load[q * 3 + k] = (long long)std::min<uint64_t>(queues[q].used[k], uint64_t(1) << 62); quota[q * 3 + k] = e->fs_quotas[q].deserved[k]; }
+    for (int k = 0; k < 3; ++k) { load[q * 3 + k] = (long long)std::min<uint64_t>(queues[q].used[k], uint64_t(1) << 62); quota[q * 3 + k] = quotas[q].deserved[k]; }
   }
   for (uint32_t q = NQ; q-- > 0;)
     if (queues[q].parent != GROVE_NONE_U32) for (int k = 0; k < 3; ++k) load[queues[q].parent * 3 + k] += load[q * 3 + k];
@@ -3087,6 +3201,9 @@ static int32_t fair_share_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
   const std::vector<uint32_t> gang_queue = e->qu_gang_queue;
   const std::vector<grove_queue_quota_t> quotas = e->fs_quotas;
   const uint32_t NQ = uint32_t(queues.size());
+  std::vector<grove_queue_quota_t> fair;   // with over-quota weights, the fair shares stand in for the quotas (the Restore below
+                                           // puts the weights and these shares back with the queue set)
+  if (e->oq_given) { rc = over_quota_shares(e, quotas.data(), fair); if (rc) return rc; }
   std::vector<uint32_t> by_rank(G), rank(G);
   std::iota(by_rank.begin(), by_rank.end(), 0u);
   std::stable_sort(by_rank.begin(), by_rank.end(), [e](uint32_t a, uint32_t b) { return e->gangs[a].priority > e->gangs[b].priority; });
@@ -3114,7 +3231,7 @@ static int32_t fair_share_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
     }
   }
   uint32_t max_depth = 1;
-  rc = fs_tables(e, rank, &max_depth);
+  rc = fs_tables(e, rank, e->oq_given ? fair : quotas, &max_depth);
   if (rc) return rc;
   // whatever goes wrong from here, the handle goes back to the caller's submission, queue set and fair-share set on the starting
   // node table (the fair-share set only when the queue set could be put back)

@@ -667,6 +667,7 @@ Err GpuBackend::EncodeLocked(const std::vector<Node>& nodes, Tables* out, const 
       out->queues.push_back(r);
       out->quotas.push_back(grove_queue_quota_t{{q.DeservedCpuMilli.value_or(GROVE_QUEUE_UNLIMITED), q.DeservedMemMiB.value_or(GROVE_QUEUE_UNLIMITED),
                                                  q.DeservedGpu.value_or(GROVE_QUEUE_UNLIMITED)}});
+      out->weights.push_back(grove_queue_weight_t{{q.OverQuotaWeightCpu.value_or(1u), q.OverQuotaWeightMem.value_or(1u), q.OverQuotaWeightGpu.value_or(1u)}, 0u});
     }
     for (const auto& [key, qn] : queueOf_) {
       auto it = idx.find(qn); auto rg = running_.find(key);
@@ -770,6 +771,7 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
   bool acrossQueues = false;                           // SetReclaimAcrossQueues with queue members: grove_run_cycle_reclaim_queues
   bool thenPreempt = false;                            // SetReclaimThenPreempt with queue members: grove_run_cycle_reclaim_preempt_queues
   bool fairShare = false;                              // SetFairShareOrder with queue members: the queue cycle in fair-share order
+  bool overQuota = false;                              // SetOverQuotaWeights: the cycles with quotas run with each queue's weights
   std::vector<uint32_t> replaces;   // reservation reuse: per gang row, the running gang it is the new version of
   {
     std::lock_guard<std::mutex> l(mu_);
@@ -784,6 +786,7 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
     preempt = ((preemption_ || reclaimReuse_) && !running_.empty()) || acrossQueues;
     reuse = (reuse_ || reclaimReuse_) && !running_.empty();
     fairShare = fairShare_ && !t.queues.empty() && !both && !preempt && !reuse && !consolidate;
+    overQuota = overQuota_;
     if (preempt || reuse) {
       std::map<std::string, uint32_t> nodeIdx;
       for (uint32_t i = 0; i < nodes.size(); ++i) nodeIdx[nodes[i].Name] = i;
@@ -898,6 +901,8 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
         if (auto it = queueOf_.find(runNames[r]); it != queueOf_.end())
           if (auto n = std::find(t.queueNames.begin(), t.queueNames.end(), it->second); n != t.queueNames.end()) runQueue[r] = uint32_t(n - t.queueNames.begin());
     }
+    if ((thenPreempt || acrossQueues) && overQuota)
+      if (auto e = chk(grove_set_over_quota(engine_, t.weights.data(), uint32_t(t.weights.size())), "grove_set_over_quota")) return e;
     if (thenPreempt) {
       if (auto e = chk(grove_run_cycle_reclaim_preempt_queues(engine_, t.quotas.data(), uint32_t(t.quotas.size()), run.data(), uint32_t(run.size()),
                                                               held.data(), uint32_t(held.size()), runQueue.data(), &st), "grove_run_cycle_reclaim_preempt_queues")) return e;
@@ -915,7 +920,16 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
   else {
     if (fairShare)
       if (auto e = chk(grove_set_fair_share(engine_, t.quotas.data(), uint32_t(t.quotas.size())), "grove_set_fair_share")) return e;
+    if (fairShare && overQuota)
+      if (auto e = chk(grove_set_over_quota(engine_, t.weights.data(), uint32_t(t.weights.size())), "grove_set_over_quota")) return e;
     if (auto e = chk(grove_run_cycle(engine_, &st), "grove_run_cycle")) return e;
+  }
+  if (overQuota && (thenPreempt || acrossQueues || fairShare)) {   // the fair shares the cycle used
+    std::vector<uint64_t> fs(t.queues.size() * 3);
+    if (auto e = chk(grove_get_fair_shares(engine_, fs.data(), uint32_t(t.queues.size())), "grove_get_fair_shares")) return e;
+    std::lock_guard<std::mutex> l(mu_);
+    fairShares_.clear();
+    for (size_t q = 0; q < t.queueNames.size(); ++q) fairShares_[t.queueNames[q]] = {fs[q * 3], fs[q * 3 + 1], fs[q * 3 + 2]};
   }
   if (stats) *stats = st;
   std::vector<grove_placement_t> pl(st.pods_bound + 1);

@@ -18,6 +18,7 @@
 #include <chrono>
 #include <condition_variable>
 #include <functional>
+#include <array>
 #include <map>
 #include <mutex>
 #include <thread>
@@ -214,11 +215,14 @@ struct TopologySpread {
 // a KAI queue's hard limits (scheduling.run.ai/v2 Queue: spec.parentQueue, spec.resources.{cpu,memory,gpu}.limit; DESIGN.md
 // section 1 "Queue limits"), in the engine's units: millicores, MiB, GPUs.  nullopt = no limit (KAI's -1).  The deserved quota
 // (spec.resources.{cpu,memory,gpu}.quota; DESIGN.md section 1 "Reclaim across queues") in the same units; nullopt = KAI's -1, the
-// queue deserves whatever it holds.  Only SetReclaimAcrossQueues reads it.
+// queue deserves whatever it holds.  Only SetReclaimAcrossQueues reads it.  The over-quota weight
+// (spec.resources.{cpu,memory,gpu}.overQuotaWeight; DESIGN.md section 1 "Over-quota weight"): the queue's share of the capacity
+// nobody deserves relative to its siblings; nullopt = 1, KAI's default.  Only SetOverQuotaWeights reads it.
 struct Queue {
   std::string Parent;                            // "" = a root queue; otherwise a queue set earlier
   std::optional<uint64_t> CpuMilli, MemMiB, Gpu;
   std::optional<uint64_t> DeservedCpuMilli, DeservedMemMiB, DeservedGpu;
+  std::optional<uint32_t> OverQuotaWeightCpu, OverQuotaWeightMem, OverQuotaWeightGpu;
 };
 
 // packed tables of one cycle, as handed to libgrove_place.so
@@ -242,6 +246,7 @@ struct Tables {
   // (GROVE_NONE_U32: none)
   std::vector<grove_queue_t> queues;
   std::vector<grove_queue_quota_t> quotas;              // per queue of `queues`, its deserved quota
+  std::vector<grove_queue_weight_t> weights;            // per queue of `queues`, its over-quota weights
   std::vector<std::string> queueNames;
   std::vector<uint32_t> queueOf;
   // consolidation (SetConsolidation): rows [specRow, gangs.size()) are gated rows restating running PodGangs, which makes them
@@ -317,6 +322,14 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   // the next turn goes to the queue furthest below its quota, priority orders PodGangs only inside a queue.  Members must sit in
   // leaf queues (a cycle with a member in a parent queue fails).  Bin-packing is not applied in such a pass.  Off by default.
   void SetFairShareOrder(bool on) { std::lock_guard<std::mutex> l(mu_); fairShare_ = on; }
+  // Over-quota weight (KAI's proportion plugin; DESIGN.md section 1 "Over-quota weight"): with it on, every cycle that runs with
+  // quotas -- SetReclaimAcrossQueues, SetReclaimThenPreempt, SetFairShareOrder -- sets each Queue's over-quota weights
+  // (grove_set_over_quota), so that a queue's fair share, its deserved quota plus its weighted slice of the capacity nobody
+  // deserves, stands in for the deserved quota.  Off by default; off behaves exactly as before.
+  void SetOverQuotaWeights(bool on) { std::lock_guard<std::mutex> l(mu_); overQuota_ = on; }
+  // the fair shares (cpu milli, mem MiB, gpu; GROVE_QUEUE_UNLIMITED where the deserved quota is unlimited) of the last cycle that
+  // ran with weights, by queue name, as KAI reports them in queue status; empty before such a cycle
+  std::map<std::string, std::array<uint64_t, 3>> FairShares() const { std::lock_guard<std::mutex> l(mu_); return fairShares_; }
   // Large PodGangs: with it on, PodGangs of up to GROVE_MAX_WIDE_GANG_PODS pods (PodGroups of up to as many) are encoded and a
   // cycle submits through grove_submit_gangs_wide; ValidatePodCliqueSet accepts base PodGangs of that size.  The running-gang
   // cycles (preemption, reservation reuse, reuse with reclaim) do not take such PodGangs: while one of those switches is on too,
@@ -426,6 +439,8 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   bool reclaimQueues_ = false;
   bool reclaimThenPreempt_ = false;
   bool fairShare_ = false;
+  bool overQuota_ = false;
+  std::map<std::string, std::array<uint64_t, 3>> fairShares_;   // FairShares()
   bool large_ = false;
   bool explain_ = false;
   std::string binpackKey_;                             // bin-packing level (off: empty)

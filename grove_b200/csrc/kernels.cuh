@@ -16,6 +16,7 @@
 //   queue.cuh    k_queue_scan / k_queue_gate  the headroom, gate and surplus caps of the queue members (grove_set_queues)
 //   fairshare.cuh k_fs_init / k_fs_gather / k_fs_key / k_fs_diff  the turn order of a fair-share cycle (grove_set_fair_share), with
 //                cub's segmented scans and stable merge sort
+//   overquota.cuh k_oq_demand / k_oq_capacity / k_oq_fill  the fair shares under over-quota weights (grove_set_over_quota)
 //   binpack.cuh  k_binpack_sum / k_binpack_keys / k_binpack_pick  the fullest domain each bin-packing member is anchored at
 //                (grove_set_binpack)
 //   imex.cuh     imex_foreign  which nodes another ComputeDomain holds in a gang's view (grove_set_compute_domains; the kImex
@@ -33,6 +34,7 @@
 #include "reclaim.cuh"
 #include "donor.cuh"
 #include "fairshare.cuh"
+#include "overquota.cuh"
 #include "diagnose.cuh"
 #include "spread.cuh"
 #include "fence.cuh"

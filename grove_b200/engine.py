@@ -29,6 +29,7 @@ SYMBOLS = [
     "grove_run_cycle_consolidate", "grove_get_moves", "grove_run_cycle_preempt_queues",
     "grove_run_cycle_reclaim_queues", "grove_run_cycle_reclaim_preempt_queues",
     "grove_set_fair_share", "grove_get_turn_order", "grove_get_fair_share_stats",
+    "grove_set_over_quota", "grove_get_fair_shares",
     "grove_set_binpack", "grove_get_binpack_picks", "grove_set_compute_domains", "grove_get_compute_domain_owners",
     "grove_shard_range", "grove_run_score_pass", "grove_shard_summary_device",
     "grove_debug_get_perm", "grove_debug_get_fit_row", "grove_debug_get_score_row",
@@ -198,6 +199,22 @@ class PlacementEngine:
         st = np.zeros(1, dtype=T.fair_share_stats_dt)
         self._check(self.lib.grove_get_fair_share_stats(self.h, _p(st)))
         return {k: st[k][0].item() for k in T.fair_share_stats_dt.names}
+
+    def set_over_quota(self, weights: np.ndarray):
+        """grove_set_over_quota: one over-quota weight row per queue of the set_queues set (tables.queue_weight_dt; KAI's default is
+        1).  run_cycle with a fair-share set, run_cycle_reclaim_queues and the reclaim pass of run_cycle_reclaim_preempt_queues then
+        take each queue's fair share -- its deserved quota plus its weighted slice of the capacity nobody deserves, capped by what
+        it asks for -- as its quota; fair_shares() reports them.  Cleared with the queue set (include/grove_place.h "over-quota
+        weight")."""
+        weights = np.ascontiguousarray(weights, dtype=T.queue_weight_dt)
+        self._check(self.lib.grove_set_over_quota(self.h, _p(weights), C.c_uint32(len(weights))))
+
+    def fair_shares(self, n_queues: int) -> np.ndarray:
+        """(n_queues, 3) uint64: the fair shares (cpu milli, mem MiB, gpu; QUEUE_UNLIMITED where deserved is) the last call that
+        ran with over-quota weights computed"""
+        out = np.zeros((max(n_queues, 1), 3), dtype=np.uint64)
+        self._check(self.lib.grove_get_fair_shares(self.h, _p(out), C.c_uint32(n_queues)))
+        return out[:n_queues]
 
     def binpack_picks(self) -> np.ndarray:
         """caller index of the first node of each gang's pick in the last cycle that ran with a set_binpack set (tables.NONE_U32:

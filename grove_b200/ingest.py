@@ -324,6 +324,29 @@ def queue_quotas_from_manifests(queue_docs, names):
     return out
 
 
+def queue_weights_from_manifests(queue_docs, names):
+    """Queue manifests + the queue names in table order (as queues_from_manifests returns them) -> tables.queue_weight_dt[n] for
+    grove_set_over_quota.  spec.resources.{cpu,memory,gpu}.overQuotaWeight is the queue's share of the capacity nobody deserves
+    relative to its siblings; absent means 1, KAI's default.  A negative or fractional weight raises ValueError naming the queue."""
+    docs = {d["metadata"]["name"]: d for d in queue_docs if d and d.get("kind", "Queue") == "Queue"}
+    out = np.zeros(len(names), dtype=T.queue_weight_dt)
+    for i, n in enumerate(names):
+        res = (docs[n].get("spec") or {}).get("resources") or {}
+        for r, key in enumerate(("cpu", "memory", "gpu")):
+            w = (res.get(key) or {}).get("overQuotaWeight")
+            if w is None:
+                out["over_quota"][i, r] = 1
+                continue
+            try:
+                x = _quantity(w)
+            except (ValueError, ZeroDivisionError):
+                x = Fraction(-1)
+            if x < 0 or x.denominator != 1 or x >= 1 << 32:
+                raise ValueError(f"Queue {n!r}: {key} overQuotaWeight {w!r} is not a whole number from 0 to 2^32 - 1")
+            out["over_quota"][i, r] = int(x)
+    return out
+
+
 def tables_from_pcs(pcs: dict, topology_levels, tas_enabled: bool = True, class_mask=0xFFFF):
     """PodCliqueSet -> (gangs, cliques, scopes, clique_names, PodGang manifests): the producer, then the encoder."""
     gangs, requests, base_of = podgangs_from_pcs(pcs, topology_levels, tas_enabled)

@@ -101,6 +101,7 @@ queue_dt = np.dtype([("parent", np.uint32), ("reserved", np.uint32), ("limit", "
 STATUS_RECLAIMER = 0x80           # status reserved0: admitted by the class pass of grove_run_cycle_reclaim_queues (or
                                   # the reclaim pass of grove_run_cycle_reclaim_preempt_queues)
 queue_quota_dt = np.dtype([("deserved", "<u8", (3,))])   # per resource, QUEUE_UNLIMITED = whatever the queue holds (KAI's -1)
+queue_weight_dt = np.dtype([("over_quota", "<u4", (3,)), ("reserved", "<u4")])   # per resource (cpu, mem, gpu); KAI's default 1
 fair_share_stats_dt = np.dtype([("iterations", "<u4"), ("turns_rerun", "<u4")])   # grove_get_fair_share_stats
 
 assert node_dt.itemsize == 32 and clique_dt.itemsize == 16 and scope_dt.itemsize == 8
@@ -108,7 +109,7 @@ assert gang_dt.itemsize == 32 and placement_dt.itemsize == 8 and status_dt.items
 assert config_dt.itemsize == 32 and stats_dt.itemsize == 64
 assert gang_diag_dt.itemsize == 16 and clique_diag_dt.itemsize == 40
 assert spread_dt.itemsize == 8 and spread_seed_dt.itemsize == 8 and queue_dt.itemsize == 56
-assert queue_quota_dt.itemsize == 24
+assert queue_quota_dt.itemsize == 24 and queue_weight_dt.itemsize == 16
 
 
 def make_nodes(n: int) -> np.ndarray:

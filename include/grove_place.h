@@ -643,6 +643,36 @@ int32_t grove_set_fair_share(grove_engine_t* e, const grove_queue_quota_t* quota
 int32_t grove_get_turn_order(grove_engine_t* e, uint32_t* out, uint32_t cap);
 int32_t grove_get_fair_share_stats(grove_engine_t* e, grove_fair_share_stats_t* out);
 
+/* ---- over-quota weight ---------------------------------------------------------------------------------
+ * A queue's fair share is its deserved quota plus a slice of the capacity nobody deserves, divided among siblings by their
+ * over-quota weights and capped by what each asks for (DESIGN.md section 1, "Over-quota weight"; after KAI-Scheduler's proportion
+ * plugin and Queue `spec.resources.*.overQuotaWeight`).  grove_set_over_quota gives one weight row per queue of the set
+ * grove_set_queues gave the current submission.  With it in place, grove_run_cycle with a fair-share set,
+ * grove_run_cycle_reclaim_queues and the reclaim pass of grove_run_cycle_reclaim_preempt_queues behave exactly as if the caller had
+ * passed the fair shares as the deserved quotas (shares, caps and donor sets); the preempt pass and every entry that takes no
+ * quotas do not read it.  The fair shares are computed once per call, at its start, per resource r, from the call's deserved
+ * quotas; every quantity below saturates at 2^62:
+ *   C[r] = the free r of the schedulable nodes of the table the call starts from + the load of every top-level queue (own used
+ *   plus its descendants').  demand_X[r] = load_X[r] + replicas * request[r] of every clique of every gang not GROVE_GANG_GATED
+ *   whose queue lies in X's subtree (surplus pods count).  The root's pool is C; at a parent with pool P each child c takes:
+ *     deserved_c[r] unlimited: fair_c[r] = GROVE_QUEUE_UNLIMITED, and t_c = min(demand_c, limit_c) of P, which c's children divide;
+ *     otherwise base_c = min(deserved_c, demand_c, limit_c), need_c = min(demand_c, limit_c) - base_c.
+ *   R = max(0, P - sum of bases - sum of t).  Then, while a round gives something: A = the finite children with need_c > 0 and
+ *   w_c > 0, W = sum of their weights, each gets g_c = min(need_c, floor(R * w_c / W)), R -= sum g, need_c -= g_c.  The leftover
+ *   (R < |A|) goes one unit each to the members of A in (w desc, queue index asc) order while R > 0.  fair_c = base_c + what c
+ *   got; c's children divide it.
+ * The set is cleared with the queue set (next grove_submit_gangs* / grove_load_nodes* / grove_set_queues) and kept by
+ * grove_update_nodes.  Refused: n_queues other than the set's queue count or a null row pointer with n_queues > 0
+ * (GROVE_ERR_INVALID_ARG); no queue set (GROVE_ERR_STATE).  grove_get_fair_shares writes 3 values per queue (cpu milli, mem MiB,
+ * gpu): the fair shares the last call that ran with weights computed (GROVE_QUEUE_UNLIMITED where deserved is); GROVE_ERR_STATE
+ * before such a call since the set was given, GROVE_ERR_LIMIT when cap_queues is below the queue count. */
+typedef struct grove_queue_weight {   /* 16 B */
+  uint32_t over_quota[3];             /* cpu, mem, gpu; KAI's default is 1, 0 = the queue gets no share of the surplus */
+  uint32_t reserved;
+} grove_queue_weight_t;
+int32_t grove_set_over_quota(grove_engine_t* e, const grove_queue_weight_t* w, uint32_t n_queues);
+int32_t grove_get_fair_shares(grove_engine_t* e, uint64_t* out, uint32_t cap_queues);
+
 /* K2: the topology-distance score matrix T[clique][node] = fit ? 1 + levels shared with the gang's anchor : 0 (u8) over the
  * snapshot the last cycle started from -- what a scheduler's Score extension point would hand out.  The admission does
  * not read it (its visiting order comes from the anchor's domain ranges), so it is built on request; GROVE_TUNE_SCORE=1

@@ -64,6 +64,11 @@ type schedulerBackend struct {
 	// fairShare: a pass with queue members and no preemption runs the queue cycle in fair-share order (grove_set_fair_share with
 	// each queue's deserved quota; GpuBackend::SetFairShareOrder in the C++ mirror)
 	fairShare bool
+	// overQuota: the passes that run with quotas (reclaimQueues, reclaimThenPreempt, fairShare) also set each queue's over-quota
+	// weights (grove_set_over_quota), so that its fair share stands in for its deserved quota; fairShares holds the shares the last
+	// such pass used, by queue name (GpuBackend::SetOverQuotaWeights / FairShares in the C++ mirror)
+	overQuota  bool
+	fairShares map[string][3]uint64
 	// largePodGangs: PodGangs of up to maxWideGangPods pods are encoded (a counts row per clique) and submitted through
 	// grove_submit_gangs_wide.  The reclaim pass takes no such PodGang: with preempt also on, one beyond maxGangPods pods or 255
 	// replicas is reported Unschedulable (GpuBackend::SetLargePodGangs in the C++ mirror).
@@ -147,6 +152,28 @@ func (b *schedulerBackend) SetFairShareOrder(on bool) {
 	b.mu.Lock()
 	defer b.mu.Unlock()
 	b.fairShare = on
+}
+
+// SetOverQuotaWeights: with it on, every pass that runs with quotas (SetReclaimAcrossQueues, SetReclaimThenPreempt,
+// SetFairShareOrder) sets each queue's over-quota weights, as KAI-Scheduler's proportion plugin divides the capacity nobody
+// deserves: a queue's fair share, its deserved quota plus its weighted slice of that capacity capped by what it asks for, stands
+// in for its deserved quota (DESIGN.md section 1 "Over-quota weight").  Off by default; off behaves exactly as before.
+func (b *schedulerBackend) SetOverQuotaWeights(on bool) {
+	b.mu.Lock()
+	defer b.mu.Unlock()
+	b.overQuota = on
+}
+
+// FairShares: the fair shares (cpu milli, mem MiB, gpu; unlimited where the deserved quota is) of the last pass that ran with
+// over-quota weights, by queue name, as KAI reports them in queue status; empty before such a pass.
+func (b *schedulerBackend) FairShares() map[string][3]uint64 {
+	b.mu.Lock()
+	defer b.mu.Unlock()
+	out := make(map[string][3]uint64, len(b.fairShares))
+	for k, v := range b.fairShares {
+		out[k] = v
+	}
+	return out
 }
 
 // SetTopologySpread sets (nil: removes) the topology spread of PodCliqueSet pcs.  Its pending base PodGangs with a Required level
@@ -235,12 +262,15 @@ func (b *schedulerBackend) encodeSpread(t *tables, rows []*groveschedulerv1alpha
 }
 
 // Queue is a KAI queue's hard limits in the engine's units (millicores, MiB, GPUs; nil = no limit, KAI's -1), its deserved quota
-// in the same units (spec.resources.*.quota; nil = KAI's -1, read only by SetReclaimAcrossQueues), and its parent ("" = a root
-// queue).  GpuBackend::SetQueue in the C++ mirror; DESIGN.md section 1 "Queue limits" and "Reclaim across queues".
+// in the same units (spec.resources.*.quota; nil = KAI's -1, read only by SetReclaimAcrossQueues), its over-quota weights
+// (spec.resources.*.overQuotaWeight; nil = 1, KAI's default, read only by SetOverQuotaWeights) and its parent ("" = a root
+// queue).  GpuBackend::SetQueue in the C++ mirror; DESIGN.md section 1 "Queue limits", "Reclaim across queues" and "Over-quota
+// weight".
 type Queue struct {
-	Parent                                        string
-	CpuMilli, MemMiB, Gpu                         *uint64
-	DeservedCpuMilli, DeservedMemMiB, DeservedGpu *uint64
+	Parent                                                     string
+	CpuMilli, MemMiB, Gpu                                      *uint64
+	DeservedCpuMilli, DeservedMemMiB, DeservedGpu              *uint64
+	OverQuotaWeightCpu, OverQuotaWeightMem, OverQuotaWeightGpu *uint32
 }
 
 const labelQueue = "kai.scheduler/queue"
@@ -351,6 +381,15 @@ func (b *schedulerBackend) encodeQueues(t *tables, rows []*groveschedulerv1alpha
 			t.quotas = append(t.quotas, quota)
 		} else if b.fairShare && !b.preempt {
 			t.fairShare = append(t.fairShare, quota)
+		}
+		if b.overQuota {
+			wt := func(x *uint32) C.uint32_t {
+				if x == nil {
+					return 1
+				}
+				return C.uint32_t(*x)
+			}
+			t.weights = append(t.weights, C.grove_queue_weight_t{over_quota: [3]C.uint32_t{wt(q.OverQuotaWeightCpu), wt(q.OverQuotaWeightMem), wt(q.OverQuotaWeightGpu)}})
 		}
 	}
 	for key, qn := range b.queueOf {
@@ -1025,6 +1064,12 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 			b.rejectedFor[key]++
 		} else if st.state == C.GROVE_GANG_ADMITTED {
 			delete(b.rejectedFor, key)
+		}
+	}
+	if len(res.fairShares) > 0 { // the fair shares the pass used (SetOverQuotaWeights)
+		b.fairShares = make(map[string][3]uint64, len(t.queueNames))
+		for qi, n := range t.queueNames {
+			b.fairShares[n] = [3]uint64{uint64(res.fairShares[qi*3]), uint64(res.fairShares[qi*3+1]), uint64(res.fairShares[qi*3+2])}
 		}
 	}
 	for gi, st := range res.status[:len(rows)] { // what an admitted member holds counts against its queue from now on

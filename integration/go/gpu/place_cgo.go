@@ -82,6 +82,9 @@ type tables struct {
 	// fair-share order: each queue's deserved quota, in `queues` order (grove_set_fair_share); set only with SetFairShareOrder in a
 	// pass with queue members and no preemption
 	fairShare []C.grove_queue_quota_t
+	// over-quota weights: each queue's, in `queues` order (grove_set_over_quota); set only with SetOverQuotaWeights, and read only
+	// by a pass that runs with quotas or fairShare
+	weights    []C.grove_queue_weight_t
 	queueNames []string
 	// consolidation (optional; ordinary passes only, never with fences): the target rows, and for each running gang of `running`
 	// the gated row that restates it (grove_run_cycle_consolidate)
@@ -95,6 +98,8 @@ type result struct {
 	victims    []C.grove_victim_t
 	moves      []C.grove_move_t // consolidation: (running gang, target row) per relocated gang
 	stats      C.grove_cycle_stats_t
+	// with over-quota weights, after a pass that ran with quotas or fairShare: 3 fair shares per queue (grove_get_fair_shares)
+	fairShares []C.uint64_t
 	// explain, after an ordinary cycle with a rejected gang: why each rejected gang did not fit (grove_diagnose)
 	gangDiag   []C.grove_gang_diag_t
 	cliqueDiag []C.grove_clique_diag_t
@@ -151,17 +156,28 @@ func (e *engine) cycle(t *tables, preempt, large, explain bool) (*result, error)
 		}
 	}
 	r := &result{}
+	// the weights go with a pass that runs with quotas: reclaim across queues, reclaim then preempt, or the fair-share order
+	weighted := len(t.weights) > 0 && len(t.queues) > 0 &&
+		((preempt && len(t.running) > 0 && len(t.runningQueue) > 0 && len(t.quotas) > 0) || len(t.fairShare) > 0)
+	usedQuotas := false // the pass below ran with quotas: the fair shares it used can be read back
+	if weighted {
+		if err := e.err(C.grove_set_over_quota(e.h, &t.weights[0], C.uint32_t(len(t.weights)))); err != nil {
+			return nil, err
+		}
+	}
 	if preempt && len(t.running) > 0 {
 		var hp *C.grove_holding_t
 		if len(t.holdings) > 0 {
 			hp = &t.holdings[0]
 		}
 		if len(t.runningQueue) > 0 && len(t.quotas) > 0 && t.thenPreempt {
+			usedQuotas = true
 			if err := e.err(C.grove_run_cycle_reclaim_preempt_queues(e.h, &t.quotas[0], C.uint32_t(len(t.quotas)), &t.running[0],
 				C.uint32_t(len(t.running)), hp, C.uint32_t(len(t.holdings)), &t.runningQueue[0], &r.stats)); err != nil {
 				return nil, err
 			}
 		} else if len(t.runningQueue) > 0 && len(t.quotas) > 0 {
+			usedQuotas = true
 			if err := e.err(C.grove_run_cycle_reclaim_queues(e.h, &t.quotas[0], C.uint32_t(len(t.quotas)), &t.running[0],
 				C.uint32_t(len(t.running)), hp, C.uint32_t(len(t.holdings)), &t.runningQueue[0], &r.stats)); err != nil {
 				return nil, err
@@ -205,6 +221,7 @@ func (e *engine) cycle(t *tables, preempt, large, explain bool) (*result, error)
 			}
 		}
 	} else if len(t.fairShare) > 0 && len(t.queues) > 0 {
+		usedQuotas = true
 		if err := e.err(C.grove_set_fair_share(e.h, &t.fairShare[0], C.uint32_t(len(t.fairShare)))); err != nil {
 			return nil, err
 		}
@@ -213,6 +230,12 @@ func (e *engine) cycle(t *tables, preempt, large, explain bool) (*result, error)
 		}
 	} else if err := e.err(C.grove_run_cycle(e.h, &r.stats)); err != nil {
 		return nil, err
+	}
+	if weighted && usedQuotas {
+		r.fairShares = make([]C.uint64_t, 3*len(t.queues))
+		if err := e.err(C.grove_get_fair_shares(e.h, (*C.uint64_t)(&r.fairShares[0]), C.uint32_t(len(t.queues)))); err != nil {
+			return nil, err
+		}
 	}
 	r.placements = make([]C.grove_placement_t, int(r.stats.pods_bound)+1)
 	var n C.uint32_t
