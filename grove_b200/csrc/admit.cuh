@@ -171,10 +171,10 @@ __device__ __forceinline__ uint32_t visit_pos(const GangRegs& g, uint32_t n) {
 // ---- the evaluator: the whole warp packs ONE candidate range ------------------------------------------
 // kFence: the nodes of the fences active for the gang (fm0 / fm1, common.cuh fenced) take no pod
 // kImex: the nodes another CD holds in the gang's view (imex.cuh imex_foreign) take no pod of its enrolled cliques (enr)
-template <bool kPref_, bool kHolds, bool kWide_ = false, bool kFence = false, bool kImex = false>
+template <bool kPref_, Mode M>
 struct Ev {
   static constexpr bool kPref = kPref_;
-  static constexpr bool kWide = kWide_;
+  static constexpr bool kWide = M == Mode::kWide, kFence = M == Mode::kFence, kImex = M == Mode::kImex;
   static constexpr bool kStaged = false;
   const Topo& tp; const Relax& rb; GangShared& sh; const GangRegs& g; uint32_t lane;
   uint32_t np;
@@ -234,13 +234,13 @@ struct Ev {
 #pragma unroll
           for (uint32_t s = 0; s < kClaimSlots; ++s) {
             const uint4 c = __ldg(line + s);
-            if (gives_back<kHolds, kImex>(c.x, g.rank)) { cpu += int(c.y); mem += int(c.z); gpu += int(c.w & 0xFFFFu); pods += int(c.w >> 16); }
+            if (gives_back<M>(c.x, g.rank)) { cpu += int(c.y); mem += int(c.z); gpu += int(c.w & 0xFFFFu); pods += int(c.w >> 16); }
           }
         }
         if (live & kHasOvf) {
           for (uint32_t i = __ldg(rb.ovf_head + n); i; i = __ldg(rb.ovf_next + i - 1)) {
             const uint4 c = __ldg(rb.ovf_claim + i - 1);
-            if (gives_back<kHolds, kImex>(c.x, g.rank)) { cpu += int(c.y); mem += int(c.z); gpu += int(c.w & 0xFFFFu); pods += int(c.w >> 16); }
+            if (gives_back<M>(c.x, g.rank)) { cpu += int(c.y); mem += int(c.z); gpu += int(c.w & 0xFFFFu); pods += int(c.w >> 16); }
           }
         }
       }
@@ -358,10 +358,10 @@ struct Ev {
 // instead of a chain of dependent L2 look-ups per 32 nodes.
 constexpr uint32_t kStageMax = 128;
 
-template <bool kPref_, bool kHolds, bool kWide_ = false, bool kFence = false, bool kImex = false>
+template <bool kPref_, Mode M>
 struct EvS {
   static constexpr bool kPref = kPref_;
-  static constexpr bool kWide = kWide_;
+  static constexpr bool kWide = M == Mode::kWide, kFence = M == Mode::kFence, kImex = M == Mode::kImex;
   static constexpr bool kStaged = true;   // node state in shared memory: an attempt costs less than the table look-ups that would skip it
   const Topo& tp; const Relax& rb; GangShared& sh; const GangRegs& g; uint32_t lane;
   int4* view;           // [kStageMax] cpu, mem, gpu, pods the gang may still take.  Signed: the claims of lower ranks may transiently exceed
@@ -419,12 +419,12 @@ struct EvS {
           for (uint32_t s = 0; s < kClaimSlots; ++s) c[s] = __ldg(line + s);
 #pragma unroll
           for (uint32_t s = 0; s < kClaimSlots; ++s)
-            if (gives_back<kHolds, kImex>(c[s].x, g.rank)) { cpu += int(c[s].y); mem += int(c[s].z); gpu += int(c[s].w & 0xFFFFu); pods += int(c[s].w >> 16); }
+            if (gives_back<M>(c[s].x, g.rank)) { cpu += int(c[s].y); mem += int(c[s].z); gpu += int(c[s].w & 0xFFFFu); pods += int(c[s].w >> 16); }
         }
         if (live[k] & kHasOvf) {
           for (uint32_t i = __ldg(rb.ovf_head + n); i; i = __ldg(rb.ovf_next + i - 1)) {
             const uint4 c = __ldg(rb.ovf_claim + i - 1);
-            if (gives_back<kHolds, kImex>(c.x, g.rank)) { cpu += int(c.y); mem += int(c.z); gpu += int(c.w & 0xFFFFu); pods += int(c.w >> 16); }
+            if (gives_back<M>(c.x, g.rank)) { cpu += int(c.y); mem += int(c.z); gpu += int(c.w & 0xFFFFu); pods += int(c.w >> 16); }
           }
         }
       }
@@ -854,18 +854,11 @@ __device__ __forceinline__ uint32_t eval_list_at(const Relax& rx, const Tables& 
 // cudaGridDependencySynchronize().
 constexpr uint32_t kEvalDeferred = 0xFFu;   // nxt_tstate: no result this round
 constexpr int kEvalWarps = 8;
-// kWide: the instantiation of a wide cycle (16-bit counts; the entry stack of each warp in Relax::wide_node).
-// kSpread: the instantiation of a cycle with topology spread members (spread.cuh): a member's candidates are those whose
-// level-l_s domain is allowed (HARD, and the first walk of SOFT) or not allowed (the second walk of SOFT).
-// kFence: the instantiation of a cycle with fences (fence.cuh): the nodes of an active fence of a gang ranked before the evaluated
-// one fail K1 fit in every view it forms (staged attempts, unstaged reads, the record - total fast path).  The capacity tables and
-// shape bits come from the committed table and stay upper bounds.
-// kQueue: the instantiation of a cycle with queue members (queue.cuh): a member whose gate is closed is REJECTED without evaluation,
-// and an admitted member packs each clique's surplus up to the replicas k_queue_gate allows.
-// kImex: the instantiation of a cycle with enrolled cliques (imex.cuh): a node another CD holds in the gang's view fails K1 fit for
-// the gang's enrolled cliques wherever a view is formed, like a fenced node.  Tables and shape bits stay ownership-blind upper bounds.
-template <bool kPref, bool kHolds, bool kWide, bool kSpread = false, bool kFence = false, bool kQueue = false, bool kImex = false>
+// M: the cycle's mode (common.cuh Mode), instantiated for every mode.
+template <bool kPref, Mode M>
 __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb, Relax rx, uint32_t max_att) {
+  constexpr bool kWide = M == Mode::kWide, kSpread = M == Mode::kSpread, kFence = M == Mode::kFence;
+  constexpr bool kQueue = M == Mode::kQueue, kImex = M == Mode::kImex;
   __shared__ GangShared shs[kEvalWarps];
   __shared__ int4 s_view[kEvalWarps][kStageMax];
   __shared__ uint32_t s_vflag[kEvalWarps][kStageMax];
@@ -961,8 +954,8 @@ __global__ void __launch_bounds__(kEvalWarps * 32, 2) k_eval(Topo tp, Tables tb,
     // shrink otherwise (claims are added, settled claims move into the committed state).  So a re-evaluation skips the
     // candidates in front of its last answer that no withdrawal touched -- gangs that meet a nearly full cluster would
     // otherwise re-run dozens of failing attempts every round.  (Single candidate level only.)
-    Ev<kPref, kHolds, kWide, kFence, kImex> ev(tp, rx, sh, g, lane);                  // candidates of any size, node state from L2
-    EvS<kPref, kHolds, kWide, kFence, kImex> evs(tp, rx, sh, g, lane, s_view[warp], s_vflag[warp], s_rk[warp]);         // candidates of <= kStageMax nodes, node state staged in shared memory
+    Ev<kPref, M> ev(tp, rx, sh, g, lane);                  // candidates of any size, node state from L2
+    EvS<kPref, M> evs(tp, rx, sh, g, lane, s_view[warp], s_vflag[warp], s_rk[warp]);         // candidates of <= kStageMax nodes, node state staged in shared memory
     if constexpr (kWide) { ev.wn = evs.wn = wide_node; ev.wm = evs.wm = wide_meta; }
     if constexpr (kFence) {   // the fences active for this gang: a lane per entry (at most 64), fixed for the round (k_apply writes tstate)
       bool a0 = false, a1 = false;

@@ -20,15 +20,31 @@ constexpr uint32_t kHold = 1u << 24;          // claim tag bit above the 24 rank
 constexpr uint32_t kEnrolled = 1u << 25;     // claim tag bit (kImex cycles): the claim is a run of an enrolled clique's pods
 constexpr uint32_t kRankBits = 0xFFFFFFu;
 
+// The mode of a relaxation cycle: which variant of the relaxation kernels it runs (engine.cu cycle_mode, once per cycle).
+enum class Mode : uint8_t {
+  kPlain,    // an ordinary cycle
+  kHolds,    // a cycle with holds (grove_run_cycle_reuse, the reclaim passes): a gang gives its own hold back to its view, and an
+             // owner publishes only what its placement needs beyond its hold
+  kWide,     // a wide submission (grove_submit_gangs_wide): 16-bit counts, each k_eval warp's entry stack in Relax::wide_node
+  kSpread,   // topology spread members (spread.cuh): a member's candidates are those whose level-l_s domain is allowed (HARD, and the
+             // first walk of SOFT) or not allowed (the second walk of SOFT); a changed result stamps its group (k_apply, k_detect)
+  kFence,    // fences (fence.cuh): the nodes of an active fence of a gang ranked before the evaluated one fail K1 fit in every view it
+             // forms (staged attempts, unstaged reads, the record - total fast path); the capacity tables and shape bits come from
+             // the committed table and stay upper bounds.  A fencing gang's flip to or from REJECTED stamps its fence (k_apply)
+  kQueue,    // queue members (queue.cuh): a member whose gate is closed is REJECTED without evaluation, an admitted one packs each
+             // clique's surplus up to the replicas k_queue_gate allows, and a changed result records its usage U (k_apply)
+  kImex,     // enrolled cliques (imex.cuh): a node another CD holds in the gang's view fails K1 fit for its enrolled cliques, like a
+             // fenced node; enrolled runs' claims carry kEnrolled and are counted per node (k_apply), and k_fold moves their CD
+             // into the node's committed owner
+};
+
 // Does the gang of rank `rank` give claim tag x back, i.e. not subtract it from its view?  The claims of the ranks after it, and
-// (kHolds: a cycle with holds) its own hold; every other hold is subtracted by everybody.  Without holds this is the plain rank
-// test: the kernels of an ordinary cycle are instantiated without the hold logic.  (kImex: a cycle with ComputeDomains, whose
-// tags may carry kEnrolled; such a cycle has no holds.)
-template <bool kHolds, bool kImex = false>
+// (kHolds) its own hold; every other hold is subtracted by everybody.  Otherwise this is the plain rank test: the kernels of an
+// ordinary cycle are instantiated without the hold logic.  (kImex: tags may carry kEnrolled.)
+template <Mode M>
 __device__ __forceinline__ bool gives_back(uint32_t x, uint32_t rank) {
-  static_assert(!(kHolds && kImex), "a ComputeDomain cycle has no holds");
-  if constexpr (kImex) return x != kClaimEmpty && (x & kRankBits) >= rank;
-  else if constexpr (kHolds) return (x >= rank && x < kHold) || x == (rank | kHold);   // (kClaimEmpty has the hold bit set)
+  if constexpr (M == Mode::kImex) return x != kClaimEmpty && (x & kRankBits) >= rank;
+  else if constexpr (M == Mode::kHolds) return (x >= rank && x < kHold) || x == (rank | kHold);   // (kClaimEmpty has the hold bit set)
   else return x >= rank && x != kClaimEmpty;
 }
 

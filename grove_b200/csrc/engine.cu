@@ -245,9 +245,10 @@ struct grove_engine {
   DevBuf<unsigned long long> d_dn_quota;
   DevBuf<long long> d_dn_load, d_dn_use;
   DevBuf<uint8_t> d_dn_fin, d_dn_bits;
-  // grove_diagnose (diagnose.cuh): whether the outputs on the device describe an ordinary cycle over the current inputs, the
-  // per-node usage lists, the batch descriptors, the per-domain capacity sums and the records
-  enum Diag : uint8_t { kDiagNoCycle, kDiagReady, kDiagRunning, kDiagChanged, kDiagSpread, kDiagFence, kDiagImex, kDiagFairShare } diag = kDiagNoCycle;
+  // grove_diagnose (diagnose.cuh): whether the outputs on the device describe an ordinary cycle over the current inputs, and its
+  // mode (kDiagReady); the per-node usage lists, the batch descriptors, the per-domain capacity sums and the records
+  enum Diag : uint8_t { kDiagNoCycle, kDiagReady, kDiagRunning, kDiagChanged, kDiagFairShare } diag = kDiagNoCycle;
+  Mode diag_mode = Mode::kPlain;
   DevBuf<uint32_t> d_dg_cnt, d_dg_off, d_dg_cur, d_dg_minr;
   DevBuf<uint4> d_dg_rec;
   DevBuf<DiagGang> d_dg_gang;
@@ -339,24 +340,28 @@ struct grove_engine {
   } while (0)
 
 static int32_t fail(grove_engine* e, int32_t code, const char* msg) { e->err = msg; return code; }
-static int32_t refuse_spread(grove_engine* e, const char* entry) {
-  e->err = std::string(entry) + ": not supported while a topology spread set with members is in place (grove_set_spread)";
-  return GROVE_ERR_STATE;
+// The optional sets of a submission, in the order a refusal reports them: when each is in place, and which others grove_run_cycle
+// runs it with.  Spread, fence, queue and ComputeDomain sets each choose the cycle's mode (cycle_mode), so they exclude each
+// other; bin-packing and fair share run in an ordinary or a queue cycle, not together.
+enum Set : uint32_t { kSetSpread = 1, kSetFence = 2, kSetQueue = 4, kSetBinpack = 8, kSetImex = 16, kSetFairShare = 32 };
+struct SetRow { const char* what; uint32_t runs_with; };
+static constexpr SetRow kSetTable[] = {
+    {"a topology spread set with members is in place (grove_set_spread)", 0},
+    {"a fence set is in place (grove_set_fences)", 0},
+    {"a queue set with members is in place (grove_set_queues)", kSetBinpack | kSetFairShare},
+    {"a bin-packing set with members is in place (grove_set_binpack)", kSetQueue},
+    {"a ComputeDomain set with an enrolled clique is in place (grove_set_compute_domains)", 0},
+    {"a fair-share set is in place (grove_set_fair_share)", kSetQueue},
+};
+static uint32_t sets_in_place(const grove_engine* e) {
+  return (e->sp_members ? kSetSpread : 0u) | (!e->fc_gangs.empty() ? kSetFence : 0u) | (e->qu_members ? kSetQueue : 0u) |
+         (e->bp_members ? kSetBinpack : 0u) | (e->im_enrolled ? kSetImex : 0u) | (e->fs_given ? kSetFairShare : 0u);
 }
-static int32_t refuse_fences(grove_engine* e, const char* entry) {
-  e->err = std::string(entry) + ": not supported while a fence set is in place (grove_set_fences)";
-  return GROVE_ERR_STATE;
-}
-static int32_t refuse_queues(grove_engine* e, const char* entry) {
-  e->err = std::string(entry) + ": not supported while a queue set with members is in place (grove_set_queues)";
-  return GROVE_ERR_STATE;
-}
-static int32_t refuse_binpack(grove_engine* e, const char* entry) {
-  e->err = std::string(entry) + ": not supported while a bin-packing set with members is in place (grove_set_binpack)";
-  return GROVE_ERR_STATE;
-}
-static int32_t refuse_imex(grove_engine* e, const char* entry) {
-  e->err = std::string(entry) + ": not supported while a ComputeDomain set with an enrolled clique is in place (grove_set_compute_domains)";
+// refuses the first set in place that `entry` does not run with (a refusal leaves grove_diagnose as it was)
+static int32_t refuse_sets(grove_engine* e, const char* entry, uint32_t allowed) {
+  const uint32_t s = sets_in_place(e) & ~allowed;
+  if (!s) return GROVE_OK;
+  e->err = std::string(entry) + ": not supported while " + kSetTable[__builtin_ctz(s)].what;
   return GROVE_ERR_STATE;
 }
 static int32_t refuse_wide(grove_engine* e, const char* entry) {
@@ -545,6 +550,45 @@ static Relax make_relax(grove_engine* e) {
 }
 
 // ---------------------------------------------------------------------------------------------
+// The mode of the cycle about to run (common.cuh Mode).  The entries let at most one of the sets that choose a mode be in place
+// (kSetTable), the running-gang entries refuse them all, and a wide submission takes no set.
+static Mode cycle_mode(const grove_engine* e) {
+  if (e->sp_members) return Mode::kSpread;
+  if (!e->fc_gangs.empty()) return Mode::kFence;
+  if (e->im_enrolled) return Mode::kImex;
+  if (e->qu_members) return Mode::kQueue;
+  if (e->wide) return Mode::kWide;
+  if (e->holds_on) return Mode::kHolds;
+  return Mode::kPlain;
+}
+
+// Each relaxation kernel is instantiated for the modes whose code differs from kPlain, and a mode runs that instantiation:
+// k_eval for every mode, k_apply for all but kWide, k_detect for kSpread, k_fold for kHolds and kImex.
+constexpr Mode apply_mode(Mode m) { return m == Mode::kWide ? Mode::kPlain : m; }
+constexpr Mode fold_mode(Mode m) { return m == Mode::kHolds || m == Mode::kImex ? m : Mode::kPlain; }
+
+struct RoundKernels {
+  void (*eval)(Topo, Tables, Relax, uint32_t);
+  void (*apply)(Tables, Relax);
+  void (*detect)(Topo, Tables, Relax, uint32_t);
+  void (*fold)(Tables, Relax, uint4*);
+};
+template <Mode M>
+static RoundKernels round_kernels(bool pref) {
+  return {pref ? k_eval<true, M> : k_eval<false, M>, k_apply<apply_mode(M)>, k_detect<M == Mode::kSpread>, k_fold<fold_mode(M)>};
+}
+static RoundKernels round_kernels(Mode m, bool pref) {
+  switch (m) {
+    case Mode::kHolds: return round_kernels<Mode::kHolds>(pref);
+    case Mode::kWide: return round_kernels<Mode::kWide>(pref);
+    case Mode::kSpread: return round_kernels<Mode::kSpread>(pref);
+    case Mode::kFence: return round_kernels<Mode::kFence>(pref);
+    case Mode::kQueue: return round_kernels<Mode::kQueue>(pref);
+    case Mode::kImex: return round_kernels<Mode::kImex>(pref);
+    default: return round_kernels<Mode::kPlain>(pref);
+  }
+}
+
 extern "C" {
 
 uint32_t grove_abi_version(void) { return GROVE_ABI_VERSION; }
@@ -615,18 +659,28 @@ void grove_engine_destroy(grove_engine_t* e) {
 }
 
 
+// the outputs no longer describe the cycle that made them over the current inputs
+static void inputs_changed(grove_engine* e) {
+  if (e->diag == grove_engine::kDiagReady) e->diag = grove_engine::kDiagChanged;
+}
+
+// every optional set belongs to the nodes and gangs it was validated against (a queue set with its fair-share set and over-quota
+// weights): a node load or a submission drops them all
+static void drop_sets(grove_engine* e) {
+  e->sp_groups = e->sp_members = 0;
+  e->fc_gangs.clear();
+  e->qu_members = 0; e->qu_given = false;
+  e->fs_given = false; e->fs_have_order = false;
+  e->oq_given = false; e->oq_have_fair = false;
+  e->bp_members = 0; e->bp_given = false;
+  e->im_enrolled = 0; e->im_given = false;
+}
+
 static int32_t load_nodes_common(grove_engine* e, const grove_node_t* host_nodes, const void* dev_nodes, uint32_t n) {
   if (n == 0 || n > GROVE_MAX_NODES) return fail(e, GROVE_ERR_INVALID_ARG, "node count out of range");
   if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
-  if (e->diag == grove_engine::kDiagReady || e->diag == grove_engine::kDiagSpread || e->diag == grove_engine::kDiagFence ||
-      e->diag == grove_engine::kDiagImex) e->diag = grove_engine::kDiagChanged;
-  e->sp_groups = e->sp_members = 0;   // a spread set belongs to the nodes and gangs it was validated against
-  e->fc_gangs.clear();                // (a fence set too)
-  e->qu_members = 0; e->qu_given = false;   // (and a queue set, with its fair-share set and over-quota weights)
-  e->fs_given = false; e->fs_have_order = false;
-  e->oq_given = false; e->oq_have_fair = false;
-  e->bp_members = 0; e->bp_given = false;   // (and a bin-packing set)
-  e->im_enrolled = 0; e->im_given = false;  // (and a ComputeDomain set)
+  inputs_changed(e);
+  drop_sets(e);
   CU_TRY(e, cudaSetDevice(e->cfg.device));
   if (host_nodes) {
     CU_TRY(e, cudaEventSynchronize(e->ev_nodes_up));  // an earlier upload may still be reading the staging buffer
@@ -678,8 +732,7 @@ int32_t grove_update_nodes(grove_engine_t* e, const uint32_t* idx, const grove_n
   if (!e || (n && (!idx || !recs))) return GROVE_ERR_INVALID_ARG;
   if (!e->nodes_loaded) return fail(e, GROVE_ERR_STATE, "no node snapshot loaded");
   if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
-  if (e->diag == grove_engine::kDiagReady || e->diag == grove_engine::kDiagSpread || e->diag == grove_engine::kDiagFence ||
-      e->diag == grove_engine::kDiagImex) e->diag = grove_engine::kDiagChanged;
+  inputs_changed(e);
   if (n == 0) return GROVE_OK;
   e->score_pass_valid = false;
   CU_TRY(e, cudaSetDevice(e->cfg.device));
@@ -782,16 +835,9 @@ static int32_t validate(grove_engine* e, const grove_gang_t* gangs, uint32_t G, 
 static int32_t submit(grove_engine* e, const grove_gang_t* gangs, uint32_t n_gangs, const grove_clique_t* cliques,
                       const std::vector<uint32_t>& ccount, uint32_t n_cliques, const grove_scope_t* scopes, uint32_t n_scopes, uint32_t max_pods) {
   if (e->in_cycle) return fail(e, GROVE_ERR_STATE, "cycle in flight");
-  if (e->diag == grove_engine::kDiagReady || e->diag == grove_engine::kDiagSpread || e->diag == grove_engine::kDiagFence ||
-      e->diag == grove_engine::kDiagImex) e->diag = grove_engine::kDiagChanged;
+  inputs_changed(e);
   if (n_gangs >= (1u << 24)) return fail(e, GROVE_ERR_LIMIT, "too many gangs");  // order rank + round tag share a stamp word
-  e->sp_groups = e->sp_members = 0;
-  e->fc_gangs.clear();
-  e->qu_members = 0; e->qu_given = false;
-  e->fs_given = false; e->fs_have_order = false;
-  e->oq_given = false; e->oq_have_fair = false;
-  e->bp_members = 0; e->bp_given = false;
-  e->im_enrolled = 0; e->im_given = false;
+  drop_sets(e);
   int32_t rc = validate(e, gangs, n_gangs, cliques, ccount.data(), n_cliques, scopes, n_scopes, max_pods);
   if (rc) return rc;
   CU_TRY(e, cudaSetDevice(e->cfg.device));
@@ -1332,7 +1378,8 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
     CU_TRY(e, cudaGetLastError());
     e->launches += 1;
   }
-  const bool spread = e->sp_members > 0;   // (the running-gang entries refuse a spread set: no holds here)
+  const Mode mode = cycle_mode(e);
+  const bool spread = mode == Mode::kSpread, fences = mode == Mode::kFence, queues = mode == Mode::kQueue, imex = mode == Mode::kImex;
   if (G && spread) {   // the classes of every domain's schedulable nodes, over the cycle-start table; no member's stamp
     CU_TRY(e, cudaMemsetAsync(e->d_sp_dcls.p, 0, sizeof(uint32_t) * e->sp_dcls_words, e->stream));
     CU_TRY(e, cudaMemsetAsync(e->d_sp_stamp.p, 0xFF, sizeof(uint32_t) * e->sp_groups, e->stream));
@@ -1340,9 +1387,6 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
     CU_TRY(e, cudaGetLastError());
     e->launches += 1;
   }
-  const bool fences = !e->fc_gangs.empty();   // (the running-gang entries and spread cycles refuse a fence set)
-  const bool queues = e->qu_members > 0;   // (the running-gang entries, spread and fenced cycles refuse a queue set)
-  const bool imex = e->im_enrolled > 0;    // (the running-gang entries and the other sets' cycles refuse an enrolled clique)
   if (G && imex) {   // the CD of every clique and of every rank's gang, owner0 in sorted order (padding: no owner), no enrolled claim
     e->h_im_rank_cd.resize(G); e->h_im_owner.resize(e->Npad);
     for (uint32_t g = 0; g < G; ++g) e->h_im_rank_cd[e->ginfo[g].order] = e->im_gang_cd[g];
@@ -1400,65 +1444,29 @@ static int32_t run_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
     // moved on, and to know when to stop).  GROVE_DEBUG_ADMIT looks after every round.
     const uint32_t batch = e->dbg_on ? 1u : std::max(1u, e->tune_batch);
     uint32_t next_round = 1;   // number of the next round to be enqueued (rounds advance one by one until the cycle is over)
+    const RoundKernels k = round_kernels(mode, e->any_preferred);
     auto enqueue_round = [&]() -> int32_t {
       if (next_round > 1 && next_round % kTagRounds == 0) {   // the stamp tags wrap: forget the stamps of the epoch that ends
         CU_TRY(e, cudaMemsetAsync(e->d_add_stamp.p, 0xFF, sizeof(uint32_t) * e->Npad, e->stream));
         CU_TRY(e, cudaMemsetAsync(e->d_rem_stamp.p, 0xFF, sizeof(uint32_t) * e->words, e->stream));
         if (spread) CU_TRY(e, cudaMemsetAsync(e->d_sp_stamp.p, 0xFF, sizeof(uint32_t) * e->sp_groups, e->stream));
       }
-      if (spread) {   // a spread cycle: the members' allowed domains first, then its own instantiations of the round's kernels
-        CU_TRY(e, launch_chained(k_spread, e->sp_groups, 256, e->stream, tp, tb, rx, 0u));
-        CU_TRY(e, launch_chained(e->any_preferred ? k_eval<true, false, false, true> : k_eval<false, false, false, true>, n_eval_ctas,
-                                 kEvalWarps * 32, e->stream, tp, tb, rx, e->tune_max_att));
-        CU_TRY(e, launch_chained(k_apply<false, true>, warp_ctas, 256, e->stream, tb, rx));
-        CU_TRY(e, launch_chained(k_detect<true>, warp_ctas, 256, e->stream, tp, tb, rx, e->tune_refresh));
-        e->launches += 4;
-        ++next_round;
-        return GROVE_OK;
-      }
-      if (fences) {   // a fenced cycle: its own instantiations of K3 and k_apply
-        CU_TRY(e, launch_chained(e->any_preferred ? k_eval<true, false, false, false, true> : k_eval<false, false, false, false, true>,
-                                 n_eval_ctas, kEvalWarps * 32, e->stream, tp, tb, rx, e->tune_max_att));
-        CU_TRY(e, launch_chained(k_apply<false, false, true>, warp_ctas, 256, e->stream, tb, rx));
-        CU_TRY(e, launch_chained(k_detect<false>, warp_ctas, 256, e->stream, tp, tb, rx, e->tune_refresh));
-        e->launches += 3;
-        ++next_round;
-        return GROVE_OK;
-      }
-      if (imex) {   // a cycle with enrolled cliques: its own instantiations of K3 and k_apply
-        CU_TRY(e, launch_chained(e->any_preferred ? k_eval<true, false, false, false, false, false, true> : k_eval<false, false, false, false, false, false, true>,
-                                 n_eval_ctas, kEvalWarps * 32, e->stream, tp, tb, rx, e->tune_max_att));
-        CU_TRY(e, launch_chained(k_apply<false, false, false, false, true>, warp_ctas, 256, e->stream, tb, rx));
-        CU_TRY(e, launch_chained(k_detect<false>, warp_ctas, 256, e->stream, tp, tb, rx, e->tune_refresh));
-        e->launches += 3;
-        ++next_round;
-        return GROVE_OK;
-      }
-      if (queues) {   // a queue cycle: its own instantiations of K3 and k_apply, then the headroom and the gates before k_detect
-        CU_TRY(e, launch_chained(e->any_preferred ? k_eval<true, false, false, false, false, true> : k_eval<false, false, false, false, false, true>,
-                                 n_eval_ctas, kEvalWarps * 32, e->stream, tp, tb, rx, e->tune_max_att));
-        CU_TRY(e, launch_chained(k_apply<false, false, false, true>, warp_ctas, 256, e->stream, tb, rx));
+      // one stream-ordered chain: evaluate -> publish -> detect, each launched while the one before drains; a spread cycle
+      // computes the members' allowed domains first, a queue cycle the headroom and the gates before k_detect
+      if (spread) CU_TRY(e, launch_chained(k_spread, e->sp_groups, 256, e->stream, tp, tb, rx, 0u));
+      CU_TRY(e, launch_chained(k.eval, n_eval_ctas, kEvalWarps * 32, e->stream, tp, tb, rx, e->tune_max_att));
+      CU_TRY(e, launch_chained(k.apply, warp_ctas, 256, e->stream, tb, rx));
+      if (queues) {
         CU_TRY(e, launch_chained(k_queue_scan, e->qu_scanned, 256, e->stream, tb, rx, 0u));
         CU_TRY(e, launch_chained(k_queue_gate, (e->qu_members + 255) / 256, 256, e->stream, tb, rx, 1u, (grove_gang_status_t*)nullptr));
-        CU_TRY(e, launch_chained(k_detect<false>, warp_ctas, 256, e->stream, tp, tb, rx, e->tune_refresh));
-        e->launches += 5;
-        ++next_round;
-        return GROVE_OK;
       }
-      // one stream-ordered chain: evaluate -> publish -> detect, each launched while the one before drains
-      // (a wide cycle never has holds: grove_run_cycle_reuse refuses wide submissions)
-      auto* k3 = e->wide ? (e->any_preferred ? k_eval<true, false, true> : k_eval<false, false, true>)
-                 : e->holds_on ? (e->any_preferred ? k_eval<true, true, false> : k_eval<false, true, false>)
-                               : (e->any_preferred ? k_eval<true, false, false> : k_eval<false, false, false>);
-      CU_TRY(e, launch_chained(k3, n_eval_ctas, kEvalWarps * 32, e->stream, tp, tb, rx, e->tune_max_att));
-      CU_TRY(e, launch_chained(e->holds_on ? k_apply<true> : k_apply<false>, warp_ctas, 256, e->stream, tb, rx));
-      CU_TRY(e, launch_chained(k_detect<false>, warp_ctas, 256, e->stream, tp, tb, rx, e->tune_refresh));
-      e->launches += 3;
+      CU_TRY(e, launch_chained(k.detect, warp_ctas, 256, e->stream, tp, tb, rx, e->tune_refresh));
+      e->launches += 3 + (spread ? 1 : 0) + (queues ? 2 : 0);
       ++next_round;
       return GROVE_OK;
     };
     auto fold = [&]() -> int32_t {   // the final gangs' claims -> committed state (relax.cuh k_fold)
-      CU_TRY(e, launch_chained(imex ? k_fold<false, true> : e->holds_on ? k_fold<true> : k_fold<false>, warp_ctas, 256, e->stream, tb, rx, e->d_nres.p));
+      CU_TRY(e, launch_chained(k.fold, warp_ctas, 256, e->stream, tb, rx, e->d_nres.p));
       CU_TRY(e, launch_chained(k_fold_mark, 1, 1, e->stream, rx));
       e->launches += 2;
       CU_TRY(e, cudaGetLastError());
@@ -1599,19 +1607,18 @@ static int32_t fair_share_cycle(grove_engine* e, grove_cycle_stats_t* stats);
 
 int32_t grove_run_cycle(grove_engine_t* e, grove_cycle_stats_t* stats) {
   if (!e) return GROVE_ERR_INVALID_ARG;
+  const uint32_t sets = sets_in_place(e);
+  for (uint32_t s = sets; s; s &= s - 1) {   // every set in place runs with every other one (a refusal leaves grove_diagnose as it was)
+    const uint32_t i = __builtin_ctz(s), clash = sets & ~(1u << i) & ~kSetTable[i].runs_with;
+    if (clash) {
+      e->err = std::string("grove_run_cycle: not supported while ") + kSetTable[i].what + " and " + kSetTable[__builtin_ctz(clash)].what;
+      return GROVE_ERR_STATE;
+    }
+  }
   if (e->fs_given) return fair_share_cycle(e, stats);
-  const bool spread = e->sp_members > 0, fences = !e->fc_gangs.empty();
-  if (spread && fences) return fail(e, GROVE_ERR_STATE, "grove_run_cycle: a spread set with members and a fence set together are not supported");
-  if (e->qu_members && (spread || fences))
-    return fail(e, GROVE_ERR_STATE, "grove_run_cycle: a queue set with members together with a spread set with members or a fence set is not supported");
-  if (e->bp_members && (spread || fences))
-    return fail(e, GROVE_ERR_STATE, "grove_run_cycle: a bin-packing set with members together with a spread set with members or a fence set is not supported");
-  if (e->im_enrolled && (spread || fences || e->qu_members || e->bp_members))
-    return fail(e, GROVE_ERR_STATE, "grove_run_cycle: a ComputeDomain set with an enrolled clique together with a spread set with members, a fence set, "
-                                    "a queue set with members or a bin-packing set with members is not supported");
+  const Mode mode = cycle_mode(e);
   const int32_t rc = run_cycle(e, stats);
-  if (rc == GROVE_OK)
-    e->diag = spread ? grove_engine::kDiagSpread : fences ? grove_engine::kDiagFence : e->im_enrolled ? grove_engine::kDiagImex : grove_engine::kDiagReady;
+  if (rc == GROVE_OK) { e->diag = grove_engine::kDiagReady; e->diag_mode = mode; }
   return rc;
 }
 
@@ -1976,16 +1983,17 @@ static constexpr size_t kDiagScratchCols = size_t(1) << 23;
 int32_t grove_diagnose(grove_engine_t* e, grove_gang_diag_t* gangs, uint32_t cap_g, grove_clique_diag_t* cliques, uint32_t cap_q) {
   if (!e) return GROVE_ERR_INVALID_ARG;
   switch (e->diag) {
-    case grove_engine::kDiagReady: break;
+    case grove_engine::kDiagReady:
+      if (e->diag_mode == Mode::kSpread)
+        return fail(e, GROVE_ERR_STATE, "grove_diagnose: the last cycle had topology spread members, which the diagnosis does not model");
+      if (e->diag_mode == Mode::kFence)
+        return fail(e, GROVE_ERR_STATE, "grove_diagnose: the last cycle had fences, which the diagnosis does not model");
+      if (e->diag_mode == Mode::kImex)
+        return fail(e, GROVE_ERR_STATE, "grove_diagnose: the last cycle had enrolled cliques (ComputeDomains), which the diagnosis does not model");
+      break;
     case grove_engine::kDiagNoCycle: return fail(e, GROVE_ERR_STATE, "grove_diagnose: no completed cycle");
     case grove_engine::kDiagRunning:
       return fail(e, GROVE_ERR_STATE, "grove_diagnose: the last cycle ran with running gangs (preempt / reuse); only grove_run_cycle is diagnosed");
-    case grove_engine::kDiagSpread:
-      return fail(e, GROVE_ERR_STATE, "grove_diagnose: the last cycle had topology spread members, which the diagnosis does not model");
-    case grove_engine::kDiagFence:
-      return fail(e, GROVE_ERR_STATE, "grove_diagnose: the last cycle had fences, which the diagnosis does not model");
-    case grove_engine::kDiagImex:
-      return fail(e, GROVE_ERR_STATE, "grove_diagnose: the last cycle had enrolled cliques (ComputeDomains), which the diagnosis does not model");
     case grove_engine::kDiagFairShare:
       return fail(e, GROVE_ERR_STATE, "grove_diagnose: the last cycle ran in fair-share order, which the diagnosis does not model");
     default: return fail(e, GROVE_ERR_STATE, "grove_diagnose: nodes or gangs were loaded, updated or submitted since the last cycle");
@@ -2408,11 +2416,7 @@ static int32_t run_cycle_holds(grove_engine* e, const uint32_t* replaces, const 
 int32_t grove_run_cycle_reuse(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs, const grove_running_gang_t* running,
                               uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
   if (!e || (n_gangs && !replaces) || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
-  if (e->sp_members) return refuse_spread(e, "grove_run_cycle_reuse");
-  if (e->qu_members) return refuse_queues(e, "grove_run_cycle_reuse");
-  if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_reuse");
-  if (e->bp_members) return refuse_binpack(e, "grove_run_cycle_reuse");
-  if (e->im_enrolled) return refuse_imex(e, "grove_run_cycle_reuse");
+  if (int32_t rc = refuse_sets(e, "grove_run_cycle_reuse", kSetFairShare)) return rc;   // (a fair-share set over a queue set without members)
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse");
   const int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);
@@ -2841,11 +2845,7 @@ static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const gr
 int32_t grove_run_cycle_preempt(grove_engine_t* e, const grove_running_gang_t* running, uint32_t n_running,
                                 const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
   if (!e || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
-  if (e->sp_members) return refuse_spread(e, "grove_run_cycle_preempt");
-  if (e->qu_members) return refuse_queues(e, "grove_run_cycle_preempt");
-  if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_preempt");
-  if (e->bp_members) return refuse_binpack(e, "grove_run_cycle_preempt");
-  if (e->im_enrolled) return refuse_imex(e, "grove_run_cycle_preempt");
+  if (int32_t rc = refuse_sets(e, "grove_run_cycle_preempt", kSetFairShare)) return rc;   // (a fair-share set over a queue set without members)
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_preempt");
   int32_t rc = check_ready(e);
@@ -2858,11 +2858,7 @@ int32_t grove_run_cycle_preempt(grove_engine_t* e, const grove_running_gang_t* r
 int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs, const grove_running_gang_t* running,
                                       uint32_t n_running, const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats) {
   if (!e || (n_gangs && !replaces) || (n_running && !running) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
-  if (e->sp_members) return refuse_spread(e, "grove_run_cycle_reuse_preempt");
-  if (e->qu_members) return refuse_queues(e, "grove_run_cycle_reuse_preempt");
-  if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_reuse_preempt");
-  if (e->bp_members) return refuse_binpack(e, "grove_run_cycle_reuse_preempt");
-  if (e->im_enrolled) return refuse_imex(e, "grove_run_cycle_reuse_preempt");
+  if (int32_t rc = refuse_sets(e, "grove_run_cycle_reuse_preempt", kSetFairShare)) return rc;   // (a fair-share set over a queue set without members)
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse_preempt");
   const int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);
@@ -2965,12 +2961,8 @@ static int32_t over_quota_shares(grove_engine* e, const grove_queue_quota_t* quo
 // The checks grove_run_cycle_preempt_queues and grove_run_cycle_reclaim_queues share.  First the sets the entries refuse (a refusal
 // here leaves grove_diagnose as it was) ...
 static int32_t check_queue_sets(grove_engine* e, const char* entry) {
-  if (e->sp_members) return refuse_spread(e, entry);
-  if (!e->fc_gangs.empty()) return refuse_fences(e, entry);
-  if (e->bp_members) return refuse_binpack(e, entry);
-  if (e->im_enrolled) return refuse_imex(e, entry);
+  if (int32_t rc = refuse_sets(e, entry, kSetQueue)) return rc;   // (a fair-share set comes last: it stands on a queue set)
   if (!e->qu_given) { e->err = std::string(entry) + ": no queue set given for the current submission (grove_set_queues)"; return GROVE_ERR_STATE; }
-  if (e->fs_given) { e->err = std::string(entry) + ": not supported while a fair-share set is in place (grove_set_fair_share)"; return GROVE_ERR_STATE; }
   return GROVE_OK;
 }
 
@@ -3189,10 +3181,6 @@ static int32_t fs_take_order(grove_engine* e, uint32_t d, std::vector<uint32_t>&
 static int32_t fair_share_cycle(grove_engine* e, grove_cycle_stats_t* stats) {
   int32_t rc = check_ready(e);
   if (rc) return rc;
-  if (e->bp_members) return refuse_binpack(e, "grove_run_cycle with a fair-share set");
-  if (e->im_enrolled) return refuse_imex(e, "grove_run_cycle with a fair-share set");
-  if (e->sp_members) return refuse_spread(e, "grove_run_cycle with a fair-share set");
-  if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle with a fair-share set");
   if (!e->qu_given) return fail(e, GROVE_ERR_STATE, "grove_run_cycle: the fair-share set has no queue set (grove_set_queues)");
   struct Diag { grove_engine* e; ~Diag() { e->diag = grove_engine::kDiagFairShare; } } diag_guard{e};
   CU_TRY(e, cudaSetDevice(e->cfg.device));
@@ -3364,11 +3352,7 @@ int32_t grove_run_cycle_consolidate(grove_engine_t* e, const uint32_t* targets, 
                                     const grove_running_gang_t* running, uint32_t n_running, const grove_holding_t* holdings,
                                     uint32_t n_holdings, grove_cycle_stats_t* stats) {
   if (!e || (n_targets && !targets) || (n_running && (!running || !spec_of)) || (n_holdings && !holdings)) return GROVE_ERR_INVALID_ARG;
-  if (e->sp_members) return refuse_spread(e, "grove_run_cycle_consolidate");
-  if (e->qu_members) return refuse_queues(e, "grove_run_cycle_consolidate");
-  if (!e->fc_gangs.empty()) return refuse_fences(e, "grove_run_cycle_consolidate");
-  if (e->bp_members) return refuse_binpack(e, "grove_run_cycle_consolidate");
-  if (e->im_enrolled) return refuse_imex(e, "grove_run_cycle_consolidate");
+  if (int32_t rc = refuse_sets(e, "grove_run_cycle_consolidate", kSetFairShare)) return rc;   // (a fair-share set over a queue set without members)
   NoDiagnosis no_diag{e};
   if (e->wide) return refuse_wide(e, "grove_run_cycle_consolidate");
   if (n_targets > GROVE_MAX_CONSOLIDATE_TARGETS) return fail(e, GROVE_ERR_LIMIT, "grove_run_cycle_consolidate: more than GROVE_MAX_CONSOLIDATE_TARGETS targets");

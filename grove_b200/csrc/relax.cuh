@@ -205,12 +205,11 @@ __global__ void __launch_bounds__(256) k_hold_release(Tables tb, Relax rx, uint4
   }
 }
 
-// one warp per evaluated gang: publish a changed result (kHolds: a cycle with holds; kSpread: a cycle with spread members, whose
-// changed results leave a stamp per group; kFence: a cycle with fences, whose gangs' flips to or from REJECTED stamp their fence;
-// kQueue: a cycle with queue members, whose changed results record their usage U for k_queue_scan; kImex: a cycle with enrolled
-// cliques, whose runs' claims carry kEnrolled and are counted per node)
-template <bool kHolds, bool kSpread = false, bool kFence = false, bool kQueue = false, bool kImex = false>
+// one warp per evaluated gang: publish a changed result (M: the cycle's mode, common.cuh Mode; a wide cycle runs kPlain)
+template <Mode M>
 __global__ void __launch_bounds__(256) k_apply(Tables tb, Relax rx) {
+  constexpr bool kHolds = M == Mode::kHolds, kSpread = M == Mode::kSpread, kFence = M == Mode::kFence;
+  constexpr bool kQueue = M == Mode::kQueue, kImex = M == Mode::kImex;
   cudaGridDependencySynchronize();   // (launched chained: engine.cu launch_chained)
   const uint32_t lane = threadIdx.x & 31;
   if (rx.ctl[kDone]) return;
@@ -399,9 +398,10 @@ __global__ void __launch_bounds__(256) k_detect(Topo tp, Tables tb, Relax rx, ui
 // one warp per gang that became final since the last fold: its claims move into the committed state.  Not every round: the
 // claims of final gangs are as good as committed for everybody who ranks after them, so the fold runs before a capacity-table
 // rebuild (the tables are built from the committed state) and when the cycle ends; k_fold_mark then moves the marker.
-// (kImex: an enrolled run's CD becomes the node's committed owner)
-template <bool kHolds, bool kImex = false>
+// (M: the cycle's mode, of which only kHolds and kImex differ from kPlain; kImex: an enrolled run's CD becomes the node's owner)
+template <Mode M>
 __global__ void __launch_bounds__(256) k_fold(Tables tb, Relax rx, uint4* nres) {
+  constexpr bool kHolds = M == Mode::kHolds, kImex = M == Mode::kImex;
   cudaGridDependencySynchronize();
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t lo = rx.ctl[kFolded], hi = rx.ctl[kFront];
