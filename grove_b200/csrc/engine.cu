@@ -220,6 +220,7 @@ struct grove_engine {
   bool in_cycle = false;
   uint64_t launches = 0;
   std::vector<grove_victim_t> victims;   // of the last grove_run_cycle_preempt
+  std::vector<grove_surplus_victim_t> surplus_victims;   // of the last grove_run_cycle_preempt_elastic
   // node-range shard of this handle (cfg.rank of cfg.world; the whole table when world <= 1): sorted node indices, cut at
   // top-level domain boundaries
   uint32_t shard_lo = 0, shard_hi = 0;
@@ -238,6 +239,10 @@ struct grove_engine {
   DevBuf<uint4> d_rc_ent, d_rc_real, d_rc_base, d_rc_rows, d_rc_patch;
   DevBuf<int32_t> d_rc_prio;
   DevBuf<uint8_t> d_rc_gone, d_rc_evict;
+  // the surplus pods of a grove_run_cycle_preempt_elastic (reclaim.cuh SurplusCsr): rows by sorted node, entries, taken mask
+  DevBuf<uint32_t> d_sp_off;
+  DevBuf<uint4> d_sp_ent;
+  DevBuf<uint8_t> d_sp_taken;
   // the donor sets of grove_run_cycle_reclaim_queues (donor.cuh): per scanned queue its pairs in victim order, the quotas, the
   // running gangs' usage, queues and chains, the per-class loads and the per-(running gang, depth) verdicts
   DevBuf<uint32_t> d_dn_off, d_dn_qid, d_dn_parent, d_dn_rq;
@@ -1254,7 +1259,7 @@ static int32_t cycle_begin(grove_engine* e) {
     CU_TRY(e, cudaGetLastError());
   }
   e->launches = 0; e->in_cycle = true; e->have_results = false; e->have_scopes = false; e->diag = grove_engine::kDiagNoCycle;
-  e->victims.clear(); e->moves.clear(); e->score_pass_valid = false;
+  e->victims.clear(); e->surplus_victims.clear(); e->moves.clear(); e->score_pass_valid = false;
   std::memset(&e->last, 0, sizeof(e->last));
   return GROVE_OK;
 }
@@ -2474,6 +2479,45 @@ static int32_t upload_running(grove_engine* e, const grove_running_gang_t* runni
   return GROVE_OK;
 }
 
+// The surplus pods of grove_run_cycle_preempt_elastic (include/grove_place.h "elastic reclaim"): the caller's records, checked by
+// the entry.  On the host, off / pod list them as the device CSR does -- rows by sorted node, the caller's order within a row --
+// with pod[i] the caller's index of entry i; run_off / run_ent list each running gang's entries.
+namespace {
+struct SurplusIn { const grove_surplus_pod_t* pod; uint32_t n; };
+struct SurplusByNode { std::vector<uint32_t> off, pod, run_off, run_ent; };
+}  // namespace
+
+static int32_t upload_surplus(grove_engine* e, const SurplusIn& in, uint32_t n_running, SurplusByNode* at, SurplusCsr* csr) {
+  const uint32_t N = e->N;
+  at->off.assign(size_t(N) + 1, 0); at->pod.resize(in.n);
+  for (uint32_t i = 0; i < in.n; ++i) ++at->off[e->inv[in.pod[i].node] + 1];
+  for (uint32_t n = 0; n < N; ++n) at->off[n + 1] += at->off[n];
+  std::vector<uint4> ent(std::max<uint32_t>(in.n, 1));
+  {
+    std::vector<uint32_t> cur(at->off.begin(), at->off.end() - 1);
+    for (uint32_t i = 0; i < in.n; ++i) {
+      const grove_surplus_pod_t& p = in.pod[i];
+      const uint32_t k = cur[e->inv[p.node]]++;
+      at->pod[k] = i;
+      ent[k] = make_uint4(p.running, p.cpu_milli, p.mem_mib, uint32_t(p.gpu) | (1u << 16));
+    }
+  }
+  at->run_off.assign(size_t(n_running) + 1, 0); at->run_ent.resize(in.n);
+  for (uint32_t k = 0; k < in.n; ++k) ++at->run_off[in.pod[at->pod[k]].running + 1];
+  for (uint32_t r = 0; r < n_running; ++r) at->run_off[r + 1] += at->run_off[r];
+  {
+    std::vector<uint32_t> cur(at->run_off.begin(), at->run_off.end() - 1);
+    for (uint32_t k = 0; k < in.n; ++k) at->run_ent[cur[in.pod[at->pod[k]].running]++] = k;
+  }
+  CU_TRY(e, e->d_sp_off.ensure(at->off.size())); CU_TRY(e, e->d_sp_ent.ensure(ent.size()));
+  CU_TRY(e, e->d_sp_taken.ensure(ent.size()));
+  CU_TRY(e, cudaMemcpyAsync(e->d_sp_off.p, at->off.data(), sizeof(uint32_t) * at->off.size(), cudaMemcpyHostToDevice, e->stream));
+  CU_TRY(e, cudaMemcpyAsync(e->d_sp_ent.p, ent.data(), sizeof(uint4) * ent.size(), cudaMemcpyHostToDevice, e->stream));
+  CU_TRY(e, cudaStreamSynchronize(e->stream));   // (pageable sources)
+  *csr = SurplusCsr{e->d_sp_off.p, e->d_sp_ent.p, e->d_sp_taken.p};
+  return GROVE_OK;
+}
+
 // The donor sets of grove_run_cycle_reclaim_queues on the device (donor.cuh): the (scanned queue, running gang) pairs in victim
 // order with the depth of the queue in the running gang's chain, and what k_donor_scan / k_donor_mark read besides, uploaded
 // once per call.  -> the number of scanned queues (those with a finite quota on some resource); 0: every E(Q) is empty.
@@ -2549,15 +2593,22 @@ static Share share_of(const grove_queue_quota_t& q, const std::array<int64_t, 3>
 // replaces (null: no gang replaces a running gang) as for grove_run_cycle_reuse; running_queue (null: no queue set) the queue of each
 // running gang in the queue set of the current submission; quotas (null: no queue classes) one row per queue of that set, and then
 // the queue classes run first (grove_run_cycle_reclaim_queues); priority: the priority classes run (after the queue classes, from
-// the state they leave: grove_run_cycle_reclaim_preempt_queues).  Inputs checked by the entry.
+// the state they leave: grove_run_cycle_reclaim_preempt_queues); surplus (null: none) the surplus pods of
+// grove_run_cycle_preempt_elastic, and then every priority class runs the surplus pass before the whole pass.  Inputs checked by
+// the entry.
 static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const grove_running_gang_t* running, uint32_t n_running,
                              const grove_holding_t* holdings, const uint32_t* running_queue, const grove_queue_quota_t* quotas,
-                             bool priority, grove_cycle_stats_t* stats) {
+                             bool priority, const SurplusIn* surplus, grove_cycle_stats_t* stats) {
   CU_TRY(e, cudaSetDevice(e->cfg.device));
   const uint32_t G = e->G, N = e->N, nblk = (N + 255) / 256;
   ReclaimCsr csr{};
   int32_t rc = upload_running(e, running, n_running, holdings, &csr);
   if (rc) return rc;
+  SurplusByNode spn;
+  SurplusCsr scsr{};
+  if (surplus) { rc = upload_surplus(e, *surplus, n_running, &spn, &scsr); if (rc) return rc; }
+  std::vector<uint8_t> taken(surplus ? std::max<uint32_t>(surplus->n, 1) : 0, 0);   // by entry of spn
+  std::vector<grove_surplus_victim_t> surplus_victims;
   CU_TRY(e, e->d_rc_evict.ensure(std::max<uint32_t>(n_running, 1)));
   // without replacements nothing holds; without a queue set no gang and no running gang is in a queue, and the queue step never runs
   std::vector<uint32_t> rep(G, GROVE_NONE_U32), run_queue(n_running, GROVE_NONE_U32);
@@ -2619,12 +2670,41 @@ static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const gr
   std::vector<std::vector<grove_placement_t>> extra(G);   // placements of the preemptors and reclaimers, by gang
   RunningByNode at;
   std::vector<int32_t> slot;   // node (caller order) -> its row in `rows` while a class chooses its victims
+  auto sp_res = [&](uint32_t i) {   // what surplus entry i takes
+    const grove_surplus_pod_t& x = surplus->pod[spn.pod[i]];
+    return Res{x.cpu_milli, x.mem_mib, x.gpu, 1};
+  };
+  auto sp_can = [&](uint32_t i) {   // may the current class take surplus entry i?
+    const uint32_t r = surplus->pod[spn.pod[i]].running;
+    return !taken[i] && evict[r] && !gone[r];
+  };
+  auto surplus_standing = [&]() {   // does an untaken surplus pod of a running gang the class may evict still stand?
+    for (uint32_t i = 0; i < spn.pod.size(); ++i) if (sp_can(i)) return true;
+    return false;
+  };
+  // the device view of a class over the running gangs `evict` marks (reclaim.cuh): add it to the free table, keeping that aside
+  // (add), or take it off again; the surplus pass's view is their untaken surplus pods, every other pass's what they still hold
+  enum class Pass { kPlain, kSurplus, kWhole };
+  auto view = [&](Pass pass, uint32_t add) -> cudaError_t {
+    cudaError_t c = cudaMemcpyAsync(e->d_rc_evict.p, evict.data(), n_running, cudaMemcpyHostToDevice, e->stream);
+    if (c != cudaSuccess) return c;
+    if (pass == Pass::kPlain) {
+      k_reclaim_view<<<nblk, 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_real.p, csr.off, csr.ent, e->d_rc_evict.p, N, add);
+    } else {
+      c = cudaMemcpyAsync(e->d_sp_taken.p, taken.data(), taken.size(), cudaMemcpyHostToDevice, e->stream);
+      if (c != cudaSuccess) return c;
+      k_elastic_view<<<nblk, 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_real.p, csr.off, csr.ent, scsr, e->d_rc_evict.p, N, add,
+                                                  pass == Pass::kWhole);
+    }
+    return cudaGetLastError();
+  };
 
   // One class: its members (gangs still rejected, in rank order) against the running gangs `evict` marks, under the queue caps
   // `caps`.  Its admitted members carry `flag`; give_back: a member admitted by the class cycle once none of them stands any more
-  // gives its room back (the priority classes' rule).
+  // gives its room back (the priority classes' rule).  pass: kPlain without surplus pods; with them, kSurplus against the untaken
+  // surplus pods alone (what stands is then an untaken surplus pod), kWhole against what the running gangs still hold.
   auto run_class = [&](const std::vector<uint32_t>& members, const std::vector<std::array<uint64_t, 3>>& caps, uint16_t flag,
-                       bool give_back) -> int32_t {
+                       bool give_back, Pass pass) -> int32_t {
     // 2. the class's members as a submission of their own.  A member holds its predecessor's holdings when that one still stands
     // and is not evictable; when it is, it is released instead.
     Sub sub;
@@ -2637,9 +2717,7 @@ static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const gr
     }
     // the class view, on the device: free + the standing holdings the class may evict; the free table itself is kept for the
     // victim choice
-    CU_TRY(e, cudaMemcpyAsync(e->d_rc_evict.p, evict.data(), n_running, cudaMemcpyHostToDevice, e->stream));
-    k_reclaim_view<<<nblk, 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_real.p, csr.off, csr.ent, e->d_rc_evict.p, N, 1u);
-    CU_TRY(e, cudaGetLastError());
+    CU_TRY(e, view(pass, 1u));
     int32_t rc = submit_sub(e, sub); if (rc) return rc;
     if (running_queue) {   // the class's queue set: own used without what the evictable gangs hold, so that its loads are load';
                            // the caps in place of the limits
@@ -2673,6 +2751,19 @@ static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const gr
         const grove_holding_t& x = holdings[running[v].holding_off + h];
         if (slot[x.node] >= 0) rows[slot[x.node]].add(held(x));
       }
+      if (surplus)   // less its surplus pods taken earlier
+        for (uint32_t k = spn.run_off[v]; k < spn.run_off[v + 1]; ++k) {
+          const uint32_t i = spn.run_ent[k], n = surplus->pod[spn.pod[i]].node;
+          if (taken[i] && slot[n] >= 0) rows[slot[n]].add(sp_res(i), -1);
+        }
+    };
+    auto left_on = [&](uint32_t x, uint32_t n) {   // does running gang x hold something on node n once its taken pods are off?
+      Res l;
+      for (uint32_t h = 0; h < running[x].n_holdings; ++h)
+        if (holdings[running[x].holding_off + h].node == n) l.add(held(holdings[running[x].holding_off + h]));
+      for (uint32_t k = spn.run_off[x]; k < spn.run_off[x + 1]; ++k)
+        if (taken[spn.run_ent[k]] && surplus->pod[spn.pod[spn.run_ent[k]]].node == n) l.add(sp_res(spn.run_ent[k]), -1);
+      return l.cpu || l.mem || l.gpu || l.pods;
     };
     auto evict_one = [&](uint32_t v, uint32_t g) {   // released, and its usage leaves its queues
       release(v);
@@ -2686,7 +2777,9 @@ static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const gr
       if (sp.state != GROVE_GANG_ADMITTED) continue;
       std::vector<uint32_t> nodes; std::vector<Res> use; std::vector<grove_placement_t> pl;
       placed(e, snap, sub, k, nodes, use, pl);
-      if (give_back && !standing()) {   // admitted by the class cycle after E(p) ran out: it stays as the ordinary pass left it.
+      if (give_back && !(pass == Pass::kSurplus ? surplus_standing() : standing())) {
+                                        // admitted by the class cycle after E(p) (in the surplus pass: its untaken surplus pods)
+                                        // ran out: it stays as the ordinary pass left it.
                                         // What the class cycle committed for it goes back: +U, and -H for a member with a hold (a
                                         // queue charge was never taken here)
         for (size_t j = 0; j < nodes.size(); ++j) back.push_back({e->inv[nodes[j]], use[j]});
@@ -2714,7 +2807,29 @@ static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const gr
                        std::max<int64_t>(use[j].gpu - mine[j].gpu, 0), std::max<int64_t>(use[j].pods - mine[j].pods, 0)};
         Res& have = rows[slot[n]];
         while (!have.covers(need)) {
-          const uint32_t v = choose_victim(at, n, running, [&](uint32_t x) { return evict[x] && !gone[x]; });
+          if (surplus) {   // surplus pods first, when those on the node are enough
+            const uint32_t row = e->inv[n];
+            Res more = have;
+            for (uint32_t i = spn.off[row]; i < spn.off[row + 1]; ++i) if (sp_can(i)) more.add(sp_res(i));
+            if (more.covers(need)) {
+              while (!have.covers(need)) {
+                uint32_t v = GROVE_NONE_U32;   // the gang by the victim rule, then its first-listed untaken pod here
+                for (uint32_t i = spn.off[row]; i < spn.off[row + 1]; ++i) {
+                  const uint32_t x = surplus->pod[spn.pod[i]].running;
+                  if (sp_can(i) && evicted_before(running, x, v)) v = x;
+                }
+                uint32_t i = spn.off[row];
+                while (!(sp_can(i) && surplus->pod[spn.pod[i]].running == v)) ++i;
+                taken[i] = 1;
+                have.add(sp_res(i));
+                surplus_victims.push_back(grove_surplus_victim_t{spn.pod[i], g});
+              }
+              break;
+            }
+            if (pass == Pass::kSurplus) return fail(e, GROVE_ERR_STATE, "elastic reclaim: a surplus preemptor's node cannot be freed by surplus pods");
+          }
+          const uint32_t v = choose_victim(at, n, running,
+                                           [&](uint32_t x) { return evict[x] && !gone[x] && (!surplus || left_on(x, n)); });
           if (v == GROVE_NONE_U32) return fail(e, GROVE_ERR_STATE, "reclaim pass: a preemptor's node cannot be freed");
           evict_one(v, g);
         }
@@ -2753,11 +2868,10 @@ static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const gr
     }
     for (uint32_t n : used) slot[n] = -1;
     rc = patch_nodes(e, back, st0); if (rc) return rc;
-    // back to the free table: take off what the evictable running gangs that still stand hold
+    // back to the free table: take off what the evictable running gangs that still stand hold (in the surplus pass: their surplus
+    // pods still untaken)
     for (uint32_t r = 0; r < n_running; ++r) evict[r] = evict[r] && !gone[r];
-    CU_TRY(e, cudaMemcpyAsync(e->d_rc_evict.p, evict.data(), n_running, cudaMemcpyHostToDevice, e->stream));
-    k_reclaim_view<<<nblk, 256, 0, e->stream>>>(e->d_nres.p, e->d_rc_real.p, csr.off, csr.ent, e->d_rc_evict.p, N, 0u);
-    CU_TRY(e, cudaGetLastError());
+    CU_TRY(e, view(pass, 0u));
     return GROVE_OK;
   };
   auto arm = [&]() -> cudaError_t {   // before the first class: the free table after the ordinary pass is kept aside
@@ -2809,7 +2923,7 @@ static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const gr
         for (uint32_t g = 0; g < G; ++g)
           if (snap.status[g].state == GROVE_GANG_REJECTED && gang_queue[g] == Q) members.push_back(g);
         std::stable_sort(members.begin(), members.end(), [&](uint32_t a, uint32_t b) { return snap.gangs[a].priority > snap.gangs[b].priority; });
-        rc = run_class(members, cap, GROVE_STATUS_RECLAIMER, false); if (rc) return rc;
+        rc = run_class(members, cap, GROVE_STATUS_RECLAIMER, false, Pass::kPlain); if (rc) return rc;
       }
     }
   }
@@ -2830,7 +2944,13 @@ static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const gr
         std::vector<uint32_t> members;   // (one priority: submission order is rank order)
         for (uint32_t g = 0; g < G; ++g)
           if (snap.status[g].state == GROVE_GANG_REJECTED && snap.gangs[g].priority == p) members.push_back(g);
-        rc = run_class(members, limit, GROVE_STATUS_PREEMPTOR, true); if (rc) return rc;
+        if (surplus && surplus_standing()) {   // the surplus pass; the whole pass takes the members it did not admit
+          rc = run_class(members, limit, GROVE_STATUS_PREEMPTOR | GROVE_STATUS_SURPLUS_ONLY, true, Pass::kSurplus); if (rc) return rc;
+          members.erase(std::remove_if(members.begin(), members.end(), [&](uint32_t g) { return snap.status[g].state != GROVE_GANG_REJECTED; }),
+                        members.end());
+          if (members.empty()) continue;
+        }
+        rc = run_class(members, limit, GROVE_STATUS_PREEMPTOR, true, surplus ? Pass::kWhole : Pass::kPlain); if (rc) return rc;
       }
     }
   }
@@ -2839,7 +2959,9 @@ static int32_t reclaim_cycle(grove_engine* e, const uint32_t* replaces, const gr
     rc = restore.put_back(); if (rc) return rc;
   }
   st0.kernel_launches += 1;   // k_reclaim_check
-  return publish_reclaim(e, snap.status, snap.place, extra, snap.sstat, st0, std::move(victims), stats);
+  rc = publish_reclaim(e, snap.status, snap.place, extra, snap.sstat, st0, std::move(victims), stats);
+  e->surplus_victims = std::move(surplus_victims);
+  return rc;
 }
 
 int32_t grove_run_cycle_preempt(grove_engine_t* e, const grove_running_gang_t* running, uint32_t n_running,
@@ -2852,7 +2974,62 @@ int32_t grove_run_cycle_preempt(grove_engine_t* e, const grove_running_gang_t* r
   if (rc) return rc;
   rc = check_running(e, running, n_running, holdings, n_holdings);
   if (rc) return rc;
-  return reclaim_cycle(e, nullptr, running, n_running, holdings, nullptr, nullptr, true, stats);
+  return reclaim_cycle(e, nullptr, running, n_running, holdings, nullptr, nullptr, true, nullptr, stats);
+}
+
+int32_t grove_run_cycle_preempt_elastic(grove_engine_t* e, const grove_running_gang_t* running, uint32_t n_running,
+                                        const grove_holding_t* holdings, uint32_t n_holdings,
+                                        const grove_surplus_pod_t* surplus, uint32_t n_surplus, grove_cycle_stats_t* stats) {
+  if (!e || (n_running && !running) || (n_holdings && !holdings) || (n_surplus && !surplus)) return GROVE_ERR_INVALID_ARG;
+  if (int32_t rc = refuse_sets(e, "grove_run_cycle_preempt_elastic", kSetFairShare)) return rc;   // (a fair-share set over a queue set without members)
+  NoDiagnosis no_diag{e};
+  if (e->wide) return refuse_wide(e, "grove_run_cycle_preempt_elastic");
+  int32_t rc = check_ready(e);
+  if (rc) return rc;
+  rc = check_running(e, running, n_running, holdings, n_holdings);
+  if (rc) return rc;
+  // every surplus pod on a node of the snapshot, of a running gang, and inside what that gang holds there
+  std::vector<std::array<int64_t, 4>> sum;   // per (running gang, node) with a surplus pod: pods, then holdings, subtracted
+  std::vector<std::pair<uint64_t, uint32_t>> key;   // ((running gang, node), its row in sum), sorted
+  for (uint32_t i = 0; i < n_surplus; ++i) {
+    if (surplus[i].running >= n_running) return fail(e, GROVE_ERR_INVALID_ARG, "surplus pod of a running gang out of range");
+    if (surplus[i].node >= e->N) return fail(e, GROVE_ERR_INVALID_ARG, "surplus pod on a node out of range");
+    key.push_back({(uint64_t(surplus[i].running) << 32) | surplus[i].node, i});
+  }
+  std::sort(key.begin(), key.end());
+  std::vector<uint32_t> row_of(n_surplus);
+  for (size_t k = 0; k < key.size(); ++k) {
+    if (k == 0 || key[k].first != key[k - 1].first) sum.push_back({0, 0, 0, 0});
+    const grove_surplus_pod_t& p = surplus[key[k].second];
+    std::array<int64_t, 4>& s = sum.back();
+    s[0] += p.cpu_milli; s[1] += p.mem_mib; s[2] += p.gpu; s[3] += 1;
+    row_of[key[k].second] = uint32_t(sum.size() - 1);
+  }
+  for (uint32_t r = 0; r < n_running && !key.empty(); ++r)
+    for (uint32_t h = 0; h < running[r].n_holdings; ++h) {
+      const grove_holding_t& x = holdings[running[r].holding_off + h];
+      const uint64_t k = (uint64_t(r) << 32) | x.node;
+      const auto it = std::lower_bound(key.begin(), key.end(), std::make_pair(k, 0u));
+      if (it == key.end() || it->first != k) continue;
+      std::array<int64_t, 4>& s = sum[row_of[it->second]];
+      s[0] -= x.cpu_milli; s[1] -= x.mem_mib; s[2] -= x.gpu; s[3] -= x.pods;
+    }
+  for (const auto& s : sum)
+    if (s[0] > 0 || s[1] > 0 || s[2] > 0 || s[3] > 0)
+      return fail(e, GROVE_ERR_INVALID_ARG, "surplus pods exceed what their running gang holds on a node");
+  if (!n_surplus) return reclaim_cycle(e, nullptr, running, n_running, holdings, nullptr, nullptr, true, nullptr, stats);
+  const SurplusIn in{surplus, n_surplus};
+  return reclaim_cycle(e, nullptr, running, n_running, holdings, nullptr, nullptr, true, &in, stats);
+}
+
+int32_t grove_get_surplus_victims(grove_engine_t* e, grove_surplus_victim_t* out, uint32_t cap, uint32_t* n_out) {
+  if (!e || !n_out) return GROVE_ERR_INVALID_ARG;
+  if (!e->have_results) return fail(e, GROVE_ERR_STATE, "no completed cycle");
+  *n_out = uint32_t(e->surplus_victims.size());
+  if (!out) return GROVE_OK;
+  if (cap < e->surplus_victims.size()) return fail(e, GROVE_ERR_LIMIT, "output buffer too small");
+  std::memcpy(out, e->surplus_victims.data(), sizeof(grove_surplus_victim_t) * e->surplus_victims.size());
+  return GROVE_OK;
 }
 
 int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replaces, uint32_t n_gangs, const grove_running_gang_t* running,
@@ -2863,7 +3040,7 @@ int32_t grove_run_cycle_reuse_preempt(grove_engine_t* e, const uint32_t* replace
   if (e->wide) return refuse_wide(e, "grove_run_cycle_reuse_preempt");
   const int32_t rc = check_reuse_inputs(e, replaces, n_gangs, running, n_running, holdings, n_holdings);
   if (rc) return rc;
-  return reclaim_cycle(e, replaces, running, n_running, holdings, nullptr, nullptr, true, stats);
+  return reclaim_cycle(e, replaces, running, n_running, holdings, nullptr, nullptr, true, nullptr, stats);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -2999,7 +3176,7 @@ int32_t grove_run_cycle_preempt_queues(grove_engine_t* e, const grove_running_ga
   NoDiagnosis no_diag{e};
   rc = check_queue_running(e, "grove_run_cycle_preempt_queues", running, n_running, holdings, n_holdings, running_queue);
   if (rc) return rc;
-  return reclaim_cycle(e, nullptr, running, n_running, holdings, running_queue, nullptr, true, stats);
+  return reclaim_cycle(e, nullptr, running, n_running, holdings, running_queue, nullptr, true, nullptr, stats);
 }
 
 // grove_run_cycle_reclaim_queues, and with priority grove_run_cycle_reclaim_preempt_queues: the same inputs, the same refusals
@@ -3020,7 +3197,7 @@ static int32_t reclaim_queues_entry(grove_engine* e, const char* entry, const gr
     rc = over_quota_shares(e, quotas, fair); if (rc) return rc;
     quotas = fair.data();
   }
-  return reclaim_cycle(e, nullptr, running, n_running, holdings, running_queue, quotas, priority, stats);
+  return reclaim_cycle(e, nullptr, running, n_running, holdings, running_queue, quotas, priority, nullptr, stats);
 }
 
 int32_t grove_run_cycle_reclaim_queues(grove_engine_t* e, const grove_queue_quota_t* quotas, uint32_t n_queues,

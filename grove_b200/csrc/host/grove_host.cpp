@@ -772,6 +772,9 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
   bool thenPreempt = false;                            // SetReclaimThenPreempt with queue members: grove_run_cycle_reclaim_preempt_queues
   bool fairShare = false;                              // SetFairShareOrder with queue members: the queue cycle in fair-share order
   bool overQuota = false;                              // SetOverQuotaWeights: the cycles with quotas run with each queue's weights
+  bool elastic = false;                                // SetElasticPreemption: one grove_run_cycle_preempt_elastic
+  std::vector<grove_surplus_pod_t> surplus;            // ... its surplus pods, and (running PodGang, its pod) of each
+  std::vector<std::pair<std::string, BoundPod>> surplusOf;
   std::vector<uint32_t> replaces;   // reservation reuse: per gang row, the running gang it is the new version of
   {
     std::lock_guard<std::mutex> l(mu_);
@@ -787,6 +790,7 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
     reuse = (reuse_ || reclaimReuse_) && !running_.empty();
     fairShare = fairShare_ && !t.queues.empty() && !both && !preempt && !reuse && !consolidate;
     overQuota = overQuota_;
+    elastic = elastic_ && preempt && !both && !reuse_ && !preemptQueues_ && !reclaimQueues_ && !reclaimThenPreempt_ && !consMax_;
     if (preempt || reuse) {
       std::map<std::string, uint32_t> nodeIdx;
       for (uint32_t i = 0; i < nodes.size(); ++i) nodeIdx[nodes[i].Name] = i;
@@ -797,6 +801,16 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
           auto it = nodeIdx.find(h.node);
           if (it == nodeIdx.end()) continue;
           held.push_back(grove_holding_t{it->second, h.cpu_milli, h.mem_mib, h.gpu, h.pods}); ++r.n_holdings;
+        }
+        if (elastic) {   // its bound pods beyond MinReplicas, PodGroup by PodGroup, the highest PodReference index first
+          std::vector<BoundPod> extra;
+          for (const BoundPod& p : kv.second.pods)
+            if (p.group < kv.second.minReplicas.size() && int64_t(p.index) >= kv.second.minReplicas[p.group] && nodeIdx.count(p.node)) extra.push_back(p);
+          std::sort(extra.begin(), extra.end(), [](const BoundPod& a, const BoundPod& b) { return a.group != b.group ? a.group < b.group : a.index > b.index; });
+          for (const BoundPod& p : extra) {
+            surplus.push_back(grove_surplus_pod_t{uint32_t(run.size()), nodeIdx.at(p.node), p.cpu_milli, p.mem_mib, p.gpu, 0});
+            surplusOf.push_back({kv.first, p});
+          }
         }
         run.push_back(r); runNames.push_back(kv.first);
       }
@@ -911,6 +925,10 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
                                                       uint32_t(held.size()), runQueue.data(), &st), "grove_run_cycle_reclaim_queues")) return e;
     } else if (auto e = chk(grove_run_cycle_preempt_queues(engine_, run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), runQueue.data(), &st),
                             "grove_run_cycle_preempt_queues")) return e;
+  }
+  else if (preempt && elastic) {
+    if (auto e = chk(grove_run_cycle_preempt_elastic(engine_, run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), surplus.data(),
+                                                     uint32_t(surplus.size()), &st), "grove_run_cycle_preempt_elastic")) return e;
   }
   else if (preempt) { if (auto e = chk(grove_run_cycle_preempt(engine_, run.data(), uint32_t(run.size()), held.data(), uint32_t(held.size()), &st), "grove_run_cycle_preempt")) return e; }
   else if (consolidate) {
@@ -1033,6 +1051,27 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
     if (gs[g].state == GROVE_GANG_REJECTED) ++rejectedFor_[t.gangNames[g]];
     else if (gs[g].state == GROVE_GANG_ADMITTED) rejectedFor_.erase(t.gangNames[g]);
   }
+  if (elastic) {   // surplus pods taken: the PodGang keeps running, the caller terminates the pods, their holdings are forgotten
+    uint32_t ns = 0;
+    if (auto e = chk(grove_get_surplus_victims(engine_, nullptr, 0, &ns), "grove_get_surplus_victims")) return e;
+    std::vector<grove_surplus_victim_t> sv(ns + 1);
+    if (auto e = chk(grove_get_surplus_victims(engine_, sv.data(), uint32_t(sv.size()), &ns), "grove_get_surplus_victims")) return e;
+    for (uint32_t i = 0; i < ns; ++i) {
+      const auto& [key, p] = surplusOf[sv[i].pod];
+      PodGangStatus& s = (*statuses)[key];
+      s.Phase = PodGangPhase::Running; s.Scheduled = true;
+      s.EvictedPods.push_back(p.ref);
+      auto r = running_.find(key);
+      if (r == running_.end()) continue;   // deleted while the cycle ran
+      RunningGang& rg = r->second;
+      auto b = std::find_if(rg.pods.begin(), rg.pods.end(), [&](const BoundPod& x) { return x.group == p.group && x.index == p.index; });
+      if (b != rg.pods.end()) rg.pods.erase(b);
+      auto h = std::find_if(rg.held.begin(), rg.held.end(), [&](const Held& x) { return x.node == p.node; });
+      if (h == rg.held.end()) continue;
+      h->cpu_milli -= p.cpu_milli; h->mem_mib -= p.mem_mib; h->gpu = uint16_t(h->gpu - p.gpu); h->pods = uint16_t(h->pods - 1);
+      if (!h->pods) rg.held.erase(h);
+    }
+  }
   if (preempt) {   // victims: DisruptionTarget on the PodGang (podgang.go:166-170), forgotten as running
     uint32_t nv = 0;
     if (auto e = chk(grove_get_victims(engine_, nullptr, 0, &nv), "grove_get_victims")) return e;
@@ -1072,10 +1111,15 @@ Err GpuBackend::RunCycle(const std::vector<Node>& nodes, std::vector<Binding>* b
     {   // what the PodGang holds from now on (a remainder adds to what its minimum took)
       RunningGang& rg = running_[key];
       rg.priority = t.gangs[i].priority;
+      rg.minReplicas.clear();
+      for (const PodGroup& grp : pg.Spec.PodGroups) rg.minReplicas.push_back(grp.MinReplicas);
+      std::map<uint32_t, uint32_t> nth;   // clique row -> its placements so far: the r-th binds PodReference refBase + r
       for (uint32_t k = 0; k < gs[i].n_pods; ++k) {
         const grove_placement_t& e = pl[gs[i].placement_off + k];
         const grove_clique_t& q = t.cliques[e.clique];
         const std::string& nn = nodes[e.node].Name;
+        const uint32_t group = t.cliqueOf[e.clique].second, index = t.refBase[e.clique] + nth[e.clique]++;
+        rg.pods.push_back(BoundPod{pg.Spec.PodGroups[group].PodReferences[index], group, index, nn, q.req_cpu_milli, q.req_mem_mib, q.req_gpu});
         auto it = std::find_if(rg.held.begin(), rg.held.end(), [&](const Held& h) { return h.node == nn; });
         if (it == rg.held.end()) { rg.held.push_back(Held{nn}); it = rg.held.end() - 1; }
         it->cpu_milli += q.req_cpu_milli; it->mem_mib += q.req_mem_mib; it->gpu = uint16_t(it->gpu + q.req_gpu); it->pods = uint16_t(it->pods + 1);

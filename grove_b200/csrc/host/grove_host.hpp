@@ -70,6 +70,8 @@ struct PodGangStatus {                                                          
   uint32_t UnboundPods = 0;               // best-effort pods (beyond MinReplicas) of a scheduled PodGang that found no node
   bool DisruptionTarget = false;          // condition PodGangConditionTypeDisruptionTarget :166-170, reason 1: "PodGang is preempted
   std::string DisruptionMessage;          // by a higher priority PodGang" -- names the preemptor; the caller terminates the pods
+  std::vector<NamespacedName> EvictedPods;  // elastic preemption: pods above their PodGroup's MinReplicas that a higher priority
+                                            // PodGang took; the caller terminates them, the PodGang keeps running
 };
 struct PodGang {
   std::string Namespace, Name;
@@ -287,6 +289,12 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   // rejects may evict running PodGangs of a lower priority.  Victims come back in `statuses` with DisruptionTarget set and
   // are forgotten here: the caller deletes their pods (the node snapshot of the next cycle shows the resources as free).
   void SetPreemption(bool on) { std::lock_guard<std::mutex> l(mu_); preemption_ = on; }
+  // Elastic preemption (PodGroup.MinReplicas, podgang.go:80-83; DESIGN.md section 1 "Elastic reclaim"): with it and SetPreemption
+  // on, and no reservation reuse, queue or consolidation switch, a cycle with running PodGangs is grove_run_cycle_preempt_elastic:
+  // the bound pods of each running PodGroup beyond MinReplicas (highest PodReference index first) are surplus, and a preemptor
+  // takes those before it evicts any PodGang whole.  A PodGang that lost pods keeps running, is not a DisruptionTarget, and comes
+  // back in `statuses` with EvictedPods naming them; their holdings are forgotten here.  Off by default.
+  void SetElasticPreemption(bool on) { std::lock_guard<std::mutex> l(mu_); elastic_ = on; }
   // Reservation reuse (ReuseReservationRef, podgang.go:65-71): with it on, a PodGang whose ReuseReservationRef names a running
   // PodGang is that gang's new version and the cycle is grove_run_cycle_reuse -- it may use what its predecessor holds, nobody
   // else may.  Once it is admitted the predecessor is forgotten as running (the caller deletes its pods; a later OnPodGangDelete
@@ -429,10 +437,17 @@ class GpuBackend : public Backend, public TopologyAwareSchedBackend {
   std::map<std::string, std::string> lastNode_;  // scheduled PodGang -> a node it landed on (ReuseReservationRef hint)
   std::map<std::string, std::vector<uint32_t>> bound_;  // scheduled PodGang still pending with unbound pods -> pods bound per PodGroup
   struct Held { std::string node; uint32_t cpu_milli = 0, mem_mib = 0; uint16_t gpu = 0, pods = 0; };
-  struct RunningGang { int32_t priority = 0; std::vector<Held> held; std::map<std::string, std::string> cdOn; };   // cdOn: node -> the
-                                                                                                                  // ComputeDomain of its enrolled pods there
+  // a pod this backend bound for a running PodGang: its PodGroup, PodReference index and what it takes on its node
+  struct BoundPod { NamespacedName ref; uint32_t group = 0, index = 0; std::string node; uint32_t cpu_milli = 0, mem_mib = 0; uint16_t gpu = 0; };
+  // cdOn: node -> the ComputeDomain of its enrolled pods there; pods, minReplicas: its bound pods and every PodGroup's MinReplicas
+  // (elastic preemption)
+  struct RunningGang {
+    int32_t priority = 0; std::vector<Held> held; std::map<std::string, std::string> cdOn;
+    std::vector<BoundPod> pods; std::vector<int32_t> minReplicas;
+  };
   std::map<std::string, RunningGang> running_;   // PodGangs scheduled by this backend and not deleted since
   bool preemption_ = false;
+  bool elastic_ = false;
   bool reuse_ = false;
   bool reclaimReuse_ = false;
   bool preemptQueues_ = false;

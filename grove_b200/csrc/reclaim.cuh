@@ -48,6 +48,44 @@ __global__ void __launch_bounds__(256) k_reclaim_view(uint4* nres, uint4* real, 
   nres[n] = r;
 }
 
+// The surplus pods of grove_run_cycle_preempt_elastic, uploaded once per call as a per-node CSR over the sorted node order: row n
+// lists the pods on n in the caller's order, each as x = running gang, y = cpu, z = mem, w = gpu | 1 << 16 (its pod slot); taken[i]
+// marks entry i as taken.  Every pod lies inside its gang's holdings on its node (the entry checks it), so no sum below can
+// borrow or carry from one packed field into the next.
+struct SurplusCsr {
+  const uint32_t* off;   // [N + 1]
+  const uint4* ent;
+  const uint8_t* taken;
+};
+
+// The views of the elastic reclaim loop, as k_reclaim_view's, for the running gangs the evict mask marks.  whole == 0: the
+// surplus view, their untaken surplus pods; whole == 1: the whole view, their holdings minus their taken surplus pods.  add > 0:
+// real = the table as it is (the pass's free table), then table += the view; add == 0: table -= the same sum.
+__global__ void __launch_bounds__(256) k_elastic_view(uint4* nres, uint4* real, const uint32_t* off, const uint4* ent, SurplusCsr s,
+                                                      const uint8_t* evict, uint32_t N, uint32_t add, uint32_t whole) {
+  const uint32_t n = blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= N) return;
+  uint32_t h0 = 0, h1 = 0, h2 = 0;   // whole: the holdings of the marked gangs
+  if (whole)
+    for (uint32_t i = off[n]; i < off[n + 1]; ++i) {
+      const uint4 h = ent[i];
+      if (evict[h.x]) { h0 += h.y; h1 += h.z; h2 += h.w; }
+    }
+  uint32_t p0 = 0, p1 = 0, p2 = 0;   // their surplus pods: the untaken ones (surplus view) or the taken ones (whole view)
+  for (uint32_t i = s.off[n]; i < s.off[n + 1]; ++i) {
+    const uint4 p = s.ent[i];
+    if (evict[p.x] && (s.taken[i] != 0) == (whole != 0)) { p0 += p.y; p1 += p.z; p2 += p.w; }
+  }
+  uint32_t s0 = p0, s1 = p1, s2 = p2;
+  if (whole) { s0 = h0 - p0; s1 = h1 - p1; s2 = h2 - p2; }
+  uint4 r = nres[n];
+  if (add) real[n] = r;
+  if (!(s0 | s1 | s2)) return;
+  if (add) { r.x += s0; r.y += s1; r.z += s2; }
+  else { r.x -= s0; r.y -= s1; r.z -= s2; }
+  nres[n] = r;
+}
+
 // rows idx[i] (sorted node) of a table -> out[i]
 __global__ void __launch_bounds__(256) k_reclaim_rows(const uint4* tab, const uint32_t* idx, uint4* out, uint32_t m) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;

@@ -24,7 +24,8 @@ SYMBOLS = [
     "grove_abi_version", "grove_engine_create", "grove_engine_destroy", "grove_last_error",
     "grove_load_nodes", "grove_update_nodes", "grove_get_nodes", "grove_submit_gangs", "grove_submit_gangs_wide", "grove_run_cycle",
     "grove_get_placements", "grove_get_gang_status", "grove_get_scope_domains", "grove_load_nodes_device",
-    "grove_build_score_matrix", "grove_run_cycle_preempt", "grove_get_victims", "grove_run_cycle_reuse",
+    "grove_build_score_matrix", "grove_run_cycle_preempt", "grove_get_victims",
+    "grove_run_cycle_preempt_elastic", "grove_get_surplus_victims", "grove_run_cycle_reuse",
     "grove_run_cycle_reuse_preempt", "grove_diagnose", "grove_set_spread", "grove_set_fences", "grove_set_queues",
     "grove_run_cycle_consolidate", "grove_get_moves", "grove_run_cycle_preempt_queues",
     "grove_run_cycle_reclaim_queues", "grove_run_cycle_reclaim_preempt_queues",
@@ -256,6 +257,29 @@ class PlacementEngine:
                                                      C.c_uint32(len(holdings)), _p(st)))
         return {k: st[k][0].item() for k in T.stats_dt.names}
 
+    def run_cycle_preempt_elastic(self, running: np.ndarray, holdings: np.ndarray, surplus: np.ndarray) -> dict:
+        """run_cycle_preempt that shrinks running gangs to their MinReplicas before evicting any whole: `surplus`
+        (T.surplus_pod_dt) lists the pods of the running gangs above MinReplicas, each gang's in the order it gives them up.  Every
+        priority class first admits what fits on free plus those pods (tables.STATUS_SURPLUS_ONLY), then evicts whole gangs for the
+        rest (include/grove_place.h "elastic reclaim"); surplus_victims() lists the pods taken, victims() the gangs evicted"""
+        running = np.ascontiguousarray(running, dtype=T.running_dt)
+        holdings = np.ascontiguousarray(holdings, dtype=T.holding_dt)
+        surplus = np.ascontiguousarray(surplus, dtype=T.surplus_pod_dt)
+        st = np.zeros(1, dtype=T.stats_dt)
+        self._check(self.lib.grove_run_cycle_preempt_elastic(self.h, _p(running), C.c_uint32(len(running)), _p(holdings),
+                                                             C.c_uint32(len(holdings)), _p(surplus), C.c_uint32(len(surplus)),
+                                                             _p(st)))
+        return {k: st[k][0].item() for k in T.stats_dt.names}
+
+    def surplus_victims(self) -> np.ndarray:
+        """(surplus pod, preemptor gang) pairs of the last run_cycle_preempt_elastic, in eviction order: the caller terminates
+        those pods, and their gangs keep running (empty after any other cycle)"""
+        n = C.c_uint32(0)
+        self._check(self.lib.grove_get_surplus_victims(self.h, None, C.c_uint32(0), C.byref(n)))
+        out = np.zeros(max(n.value, 1), dtype=T.surplus_victim_dt)
+        self._check(self.lib.grove_get_surplus_victims(self.h, _p(out), C.c_uint32(len(out)), C.byref(n)))
+        return out[: n.value]
+
     def run_cycle_reuse(self, replaces: np.ndarray, running: np.ndarray, holdings: np.ndarray) -> dict:
         """the ordinary cycle in which gang g with replaces[g] = r != NONE_U32 is the new version of running gang r
         (PodGangSpec.ReuseReservationRef): it may use what r holds (`running` T.running_dt, `holdings` T.holding_dt), nobody else
@@ -333,9 +357,9 @@ class PlacementEngine:
         return {k: st[k][0].item() for k in T.stats_dt.names}
 
     def victims(self) -> np.ndarray:
-        """(running gang, preemptor gang) pairs of the last run_cycle_preempt / run_cycle_reuse_preempt /
-        run_cycle_preempt_queues / run_cycle_reclaim_queues / run_cycle_reclaim_preempt_queues: the caller sets
-        DisruptionTarget on them"""
+        """(running gang, preemptor gang) pairs of the last run_cycle_preempt / run_cycle_preempt_elastic /
+        run_cycle_reuse_preempt / run_cycle_preempt_queues / run_cycle_reclaim_queues / run_cycle_reclaim_preempt_queues: the
+        caller sets DisruptionTarget on them"""
         n = C.c_uint32(0)
         self._check(self.lib.grove_get_victims(self.h, None, C.c_uint32(0), C.byref(n)))
         out = np.zeros(max(n.value, 1), dtype=T.victim_dt)

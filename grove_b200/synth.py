@@ -192,6 +192,17 @@ def config_c4(n=50000, g=10000, seed=SEED_BASE + 4, max_used_pct=90):
     return dict(name="C4", n_levels=4, nodes=nodes, tables=b.build())
 
 
+def c4_surplus(cliques, share=0.5, seed=SEED_BASE + 419):
+    """A C4-style submission whose worker PodGroups scale out: about `share` of the worker cliques (MinReplicas 4) ask for 1-3 pods
+    more than MinReplicas, which a cycle binds best effort -- once running, the surplus pods grove_run_cycle_preempt_elastic may
+    take back.  -> a copy of `cliques`"""
+    out = cliques.copy()
+    work = np.nonzero(out["min_replicas"] == 4)[0]
+    pick = work[_rand_below(seed, 30, len(work), 1000) < int(share * 1000)]
+    out["replicas"][pick] = out["min_replicas"][pick] + 1 + _rand_below(seed, 31, len(pick), 3).astype(np.uint8)
+    return out
+
+
 def c4_spread_groups(gangs, cliques, size=8, level=0, mode=T.SPREAD_HARD, max_skew=1):
     """Topology spread groups over a C4-style submission (grove_set_spread): its base gangs whose Required level is `level` or
     deeper, in groups of `size` by (priority, template) -- the replicas of one PodCliqueSet.  -> (T.spread_dt groups, gang_group)"""

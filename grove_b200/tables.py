@@ -49,6 +49,12 @@ holding_dt = np.dtype([("node", np.uint32), ("cpu_milli", np.uint32), ("mem_mib"
 running_dt = np.dtype([("priority", np.int32), ("holding_off", np.uint32), ("n_holdings", np.uint32), ("reserved", np.uint32)])
 victim_dt = np.dtype([("running", np.uint32), ("preemptor", np.uint32)])
 STATUS_PREEMPTOR = 0x1
+# elastic reclaim (grove_run_cycle_preempt_elastic, include/grove_place.h "elastic reclaim"): one pod of a running gang above its
+# PodGroup's MinReplicas, and a (surplus pod, preemptor) pair
+surplus_pod_dt = np.dtype([("running", np.uint32), ("node", np.uint32), ("cpu_milli", np.uint32), ("mem_mib", np.uint32),
+                           ("gpu", np.uint16), ("reserved", np.uint16)])
+surplus_victim_dt = np.dtype([("pod", np.uint32), ("preemptor", np.uint32)])
+STATUS_SURPLUS_ONLY = 0x100       # status reserved0, with STATUS_PREEMPTOR: admitted by the surplus pass (took surplus pods only)
 status_dt = np.dtype([
     ("state", "u1"), ("level", "u1"), ("reserved0", "<u2"), ("score_num", "<u2"), ("score_den", "<u2"),
     ("n_pods", "<u4"), ("placement_off", "<u4"), ("domain_node", "<u4"), ("reserved1", "<u4", (3,)),
@@ -110,6 +116,7 @@ assert config_dt.itemsize == 32 and stats_dt.itemsize == 64
 assert gang_diag_dt.itemsize == 16 and clique_diag_dt.itemsize == 40
 assert spread_dt.itemsize == 8 and spread_seed_dt.itemsize == 8 and queue_dt.itemsize == 56
 assert queue_quota_dt.itemsize == 24 and queue_weight_dt.itemsize == 16
+assert surplus_pod_dt.itemsize == 20 and surplus_victim_dt.itemsize == 8
 
 
 def make_nodes(n: int) -> np.ndarray:

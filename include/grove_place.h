@@ -154,7 +154,9 @@ typedef struct grove_gang_status {
                               GROVE_STATUS_OVER_LIMIT / GROVE_STATUS_SURPLUS_CAPPED = a queue member held back by its queue
                               chain's limits (grove_set_queues), GROVE_STATUS_RECLAIMER = admitted by the class pass of
                               grove_run_cycle_reclaim_queues (or the reclaim pass of
-                              grove_run_cycle_reclaim_preempt_queues, whose preempt pass sets GROVE_STATUS_PREEMPTOR); else 0 */
+                              grove_run_cycle_reclaim_preempt_queues, whose preempt pass sets GROVE_STATUS_PREEMPTOR),
+                              GROVE_STATUS_SURPLUS_ONLY = with GROVE_STATUS_PREEMPTOR, admitted by the surplus pass of
+                              grove_run_cycle_preempt_elastic; else 0 */
   uint16_t score_num;      /* PlacementScore = score_num / score_den (podgang.go:187-189): over the gang, its scopes and
                               its cliques that carry a pack constraint, (levels honoured) / (levels asked for), where
                               asked = Preferred if set else Required; 1/1 when nothing was asked or everything held;
@@ -275,6 +277,50 @@ typedef struct grove_victim {
 int32_t grove_run_cycle_preempt(grove_engine_t* e, const grove_running_gang_t* running, uint32_t n_running,
                                 const grove_holding_t* holdings, uint32_t n_holdings, grove_cycle_stats_t* stats);
 int32_t grove_get_victims(grove_engine_t* e, grove_victim_t* out, uint32_t cap, uint32_t* n_out);
+
+/* ---- elastic reclaim ------------------------------------------------------------------------------
+ * The reclaim pass, shrinking running gangs to their MinReplicas before evicting any whole (DESIGN.md section 1, "Elastic
+ * reclaim").  The reference pins the contract (PodGroup.MinReplicas, podgang.go:80-83: "guaranteed gang scheduling is only
+ * provided for MinReplicas"); the arithmetic is ours.  Inputs are those of grove_run_cycle_preempt plus the SURPLUS PODS: one
+ * record per pod of a running gang above its PodGroup's MinReplicas, a gang's pods in the order it gives them up (for Grove the
+ * highest PodReference index first).  A surplus pod is part of its gang's holdings on its node and takes 1 pod slot plus its cpu,
+ * mem and gpu.  F is the free table; E(p) the standing running gangs of a priority below p.  A taken surplus pod is gone, its
+ * gang keeps standing.
+ *   1. The ordinary pass: grove_run_cycle.
+ *   2. Every priority p of a gang still REJECTED, descending, while E(p) is non-empty; its members are its REJECTED gangs in rank
+ *      order, each evaluated once as grove_run_cycle_preempt evaluates it (K3, same candidate order, ordinary-pass anchor).
+ *      Pass 1, only when some untaken surplus pod of E(p) stands: each member against F + the untaken surplus pods of E(p),
+ *      skipped once none stands; admitted: GROVE_STATUS_PREEMPTOR | GROVE_STATUS_SURPLUS_ONLY, and it takes surplus pods only.
+ *      Pass 2, the members pass 1 did not admit: each against F + what the standing gangs of E(p) still hold (holdings minus their
+ *      taken pods), skipped once E(p) is empty; admitted: GROVE_STATUS_PREEMPTOR.
+ *   3. The node step of an admitted g, node by node in the order its placement first names them, need = what g puts there:
+ *      while F does not cover need: if F + the untaken surplus pods there of the standing gangs of E(p) covers it, take such pods
+ *      one at a time until F does (the gang by the victim rule -- lowest priority, then highest running index -- then its
+ *      first-listed untaken pod on the node) and stop; else evict WHOLE, by the victim rule, the next gang of E(p) that still holds
+ *      something on the node: everything it still holds anywhere, its untaken surplus pods included, returns to F.  Then F -= need.
+ * grove_get_victims lists the whole-gang evictions, grove_get_surplus_victims the (surplus pod, preemptor) pairs, each in
+ * eviction order; a gang that lost pods is not a victim unless it was later evicted whole.  With n_surplus == 0 every output
+ * equals grove_run_cycle_preempt's.  Refusals: those of grove_run_cycle_preempt, with the same codes; GROVE_ERR_INVALID_ARG for a
+ * surplus pod whose running gang or node is out of range, or a (running gang, node) whose surplus pods add up to more than its
+ * holdings there in cpu, mem, gpu or pods.  grove_diagnose refuses the cycle that follows.  grove_get_surplus_victims returns
+ * GROVE_ERR_STATE before any cycle and 0 pairs after a cycle of any other entry. */
+typedef struct grove_surplus_pod {   /* 20 B */
+  uint32_t running;                  /* index into the running array */
+  uint32_t node;                     /* caller's node index */
+  uint32_t cpu_milli, mem_mib;
+  uint16_t gpu;
+  uint16_t reserved;
+} grove_surplus_pod_t;
+typedef struct grove_surplus_victim {
+  uint32_t pod;                      /* index into the surplus array */
+  uint32_t preemptor;                /* gang index of the submission */
+} grove_surplus_victim_t;
+#define GROVE_STATUS_SURPLUS_ONLY 0x100u /* grove_gang_status_t.reserved0: a preemptor admitted by pass 1 of
+                                            grove_run_cycle_preempt_elastic (it evicted surplus pods only) */
+int32_t grove_run_cycle_preempt_elastic(grove_engine_t* e, const grove_running_gang_t* running, uint32_t n_running,
+                                        const grove_holding_t* holdings, uint32_t n_holdings,
+                                        const grove_surplus_pod_t* surplus, uint32_t n_surplus, grove_cycle_stats_t* stats);
+int32_t grove_get_surplus_victims(grove_engine_t* e, grove_surplus_victim_t* out, uint32_t cap, uint32_t* n_out);
 
 /* ---- reservation reuse ---------------------------------------------------------------------------
  * The API names it (PodGangSpec.ReuseReservationRef, podgang.go:65-71: "During updates, an operator can suggest to reuse the

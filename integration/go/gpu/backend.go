@@ -51,6 +51,10 @@ type schedulerBackend struct {
 	levels   []string                                    // ClusterTopology.Spec.Levels[].Key, broadest first
 	running  map[string]runningGang                      // PodGangs scheduled by this backend: priority + holdings (reclaim pass)
 	preempt  bool
+	// elastic: with preempt also on and no queue or consolidation switch, a pass with running gangs is
+	// grove_run_cycle_preempt_elastic: preemptors take the running gangs' pods beyond MinReplicas before evicting any gang whole
+	// (GpuBackend::SetElasticPreemption in the C++ mirror)
+	elastic bool
 	// preemptQueues: with preempt also on, queue members stay in the pass and a pass with members is
 	// grove_run_cycle_preempt_queues (GpuBackend::SetPreemptionWithinQueues in the C++ mirror)
 	preemptQueues bool
@@ -112,6 +116,16 @@ const (
 	labelPartOf      = "app.kubernetes.io/part-of"
 	labelBasePodGang  = "grove.io/base-podgang"
 )
+
+// SetElasticPreemption: with it and preemption on (no queue or consolidation switch), a pass with running PodGangs runs
+// grove_run_cycle_preempt_elastic: the bound pods of each running PodGroup beyond MinReplicas are surplus, and a preemptor takes
+// those before it evicts any PodGang whole (DESIGN.md section 1 "Elastic reclaim").  A PodGang that lost pods keeps running and
+// is not a DisruptionTarget; the backend deletes those pods and forgets what they held.  Off by default.
+func (b *schedulerBackend) SetElasticPreemption(on bool) {
+	b.mu.Lock()
+	defer b.mu.Unlock()
+	b.elastic = on
+}
 
 // SetPreemptionWithinQueues: with it and preemption on, queue members are no longer kept out of a pass with preemption, and a
 // pass with members runs grove_run_cycle_preempt_queues: a member its queue chain turns away may evict lower-priority PodGangs of
@@ -1041,6 +1055,8 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 			t.cd, t.owner0 = cd, owner0
 		}
 	}
+	// elastic reclaim: t.surplus lists the bound pods of each gang of t.running beyond its PodGroups' MinReplicas
+	t.elastic = preempt && b.elastic && !b.preemptQueues && !b.reclaimQueues && !b.reclaimThenPreempt && b.consMax == 0
 	rejectedFor := map[string]int{}
 	for k, v := range b.rejectedFor {
 		rejectedFor[k] = v
@@ -1165,6 +1181,9 @@ func (b *schedulerBackend) runCycle(ctx context.Context) error {
 		if err := b.client.Status().Update(ctx, pg); err != nil {
 			return err
 		}
+	}
+	for _, v := range res.surplusVictims { // a pod beyond MinReplicas: deleted, its PodGang keeps running (podgang.go:80-83)
+		b.evictSurplusPod(ctx, int(v.pod), rows[v.preemptor])
 	}
 	for _, v := range res.victims { // podgang.go:166-170, reason 1
 		b.markDisruptionTarget(ctx, int(v.running), rows[v.preemptor])

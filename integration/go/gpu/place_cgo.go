@@ -55,6 +55,11 @@ type tables struct {
 	// reclaim pass (optional): PodGangs this backend scheduled earlier and what they hold per node
 	running  []C.grove_running_gang_t
 	holdings []C.grove_holding_t
+	// elastic reclaim: the pass is grove_run_cycle_preempt_elastic over these surplus pods (the bound pods of the running gangs
+	// beyond MinReplicas, each gang's highest PodReference index first); set only with SetElasticPreemption and preemption, in a
+	// pass without queue members
+	elastic bool
+	surplus []C.grove_surplus_pod_t
 	// topology spread (optional; never together with the reclaim pass): the groups, each gang row's group (GROVE_NONE_U32 =
 	// none) and the running replicas
 	spreadGroups []C.grove_spread_t
@@ -96,6 +101,8 @@ type result struct {
 	placements []C.grove_placement_t
 	status     []C.grove_gang_status_t
 	victims    []C.grove_victim_t
+	// elastic reclaim: (surplus pod of tables.surplus, preemptor row) per pod taken (grove_get_surplus_victims)
+	surplusVictims []C.grove_surplus_victim_t
 	moves      []C.grove_move_t // consolidation: (running gang, target row) per relocated gang
 	stats      C.grove_cycle_stats_t
 	// with over-quota weights, after a pass that ran with quotas or fairShare: 3 fair shares per queue (grove_get_fair_shares)
@@ -186,6 +193,25 @@ func (e *engine) cycle(t *tables, preempt, large, explain bool) (*result, error)
 			if err := e.err(C.grove_run_cycle_preempt_queues(e.h, &t.running[0], C.uint32_t(len(t.running)), hp,
 				C.uint32_t(len(t.holdings)), &t.runningQueue[0], &r.stats)); err != nil {
 				return nil, err
+			}
+		} else if t.elastic {
+			var sp *C.grove_surplus_pod_t
+			if len(t.surplus) > 0 {
+				sp = &t.surplus[0]
+			}
+			if err := e.err(C.grove_run_cycle_preempt_elastic(e.h, &t.running[0], C.uint32_t(len(t.running)), hp,
+				C.uint32_t(len(t.holdings)), sp, C.uint32_t(len(t.surplus)), &r.stats)); err != nil {
+				return nil, err
+			}
+			var n C.uint32_t
+			if err := e.err(C.grove_get_surplus_victims(e.h, nil, 0, &n)); err != nil {
+				return nil, err
+			}
+			if n > 0 {
+				r.surplusVictims = make([]C.grove_surplus_victim_t, int(n))
+				if err := e.err(C.grove_get_surplus_victims(e.h, &r.surplusVictims[0], n, &n)); err != nil {
+					return nil, err
+				}
 			}
 		} else if err := e.err(C.grove_run_cycle_preempt(e.h, &t.running[0], C.uint32_t(len(t.running)), hp,
 			C.uint32_t(len(t.holdings)), &r.stats)); err != nil {
